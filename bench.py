@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — RegisterFrame throughput of the B200-native CT-ICP engine on BASELINE.json's metric.
+"""bench.py — RegisterFrame throughput of the H100-native CT-ICP engine on BASELINE.json's metric.
 
 A "step" is one cticp RegisterFrame of one synthetic KITTI-shape 64-beam scan (HDL-64E ring table, ~130k returns of the
 "suburb" scene: F ~ 12k frame points, K ~ 2.6k keypoints) with the driving options of BASELINE.json configs[1] (solver GN,
@@ -16,10 +16,15 @@ frames are registered untimed.
               corrected_points, all_corrected_points and keypoints are transformed, copied back and assembled into
               caller-owned arrays of 64-byte WPoint3D records inside the timed region
   roofline    k_gn_persistent (all ICP iterations of a frame in one launch: gather + selection + reduce + solve):
-              algorithmic bytes per launch / CUDA-event time per launch vs the measured HBM copy bandwidth
+              algorithmic bytes per launch / CUDA-event time per launch vs the H100 SXM data-sheet HBM3 bandwidth
   cpu_baseline  the CPU oracle (restatement of the reference's path with the reference's threading) on the same frames
   extra_workloads  configs[2] (driving_config.yaml, solver CERES as a device LM/IRLS loop) and configs[4] (dense 128-beam
-              scans, 20 forced GN iterations) measured the same way on fewer frames, each with its own cpu_baseline
+              scans, 20 forced GN iterations) measured the same way over --steps timed frames (shorter preroll), each with
+              its own cpu_baseline on fewer frames
+
+`--dump-outputs DIR` writes what the timed path (register_staged) returned for its last timed step as DIR/<name>.npy
+(float64): the frame's begin / end poses, the summary's counters and its three point vectors. The scans are seeded, so
+two builds run with the same arguments can be compared output for output.
 
 `--impl reference` times only the CPU oracle (the reference itself cannot be built offline, see DESIGN.md).
 N > 1 (torchrun): every rank registers the same scans with the keypoints sharded rank/world; the JTJ/JTr sums are
@@ -42,16 +47,16 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 METRIC = "scans/sec (RegisterFrame) on 64-beam ~120k-pt clouds"
 UNIT = "scans/s"
-WORKLOAD = "configs[1]: KITTI-shape 64-beam synthetic scans, CT_ICP_GN point-to-plane, 5 ICP iters, 1xB200"
+WORKLOAD = "configs[1]: KITTI-shape 64-beam synthetic scans, CT_ICP_GN point-to-plane, 5 ICP iters, 1xH100"
 
 
 WORKLOADS = {
     # name: (sensor, description)
     "kitti64_gn": ("HDL64E", WORKLOAD),
     "kitti64_ceres": ("HDL64E", "configs[2]: KITTI-shape 64-beam synthetic scans, driving_config.yaml (solver CERES as device "
-                                "LM/IRLS, Cauchy, 5x5 iterations, 900 residuals), 1xB200"),
+                                "LM/IRLS, Cauchy, 5x5 iterations, 900 residuals), 1xH100"),
     "dense128_gn": ("DENSE128", "configs[4]: dense 128-beam ~290k-pt synthetic scans, CT_ICP_GN, 20 ICP iterations forced, "
-                                "voxel 0.25 / sample 0.5, 1xB200"),
+                                "voxel 0.25 / sample 0.5, 1xH100"),
 }
 _WORKLOAD = "kitti64_gn"
 SCENE_PROFILE = "suburb"
@@ -105,7 +110,7 @@ def make_options(b):
 
 
 class ClockSampler:
-    """SM clock and clock-event (throttle) reasons sampled DURING the timed region (B200_PROFILING.md's clocks line).
+    """SM clock and clock-event (throttle) reasons sampled DURING the timed region.
 
     In-process NVML (pynvml) from a daemon thread every 20 ms (the timed regions are only tens of ms long; at 5 ms the queries began to show in the step times) — two cheap queries per sample, no child process next
     to the HOST-timed end-to-end steps; `nvidia-smi -lms 200` is the fallback (CTICP_BENCH_CLOCKS=smi forces it)."""
@@ -205,7 +210,7 @@ def make_scans(n_frames, sensor_name):
 
 def workload_config(workload_text, world, seq, first, count, frame_points, keypoints, iters, preroll):
     """The `config` object of a bench line: identical keys and values for the native and the reference arm."""
-    return {"workload": workload_text.replace("1xB200", "%dxB200" % world),
+    return {"workload": workload_text.replace("1xH100", "%dxH100" % world),
             "scene": "synthetic '%s' scene, %s" % (SCENE_PROFILE, "ct_icp_b200/synthetic.py"),
             "points_per_scan": round(float(np.mean([len(s["xyz"]) for s in seq[first:first + count]])), 1),
             "frame_points": round(frame_points, 1), "keypoints": round(keypoints, 1),
@@ -245,23 +250,8 @@ CPU_SAMPLE_NOTE = ("CPU oracle restating the reference's RegisterFrame with the 
                    "uses tsl::robin_map (oracle/orc_core.h)")
 
 
-def load_traffic():
-    """dram bytes per launch of the GN kernel from the committed ncu capture summary (profiles/), if any."""
-    for name in ("r03_gn_persistent_ncu_summary.json", "r02_gn_persistent_ncu_summary.json", "gather_kernel_ncu_summary.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                return json.load(f).get("dram_bytes_per_launch")
-        except Exception:
-            continue
-    return None
-
-
-def measured_peak_gbs():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+# NVIDIA's data sheet for the H100 SXM (HBM3): the denominator of roofline.frac, not a bandwidth this bench measured
+HBM_PEAK_GBS = 3350.0
 
 
 class Dist:
@@ -302,8 +292,9 @@ def pose_vector(sm):
                     list(sm.frame.end_pose.quat))
 
 
-def run_native(eng, D, seq, preroll, W, K, n_roof, with_dropin=True, parity_frames=0):
-    """All GPU passes of one workload over `seq`. Returns the fields of the bench line (rank 0) — timing is max over ranks."""
+def run_native(eng, D, seq, preroll, W, K, n_roof, with_dropin=True, parity_frames=0, dump=None):
+    """All GPU passes of one workload over `seq`. Returns the fields of the bench line (rank 0) — timing is max over ranks.
+    dump: a dict that receives the outputs of pass A's last timed step (see dump_arrays)."""
     from ct_icp_b200 import _abi as abi
     torch = D.torch
     world, rank, device = D.world, D.rank, D.device
@@ -351,6 +342,8 @@ def run_native(eng, D, seq, preroll, W, K, n_roof, with_dropin=True, parity_fram
         f_sum += sm.num_corrected_points
         iters_sum += t.icp_iterations
     D.barrier()
+    if dump is not None:
+        dump.update(dump_arrays(od, sm))
     total_ms = D.max_over_ranks(float(np.sum(step_ms)))
     out = {"value": K / (total_ms / 1e3), "ms_per_step": total_ms / K, "gpu_launches": launches,
            "frame_points": f_sum / K, "keypoints": kp_sum / K, "iters": iters_sum / K}
@@ -374,12 +367,11 @@ def run_native(eng, D, seq, preroll, W, K, n_roof, with_dropin=True, parity_fram
         od.set_gather_timing(False)
         stencil = 27        # (2r+1)^3 with r = ceil(0.8 / 1.0) = 1
         alg_bytes = g_kp * (16 + 16 * stencil) + 16 * g_pts          # SURVEY §8d: keypoint + slot probes + map points
-        peak, peak_src = measured_peak_gbs()
         if g_launch and g_ms > 0:
             achieved = (alg_bytes / g_launch) / (g_ms / g_launch * 1e-3) / 1e9
             roofline = {"bound": "hbm", "kernel": "k_gn_persistent (all ICP iterations of a frame: gather + selection + reduce + solve)",
-                        "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": load_traffic(),
-                        "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes / g_launch,
+                        "achieved": achieved, "peak": HBM_PEAK_GBS, "unit": "GB/s", "frac": achieved / HBM_PEAK_GBS,
+                        "peak_source": "H100 SXM data sheet, 3.35 TB/s", "algorithmic_bytes_per_launch": alg_bytes / g_launch,
                         "us_per_launch": g_ms / g_launch * 1e3, "keypoint_iterations_per_launch": g_kp / g_launch,
                         "us_per_1k_keypoint_iterations": (g_ms * 1e3) / max(g_kp, 1) * 1e3,
                         "mean_stencil_points": g_pts / max(g_kp, 1), "launches_timed": g_launch,
@@ -457,6 +449,40 @@ def run_native(eng, D, seq, preroll, W, K, n_roof, with_dropin=True, parity_fram
     return out
 
 
+def dump_arrays(od, sm):
+    """What a caller of register_staged receives for one frame: the summary's poses and counters, and its three point
+    vectors (fetched on demand, after the timed region) as world coordinates."""
+    from ct_icp_b200 import _abi as abi
+
+    def pose(p):
+        return list(p.tr) + list(p.quat) + [p.dest_timestamp]
+    out = {"frame_pose": np.array([pose(sm.frame.begin_pose), pose(sm.frame.end_pose)], dtype=np.float64),
+           "summary": np.array([sm.success, sm.sample_size, sm.number_of_residuals, sm.num_corrected_points,
+                                sm.num_all_corrected_points, sm.num_keypoints, sm.icp_summary.num_iters,
+                                sm.distance_correction, sm.relative_distance, sm.relative_orientation,
+                                sm.ego_orientation], dtype=np.float64)}
+    for name, which in (("corrected_points", abi.POINTS_CORRECTED), ("all_corrected_points", abi.POINTS_ALL_CORRECTED),
+                        ("keypoints", abi.POINTS_KEYPOINTS)):
+        out[name] = np.ascontiguousarray(od.points(which)["world"], dtype=np.float64)
+    return out
+
+
+DUMP_LIMIT = 64 << 20
+
+
+def write_dump(arrays, out_dir):
+    """DIR/<name>.npy; above DUMP_LIMIT bytes in all, every point array keeps the same fixed, seeded sample fraction of its
+    rows (in their original order)."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    keep = min(1.0, DUMP_LIMIT / total) if total else 1.0
+    for name, a in arrays.items():
+        if keep < 1.0 and a.ndim == 2 and len(a) > 16:
+            n = max(1, int(len(a) * keep * 0.99))
+            a = a[np.sort(np.random.default_rng(1234).choice(len(a), n, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def cpu_baseline_for(seq, first, steps, cores):
     v, times, f, k, it = run_oracle(seq, first, steps)
     threads = oracle_threads()
@@ -477,6 +503,8 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the configs[2] / configs[4] extra workloads")
     ap.add_argument("--workload", default="kitti64_gn", choices=sorted(WORKLOADS),
                     help="kitti64_gn is BASELINE.json's metric configuration (the bench line)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64, at most 64 MB in all)")
     args = ap.parse_args()
     global _WORKLOAD, WORKLOAD
     _WORKLOAD = args.workload
@@ -519,7 +547,8 @@ def main():
     clocks = ClockSampler(D.device)
     D.barrier()
     clocks.start()
-    res = run_native(eng, D, seq, preroll, W, K, n_roof, with_dropin=True, parity_frames=6 if world > 1 else 0)
+    dump = {} if args.dump_outputs and rank == 0 else None
+    res = run_native(eng, D, seq, preroll, W, K, n_roof, with_dropin=True, parity_frames=6 if world > 1 else 0, dump=dump)
     clock_info = clocks.stop()     # sampled from the start of the device-timed steps to the end of the e2e steps
 
     cpu_baseline = None
@@ -530,7 +559,7 @@ def main():
     extras = None
     if args.workload == "kitti64_gn" and not args.no_extras:
         extras = {}
-        plan = {"kitti64_ceres": (args.preroll, 3, 12, 10), "dense128_gn": (6, 3, 6, 2)}
+        plan = {"kitti64_ceres": (args.preroll, 3, K, min(K, 10)), "dense128_gn": (6, 3, K, min(K, 2))}
         if world > 1:
             plan.pop("kitti64_ceres")   # N > 1: only the configuration the sweep of BASELINE.json configs[4] is about
         for name, (xp, xw, xk, xcpu) in plan.items():
@@ -569,6 +598,8 @@ def main():
         if extras is not None:
             line["extra_workloads"] = extras
         print(json.dumps(line))
+    if dump:
+        write_dump(dump, args.dump_outputs)
     if D.dist is not None:
         D.dist.destroy_process_group()
     return 0

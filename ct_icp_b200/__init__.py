@@ -1,7 +1,7 @@
-"""ct_icp_b200 — B200-native CT-ICP registration engine behind the ct_icp::Odometry API surface.
+"""ct_icp_b200 — H100-native CT-ICP registration engine behind the ct_icp::Odometry API surface.
 
 Python host mirror of the reference interface (ct_icp::Odometry, CTICPOptions, OdometryOptions,
-MultipleResolutionVoxelMap) over the C ABI in include/cticp.h. All compute runs in hand-written sm_100a kernels
+MultipleResolutionVoxelMap) over the C ABI in include/cticp.h. All compute runs in hand-written sm_90a kernels
 (ct_icp_b200/csrc); this package only marshals arrays and option structs.
 """
 from . import _abi as abi

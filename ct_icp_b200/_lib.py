@@ -1,7 +1,7 @@
 """Loads the engine (ct_icp_b200/libcticp_b200.so, built by __graft_entry__.build() / csrc/Makefile).
 
-There is no CPU fallback: a missing library raises, and creating an Odometry / VoxelMap without a usable sm_100
-device fails with CTICP_ERR_NO_DEVICE.
+There is no CPU fallback: a missing library raises, and creating an Odometry / VoxelMap without a usable sm_90
+(H100) device fails with CTICP_ERR_NO_DEVICE.
 """
 import ctypes
 import os
@@ -19,7 +19,7 @@ class EngineNotBuilt(RuntimeError):
 
 
 def build(verbose=False):
-    """nvcc -gencode arch=compute_100a,code=sm_100a … → libcticp_b200.so (cross-compiles without a GPU)."""
+    """nvcc -gencode arch=compute_90a,code=sm_90a … → libcticp_b200.so (cross-compiles without a GPU)."""
     import subprocess
     r = subprocess.run(["make", "-C", os.path.join(_PKG, "csrc"), "-j8"], capture_output=True, text=True)
     if verbose or r.returncode != 0:

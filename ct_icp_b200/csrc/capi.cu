@@ -55,7 +55,7 @@ void RequireDevice(int device) {
     CAPI_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     CAPI_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) throw std::runtime_error("NO_DEVICE: this build targets sm_100a (Blackwell B200) only");
+    if (prop.major != 9 || prop.minor != 0) throw std::runtime_error("NO_DEVICE: this build targets sm_90a (Hopper H100) only");
 }
 }  // namespace
 

@@ -255,8 +255,8 @@ __global__ void k_remove_far(MapLevel L, MapCounters *ctr, V3 loc, double distan
 
 // ---- the whole map update of a frame (odometry.cpp:855-953: transform of the sub-sampled frame with the final pose pair,
 // RemoveElementsFarFromLocation, InsertPointCloud on every resolution) in ONE cooperative launch: phases separated by
-// grid barriers instead of 2 + 2 x levels kernels and their memsets (29 us of a 310 us step in round 1, most of it the
-// fixed cost of five short dependent launches).
+// grid barriers instead of 2 + 2 x levels kernels and their memsets (most of their time was the fixed cost of five
+// short dependent launches).
 struct FusedUpdateArgs {
     MapLevel levels[CTICP_MAX_RESOLUTIONS];
     int num_levels;
@@ -464,12 +464,12 @@ void DeviceMap::InsertDevice(const double *d_world_xyz, const int *d_n, size_t n
     }
     const int frame_ordinal = (int) frame_count_++;
     const int threads = 256;
-    const int blocks = (int) std::min<size_t>((n_upper + threads - 1) / threads, 148 * 8);
+    const int blocks = (int) std::min<size_t>((n_upper + threads - 1) / threads, 132 * 8);
     for (size_t i = 0; i < levels_.size(); ++i) {
         MapCounters *ctr = d_counters_ + i;
         CT_CUDA_CHECK(cudaMemsetAsync(&ctr->num_touched, 0, sizeof(unsigned), stream_));
         k_insert_claim<<<blocks, threads, 0, stream_>>>(levels_[i], ctr, d_world_xyz, d_n, d_next_, d_touched_);
-        const int cblocks = (int) std::min<size_t>((n_upper + kInsertWarps - 1) / kInsertWarps, 148 * 8);
+        const int cblocks = (int) std::min<size_t>((n_upper + kInsertWarps - 1) / kInsertWarps, 132 * 8);
         k_insert_commit<<<cblocks, kInsertWarps * 32, 0, stream_>>>(levels_[i], ctr, d_world_xyz, d_next_, d_touched_,
                                                                      d_frame_origins_, frame_ordinal);
         launches_ += 2;
@@ -514,7 +514,7 @@ void DeviceMap::UpdateFused(const float4 *d_frame, const float4 *d_frame_lo, con
         frame_ordinal = (int) frame_count_++;
     }
     if (fused_grid_ == 0) {
-        int per_sm = 0, dev = 0, sms = 148;
+        int per_sm = 0, dev = 0, sms = 132;
         CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_map_update_fused, kInsertWarps * 32, 0));
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);

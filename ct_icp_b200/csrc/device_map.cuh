@@ -4,7 +4,7 @@
 // becomes, per resolution, one open-addressed table of 16-byte slots {key, count} with linear probing, and one
 // fixed-stride float4 point array in which slot s owns points [s*B, s*B + count).  Points are stored as fp32 offsets
 // from their voxel's origin (voxel * resolution), so storage error is <= 6e-8 m at any world coordinate while all
-// geometry is evaluated in fp64 (SURVEY §7 "Precision").  HBM is plentiful (180 GB): the fixed stride removes the
+// geometry is evaluated in fp64 (SURVEY §7 "Precision").  HBM is plentiful (80 GB): the fixed stride removes the
 // allocator, the second dependent pointer load of the reference (bucket → vector → heap block) and makes a voxel's
 // points one contiguous <= B*16-byte run.
 #pragma once

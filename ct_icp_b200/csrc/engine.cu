@@ -1,4 +1,4 @@
-// engine.cu — host orchestration of the B200-native odometry (see engine.h).
+// engine.cu — host orchestration of the H100-native odometry (see engine.h).
 #include "engine.h"
 
 #include <algorithm>
@@ -97,7 +97,7 @@ Engine::Engine(const cticp_odometry_options &options, int device) : options_(opt
     CT_CUDA_CHECK(cudaSetDevice(device));
     cudaDeviceProp prop;
     CT_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) throw std::runtime_error("NO_DEVICE: this build targets sm_100a (Blackwell B200) only");
+    if (prop.major != 9 || prop.minor != 0) throw std::runtime_error("NO_DEVICE: this build targets sm_90a (Hopper H100) only");
 
     // Odometry::Odometry, odometry.cpp:697-734: motion_compensation overrides the ICP parametrisation
     switch (options_.motion_compensation) {
@@ -364,8 +364,8 @@ void Engine::IngestImpl(const ScanView &scan, const FrameInfo &info, int64_t sta
         pipe_->DistortFrame(tr.begin_pose.pose.q, tr.begin_pose.pose.t, tr.end_pose.pose.q, tr.end_pose.pose.t);
 }
 
-// Host team of the O(N) passes: half of the machine shared by the ranks of this node, 2..16 threads (measured on
-// the 128-CPU B200 host: packing 130k points takes 0.25 ms on 2 threads, 0.085 on 8, 0.073 on 16).
+// Host team of the O(N) passes: half of the machine shared by the ranks of this node, 2..16 threads (packing a 130k-point
+// scan scales up to about 8 threads and gains little beyond 16).
 int Engine::HostTeamSize(int ranks_on_node) {
     const int hw = std::max(1, (int) std::thread::hardware_concurrency());
     // half of the machine divided between the ranks (round 1 gave each rank hw / (4 ranks): 4 threads at 8 ranks on the
@@ -377,10 +377,9 @@ int Engine::HostTeamSize(int ranks_on_node) {
 }
 
 // ---- host fork-join pool -------------------------------------------------------------------------------------
-// The CPUs of the caller's socket (those the process may use): the team is kept on ONE socket. Measured on the 2 x 32-core
-// host of the B200 box (profiles/README.md): a team scattered over both sockets packs a 130k-point scan in 145-175 us,
-// the same team confined to either socket in 100-110 us (the pinned staging buffer and the caller's arrays are then
-// local to everyone, and the parts' barrier does not cross the socket link).
+// The CPUs of the caller's socket (those the process may use): the team is kept on ONE socket. On a two-socket host a
+// team scattered over both sockets packs a scan markedly slower than the same team confined to either socket (the pinned
+// staging buffer and the caller's arrays are then local to everyone, and the parts' barrier does not cross the socket link).
 static bool SocketCpuSet(cpu_set_t *out) {
     const char *env = getenv("CTICP_HOST_AFFINITY");
     if (env && atoi(env) == 0) return false;
@@ -516,7 +515,7 @@ template <typename T> inline T LoadUnaligned(const char *p) {   // PointCloud2 r
 
 namespace {
 // one packed point: hi = float32(x, y, z, alpha) with a non-temporal store (the packed scan is consumed by the DMA engine,
-// not by this core — keeping it out of the CPU caches took the H2D copy from ~12 GB/s, snooped dirty lines, to PCIe
+// not by this core — keeping it out of the CPU caches spares the H2D copy from snooping dirty lines, so it runs at PCIe
 // speed); for float64 sources also the residual plane lo = value - hi, and whether any coordinate needs it
 template <typename XT>
 inline void PackPoint(XT x, XT y, XT z, double a, float4 *dst, bool *any_lo) {

@@ -1,4 +1,4 @@
-// engine.h — host orchestration of one odometry instance: the B200-native ct_icp::Odometry.
+// engine.h — host orchestration of one odometry instance: the H100-native ct_icp::Odometry.
 //
 // Mirrors the control flow of src/ct_icp/odometry.cpp (RegisterFrame :199-214, InitializeMotion :276-330,
 // InitializeFrame :333-382, DoRegister :386-501, TryRegister :525-601, AssessRegistration :604-684,
@@ -60,8 +60,8 @@ void PackBlockF64Avx2(const double *xyz, const double *t, size_t b, size_t e, do
 // Minimal fork-join pool for the host passes over a scan (timestamp min/max, float4 packing): the only O(N) host
 // work of RegisterFrame. After a job the workers keep polling for the next one for ~1 ms before they go to sleep on a
 // condition variable (what OpenMP runtimes do by default, cf. GOMP_SPINCOUNT): when frames arrive back to back the
-// team starts within a microsecond instead of a futex wake-up per worker (~50 us for 15 workers); at sensor rate
-// (10-20 Hz) the polling is a ~1 % duty cycle. The caller polls for completion as well (the job is ~50 us long).
+// team starts within a microsecond instead of a futex wake-up per worker; at sensor rate (10-20 Hz) the polling is a
+// ~1 % duty cycle. The caller polls for completion as well (the job is a few tens of microseconds long).
 struct CallbackError : std::runtime_error {
     using std::runtime_error::runtime_error;
 };
@@ -188,9 +188,8 @@ private:
     // copy-engine operation and no host round trip between the ICP loop and the map update.
     bool device_tail_ = true;      // CTICP_DEVICE_TAIL=0: AssessRegistration / UpdateMap on the host for every frame
     bool tail_in_kernel_ = false;  // CTICP_TAIL_IN_KERNEL=1: solver GN's persistent kernel decides the tail itself at the end of
-                                   // its loop instead of a separate k_frame_policy launch (three launches per frame; measured
-                                   // neutral, profiles/r03h_bench*.json: 0.2479 vs 0.2483 ms per step — the default keeps the
-                                   // policy in its own one-warp kernel, the same for every solver)
+                                   // its loop instead of a separate k_frame_policy launch (three launches per frame; the
+                                   // default keeps the policy in its own one-warp kernel, the same for every solver)
     bool tail_armed_ = false;      // the coming TryRegister enqueues the device tail (tail_in_ is filled)
     bool tail_launched_ = false;   // the last TryRegister did: h_verdict_ holds this frame's verdict
     FramePolicyIn tail_in_{};

@@ -89,7 +89,7 @@ __global__ void k_grid_mark(const int *__restrict__ d_n, int use_perm, uint64_t 
 // emit: compact the winners in permuted order and (optionally) scatter them through a second permutation (the
 // second shuffle). One CTA per tile of 1024 positions: the exclusive prefix of a position is
 //   Σ tile_count[tiles before] (every CTA re-adds those <= 512 counters) + a CTA-local scan of the tile's flags,
-// which replaces a serial single-CTA scan over all positions (64 us for 130k points) by a fully parallel pass.
+// which replaces a serial single-CTA scan over all positions by a fully parallel pass.
 struct EmitScratch {
     uint32_t red[2][kTileThreads / 32];
     uint32_t warp[kTileThreads / 32];
@@ -190,8 +190,8 @@ k_grid_emit(const float4 *__restrict__ pts, const float4 *__restrict__ lo, const
 }
 
 // ---- both grid selections of a frame (sub_sample_frame N -> F, grid_sampling F -> K) in ONE cooperative launch: seven
-// phases separated by grid barriers instead of six kernels + four memsets. (Each of those kernels lasts 4-11 us for work
-// worth about one: launch ramp, tail, and the dependency on its predecessor; 46 us of a 310 us step in round 1.)
+// phases separated by grid barriers instead of six kernels + four memsets. (Each of those kernels lasted several times
+// its work: launch ramp, tail, and the dependency on its predecessor.)
 struct FusedSampleArgs {
     const float4 *raw;
     const float4 *raw_lo;              // residual plane of the scan (nullptr: float32-representable)
@@ -413,7 +413,7 @@ FramePipeline::~FramePipeline() {
     cudaFree(d_tile2_); cudaFree(d_src2_);
 }
 
-int FramePipeline::Blocks(size_t n) const { return (int) std::max<size_t>(1, std::min<size_t>((n + 255) / 256, 148 * 8)); }
+int FramePipeline::Blocks(size_t n) const { return (int) std::max<size_t>(1, std::min<size_t>((n + 255) / 256, 132 * 8)); }
 
 void FramePipeline::EnsureLo() {
     if (d_raw_lo_) return;
@@ -544,7 +544,7 @@ void FramePipeline::SampleFused(double voxel_size, double sample_voxel_size, uin
         CT_CUDA_CHECK(cudaMalloc(&d_src2_, sizeof(uint32_t) * max_points_));
         int per_sm = 0;
         CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_sample_fused, kTileThreads, 0));
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         int want = 4;   // CTAs per SM: more hide the latency of the probes, fewer make the grid barriers cheaper (A/B knob)

@@ -173,7 +173,7 @@ private:
     static constexpr int kMaxEvents = 64;
     cudaEvent_t ev_begin_[kMaxEvents], ev_end_[kMaxEvents];
     int ev_used_ = 0;
-    int num_sms_ = 148;
+    int num_sms_ = 132;
     int max_coresident_[2] = {0, 0};   // k_gn_persistent<false / true>
     int kp_per_cta_ = 8;               // keypoints per gather CTA below which the persistent grid is not widened further
     bool use_persistent_ = true;

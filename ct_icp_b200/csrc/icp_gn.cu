@@ -30,8 +30,8 @@ namespace cg = cooperative_groups;
     } while (0)
 
 // Warps per CTA of the gather kernels (one keypoint per warp at a time). Fewer, fatter CTAs make the grid-wide
-// barriers and the reduction of the per-CTA partial sums cheaper, and more warps share one SM's instruction cache:
-// measured on config 2 (K ~ 1.2k), GN loop per frame: 4 warps 0.27 ms, 8 warps 0.193 ms, 16 warps 0.181 ms
+// barriers and the reduction of the per-CTA partial sums cheaper, and more warps share one SM's instruction cache: on
+// config 2 (K ~ 1.2k) the GN loop per frame got faster from 4 to 8 to 16 warps (CTICP_GATHER_WARPS selects it)
 // (16 warps x 128 registers = the whole register file: one CTA per SM, ~77 CTAs).
 #ifndef CTICP_GATHER_WARPS
 #define CTICP_GATHER_WARPS 16
@@ -165,9 +165,9 @@ __device__ __noinline__ void warp_gn_solve(const double *acc, SolveScratch &S, I
 // and, when every row of the range is there, the CTA reduces the rows IN KEYPOINT ORDER into the 90 accumulators
 // (gn_cta_reduce_rows): the result does not depend on which warp computed which row, so the work can be handed out
 // dynamically — a warp whose keypoint has a sparse stencil takes the next one while a neighbour is still busy with a
-// dense one — and the registration stays bit-reproducible. Measured before this (profiles/r03b_warp_stamps.log, K = 2430 on
-// 2352 gather warps, static tiles of two): a tile took 9.5k cycles at the median, 17k at p90 and 26k at the maximum, and
-// every iteration waited for that maximum while half of the warps had no tile at all.
+// dense one — and the registration stays bit-reproducible. Per-warp clock64 stamps of the static tiles of
+// two that came before showed a long tail of slow tiles, and every iteration waited for the slowest while half of the
+// warps had no tile at all.
 struct GnPose {
     Q4 qb, qe;
     V3 tb, te;
@@ -203,7 +203,7 @@ struct __align__(16) CtaRows {
 __device__ __forceinline__ int gn_tile_width(int span) {
     // one keypoint per grab while the range is at most two rounds of the CTA's warps (the loop is bound by the slowest
     // keypoint there: balance counts); beyond that one tile per warp, as wide as it gets (throughput: the lane-per-keypoint
-    // phases cost 1/W per keypoint — measured on the dense workload, K = 32k: tiles of 7 cost 6 % more than tiles of 14)
+    // phases cost 1/W per keypoint — on the dense workload, K = 32k, tiles of 7 were slower than tiles of 14)
     if (span <= 2 * CTICP_GATHER_WARPS) return 1;
     const int W = (span + CTICP_GATHER_WARPS - 1) / CTICP_GATHER_WARPS;
     return W < kTileMax ? W : kTileMax;
@@ -449,7 +449,7 @@ __device__ __forceinline__ GnPose load_pose(const IcpState *st) {
     return p;
 }
 
-static_assert(sizeof(GnShared) <= 227 * 1024, "k_gn_persistent: dynamic shared memory of one CTA (sm_100: 227 KB)");
+static_assert(sizeof(GnShared) <= 227 * 1024, "k_gn_persistent: dynamic shared memory of one CTA (sm_90: 227 KB)");
 extern __shared__ __align__(16) unsigned char gn_smem_raw[];
 
 // mode 0: gather + (last CTA) reduce + solve + pose update          [one launch per ICP iteration]
@@ -510,8 +510,8 @@ k_gn_iterate(GatherLaunch cfg, const float4 *__restrict__ keypoints, const int *
 // The loop's dependencies are asymmetric: the solver CTA needs every gather CTA's partial row; a gather CTA needs the solver
 // CTA's new pose — it never needs the OTHER gather CTAs. So a gather CTA only ARRIVES (fence + one atomic, no wait) and then
 // polls the epoch word the solver CTA bumps after publishing the state, and the solver CTA polls the arrival counter. Per
-// iteration that is one L2 round trip on each side instead of two cg::grid.sync() (measured 2.0 us each on 148 CTAs,
-// profiles/r03c_coop_launch_cost.txt: 8k of the ~47k cycles of an iteration) plus the separate fetch of the pose.
+// iteration that is one L2 round trip on each side instead of two cg::grid.sync() (each a full
+// grid-wide round trip; tools/micro/coop_launch_cost.cu measures one) plus the separate fetch of the pose.
 // The launch stays cooperative: the CTAs must be co-resident for the polls to make progress. Every poll is bounded: a
 // protocol error ends the kernel with st->failed = 2 instead of hanging the device.
 // Two sets of words alternate between launches; the solver CTA of a launch zeroes the set of the NEXT launch (nobody touches

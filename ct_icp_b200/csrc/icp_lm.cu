@@ -778,7 +778,7 @@ __device__ __forceinline__ void lm_step_device(const LmParams &P, int phase, LmS
     const int R = lm->num_residuals_global;
     // The scalar bookkeeping of TrustRegionMinimizer is a few dozen numbers: every loop over the 12 tangent directions /
     // 14 parameters runs one element per lane (reductions by shuffles), lane 0 keeps only the branchy decisions. (The
-    // first cut ran them as serial loops on lane 0 against shared memory: 30k cycles per step on B200.)
+    // first cut ran them as serial loops on lane 0 against shared memory, several times slower.)
 
     // unpack the evaluation: U = J^T J, gu = J^T r, cost (+ regularisers at the evaluated point)
     for (int e = lane; e < 78; e += 32) {
@@ -1081,7 +1081,7 @@ struct __align__(16) LmPShared {
     int flag;
     int next;   // tile counter of the residual assembly (lm_grab_tile)
 };
-static_assert(sizeof(LmPShared) <= 227 * 1024, "k_lm_persistent: dynamic shared memory of one CTA (sm_100: 227 KB)");
+static_assert(sizeof(LmPShared) <= 227 * 1024, "k_lm_persistent: dynamic shared memory of one CTA (sm_90: 227 KB)");
 extern __shared__ __align__(16) unsigned char lm_smem_raw[];
 
 // what the worker CTAs read of the LM state: the point to evaluate, the problem size, the stop flag

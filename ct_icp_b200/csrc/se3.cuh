@@ -1,4 +1,4 @@
-// se3.cuh — fp64 SE3 / quaternion algebra shared by host orchestration and sm_100a kernels.
+// se3.cuh — fp64 SE3 / quaternion algebra shared by host orchestration and sm_90a kernels.
 //
 // Restates the arithmetic the reference gets from Eigen + slam::TSE3/TPose
 // (include/SlamCore/types.h:100-139, 192-219, 313-366, 434-470): quaternion product, q·v, slerp (not renormalised),
@@ -227,9 +227,9 @@ CT_HD V3 ct_transform_c(Q4 qb, V3 tb, Q4 qe, V3 te, double alpha, V3 raw, const 
 // ---- conversions without the XU pipe ---------------------------------------------------------------------------------
 // F2F.F64.F32 / I2F.F64 / F2I.F64 and the 64-bit MUFU seeds of divisions and square roots execute on the XU pipe: few lanes
 // per clock and a long latency, and every one of them sits ON the dependent chain of a keypoint (the gather kernels are
-// bound by that chain, not by any pipe's throughput: profiles/README.md). The first round-2 build executed ~100 of them per
+// bound by that chain, not by any pipe's throughput). The first round-2 build executed ~100 of them per
 // keypoint-iteration; these helpers do the same conversions with integer / fp64-add instructions (exact, all values),
-// worth 8 % of the GN loop together with the polynomial sin / cos and the 1/n table:
+// which shortened the GN loop together with the polynomial sin / cos and the 1/n table:
 // float → double: re-bias the exponent, shift the mantissa. Branch-free: fp32 denormals (|x| < 1.2e-38 — no coordinate or
 // offset in metres is one) become zero, inf / nan become huge finite values (never inside a search radius).
 __device__ __forceinline__ double f32_to_f64(float f) {

@@ -34,13 +34,13 @@ struct SolveScratch {
 // for which elimination without pivoting is backward stable; the result agrees with a pivoted LDL^T to ~1e-13 relative.
 // History of the serial tail this sits in: round 1 kept rows in registers but broadcast all 13 columns at every step and
 // back-substituted (~3.5k instructions); the first round-2 form updated the matrix in shared memory (5 entries per lane and
-// pivot, two barriers per pivot: ~0.5k instructions but 3.9k cycles per solve — every pivot waits for a store -> barrier ->
+// pivot, two barriers per pivot: ~0.5k instructions but a long serial chain — every pivot waits for a store -> barrier ->
 // load round trip); this one is ~0.5k instructions with only shuffle latency between pivots.
 static __device__ __forceinline__ void warp_ldlt_solve12(SolveScratch &S, int lane) {
     // Gauss-Jordan on the augmented 12 x 13 system, IN REGISTERS: lane r holds row r; step p broadcasts the pivot row's
     // remaining entries by shuffles, every lane forms the reciprocal of the pivot itself, and each row is updated with
     // fully unrolled, compile-time column indices. (The shared-memory form before it paid two barriers plus a
-    // store -> load round trip per pivot: 3.9k cycles per solve on B200; the stamps are in profiles/.) Same operations on the
+    // store -> load round trip per pivot.) Same operations on the
     // same operands as before: the pivot row is scaled by 1 / pivot, row r loses (a_rp / pivot) x the OLD pivot row.
     const int r = lane < 12 ? lane : 0;   // lanes 12..31 mirror row 0 (their results are discarded)
     double a[13];
@@ -66,8 +66,8 @@ static __device__ __forceinline__ void warp_ldlt_solve12(SolveScratch &S, int la
 // The same elimination on the augmented matrix in shared memory, as a 12-trip loop (five entries per lane and pivot): ~60
 // instructions of code instead of ~500. For callers whose serial tail is bound by INSTRUCTION FETCH rather than latency —
 // the CERES minimizer step runs ~1k instructions once per evaluation on one warp, cold in the 32 KB L1.5 I-cache every time
-// (the workers' code streams through the cache in between): measured 30k cycles per step with this form, 53k with the
-// unrolled register form above inlined, 61k with it as a call (profiles/README.md).
+// (the workers' code streams through the cache in between): this form measured faster per step than the unrolled
+// register form above, inlined or as a call.
 static __device__ __forceinline__ void warp_ldlt_solve12_compact(SolveScratch &S, int lane) {
     if (lane < 12) S.A[lane][12] = S.b[lane];   // augmented column
     int er[5], ec[5];

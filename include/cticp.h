@@ -1,5 +1,5 @@
 /*
- * cticp.h — C ABI of the B200-native CT-ICP registration engine.
+ * cticp.h — C ABI of the H100-native CT-ICP registration engine.
  *
  * This is the drop-in boundary underneath the C++ facade `ct_icp::Odometry`
  * (ct_icp_b200/include/ct_icp/odometry.h). Plain pointers and sizes only; no
@@ -15,7 +15,7 @@
  *     ros/catkin_ws/ct_icp_odometry/src/ct_icp_odometry_node.cxx:67).
  *   - input clouds are borrowed for the duration of the call only.
  *   - there is NO CPU fallback: cticp_create fails with CTICP_ERR_NO_DEVICE
- *     when no sm_100 device is usable.
+ *     when no sm_90 (H100) device is usable.
  *   - ingest precision: a scan is kept on the device as (x, y, z, alpha) in
  *     fp32 — what LiDAR drivers emit (KITTI .bin, PointCloud2 FLOAT32) — and all
  *     geometry is evaluated in fp64 from there. The reference reads the scan

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90) CUDA device: pytest -m gpu")
 
 
 @pytest.fixture(scope="session")

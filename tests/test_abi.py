@@ -73,7 +73,7 @@ def test_reference_default_values():
 
 
 def test_no_cpu_fallback():
-    """Without a usable sm_100 device every constructor fails loudly with CTICP_ERR_NO_DEVICE."""
+    """Without a usable sm_90 device every constructor fails loudly with CTICP_ERR_NO_DEVICE."""
     import torch
     if torch.cuda.is_available():
         pytest.skip("a CUDA device is present")

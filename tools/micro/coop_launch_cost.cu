@@ -1,8 +1,8 @@
 // Micro-benchmark: what does a cooperative launch cost on the device timeline, next to a plain launch of the same grid?
-// Chains of N dependent short kernels on one stream, timed with events; grid = 4 CTAs x 148 SMs x 256 threads, each kernel
+// Chains of N dependent short kernels on one stream, timed with events; grid = 4 CTAs per SM (all SMs) x 256 threads, each kernel
 // with `syncs` grid-wide barriers — cg::grid.sync() under cudaLaunchCooperativeKernel vs a hand-rolled arrive/epoch
 // barrier under a plain launch (all CTAs co-resident by construction).
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o coop_launch_cost coop_launch_cost.cu ; run: ./coop_launch_cost
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o coop_launch_cost coop_launch_cost.cu ; run: ./coop_launch_cost
 #include <cooperative_groups.h>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -60,7 +60,7 @@ int main() {
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0);
     cudaEventCreate(&e1);
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     const int chain = 30;
     for (int per_sm : {1, 4}) {

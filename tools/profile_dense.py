@@ -1,5 +1,6 @@
+import os
 import sys
-sys.path.insert(0,'/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench, ct_icp_b200
 from ct_icp_b200 import synthetic as syn
 bench._WORKLOAD="dense128_gn"

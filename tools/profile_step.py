@@ -1,5 +1,5 @@
 """Profiling driver: registers `--frames` HDL-64 scans (device-resident input) so that ncu can list every launch
-of steady-state RegisterFrame steps. Run under ncu (see profiles/README.md); numbers printed under a profiler are
+of steady-state RegisterFrame steps. Run under ncu; numbers printed under a profiler are
 never bench values."""
 import argparse
 import os
