@@ -29,7 +29,7 @@ public:
     bool raw_has_lo() const { return raw_lo_; }
     bool frame_has_lo() const { return frame_lo_; }
     bool frame_distorted() const { return distorted_; }
-    const float4 *d_raw_lo() const { return raw_lo_ ? d_raw_lo_ : nullptr; }
+    const float4 *d_raw_lo() const { return raw_lo_ ? raw_lo_ptr_ : nullptr; }
     const float4 *d_frame_lo() const { return frame_lo_ ? d_frame_lo_ : nullptr; }
     const float4 *d_keypoints_lo() const { return frame_lo_ ? d_kp_lo_ : nullptr; }
     size_t MaxPoints() const { return max_points_; }
@@ -38,7 +38,11 @@ public:
     // UploadBegin(n), then UploadRange over a partition of [0, n) in any order
     void UploadBegin(size_t n);
     void UploadRange(size_t begin, size_t end);
-    void UploadFromDevice(const float4 *d_src, const float4 *d_src_lo, size_t n);   // scan already packed and resident in HBM
+    // scan already packed and resident in HBM: read in place (no copy) until the next Upload* — the caller keeps d_src /
+    // d_src_lo alive until then, or until DetachRaw()
+    void UploadFromDevice(const float4 *d_src, const float4 *d_src_lo, size_t n);
+    // copy a scan read in place into the pipeline's own buffers (before the caller frees it); stream-ordered
+    void DetachRaw();
 
     // Odometry::InitializeFrame: shuffle → sub_sample_frame → (frames 0,1: timestamp := end) → shuffle
     void SubSampleFrame(double voxel_size, uint64_t seed, uint64_t counter1, uint64_t counter2, bool override_alpha,
@@ -70,7 +74,7 @@ public:
     }
     const int *d_counts() const { return d_counts_; }
 
-    const float4 *d_raw() const { return d_raw_; }
+    const float4 *d_raw() const { return raw_ptr_; }
     const float4 *d_frame() const { return d_frame_; }
     const float4 *d_keypoints() const { return d_keypoints_; }
     float4 *d_keypoints_mut() { return d_keypoints_; }
@@ -90,16 +94,21 @@ public:
                     double voxel_size, int use_perm1, uint64_t seed, uint64_t c1, int use_perm2, uint64_t c2,
                     int override_alpha, float alpha_value, float4 *out, float4 *out_lo, uint32_t *out_src, int *d_n_out);
     float4 *d_frame_lo_mut() { EnsureLo(); return d_frame_lo_; }
-    float4 *d_raw_mut() { return d_raw_; }
     double *d_frame_world_mut() { return d_frame_world_; }
     float4 *d_frame_mut() { return d_frame_; }
     uint32_t *d_frame_src_mut() { return d_frame_src_; }
 
 private:
     int Blocks(size_t n) const;
+    void BeginScan(size_t n);
+    // N of a new scan reaches counts[0] as an argument of the first kernel that reads it (no 4-byte H2D copy in front of
+    // the sampler): n_ when d_n is counts[0] and that kernel has not been launched yet for this scan, else -1
+    int TakeHostN(const int *d_n);
 
     cudaStream_t stream_;
     size_t max_points_, n_ = 0, h2d_bytes_ = 0;
+    bool n_on_device_ = true;
+    const float4 *raw_ptr_ = nullptr, *raw_lo_ptr_ = nullptr;   // the scan being read: d_raw_ / d_raw_lo_ or a staged scan
     uint32_t grid_cap_ = 0;
     float4 *h_stage_ = nullptr;
     int *h_counts_ = nullptr;
@@ -109,16 +118,16 @@ private:
     uint32_t *d_frame_src_ = nullptr, *d_kp_src_ = nullptr, *d_tmp_src_ = nullptr;
     unsigned long long *d_grid_ = nullptr;
     int *d_slot_of_ = nullptr;
-    uint32_t *d_tile_count_ = nullptr, *d_flags_ = nullptr, *d_src_ = nullptr;   // flags live right after the tile counters
+    uint32_t *d_src_ = nullptr, *d_win_ = nullptr;   // point of each position / compacted winners before the second shuffle
+    unsigned long long *d_desc_ = nullptr;            // look-back descriptors of the selections (frame_pipeline.cu)
     int *d_counts_ = nullptr;
     double *d_frame_world_ = nullptr, *d_all_world_ = nullptr;
-    uint32_t *d_tile2_ = nullptr, *d_src2_ = nullptr;   // second selection of the fused sampler
+    unsigned long long *d_grid2_ = nullptr;   // hash grid of the fused sampler's second selection
     int fused_grid_ = 0;
-    // k_sample_fused leaves the hash grid and selection 1's flag / tile arrays clean for the next frame (CTICP_SAMPLE_PRECLEAR=0:
-    // every launch clears them itself): the capacity / word count that are clean right now
+    // k_sample_fused leaves the hash grid clean for the next frame (CTICP_SAMPLE_PRECLEAR=0: every launch clears it itself):
+    // the capacity that is clean right now
     bool preclear_ = true;
     uint32_t clean_cap_ = 0;
-    size_t clean_words_ = 0;
     uint32_t *d_adaptive_ = nullptr;   // tile counters + flags + src of the band-major position space
     size_t adaptive_capacity_ = 0;
     int launches_ = 0;
