@@ -70,6 +70,8 @@ class Binding:
             "map_clear": (C.c_int, [vp]),
             "icp_register": (C.c_int, [vp, P(abi.IcpOptions), P(abi.StrategyOptions), vp, sz, P(abi.Frame),
                                        P(abi.Frame), P(abi.MotionModelOptions), P(abi.IcpSummary)]),
+            "icp_register_batch": (C.c_int, [vp, P(abi.IcpOptions), sz, P(vp), P(sz), P(abi.Frame), P(vp),
+                                             P(abi.MotionModelOptions), P(abi.IcpSummary)]),
             "icp_gn_normal_equations": (C.c_int, [vp, P(abi.IcpOptions), vp, sz, P(abi.Frame), P(abi.Frame),
                                                   P(abi.MotionModelOptions), vp, vp, P(i32)]),
             "grid_sample_indices": (i64, [C.c_int, vp, sz, sz, dbl, vp, sz]),
@@ -275,6 +277,34 @@ class VoxelMap:
             C.byref(previous_frame) if previous_frame is not None else None,
             C.byref(motion_options) if motion_options is not None else None, C.byref(summary)))
         return summary
+
+    def icp_register_batch(self, icp_options, keypoints_list, frames, previous_frames=None, motion_options=None):
+        """B independent registrations (solver GN) in one launch (cticp_icp_register_batch). keypoints_list: B arrays of
+        abi.wpoint_dtype() (world rewritten in place); frames: B abi.Frame (updated in place); previous_frames: None or
+        B entries, each an abi.Frame or None (no motion prior for that problem). Returns the B abi.IcpSummary."""
+        B = len(keypoints_list)
+        if len(frames) != B or (previous_frames is not None and len(previous_frames) != B):
+            raise ValueError("keypoints_list, frames and previous_frames must have one entry per problem")
+        for kp in keypoints_list:
+            assert kp.dtype == abi.wpoint_dtype() and kp.flags.c_contiguous
+        m = max(B, 1)
+        kps = (C.c_void_p * m)(*[kp.ctypes.data if len(kp) else None for kp in keypoints_list])
+        ns = (C.c_size_t * m)(*[len(kp) for kp in keypoints_list])
+        fr = (abi.Frame * m)()
+        for b, f in enumerate(frames):
+            C.memmove(C.addressof(fr[b]), C.addressof(f), C.sizeof(abi.Frame))
+        prev = None
+        if previous_frames is not None:
+            prev = (C.c_void_p * m)(*[C.addressof(p) if p is not None else None for p in previous_frames])
+        out = (abi.IcpSummary * m)()
+        rc = self.b.fn("icp_register_batch")(
+            self.h, C.byref(icp_options), B, kps, ns, fr, prev,
+            C.byref(motion_options) if motion_options is not None else None, out)
+        if rc >= 0 or rc == abi.ERR_INTERNAL:   # ERR_INTERNAL: a timed-out problem; every output is written all the same
+            for b, f in enumerate(frames):
+                C.memmove(C.addressof(f), C.addressof(fr[b]), C.sizeof(abi.Frame))
+        self.b.check(rc)
+        return [out[b].copy() for b in range(B)]
 
     def gn_normal_equations(self, icp_options, keypoints, frame, previous_frame=None, motion_options=None):
         assert keypoints.dtype == abi.wpoint_dtype() and keypoints.flags.c_contiguous

@@ -657,26 +657,47 @@ struct DeviceKeypoints {
         cudaFree(d_state);
     }
 };
-void UploadRegistrationInputs(cticp_map *m, const cticp_wpoint *keypoints, size_t n, const cticp_frame *frame,
-                              const cticp_frame *previous_frame, const cticp_motion_model_options *mo,
-                              DeviceKeypoints &D, IcpState &S) {
+// keypoints → (fp32 raw xyz, alpha) in kp[0..n) and its residual plane in lo[0..n); returns whether some value is not
+// float32-representable. Throws TimestampError for a timestamp outside the frame, before writing anything else.
+bool PackKeypoints(const cticp_wpoint *keypoints, size_t n, const cticp_frame *frame, float4 *kp, float4 *lo) {
     const double bts = frame->begin_pose.dest_timestamp, ets = frame->end_pose.dest_timestamp;
-    std::vector<float4> kp(n), lo(n);
     for (size_t i = 0; i < n; ++i) {
         const double t = keypoints[i].timestamp;
         if (!(bts <= t && t <= ets)) throw TimestampError("The timestamp cannot be interpolated between the two poses");
+    }
+    bool has_lo = false;
+    for (size_t i = 0; i < n; ++i) {
+        const double t = keypoints[i].timestamp;
         const double v[4] = {keypoints[i].raw[0], keypoints[i].raw[1], keypoints[i].raw[2], AlphaOf(t, bts, ets)};
         kp[i] = make_float4((float) v[0], (float) v[1], (float) v[2], (float) v[3]);
         lo[i] = make_float4((float) (v[0] - (double) kp[i].x), (float) (v[1] - (double) kp[i].y),
                             (float) (v[2] - (double) kp[i].z), (float) (v[3] - (double) kp[i].w));
-        if (lo[i].x != 0.f || lo[i].y != 0.f || lo[i].z != 0.f || lo[i].w != 0.f) D.has_lo = true;
+        if (lo[i].x != 0.f || lo[i].y != 0.f || lo[i].z != 0.f || lo[i].w != 0.f) has_lo = true;
     }
+    return has_lo;
+}
+// the registration state at the initial frame (+ PreviousFrameMotionModel when previous_frame and mo are given)
+void InitialState(const cticp_frame *frame, const cticp_frame *previous_frame, const cticp_motion_model_options *mo,
+                  IcpState &S);
+void UploadRegistrationInputs(cticp_map *m, const cticp_wpoint *keypoints, size_t n, const cticp_frame *frame,
+                              const cticp_frame *previous_frame, const cticp_motion_model_options *mo,
+                              DeviceKeypoints &D, IcpState &S) {
+    std::vector<float4> kp(n), lo(n);
+    D.has_lo = PackKeypoints(keypoints, n, frame, kp.data(), lo.data());
     CAPI_CUDA(cudaMalloc(&D.d_kp, sizeof(float4) * std::max<size_t>(n, 1)));
     CAPI_CUDA(cudaMalloc(&D.d_lo, sizeof(float4) * std::max<size_t>(n, 1)));
     CAPI_CUDA(cudaMemcpyAsync(D.d_lo, lo.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, m->stream));
     CAPI_CUDA(cudaMalloc(&D.d_n, sizeof(int)));
     CAPI_CUDA(cudaMalloc(&D.d_state, sizeof(IcpState)));
     const int ni = (int) n;
+    InitialState(frame, previous_frame, mo, S);
+    CAPI_CUDA(cudaMemcpyAsync(D.d_kp, kp.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, m->stream));
+    CAPI_CUDA(cudaMemcpyAsync(D.d_n, &ni, sizeof(int), cudaMemcpyHostToDevice, m->stream));
+    CAPI_CUDA(cudaMemcpyAsync(D.d_state, &S, sizeof(IcpState), cudaMemcpyHostToDevice, m->stream));
+    CAPI_CUDA(cudaStreamSynchronize(m->stream));
+}
+void InitialState(const cticp_frame *frame, const cticp_frame *previous_frame, const cticp_motion_model_options *mo,
+                  IcpState &S) {
     memset(&S, 0, sizeof(S));
     const Q4 qb = qnormalized(Q4{frame->begin_pose.quat[0], frame->begin_pose.quat[1], frame->begin_pose.quat[2], frame->begin_pose.quat[3]});
     const Q4 qe = qnormalized(Q4{frame->end_pose.quat[0], frame->end_pose.quat[1], frame->end_pose.quat[2], frame->end_pose.quat[3]});
@@ -699,10 +720,33 @@ void UploadRegistrationInputs(cticp_map *m, const cticp_wpoint *keypoints, size_
         for (int d = 0; d < 4; ++d) S.prev_qe[d] = previous_frame->end_pose.quat[d];
     }
     icp_state_refresh_slerp(S);
-    CAPI_CUDA(cudaMemcpyAsync(D.d_kp, kp.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, m->stream));
-    CAPI_CUDA(cudaMemcpyAsync(D.d_n, &ni, sizeof(int), cudaMemcpyHostToDevice, m->stream));
-    CAPI_CUDA(cudaMemcpyAsync(D.d_state, &S, sizeof(IcpState), cudaMemcpyHostToDevice, m->stream));
-    CAPI_CUDA(cudaStreamSynchronize(m->stream));
+}
+// The final state → the frame (in/out), the rewritten world points and the summary: what cticp_icp_register reports
+void WriteRegistrationOutputs(const IcpState &S, cticp_wpoint *keypoints, size_t n, cticp_frame *frame,
+                              cticp_icp_summary *out_summary) {
+    for (int d = 0; d < 4; ++d) {
+        frame->begin_pose.quat[d] = S.qb[d];
+        frame->end_pose.quat[d] = S.qe[d];
+    }
+    for (int d = 0; d < 3; ++d) {
+        frame->begin_pose.tr[d] = S.tb[d];
+        frame->end_pose.tr[d] = S.te[d];
+    }
+    // world_kpts[i] ← InterpolatePose(begin, end, t_i) * raw_i with the final pose pair (ct_icp.cpp:964-966, :688)
+    const Q4 qb{S.qb[0], S.qb[1], S.qb[2], S.qb[3]}, qe{S.qe[0], S.qe[1], S.qe[2], S.qe[3]};
+    const V3 tb{S.tb[0], S.tb[1], S.tb[2]}, te{S.te[0], S.te[1], S.te[2]};
+    const double bts = frame->begin_pose.dest_timestamp, ets = frame->end_pose.dest_timestamp;
+    for (size_t i = 0; i < n; ++i) {
+        const V3 w = ct_transform(qb, tb, qe, te, AlphaOf(keypoints[i].timestamp, bts, ets),
+                                  V3{keypoints[i].raw[0], keypoints[i].raw[1], keypoints[i].raw[2]});
+        keypoints[i].world[0] = w.x; keypoints[i].world[1] = w.y; keypoints[i].world[2] = w.z;
+    }
+    if (out_summary) {
+        memset(out_summary, 0, sizeof(*out_summary));
+        out_summary->success = !S.failed;
+        out_summary->num_residuals_used = S.n_used;
+        out_summary->num_iters = S.iter;
+    }
 }
 }  // namespace
 
@@ -731,31 +775,71 @@ int cticp_icp_register(cticp_map *m, const cticp_icp_options *options, const cti
         }
         CAPI_CUDA(cudaMemcpyAsync(&S, D.d_state, sizeof(IcpState), cudaMemcpyDeviceToHost, m->stream));
         CAPI_CUDA(cudaStreamSynchronize(m->stream));
-        for (int d = 0; d < 4; ++d) {
-            frame->begin_pose.quat[d] = S.qb[d];
-            frame->end_pose.quat[d] = S.qe[d];
-        }
-        for (int d = 0; d < 3; ++d) {
-            frame->begin_pose.tr[d] = S.tb[d];
-            frame->end_pose.tr[d] = S.te[d];
-        }
-        // world_kpts[i] ← InterpolatePose(begin, end, t_i) * raw_i with the final pose pair (ct_icp.cpp:964-966, :688)
-        const Q4 qb{S.qb[0], S.qb[1], S.qb[2], S.qb[3]}, qe{S.qe[0], S.qe[1], S.qe[2], S.qe[3]};
-        const V3 tb{S.tb[0], S.tb[1], S.tb[2]}, te{S.te[0], S.te[1], S.te[2]};
-        const double bts = frame->begin_pose.dest_timestamp, ets = frame->end_pose.dest_timestamp;
-        for (size_t i = 0; i < n; ++i) {
-            const V3 w = ct_transform(qb, tb, qe, te, AlphaOf(keypoints[i].timestamp, bts, ets),
-                                      V3{keypoints[i].raw[0], keypoints[i].raw[1], keypoints[i].raw[2]});
-            keypoints[i].world[0] = w.x; keypoints[i].world[1] = w.y; keypoints[i].world[2] = w.z;
-        }
-        if (out_summary) {
-            memset(out_summary, 0, sizeof(*out_summary));
-            out_summary->success = !S.failed;
-            out_summary->num_residuals_used = S.n_used;
-            out_summary->num_iters = S.iter;
-        }
+        WriteRegistrationOutputs(S, keypoints, n, frame, out_summary);
         if (S.failed == 2) throw std::runtime_error("Error During Optimization");
         if (S.failed) g_last_error = "[CT_ICP]Error : not enough keypoints selected in ct-icp !";
+        return (int) CTICP_OK;
+    });
+}
+
+int cticp_icp_register_batch(cticp_map *m, const cticp_icp_options *options, size_t batch,
+                             cticp_wpoint *const *keypoints, const size_t *n, cticp_frame *frames,
+                             const cticp_frame *const *previous_frames, const cticp_motion_model_options *motion_options,
+                             cticp_icp_summary *out_summaries) {
+    return Guard([&] {
+        if (!m || !options || !keypoints || !n || !frames) throw std::invalid_argument("null argument");
+        if (batch == 0 || batch > 64) throw std::invalid_argument("batch must be in [1, 64]");
+        size_t total = 0;
+        for (size_t b = 0; b < batch; ++b) {
+            if (!keypoints[b] && n[b] > 0) throw std::invalid_argument("null keypoints");
+            total += n[b];
+        }
+        if (total > (size_t) INT32_MAX) throw std::invalid_argument("too many keypoints in one batch");
+        if (options->solver != CTICP_SOLVER_GN) throw UnsupportedError("cticp_icp_register_batch: solver GN only");
+        if (options->max_number_neighbors > 32 || options->max_number_neighbors < 1)
+            throw UnsupportedError("max_number_neighbors must be in [1, 32]");
+        CAPI_CUDA(cudaSetDevice(m->device));
+        if (!m->icp->batch_supported())
+            throw UnsupportedError("cticp_icp_register_batch needs the persistent Gauss-Newton loop with flag synchronisation");
+        // every problem's inputs are checked (timestamps) and packed before anything reaches the device
+        std::vector<float4> kp(std::max<size_t>(total, 1)), lo(std::max<size_t>(total, 1));
+        std::vector<IcpState> S(batch);
+        std::vector<char> has_lo(batch);
+        bool any_lo = false;
+        for (size_t b = 0, base = 0; b < batch; base += n[b], ++b) {
+            has_lo[b] = PackKeypoints(keypoints[b], n[b], &frames[b], kp.data() + base, lo.data() + base);
+            any_lo = any_lo || has_lo[b];
+            InitialState(&frames[b], previous_frames ? previous_frames[b] : nullptr, motion_options, S[b]);
+        }
+        if (any_lo)   // a problem that a solo call would run without a residual plane gets -0.0f: x + (-0.0) == x, every x
+            for (size_t b = 0, base = 0; b < batch; base += n[b], ++b)
+                if (!has_lo[b])
+                    for (size_t i = 0; i < n[b]; ++i) lo[base + i] = make_float4(-0.f, -0.f, -0.f, -0.f);
+        struct Buffers {
+            float4 *kp = nullptr, *lo = nullptr;
+            IcpState *states = nullptr;
+            ~Buffers() { cudaFree(kp); cudaFree(lo); cudaFree(states); }
+        } D;
+        CAPI_CUDA(cudaMalloc(&D.kp, sizeof(float4) * kp.size()));
+        CAPI_CUDA(cudaMalloc(&D.states, sizeof(IcpState) * batch));
+        CAPI_CUDA(cudaMemcpyAsync(D.kp, kp.data(), sizeof(float4) * total, cudaMemcpyHostToDevice, m->stream));
+        if (any_lo) {
+            CAPI_CUDA(cudaMalloc(&D.lo, sizeof(float4) * lo.size()));
+            CAPI_CUDA(cudaMemcpyAsync(D.lo, lo.data(), sizeof(float4) * total, cudaMemcpyHostToDevice, m->stream));
+        }
+        CAPI_CUDA(cudaMemcpyAsync(D.states, S.data(), sizeof(IcpState) * batch, cudaMemcpyHostToDevice, m->stream));
+        m->icp->set_keypoints_lo(D.lo);
+        m->icp->EnqueueGaussNewtonBatch(*m->map, *options, (int) batch, n, D.kp, options->num_iters_icp, D.states);
+        CAPI_CUDA(cudaMemcpyAsync(S.data(), D.states, sizeof(IcpState) * batch, cudaMemcpyDeviceToHost, m->stream));
+        CAPI_CUDA(cudaStreamSynchronize(m->stream));
+        bool timeout = false, not_enough = false;
+        for (size_t b = 0; b < batch; ++b) {
+            WriteRegistrationOutputs(S[b], keypoints[b], n[b], &frames[b], out_summaries ? &out_summaries[b] : nullptr);
+            timeout = timeout || S[b].failed == 2;
+            not_enough = not_enough || S[b].failed;
+        }
+        if (timeout) throw std::runtime_error("Error During Optimization");
+        if (not_enough) g_last_error = "[CT_ICP]Error : not enough keypoints selected in ct-icp !";
         return (int) CTICP_OK;
     });
 }

@@ -2,6 +2,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <vector>
+
 #include "../../include/cticp.h"
 #include "device_map.h"
 
@@ -98,6 +100,17 @@ public:
                             int shard_rank = 0, int shard_world = 1, void *nccl_comm = nullptr,
                             const FrameTailArgs *tail = nullptr);
 
+    // B independent Gauss-Newton registrations against `map` with shared options, in ONE launch of the persistent kernel
+    // (k_gn_persistent over groups). Problem b's h_n[b] keypoints are at [kp_base_b, kp_base_b + h_n[b]) of d_keypoints,
+    // kp_base_b = h_n[0] + … + h_n[b - 1] (the residual plane, when set_keypoints_lo gave one, alike); its state is
+    // d_states[b]. CTA policy and its bit-identity contract: BatchGatherCtas (icp_gn.cu). Throws CapacityError when
+    // the device cannot hold two CTAs per problem; requires batch_supported().
+    void EnqueueGaussNewtonBatch(const DeviceMap &map, const cticp_icp_options &opt, int batch, const size_t *h_n,
+                                 const float4 *d_keypoints, int num_iters, IcpState *d_states);
+    // the batch has no launch-per-iteration form (CTICP_PERSISTENT=0) and cannot use grid-wide barriers, which would
+    // couple groups with different iteration counts (-DCTICP_GN_GRID_BARRIERS builds)
+    bool batch_supported() const;
+
     // solver CERES reproduced as a device Levenberg-Marquardt / IRLS loop (icp_lm.cu)
     // k_hint sizes the grids (estimate of the keypoint count), k_capacity the per-keypoint buffers (upper bound)
     void EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
@@ -148,6 +161,9 @@ private:
     int lm_coresident_[6] = {0, 0, 0, 0, 0, 0};   // k_lm_persistent<mode, peers>
     void FreeLmBuffers();
     GnParams MakeParams(const DeviceMap &map, const cticp_icp_options &opt) const;
+    int GnCoresident(bool peers);          // co-resident CTAs of k_gn_persistent<peers> on this device
+    int PrepareLoopWords(int groups);      // the word set of the next persistent launch: zero for groups [0, groups)
+    void LoopWordsLaunched(int groups);    // bookkeeping after that launch was enqueued
 
     cudaStream_t stream_;
     const float4 *kp_lo_ = nullptr;
@@ -158,8 +174,13 @@ private:
     double *d_sys_ = nullptr;      // 12*12 + 12 + 4 debug output of the solve kernel
     double *d_acc_ = nullptr;      // reduced accumulator (multi-GPU all-reduce buffer)
     unsigned int *d_ticket_ = nullptr;   // last-CTA-done counter of k_gn_iterate
-    unsigned int *d_sync_words_ = nullptr;   // two sets of (arrive counter, epoch) of k_gn_persistent, alternating per launch
+    unsigned int *d_sync_words_ = nullptr;   // per group, two sets of (arrive counter, epoch) of k_gn_persistent, alternating per launch
     int sync_set_ = 0;
+    int sync_groups_ = 1;                    // groups d_sync_words_ holds (grow-only)
+    int sync_clean_[2] = {1, 1};             // per set: groups [0, sync_clean_[s]) have zero words
+    int *d_groups_ = nullptr;                // batched launches: first_cta | kp_base | keypoint counts (grow-only)
+    int groups_cap_ = 0;                     // ints d_groups_ holds
+    std::vector<int> h_groups_;
     // solver CERES (icp_lm.cu)
     void *d_lm_state_ = nullptr, *d_lm_stats_ = nullptr, *d_lm_blocks_ = nullptr;
     int *d_lm_sel_ = nullptr;

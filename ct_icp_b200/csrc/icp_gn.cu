@@ -364,6 +364,12 @@ struct GnShared {
     FrameVerdict verdict;   // persistent kernel, solver CTA: the frame's tail decided at the end of the loop (frame_policy.h)
     int flag;
     int done;         // gather CTAs: the published `done` flag, fetched together with the pose (one memory round trip)
+    struct {          // k_gn_persistent: the group's words, read where used (no registers held across the gather)
+        IcpState *st;
+        double *partials;   // gather CTA: its partial row; solver CTA: the group's first row
+        unsigned int *arrive, *epoch;
+        int gather_ctas;
+    } grp;
     unsigned long long mbar[kGatherWarps];   // -DCTICP_SEL_BULK: one mbarrier per warp for the bulk copies
 };
 
@@ -524,6 +530,19 @@ struct LoopSync {
     unsigned int *epoch;    // = iterations published by the solver CTA
     unsigned int *next_arrive, *next_epoch;   // the other set
 };
+// A batched launch (IcpSolver::EnqueueGaussNewtonBatch) gives every group its own words: group g's are those of group 0
+// moved by g * kSyncGroupWords (both sets of a group: 2 x (arrive line, epoch line) of 128 bytes each)
+constexpr int kSyncGroupWords = 128;
+
+// The groups of one k_gn_persistent launch. Group g owns the CTAs [first_cta[g], first_cta[g + 1]) of the grid — the first
+// is g's solver CTA, the others gather g's keypoints — its keypoints [kp_base[g], kp_base[g] + count[g]) of the launch's
+// keypoint (and residual plane) array, the state st[g], the partial rows [first_cta[g] - g, first_cta[g + 1] - g - 1) and
+// its own loop words. Groups never wait on each other. `table` (device) = first_cta[0..B] | kp_base[0..B-1];
+// num_groups == 1: the whole grid is one group with its keypoints at index 0, and `table` is not read.
+struct GnGroups {
+    const int *table;
+    int num_groups;
+};
 constexpr long long kLoopSyncTimeout = 4000000000LL;   // SM cycles (~2 s)
 __device__ __forceinline__ bool loop_wait_at_least(const unsigned int *word, unsigned int want,
                                                    long long timeout = kLoopSyncTimeout) {
@@ -542,6 +561,11 @@ __device__ __forceinline__ bool loop_wait_at_least(const unsigned int *word, uns
 // CTAs work on iteration 0, the solver warp runs the solve once on a dummy system to pull its code into the instruction
 // cache. With `tail.enabled` the solver CTA also decides the frame's tail after the loop (frame_policy.h).
 //
+// Groups (GnGroups): one launch can run B independent registrations against the same map, each on its own contiguous range
+// of CTAs with its own solver CTA, state, partial rows and loop words; everything above holds per group. A group that
+// converges or fails leaves the loop alone while the others go on, and one group's serial tail overlaps the others'
+// gathers. The single registration (solo L3 call, odometry) is the one-group case; kPeers and the frame tail are single-group.
+//
 // kPeers (multi-GPU, keypoints sharded): between its reduction and its solve the solver CTA exchanges the accumulator
 // with the other ranks' solver CTAs through NVLink peer memory (peer_exchange.cuh) — the all-reduce of SURVEY §8e
 // happens INSIDE the loop, so the sharded loop is still one launch and costs one NVLink round trip per iteration.
@@ -549,14 +573,30 @@ template <bool kPeers>
 __global__ void __launch_bounds__(kGatherWarps * 32, 1)
 k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const int *__restrict__ d_num_keypoints,
                 IcpState *st, double *__restrict__ partials, int num_iters, PeerLinks links, LoopSync sync,
-                FrameTailArgs tail) {
+                FrameTailArgs tail, GnGroups groups) {
 #ifndef CTICP_GN_FLAG_SYNC
     cg::grid_group grid = cg::this_grid();
 #endif
     GnShared &sh = *reinterpret_cast<GnShared *>(gn_smem_raw);
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const GnParams &P = cfg.P;
-    const bool solver_cta = blockIdx.x == 0;
+    // this CTA's group (GnGroups): from here on the group is the whole registration — `cta` is the index within the
+    // group, `group_ctas` its size, and st / partials / sync / the keypoint count are the group's own
+    int g = 0, cta = blockIdx.x, group_ctas = gridDim.x, kp_base = 0;
+    if (groups.num_groups > 1) {
+        const int *first_cta = groups.table;
+        while (first_cta[g + 1] <= (int) blockIdx.x) ++g;
+        cta = (int) blockIdx.x - first_cta[g];
+        group_ctas = first_cta[g + 1] - first_cta[g];
+        kp_base = groups.table[groups.num_groups + 1 + g];
+        st += g;
+        partials += (size_t) (first_cta[g] - g) * kAcc;   // the gather CTAs of the groups before this one
+        sync.arrive += kSyncGroupWords * g;
+        sync.epoch += kSyncGroupWords * g;
+        sync.next_arrive += kSyncGroupWords * g;
+        sync.next_epoch += kSyncGroupWords * g;
+    }
+    const bool solver_cta = cta == 0;
 #ifdef CTICP_GN_FLAG_SYNC
     if (solver_cta && threadIdx.x == 0) {   // the next launch's words (idle during this launch)
         *sync.next_arrive = 0u;
@@ -565,8 +605,15 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
 #endif
     unsigned int peer_seq = 0;   // sequence number of the last exchange (solver CTA only)
     if (kPeers && solver_cta) peer_seq = *links.seq;
-    const int gather_ctas = gridDim.x - 1;
+    const int gather_ctas = group_ctas - 1;
     const int *stencil = stencil_table_fill(sh.stencil, cfg.G.r);
+    if (threadIdx.x == 0) {
+        sh.grp.st = st;
+        sh.grp.partials = solver_cta ? partials : partials + (size_t) (cta - 1) * kAcc;
+        sh.grp.arrive = sync.arrive;
+        sh.grp.epoch = sync.epoch;
+        sh.grp.gather_ctas = gather_ctas;
+    }
     __syncthreads();
 
     if (solver_cta) {   // working copy of the state in shared memory: the serial tail never waits for global memory
@@ -601,7 +648,7 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
     long long t_loop = 0, t_solve = 0;
     if (solver_cta && threadIdx.x == 0) t_loop = clock64();
     // this rank's keypoint range and the tile width: constant over the iterations (integer divisions)
-    const int K = *d_num_keypoints;
+    const int K = d_num_keypoints[g];
     int kp_lo = 0, kp_hi = K;
     if (P.shard_world > 1) {
         kp_lo = (int) ((long long) K * P.shard_rank / P.shard_world);
@@ -610,8 +657,8 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
     // this CTA's balanced share of the range
     int c_lo = 0, c_hi = 0;
     if (!solver_cta) {
-        c_lo = kp_lo + (int) ((long long) (kp_hi - kp_lo) * (blockIdx.x - 1) / gather_ctas);
-        c_hi = kp_lo + (int) ((long long) (kp_hi - kp_lo) * blockIdx.x / gather_ctas);
+        c_lo = kp_base + kp_lo + (int) ((long long) (kp_hi - kp_lo) * (cta - 1) / gather_ctas);
+        c_hi = kp_base + kp_lo + (int) ((long long) (kp_hi - kp_lo) * cta / gather_ctas);
     }
     for (int it = 0; it < num_iters; ++it) {
         // `done` is uniform over the grid: published before the previous grid barrier (the solver CTA reads its own copy)
@@ -624,13 +671,14 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
 #ifdef CTICP_GN_FLAG_SYNC
                 // the state of iteration `it` is published (it == 0: uploaded by the host before the launch)
                 // (sharded: the solver CTA may itself be waiting for a late peer rank, up to PeerLinks::timeout_cycles)
-                const bool ok = it == 0 || loop_wait_at_least(sync.epoch, (unsigned int) it,
+                const bool ok = it == 0 || loop_wait_at_least(sh.grp.epoch, (unsigned int) it,
                                                               kLoopSyncTimeout + (kPeers ? links.timeout_cycles : 0LL));
 #else
                 const bool ok = true;
 #endif
-                const int done = __ldcg(&st->done);   // issued with the pose loads: one round trip, not two
-                sh.pose = load_pose(st);
+                const IcpState *gst = sh.grp.st;
+                const int done = __ldcg(&gst->done);   // issued with the pose loads: one round trip, not two
+                sh.pose = load_pose(gst);
                 sh.done = ok ? done : 1;
                 sh.rows.next = 0;
             }
@@ -640,15 +688,15 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
             // (CTICP_DEBUG_FLAGS & 2, timing only: an empty range — the barriers and the reduction without the gather work)
             const bool skip = (P.debug_flags & 2) != 0;
             gn_cta_gather(cfg, stencil, keypoints, skip ? 0 : c_lo, skip ? 0 : c_hi, sh, lane, w,
-                          partials + (size_t) (blockIdx.x - 1) * kAcc, A, bulk_ptr, P.rigid_first && it == 0);
+                          sh.grp.partials, A, bulk_ptr, P.rigid_first && it == 0);
             CT_STAMP(const long long t_g = clock64();)
 #ifdef CTICP_GN_FLAG_SYNC
             __threadfence();   // (the writers of the partial row)
             __syncthreads();
-            if (threadIdx.x == 0) atomicAdd(sync.arrive, 1u);
+            if (threadIdx.x == 0) atomicAdd(sh.grp.arrive, 1u);
 #endif
             CT_STAMP(if (P.dbg_warp && lane == 0 && it < kDbgIters) {
-                unsigned long long *o = P.dbg_warp + ((size_t) it * (gather_ctas * kGatherWarps) + (w * gather_ctas + (blockIdx.x - 1))) * kDbgSlots;
+                unsigned long long *o = P.dbg_warp + ((size_t) it * (gather_ctas * kGatherWarps) + (w * gather_ctas + (cta - 1))) * kDbgSlots;
                 o[0] = (unsigned long long) A.dbg[0]; o[1] = (unsigned long long) A.dbg[1];
                 o[2] = (unsigned long long) A.dbg[2];
                 o[3] = (unsigned long long) (t_g0 - t_it);         // pose fetch + barrier
@@ -662,16 +710,16 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
         CT_STAMP(const long long t_bar = clock64();)
 #ifdef CTICP_GN_FLAG_SYNC
         if (solver_cta) {
-            if (threadIdx.x == 0) sh.flag = loop_wait_at_least(sync.arrive, (unsigned int) (gather_ctas * (it + 1))) ? 1 : 0;
+            if (threadIdx.x == 0) sh.flag = loop_wait_at_least(sh.grp.arrive, (unsigned int) (sh.grp.gather_ctas * (it + 1))) ? 1 : 0;
             __syncthreads();
             if (!sh.flag) {   // a gather CTA never arrived: give up (the host raises "Error During Optimization")
                 if (threadIdx.x == 0) {
                     sh.state.failed = 2;
                     sh.state.done = 1;
-                    st->failed = 2;
-                    st->done = 1;
+                    sh.grp.st->failed = 2;
+                    sh.grp.st->done = 1;
                     __threadfence();
-                    atomicExch(sync.epoch, 0x7fffffffu);
+                    atomicExch(sh.grp.epoch, 0x7fffffffu);
                 }
                 break;
             }
@@ -681,12 +729,12 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
 #endif
         CT_STAMP(if (!solver_cta && P.dbg_warp && lane == 0 && w == 0 && it < kDbgIters) {
             // (slot 5 of this CTA's first warp is overwritten with the wait at the barrier that follows the gather)
-            unsigned long long *o = P.dbg_warp + ((size_t) it * (gather_ctas * kGatherWarps) + (blockIdx.x - 1)) * kDbgSlots;
+            unsigned long long *o = P.dbg_warp + ((size_t) it * (gather_ctas * kGatherWarps) + (cta - 1)) * kDbgSlots;
             o[5] = (unsigned long long) (clock64() - t_bar);
         })
         if (solver_cta) {
             const long long t_begin = threadIdx.x == 0 ? clock64() : 0;
-            gn_reduce_rows(sh, partials, gather_ctas, lane, w);
+            gn_reduce_rows(sh, sh.grp.partials, sh.grp.gather_ctas, lane, w);
             // -DCTICP_DEBUG_TIMERS: SM cycles summed over the iterations — dbg_t[0] reduction of the partial rows,
             // [1] everything from there to the published state, [2] the 12x12 solve, [3] the pose update
             CT_STAMP(if (threadIdx.x == 0) sh.state.dbg_t[0] += (unsigned long long) (clock64() - t_begin);)
@@ -718,16 +766,16 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
                 __syncwarp();
                 // publish: the gather CTAs read the pose pair / done flag of the next iteration from global memory
                 const int *src = reinterpret_cast<const int *>(ws);
-                int *dst = reinterpret_cast<int *>(st);
+                int *dst = reinterpret_cast<int *>(sh.grp.st);
                 for (int i = lane; i < (int) (sizeof(IcpState) / sizeof(int)); i += 32) __stcg(dst + i, src[i]);
                 CT_STAMP(if (lane == 0) {
                     ws->dbg_t[1] += (unsigned long long) (clock64() - t_rest);
-                    __stcg(&st->dbg_t[1], ws->dbg_t[1]);
+                    __stcg(&sh.grp.st->dbg_t[1], ws->dbg_t[1]);
                 })
 #ifdef CTICP_GN_FLAG_SYNC
                 __threadfence();   // (the lanes that wrote the state)
                 __syncwarp();
-                if (lane == 0) atomicExch(sync.epoch, (unsigned int) (it + 1));
+                if (lane == 0) atomicExch(sh.grp.epoch, (unsigned int) (it + 1));
 #endif
             }
 #ifdef CTICP_GN_FLAG_SYNC
@@ -903,6 +951,7 @@ IcpSolver::~IcpSolver() {
     cudaFree(d_acc_);
     cudaFree(d_ticket_);
     cudaFree(d_sync_words_);
+    cudaFree(d_groups_);
     FreeLmBuffers();
     for (int i = 0; i < kMaxEvents; ++i) {
         cudaEventDestroy(ev_begin_[i]);
@@ -941,6 +990,150 @@ static int GatherBlocks(size_t k_hint, int max_blocks, int kp_per_cta) {
     // tiles, too large only adds idle CTAs whose zero partials have to be summed.
     size_t want = (k_hint + kp_per_cta - 1) / kp_per_cta;
     return (int) std::max<size_t>(1, std::min(want, (size_t) max_blocks));
+}
+
+// CTA policy of a batched k_gn_persistent launch: gather[b] = the gather CTAs of problem b (each problem also has its solver
+// CTA). Contract:
+//  - When every problem fits with what a solo call would give it — solo_b = GatherBlocks(n_b + 16, coresident - 1), the
+//    grid of EnqueueGaussNewton — and Σ (1 + solo_b) <= coresident, gather[b] = solo_b. Keypoint ranges, tiles and the
+//    order of every reduction are then those of the solo call: each problem's result is bit-identical to it.
+//  - Otherwise the coresident - batch CTAs left for gathering are dealt one at a time to the problem with the most keypoints
+//    per gather CTA (exact integer comparison, ties to the lower index), starting from 1 each and never beyond solo_b. The
+//    busiest CTA sets a group's iteration time, so this balances the groups. The result then differs from the solo call's
+//    by summation order only, and is a function of (n, coresident): bit-reproducible run to run.
+// Requires 2 * batch <= coresident.
+static void BatchGatherCtas(const size_t *n, int batch, int coresident, int kp_per_cta, int *gather) {
+    long long total = 0;
+    std::vector<int> solo(batch);
+    for (int b = 0; b < batch; ++b) {
+        solo[b] = GatherBlocks(n[b] + 16, std::max(1, coresident - 1), kp_per_cta);
+        total += 1 + solo[b];
+    }
+    if (total <= coresident) {
+        for (int b = 0; b < batch; ++b) gather[b] = solo[b];
+        return;
+    }
+    for (int b = 0; b < batch; ++b) gather[b] = 1;
+    for (int left = coresident - 2 * batch; left > 0; --left) {
+        int best = -1;
+        for (int b = 0; b < batch; ++b) {
+            if (gather[b] >= solo[b]) continue;
+            // n_b / gather_b > n_best / gather_best
+            if (best < 0 || (unsigned long long) n[b] * gather[best] > (unsigned long long) n[best] * gather[b]) best = b;
+        }
+        if (best < 0) break;
+        gather[best] += 1;
+    }
+}
+
+int IcpSolver::GnCoresident(bool peers) {
+    int &coresident = max_coresident_[peers ? 1 : 0];
+    if (coresident == 0) {
+        void *kernel = peers ? (void *) k_gn_persistent<true> : (void *) k_gn_persistent<false>;
+        int per_sm = 0;
+        CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGatherWarps * 32, sizeof(GnShared)));
+        coresident = std::max(1, per_sm * num_sms_);
+    }
+    return coresident;
+}
+
+// Loop words: group g, set s at d_sync_words_ + kSyncGroupWords * g + 64 * s (arrive; epoch 32 words further). Launches
+// alternate between the sets, and the solver CTA of every group zeroes its words of the other set, so back-to-back launches
+// of as many groups need no memset. A launch with more groups than the set has clean zeroes the missing groups first.
+static LoopSync LoopSyncOf(unsigned int *words, int set) {
+    LoopSync sync;
+    sync.arrive = words + 64 * set;
+    sync.epoch = sync.arrive + 32;
+    sync.next_arrive = words + 64 * (set ^ 1);
+    sync.next_epoch = sync.next_arrive + 32;
+    return sync;
+}
+int IcpSolver::PrepareLoopWords(int groups) {
+    if (groups > sync_groups_) {
+        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+        cudaFree(d_sync_words_);
+        d_sync_words_ = nullptr;
+        CT_CUDA_CHECK(cudaMalloc(&d_sync_words_, sizeof(unsigned int) * kSyncGroupWords * groups));
+        CT_CUDA_CHECK(cudaMemset(d_sync_words_, 0, sizeof(unsigned int) * kSyncGroupWords * groups));
+        sync_groups_ = groups;
+        sync_clean_[0] = sync_clean_[1] = groups;
+    }
+    const int s = sync_set_, c = sync_clean_[s];
+    if (c < groups) {   // both sets of groups [c, groups): idle, as every earlier launch on the stream has ended
+        CT_CUDA_CHECK(cudaMemsetAsync(d_sync_words_ + (size_t) kSyncGroupWords * c, 0,
+                                      sizeof(unsigned int) * kSyncGroupWords * (groups - c), stream_));
+        if (sync_clean_[s ^ 1] >= c) sync_clean_[s ^ 1] = std::max(sync_clean_[s ^ 1], groups);
+        sync_clean_[s] = groups;
+    }
+    return s;
+}
+void IcpSolver::LoopWordsLaunched(int groups) {
+    sync_clean_[sync_set_] = 0;
+    sync_clean_[sync_set_ ^ 1] = std::max(sync_clean_[sync_set_ ^ 1], groups);
+    sync_set_ ^= 1;
+}
+
+bool IcpSolver::batch_supported() const {
+#ifdef CTICP_GN_FLAG_SYNC
+    return use_persistent_;
+#else
+    return false;
+#endif
+}
+
+void IcpSolver::EnqueueGaussNewtonBatch(const DeviceMap &map, const cticp_icp_options &opt, int batch, const size_t *h_n,
+                                        const float4 *d_keypoints, int num_iters, IcpState *d_states) {
+    if (!batch_supported()) throw std::logic_error("batched Gauss-Newton needs the persistent flag-synchronised loop");
+    if (opt.max_number_neighbors > 32 || opt.max_number_neighbors < 1)
+        throw std::invalid_argument("max_number_neighbors must be in [1, 32]");
+    if (batch < 1) throw std::invalid_argument("batch must be at least 1");
+    GatherLaunch cfg;
+    cfg.P = MakeParams(map, opt);
+    cfg.G.L = map.Level(cfg.P.level);
+    cfg.G.r = cfg.P.r;
+    cfg.G.radius2 = cfg.P.radius * cfg.P.radius;
+    cfg.G.kmax = cfg.P.kmax;
+    const int coresident = GnCoresident(false);
+    if (2 * batch > coresident)
+        throw CapacityError("batch of " + std::to_string(batch) + " registrations: the device holds " +
+                                std::to_string(coresident) + " CTAs of the Gauss-Newton kernel, two per registration needed");
+    // table: first_cta[0..B] | kp_base[0..B-1] | count[0..B-1]
+    h_groups_.assign(3 * (size_t) batch + 1, 0);
+    int *first_cta = h_groups_.data(), *kp_base = first_cta + batch + 1, *count = kp_base + batch;
+    std::vector<int> gather(batch);
+    BatchGatherCtas(h_n, batch, coresident, kp_per_cta_, gather.data());
+    long long base = 0;
+    for (int b = 0; b < batch; ++b) {
+        first_cta[b + 1] = first_cta[b] + 1 + gather[b];
+        kp_base[b] = (int) base;
+        count[b] = (int) h_n[b];
+        base += (long long) h_n[b];
+    }
+    if (base > (long long) INT32_MAX) throw std::invalid_argument("too many keypoints in one batch");
+    const int grid = first_cta[batch];
+    if ((int) h_groups_.size() > groups_cap_) {
+        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+        cudaFree(d_groups_);
+        d_groups_ = nullptr;
+        CT_CUDA_CHECK(cudaMalloc(&d_groups_, sizeof(int) * h_groups_.size()));
+        groups_cap_ = (int) h_groups_.size();
+    }
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_groups_, h_groups_.data(), sizeof(int) * h_groups_.size(), cudaMemcpyHostToDevice, stream_));
+    EnsurePartials(grid);
+    LoopSync sync = LoopSyncOf(d_sync_words_, PrepareLoopWords(batch));
+    const float4 *kp = d_keypoints;
+    const int *nk = d_groups_ + 2 * batch + 1;
+    double *parts = d_partials_;
+    int iters = num_iters;
+    PeerLinks links{};
+    FrameTailArgs tail_args{};
+    GnGroups groups{d_groups_, batch};
+    void *args[] = {&cfg, &kp, &nk, &d_states, &parts, &iters, &links, &sync, &tail_args, &groups};
+    CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_gn_persistent<false>, dim3(grid), dim3(kGatherWarps * 32), args,
+                                              sizeof(GnShared), stream_));
+    LoopWordsLaunched(batch);
+    gather_launches_ += 1;
+    launches_ += 1;
 }
 
 void IcpSolver::PrintWarpStamps(int iters) {
@@ -1002,12 +1195,7 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
     if (use_persistent_ && (!nccl_comm || peers)) {
         // one cooperative launch for the whole loop; the grid must be co-resident (grid-wide barriers)
         void *kernel = peers ? (void *) k_gn_persistent<true> : (void *) k_gn_persistent<false>;
-        int &coresident = max_coresident_[peers ? 1 : 0];
-        if (coresident == 0) {
-            int per_sm = 0;
-            CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGatherWarps * 32, sizeof(GnShared)));
-            coresident = std::max(1, per_sm * num_sms_);
-        }
+        const int coresident = GnCoresident(peers);
         const int blocks = GatherBlocks(k_share, std::max(1, coresident - 1), kp_per_cta_);
         EnsurePartials(blocks + 1);
         int grid = std::min(blocks + 1, coresident);
@@ -1030,18 +1218,15 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
             cfg.P.dbg_warp = d_dbg_warp_;
         }
 #endif
-        LoopSync sync;
-        sync.arrive = d_sync_words_ + 64 * sync_set_;
-        sync.epoch = sync.arrive + 32;
-        sync.next_arrive = d_sync_words_ + 64 * (sync_set_ ^ 1);
-        sync.next_epoch = sync.next_arrive + 32;
-        sync_set_ ^= 1;
+        LoopSync sync = LoopSyncOf(d_sync_words_, PrepareLoopWords(1));
         FrameTailArgs tail_args{};
         if (tail) tail_args = *tail;
-        void *args[] = {&cfg, &kp, &nk, &d_state, &parts, &iters, &links, &sync, &tail_args};
+        GnGroups groups{nullptr, 1};
+        void *args[] = {&cfg, &kp, &nk, &d_state, &parts, &iters, &links, &sync, &tail_args, &groups};
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
         if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
         CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kGatherWarps * 32), args, sizeof(GnShared), stream_));
+        LoopWordsLaunched(1);
         if (timed) cudaEventRecord(ev_end_[ev_used_++], stream_);
         gather_launches_ += 1;
         launches_ += 1;

@@ -507,6 +507,25 @@ int cticp_icp_register(cticp_map *m, const cticp_icp_options *options,
                        const cticp_motion_model_options *motion_options,
                        cticp_icp_summary *out_summary);
 
+/* B independent CT_ICP_Registration::Register problems (solver GN) against one map, in one persistent launch.
+ * options and motion_options are shared; keypoints[b] (n[b] records, world rewritten), frames[b] (in/out) and
+ * previous_frames[b] are per problem. previous_frames (nullable) is an array of B nullable pointers: problem b has the
+ * PreviousFrameMotionModel prior iff previous_frames && previous_frames[b] && motion_options.
+ * Each problem follows the semantics of cticp_icp_register: timestamp check, partial update on failure, world rewrite and
+ * summary. Contract: when every problem gets the CTAs a solo call would give it (the problems fit the device together)
+ * each result is bit-identical to cticp_icp_register's; otherwise the CTAs are shared in proportion to n[b] and a result
+ * differs from the solo one by floating-point summation order only, bit-reproducible from run to run.
+ * Errors: CTICP_ERR_INVALID_ARGUMENT for null pointers (keypoints[b] may be NULL when n[b] == 0) or batch outside
+ * [1, 64]; CTICP_ERR_UNSUPPORTED for a solver other than GN, max_number_neighbors outside [1, 32], or an engine without
+ * the persistent GN loop (CTICP_PERSISTENT=0, -DCTICP_GN_GRID_BARRIERS builds); CTICP_ERR_TIMESTAMP when a keypoint of
+ * any problem lies outside its frame (nothing is run and no frame is modified); CTICP_ERR_INTERNAL ("Error During
+ * Optimization") when some problem's loop timed out — every problem's outputs are written all the same. */
+int cticp_icp_register_batch(cticp_map *m, const cticp_icp_options *options, size_t batch,
+                             cticp_wpoint *const *keypoints, const size_t *n, cticp_frame *frames,
+                             const cticp_frame *const *previous_frames,
+                             const cticp_motion_model_options *motion_options,
+                             cticp_icp_summary *out_summaries);
+
 /* Debug tap for parity tests: normal equations of ONE Gauss-Newton linearisation at `frame`
  * (A 12×12 row-major AFTER the 1/n normalisation and regularisers of ct_icp.cpp:877-910, b 12, n used). */
 int cticp_icp_gn_normal_equations(cticp_map *m, const cticp_icp_options *options,

@@ -29,5 +29,16 @@ for s in syn.make_sequence(frames, syn.SMALL16, seed=1234):
     assert sm.success, sm.error_message
     n = len(od.all_corrected_points())
     print(s["frame_idx"], "K", sm.num_keypoints, "residuals", sm.number_of_residuals, "points", n, flush=True)
+if solver == "GN":
+    # batched GN (k_gn_persistent over groups): three small problems against the odometry's map, the last one failing
+    # with fewer than 100 residuals
+    kp = od.keypoints()
+    frame = od.Trajectory()[-1]
+    kps = [kp[:200].copy(), kp[200:400].copy(), kp[:50].copy()]
+    io = o.ct_icp_options.copy()
+    io.num_iters_icp = 4
+    ss = od.GetMapPointer().icp_register_batch(io, kps, [frame.copy() for _ in kps])
+    assert not ss[2].success
+    print("batch", [(s.success, s.num_residuals_used, s.num_iters) for s in ss], flush=True)
 od.close()
 print("sanitize target OK", solver)
