@@ -162,8 +162,7 @@ private:
     void FreeLmBuffers();
     GnParams MakeParams(const DeviceMap &map, const cticp_icp_options &opt) const;
     int GnCoresident(bool peers);          // co-resident CTAs of k_gn_persistent<peers> on this device
-    int PrepareLoopWords(int groups);      // the word set of the next persistent launch: zero for groups [0, groups)
-    void LoopWordsLaunched(int groups);    // bookkeeping after that launch was enqueued
+    unsigned int ReserveLoopTags(int rows, int groups, int num_iters);   // k_gn_persistent's words and tags (icp_gn.cu)
 
     cudaStream_t stream_;
     const float4 *kp_lo_ = nullptr;
@@ -174,10 +173,10 @@ private:
     double *d_sys_ = nullptr;      // 12*12 + 12 + 4 debug output of the solve kernel
     double *d_acc_ = nullptr;      // reduced accumulator (multi-GPU all-reduce buffer)
     unsigned int *d_ticket_ = nullptr;   // last-CTA-done counter of k_gn_iterate
-    unsigned int *d_sync_words_ = nullptr;   // per group, two sets of (arrive counter, epoch) of k_gn_persistent, alternating per launch
-    int sync_set_ = 0;
-    int sync_groups_ = 1;                    // groups d_sync_words_ holds (grow-only)
-    int sync_clean_[2] = {1, 1};             // per set: groups [0, sync_clean_[s]) have zero words
+    unsigned long long *d_loop_rows_ = nullptr;   // k_gn_persistent: tagged partial rows of the gather CTAs (grow-only)
+    unsigned long long *d_loop_pose_ = nullptr;   // k_gn_persistent: tagged pose words, one block per group (grow-only)
+    int loop_rows_cap_ = 0, loop_groups_cap_ = 0;
+    unsigned int loop_tag_ = 1;                   // next tag to hand out (never 0)
     int *d_groups_ = nullptr;                // batched launches: first_cta | kp_base | keypoint counts (grow-only)
     int groups_cap_ = 0;                     // ints d_groups_ holds
     std::vector<int> h_groups_;

@@ -17,6 +17,7 @@
 #include "frame_policy.h"
 #include "peer_exchange.cuh"
 #include "small_solve.cuh"
+#include "tagged_words.cuh"
 
 namespace cticp {
 namespace cg = cooperative_groups;
@@ -366,12 +367,29 @@ struct GnShared {
     int done;         // gather CTAs: the published `done` flag, fetched together with the pose (one memory round trip)
     struct {          // k_gn_persistent: the group's words, read where used (no registers held across the gather)
         IcpState *st;
-        double *partials;   // gather CTA: its partial row; solver CTA: the group's first row
-        unsigned int *arrive, *epoch;
+        unsigned long long *rows;   // tagged partial rows: gather CTA, its own; solver CTA, the group's first
+        unsigned long long *pose;   // the group's tagged pose words
         int gather_ctas;
     } grp;
     unsigned long long mbar[kGatherWarps];   // -DCTICP_SEL_BULK: one mbarrier per warp for the bulk copies
 };
+
+// the per-warp column sums of a row reduction (columns lane, lane + 32, lane + 64) → their sum in warp order in
+// sh.acc[0][0..kAcc). Called by all threads, after a barrier that follows every earlier read of sh.acc.
+__device__ __forceinline__ void gn_sum_warp_partials(GnShared &sh, double a0, double a1, double a2, int lane, int w) {
+    sh.acc[w][lane] = a0;
+    sh.acc[w][lane + 32] = a1;
+    sh.acc[w][lane + 64] = a2;
+    __syncthreads();
+    double sum = 0;
+    if (threadIdx.x < kAcc) {
+#pragma unroll
+        for (int ww = 0; ww < kGatherWarps; ++ww) sum += sh.acc[ww][threadIdx.x];
+    }
+    __syncthreads();
+    if (threadIdx.x < kAcc) sh.acc[0][threadIdx.x] = sum;
+    __syncthreads();
+}
 
 // deterministic reduction of `rows` partial rows by one CTA: warp g sums the rows b = g (mod kGatherWarps), three
 // columns per lane, all of a warp's loads in flight before the first add; then the per-warp sums in fixed order.
@@ -401,26 +419,15 @@ __device__ __forceinline__ void gn_reduce_rows(GnShared &sh, const double *__res
             }
     }
     __syncthreads();
-    sh.acc[w][lane] = a0;
-    sh.acc[w][lane + 32] = a1;
-    sh.acc[w][lane + 64] = a2;
-    __syncthreads();
-    double sum = 0;
-    if (threadIdx.x < kAcc) {
-#pragma unroll
-        for (int ww = 0; ww < kGatherWarps; ++ww) sum += sh.acc[ww][threadIdx.x];
-    }
-    __syncthreads();
-    if (threadIdx.x < kAcc) sh.acc[0][threadIdx.x] = sum;
-    __syncthreads();
+    gn_sum_warp_partials(sh, a0, a1, a2, lane, w);
 }
 
 // The gather half of an iteration for one CTA: its range [c_lo, c_hi) of the keypoints, in chunks of kRowCap rows →
-// the CTA's partial row (kAcc doubles) at `partial_out` (global). On entry sh.pose is valid and sh.rows.next == 0, both
-// visible to the CTA (the thread that fetched the pose set them before a barrier). All threads call.
-__device__ __forceinline__ void gn_cta_gather(const GatherLaunch &cfg, const int *stencil, const float4 *__restrict__ keypoints,
-                                              int c_lo, int c_hi, GnShared &sh, int lane, int w, double *partial_out,
-                                              GnWarpAcc &A, void *bulk, bool rigid) {
+// the CTA's partial row (kAcc doubles): thread t < kAcc returns entry t. On entry sh.pose is valid and sh.rows.next == 0,
+// both visible to the CTA (the thread that fetched the pose set them before a barrier). All threads call.
+__device__ __forceinline__ double gn_cta_gather(const GatherLaunch &cfg, const int *stencil, const float4 *__restrict__ keypoints,
+                                                int c_lo, int c_hi, GnShared &sh, int lane, int w, GnWarpAcc &A, void *bulk,
+                                                bool rigid) {
     const int W = gn_tile_width(c_hi - c_lo);
     double carry = 0;
     for (int base = c_lo;; base += kRowCap) {
@@ -433,16 +440,14 @@ __device__ __forceinline__ void gn_cta_gather(const GatherLaunch &cfg, const int
     }
     gn_store_warp_row(sh.acc[w], A, lane);
     __syncthreads();
-    if (threadIdx.x < kAcc) {
-        const int t = threadIdx.x;
-        double s = 0;
-        if (t <= kAccSumSq) s = carry;
-        else if (t == kAccStencil || t == kAccKeypoints || t == kAccValidNb) {
+    const int t = threadIdx.x;
+    double s = 0;
+    if (t <= kAccSumSq) s = carry;
+    else if (t == kAccStencil || t == kAccKeypoints || t == kAccValidNb) {
 #pragma unroll
-            for (int ww = 0; ww < kGatherWarps; ++ww) s += sh.acc[ww][t];
-        }
-        __stcg(partial_out + t, s);
+        for (int ww = 0; ww < kGatherWarps; ++ww) s += sh.acc[ww][t];
     }
+    return s;
 }
 
 __device__ __forceinline__ GnPose load_pose(const IcpState *st) {
@@ -492,8 +497,9 @@ k_gn_iterate(GatherLaunch cfg, const float4 *__restrict__ keypoints, const int *
             c_lo = lo + (int) ((long long) (hi - lo) * blockIdx.x / gridDim.x);
             c_hi = lo + (int) ((long long) (hi - lo) * (blockIdx.x + 1) / gridDim.x);
         }
-        gn_cta_gather(cfg, stencil, keypoints, c_lo, c_hi, sh, lane, w, partials + (size_t) blockIdx.x * kAcc, A, bulk_ptr,
-                      active && P.rigid_first && __ldcg(&st->iter) == 0);
+        const double s = gn_cta_gather(cfg, stencil, keypoints, c_lo, c_hi, sh, lane, w, A, bulk_ptr,
+                                       active && P.rigid_first && __ldcg(&st->iter) == 0);
+        if (threadIdx.x < kAcc) __stcg(partials + (size_t) blockIdx.x * kAcc + threadIdx.x, s);
     }
     // ---- last CTA to finish reduces the partials (fixed order) and takes the Gauss-Newton step -----------------
     __threadfence();
@@ -512,57 +518,137 @@ k_gn_iterate(GatherLaunch cfg, const float4 *__restrict__ keypoints, const int *
     warp_gn_solve(sh.acc[0], sh.solve, st, P, mode, sys_out, lane);
 }
 
-// ---- synchronisation of the persistent loop: two flags instead of two grid-wide barriers per iteration ------------------
+// ---- synchronisation of the persistent loop: tagged words (tagged_words.cuh), no fence, no flag, no atomic ---------------
 // The loop's dependencies are asymmetric: the solver CTA needs every gather CTA's partial row; a gather CTA needs the solver
-// CTA's new pose — it never needs the OTHER gather CTAs. So a gather CTA only ARRIVES (fence + one atomic, no wait) and then
-// polls the epoch word the solver CTA bumps after publishing the state, and the solver CTA polls the arrival counter. Per
-// iteration that is one L2 round trip on each side instead of two cg::grid.sync() (each a full
-// grid-wide round trip; tools/micro/coop_launch_cost.cu measures one) plus the separate fetch of the pose.
+// CTA's new pose and `done` flag — it never needs the OTHER gather CTAs. Both hand-offs are tagged words:
+//  - a gather CTA stores its row of iteration `it` as 2 x kAcc words tagged `tag + it` (each double as its two 32-bit
+//    halves) and goes straight on to wait for the next pose; the solver CTA's warps consume the rows in a fixed order, each
+//    as soon as its words carry that tag (gn_reduce_tagged_rows), so the reduction ends about one L2 trip after the last
+//    row lands;
+//  - after the solve the solver warp publishes the pose pair, the slerp constants and `done` as kPosePairs word pairs
+//    tagged `tag + it + 1`; warp 0 of a gather CTA polls them until every pair carries that tag: the poll is the fetch.
+// One buffer per direction is enough. A gather CTA rewrites its row only after it has read the next pose, which the solver
+// publishes only after it has consumed every row of the iteration; the solver rewrites the pose words only after every row
+// of the next iteration has arrived, i.e. after every gather CTA has read them. Tags come from a per-solver counter
+// (IcpSolver::ReserveLoopTags): a launch reserves num_iters + 1 consecutive values and the words are zeroed when allocated
+// and before the counter wraps, so a word left by another iteration or launch never carries the tag a poll waits for.
+// Iteration 0 reads the state the host uploaded; the full IcpState goes to `st` once, when the solver CTA leaves the loop.
 // The launch stays cooperative: the CTAs must be co-resident for the polls to make progress. Every poll is bounded: a
 // protocol error ends the kernel with st->failed = 2 instead of hanging the device.
-// Two sets of words alternate between launches; the solver CTA of a launch zeroes the set of the NEXT launch (nobody touches
-// it meanwhile), so no memset sits between the sampler and this kernel.
 #ifndef CTICP_GN_GRID_BARRIERS
 #define CTICP_GN_FLAG_SYNC 1
 #endif
-struct LoopSync {
-    unsigned int *arrive;   // += 1 by every gather CTA at the end of its gather
-    unsigned int *epoch;    // = iterations published by the solver CTA
-    unsigned int *next_arrive, *next_epoch;   // the other set
+constexpr int kRowWords = 2 * kAcc;   // tagged words of a partial row
+// pose words of a group: the bytes of GnPose as 32-bit halves, then `done` (and an unused half), in word pairs
+constexpr int kPosePairs = 18;
+constexpr int kPoseGroupWords = 48;   // one group's pose words (three 128-byte lines)
+static_assert(sizeof(GnPose) == 8 * (kPosePairs - 1) && 2 * kPosePairs <= kPoseGroupWords, "pose words");
+struct GnLoopWords {
+    unsigned long long *rows;   // partial rows of the gather CTAs, kRowWords each (group g's after those of groups < g)
+    unsigned long long *pose;   // kPoseGroupWords per group
+    unsigned int tag;           // tag of iteration 0's rows; iteration it's rows and pose words carry tag + it
 };
-// A batched launch (IcpSolver::EnqueueGaussNewtonBatch) gives every group its own words: group g's are those of group 0
-// moved by g * kSyncGroupWords (both sets of a group: 2 x (arrive line, epoch line) of 128 bytes each)
-constexpr int kSyncGroupWords = 128;
 
 // The groups of one k_gn_persistent launch. Group g owns the CTAs [first_cta[g], first_cta[g + 1]) of the grid — the first
 // is g's solver CTA, the others gather g's keypoints — its keypoints [kp_base[g], kp_base[g] + count[g]) of the launch's
 // keypoint (and residual plane) array, the state st[g], the partial rows [first_cta[g] - g, first_cta[g + 1] - g - 1) and
-// its own loop words. Groups never wait on each other. `table` (device) = first_cta[0..B] | kp_base[0..B-1];
+// its own pose words. Groups never wait on each other. `table` (device) = first_cta[0..B] | kp_base[0..B-1];
 // num_groups == 1: the whole grid is one group with its keypoints at index 0, and `table` is not read.
 struct GnGroups {
     const int *table;
     int num_groups;
 };
 constexpr long long kLoopSyncTimeout = 4000000000LL;   // SM cycles (~2 s)
-__device__ __forceinline__ bool loop_wait_at_least(const unsigned int *word, unsigned int want,
-                                                   long long timeout = kLoopSyncTimeout) {
+
+// The solver CTA's reduction of the `n` tagged rows of iteration `tag`, bit for bit the sum of gn_reduce_rows: warp w
+// consumes its rows w, w + kGatherWarps, … in that order, each as soon as its words carry the tag (the rows land over the
+// whole gather, so most are added before the last one arrives); then the per-warp sums in warp order. Result in
+// sh.acc[0][0..kAcc). Returns false (uniform) when a row has not arrived within kLoopSyncTimeout. Called by all threads.
+// One row per warp at a time: loads of more rows in flight need registers that this kernel's gather path then spills to
+// local memory (on the bench workload the GN launch took 161 us with five rows in flight, 157 us with two, 151 us with one).
+__device__ __forceinline__ bool gn_reduce_tagged_rows(GnShared &sh, const unsigned long long *rows, int n, unsigned int tag,
+                                                      int lane, int w) {
+    double a0 = 0, a1 = 0, a2 = 0;
+    bool ok = true;
     const long long t0 = clock64();
-    while (*reinterpret_cast<const volatile unsigned int *>(word) < want)
-        if (clock64() - t0 > timeout) return false;
-    __threadfence();
+    for (int b = w; b < n && ok; b += kGatherWarps) {
+        const unsigned long long *row = rows + (size_t) b * kRowWords + 2 * lane;
+        ulonglong2 c0, c1, c2;
+        while (true) {
+            c0 = tagged_load_u64x2(row);
+            c1 = tagged_load_u64x2(row + 64);
+            c2 = tagged_load_u64x2(row + 128);
+            if (pair_tagged(c0, tag) && pair_tagged(c1, tag) && pair_tagged(c2, tag)) break;
+            if (clock64() - t0 > kLoopSyncTimeout) {
+                ok = false;
+                break;
+            }
+        }
+        if (ok) {
+            a0 += pair_double(c0);
+            a1 += pair_double(c1);
+            a2 += pair_double(c2);
+        }
+    }
+    if (!__syncthreads_and(ok)) return false;
+    gn_sum_warp_partials(sh, a0, a1, a2, lane, w);
     return true;
+}
+
+// solver warp: the pose words of the next iteration, tagged `tag`, from the working state (GnPose's layout, then `done`)
+__device__ __forceinline__ void gn_publish_pose(unsigned long long *words, const IcpState &s, unsigned int tag, int lane) {
+    if (lane >= kPosePairs) return;
+    unsigned int lo, hi;
+    if (lane < 16) {
+        const double *d = lane < 4 ? s.qb + lane : lane < 8 ? s.qe + (lane - 4) : lane < 11 ? s.tb + (lane - 8)
+                        : lane < 14 ? s.te + (lane - 11) : lane == 14 ? &s.slerp_theta : &s.slerp_inv_sin;
+        lo = (unsigned int) __double2loint(*d);
+        hi = (unsigned int) __double2hiint(*d);
+    } else if (lane == 16) {
+        lo = (unsigned int) s.slerp_linear;
+        hi = (unsigned int) s.slerp_negate;
+    } else {
+        lo = (unsigned int) s.done;
+        hi = 0;
+    }
+    tagged_store_u64x2(words + 2 * lane, tagged_word(tag, lo), tagged_word(tag, hi));
+}
+
+// warp 0 of a gather CTA: polls the pose words until every pair carries `tag`, then → sh.pose / sh.done (a poll that runs
+// out of time reads as done: the CTA leaves the loop)
+__device__ __forceinline__ void gn_fetch_pose(GnShared &sh, unsigned int tag, long long timeout, int lane) {
+    const unsigned long long *src = sh.grp.pose + 2 * lane;
+    const bool mine = lane < kPosePairs;
+    ulonglong2 v = make_ulonglong2(0ull, 0ull);
+    const long long t0 = clock64();
+    bool ok = true;
+    while (true) {
+        if (mine) v = tagged_load_u64x2(src);
+        if (__all_sync(0xffffffffu, !mine || pair_tagged(v, tag))) break;
+        if (__any_sync(0xffffffffu, clock64() - t0 > timeout)) {
+            ok = false;
+            break;
+        }
+    }
+    if (lane < kPosePairs - 1) {
+        unsigned int *dst = reinterpret_cast<unsigned int *>(&sh.pose) + 2 * lane;
+        dst[0] = word_payload(v.x);
+        dst[1] = word_payload(v.y);
+    } else if (lane == kPosePairs - 1)
+        sh.done = ok ? (int) word_payload(v.x) : 1;
 }
 
 // ---- persistent variant: the WHOLE Gauss-Newton loop in one cooperative launch --------------------------------
 // CTA 0 is the solver CTA (deterministic reduction of the partials + 12x12 solve + pose update, by the same warp on
 // the same SM every iteration, so its instructions stay in that SM's instruction cache: executed cold, the serial tail
-// costs tens of microseconds per iteration, warm a few); CTAs 1..G gather. The two sides meet through the arrive / epoch
-// words above (-DCTICP_GN_GRID_BARRIERS: two grid-wide barriers per iteration, the round's earlier form). While the gather
-// CTAs work on iteration 0, the solver warp runs the solve once on a dummy system to pull its code into the instruction
-// cache. With `tail.enabled` the solver CTA also decides the frame's tail after the loop (frame_policy.h).
+// costs tens of microseconds per iteration, warm a few); CTAs 1..G gather. The two sides meet through the tagged words
+// above (-DCTICP_GN_GRID_BARRIERS: two grid-wide barriers per iteration around the same hand-off, the round's earlier
+// form). While the gather CTAs work on iteration 0, the solver warp runs the solve once on a dummy system to pull its code
+// into the instruction cache. With `tail.enabled` the solver CTA also decides the frame's tail after the loop
+// (frame_policy.h).
 //
 // Groups (GnGroups): one launch can run B independent registrations against the same map, each on its own contiguous range
-// of CTAs with its own solver CTA, state, partial rows and loop words; everything above holds per group. A group that
+// of CTAs with its own solver CTA, state, partial rows and pose words; everything above holds per group. A group that
 // converges or fails leaves the loop alone while the others go on, and one group's serial tail overlaps the others'
 // gathers. The single registration (solo L3 call, odometry) is the one-group case; kPeers and the frame tail are single-group.
 //
@@ -572,8 +658,7 @@ __device__ __forceinline__ bool loop_wait_at_least(const unsigned int *word, uns
 template <bool kPeers>
 __global__ void __launch_bounds__(kGatherWarps * 32, 1)
 k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const int *__restrict__ d_num_keypoints,
-                IcpState *st, double *__restrict__ partials, int num_iters, PeerLinks links, LoopSync sync,
-                FrameTailArgs tail, GnGroups groups) {
+                IcpState *st, int num_iters, PeerLinks links, GnLoopWords words, FrameTailArgs tail, GnGroups groups) {
 #ifndef CTICP_GN_FLAG_SYNC
     cg::grid_group grid = cg::this_grid();
 #endif
@@ -581,8 +666,9 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const GnParams &P = cfg.P;
     // this CTA's group (GnGroups): from here on the group is the whole registration — `cta` is the index within the
-    // group, `group_ctas` its size, and st / partials / sync / the keypoint count are the group's own
+    // group, `group_ctas` its size, and st / rows / pose words / the keypoint count are the group's own
     int g = 0, cta = blockIdx.x, group_ctas = gridDim.x, kp_base = 0;
+    unsigned long long *rows = words.rows, *pose_words = words.pose;
     if (groups.num_groups > 1) {
         const int *first_cta = groups.table;
         while (first_cta[g + 1] <= (int) blockIdx.x) ++g;
@@ -590,28 +676,18 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
         group_ctas = first_cta[g + 1] - first_cta[g];
         kp_base = groups.table[groups.num_groups + 1 + g];
         st += g;
-        partials += (size_t) (first_cta[g] - g) * kAcc;   // the gather CTAs of the groups before this one
-        sync.arrive += kSyncGroupWords * g;
-        sync.epoch += kSyncGroupWords * g;
-        sync.next_arrive += kSyncGroupWords * g;
-        sync.next_epoch += kSyncGroupWords * g;
+        rows += (size_t) (first_cta[g] - g) * kRowWords;   // the gather CTAs of the groups before this one
+        pose_words += (size_t) kPoseGroupWords * g;
     }
     const bool solver_cta = cta == 0;
-#ifdef CTICP_GN_FLAG_SYNC
-    if (solver_cta && threadIdx.x == 0) {   // the next launch's words (idle during this launch)
-        *sync.next_arrive = 0u;
-        *sync.next_epoch = 0u;
-    }
-#endif
     unsigned int peer_seq = 0;   // sequence number of the last exchange (solver CTA only)
     if (kPeers && solver_cta) peer_seq = *links.seq;
     const int gather_ctas = group_ctas - 1;
     const int *stencil = stencil_table_fill(sh.stencil, cfg.G.r);
     if (threadIdx.x == 0) {
         sh.grp.st = st;
-        sh.grp.partials = solver_cta ? partials : partials + (size_t) (cta - 1) * kAcc;
-        sh.grp.arrive = sync.arrive;
-        sh.grp.epoch = sync.epoch;
+        sh.grp.rows = solver_cta ? rows : rows + (size_t) (cta - 1) * kRowWords;
+        sh.grp.pose = pose_words;
         sh.grp.gather_ctas = gather_ctas;
     }
     __syncthreads();
@@ -661,40 +737,35 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
         c_hi = kp_base + kp_lo + (int) ((long long) (kp_hi - kp_lo) * cta / gather_ctas);
     }
     for (int it = 0; it < num_iters; ++it) {
-        // `done` is uniform over the grid: published before the previous grid barrier (the solver CTA reads its own copy)
+        const unsigned int tag = words.tag + (unsigned int) it;
         if (solver_cta) {
             if (sh.state.done) break;
         } else {
             GnWarpAcc A;
             CT_STAMP(const long long t_it = clock64();)
-            if (threadIdx.x == 0) {   // phases A / C read the pose from shared memory: 34 registers less to keep live
-#ifdef CTICP_GN_FLAG_SYNC
-                // the state of iteration `it` is published (it == 0: uploaded by the host before the launch)
-                // (sharded: the solver CTA may itself be waiting for a late peer rank, up to PeerLinks::timeout_cycles)
-                const bool ok = it == 0 || loop_wait_at_least(sh.grp.epoch, (unsigned int) it,
-                                                              kLoopSyncTimeout + (kPeers ? links.timeout_cycles : 0LL));
-#else
-                const bool ok = true;
-#endif
-                const IcpState *gst = sh.grp.st;
-                const int done = __ldcg(&gst->done);   // issued with the pose loads: one round trip, not two
-                sh.pose = load_pose(gst);
-                sh.done = ok ? done : 1;
-                sh.rows.next = 0;
+            if (w == 0) {   // phases A / C read the pose from shared memory: 34 registers less to keep live
+                if (it == 0) {   // the state the host uploaded
+                    if (lane == 0) {
+                        const IcpState *gst = sh.grp.st;
+                        const int done = __ldcg(&gst->done);   // issued with the pose loads: one round trip, not two
+                        sh.pose = load_pose(gst);
+                        sh.done = done;
+                    }
+                } else {
+                    // (sharded: the solver CTA may itself be waiting for a late peer rank, up to PeerLinks::timeout_cycles)
+                    gn_fetch_pose(sh, tag, kLoopSyncTimeout + (kPeers ? links.timeout_cycles : 0LL), lane);
+                }
+                if (lane == 0) sh.rows.next = 0;
             }
             __syncthreads();
             if (sh.done) break;
             CT_STAMP(const long long t_g0 = clock64();)
-            // (CTICP_DEBUG_FLAGS & 2, timing only: an empty range — the barriers and the reduction without the gather work)
+            // (CTICP_DEBUG_FLAGS & 2, timing only: an empty range — the hand-off and the reduction without the gather work)
             const bool skip = (P.debug_flags & 2) != 0;
-            gn_cta_gather(cfg, stencil, keypoints, skip ? 0 : c_lo, skip ? 0 : c_hi, sh, lane, w,
-                          sh.grp.partials, A, bulk_ptr, P.rigid_first && it == 0);
+            const double s = gn_cta_gather(cfg, stencil, keypoints, skip ? 0 : c_lo, skip ? 0 : c_hi, sh, lane, w, A, bulk_ptr,
+                                           P.rigid_first && it == 0);
+            if (threadIdx.x < kAcc) tagged_store_double(sh.grp.rows + 2 * threadIdx.x, tag, s);
             CT_STAMP(const long long t_g = clock64();)
-#ifdef CTICP_GN_FLAG_SYNC
-            __threadfence();   // (the writers of the partial row)
-            __syncthreads();
-            if (threadIdx.x == 0) atomicAdd(sh.grp.arrive, 1u);
-#endif
             CT_STAMP(if (P.dbg_warp && lane == 0 && it < kDbgIters) {
                 unsigned long long *o = P.dbg_warp + ((size_t) it * (gather_ctas * kGatherWarps) + (w * gather_ctas + (cta - 1))) * kDbgSlots;
                 o[0] = (unsigned long long) A.dbg[0]; o[1] = (unsigned long long) A.dbg[1];
@@ -708,23 +779,7 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
 #endif
         }
         CT_STAMP(const long long t_bar = clock64();)
-#ifdef CTICP_GN_FLAG_SYNC
-        if (solver_cta) {
-            if (threadIdx.x == 0) sh.flag = loop_wait_at_least(sh.grp.arrive, (unsigned int) (sh.grp.gather_ctas * (it + 1))) ? 1 : 0;
-            __syncthreads();
-            if (!sh.flag) {   // a gather CTA never arrived: give up (the host raises "Error During Optimization")
-                if (threadIdx.x == 0) {
-                    sh.state.failed = 2;
-                    sh.state.done = 1;
-                    sh.grp.st->failed = 2;
-                    sh.grp.st->done = 1;
-                    __threadfence();
-                    atomicExch(sh.grp.epoch, 0x7fffffffu);
-                }
-                break;
-            }
-        }
-#else
+#ifndef CTICP_GN_FLAG_SYNC
         grid.sync();
 #endif
         CT_STAMP(if (!solver_cta && P.dbg_warp && lane == 0 && w == 0 && it < kDbgIters) {
@@ -733,11 +788,24 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
             o[5] = (unsigned long long) (clock64() - t_bar);
         })
         if (solver_cta) {
-            const long long t_begin = threadIdx.x == 0 ? clock64() : 0;
-            gn_reduce_rows(sh, sh.grp.partials, sh.grp.gather_ctas, lane, w);
+            CT_STAMP(const long long t_red = clock64();)
+            if (!gn_reduce_tagged_rows(sh, sh.grp.rows, sh.grp.gather_ctas, tag, lane, w)) {
+                // a gather CTA's row never arrived: give up (the host raises "Error During Optimization"); pose words of
+                // the next iteration with done = 1 release every gather CTA that waits for them
+                if (w == 0) {
+                    if (lane == 0) {
+                        sh.state.failed = 2;
+                        sh.state.done = 1;
+                    }
+                    __syncwarp();
+                    gn_publish_pose(sh.grp.pose, sh.state, tag + 1u, lane);
+                }
+                break;
+            }
             // -DCTICP_DEBUG_TIMERS: SM cycles summed over the iterations — dbg_t[0] reduction of the partial rows,
-            // [1] everything from there to the published state, [2] the 12x12 solve, [3] the pose update
-            CT_STAMP(if (threadIdx.x == 0) sh.state.dbg_t[0] += (unsigned long long) (clock64() - t_begin);)
+            // [1] everything from there to the published pose, [2] the 12x12 solve, [3] the pose update
+            const long long t_begin = threadIdx.x == 0 ? clock64() : 0;
+            CT_STAMP(if (threadIdx.x == 0) sh.state.dbg_t[0] += (unsigned long long) (t_begin - t_red);)
             CT_STAMP(const long long t_rest = clock64();)
             bool peers_ok = true;
             if (kPeers) {
@@ -758,51 +826,43 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
                 } else
                     warp_gn_solve(sh.acc[0], sh.solve, ws, P, 0, nullptr, lane);
                 __syncwarp();
+                // the gather CTAs wait for the pose words only when they have another iteration to run
+                if (it + 1 < num_iters) gn_publish_pose(sh.grp.pose, *ws, tag + 1u, lane);
                 if (lane == 0) {
                     t_solve += clock64() - t_begin;
                     ws->cycles_total = (unsigned long long) (clock64() - t_loop);
                     ws->cycles_solve = (unsigned long long) t_solve;
                 }
-                __syncwarp();
-                // publish: the gather CTAs read the pose pair / done flag of the next iteration from global memory
-                const int *src = reinterpret_cast<const int *>(ws);
-                int *dst = reinterpret_cast<int *>(sh.grp.st);
-                for (int i = lane; i < (int) (sizeof(IcpState) / sizeof(int)); i += 32) __stcg(dst + i, src[i]);
-                CT_STAMP(if (lane == 0) {
-                    ws->dbg_t[1] += (unsigned long long) (clock64() - t_rest);
-                    __stcg(&sh.grp.st->dbg_t[1], ws->dbg_t[1]);
-                })
-#ifdef CTICP_GN_FLAG_SYNC
-                __threadfence();   // (the lanes that wrote the state)
-                __syncwarp();
-                if (lane == 0) atomicExch(sh.grp.epoch, (unsigned int) (it + 1));
-#endif
+                CT_STAMP(if (lane == 0) ws->dbg_t[1] += (unsigned long long) (clock64() - t_rest);)
             }
-#ifdef CTICP_GN_FLAG_SYNC
             __syncthreads();   // warp 0 is done with sh.acc / sh.state before the next iteration's reduction
-#else
-            __threadfence();
-#endif
         }
 #ifndef CTICP_GN_FLAG_SYNC
         grid.sync();
 #endif
     }
     if (kPeers && solver_cta && threadIdx.x == 0) *links.seq = peer_seq;
+    if (!solver_cta) return;
+    __syncthreads();   // sh.state is final
+    if (w != 0) return;
+    // the registration's state, published once on every way out of the loop (the host, k_frame_policy and later launches
+    // read it after this kernel)
+    {
+        const int *src = reinterpret_cast<const int *>(&sh.state);
+        int *dst = reinterpret_cast<int *>(sh.grp.st);
+        for (int i = lane; i < (int) (sizeof(IcpState) / sizeof(int)); i += 32) dst[i] = src[i];
+    }
     // ---- the tail of the registration (frame_policy.h): AssessRegistration + the insertion policy on the final state, the
     // verdict to HBM (the speculative map update launched behind this kernel reads it) and to mapped pinned host memory
-    if (solver_cta && tail.enabled) {
-        __syncthreads();   // sh.state is final
-        if (w == 0) {
-            const int *src = reinterpret_cast<const int *>(&sh.state);
-            int *dst = reinterpret_cast<int *>(&sh.verdict.state);
-            for (int i = lane; i < (int) (sizeof(IcpState) / sizeof(int)); i += 32) dst[i] = src[i];
-            if (lane < 4) sh.verdict.counts[lane] = __ldcg(tail.counts + lane);
-            __syncwarp();
-            if (lane == 0) frame_policy_decide(sh.verdict, tail.in);
-            __syncwarp();
-            frame_verdict_publish(sh.verdict, tail.dv, tail.hv, lane);
-        }
+    if (tail.enabled) {
+        const int *src = reinterpret_cast<const int *>(&sh.state);
+        int *dst = reinterpret_cast<int *>(&sh.verdict.state);
+        for (int i = lane; i < (int) (sizeof(IcpState) / sizeof(int)); i += 32) dst[i] = src[i];
+        if (lane < 4) sh.verdict.counts[lane] = __ldcg(tail.counts + lane);
+        __syncwarp();
+        if (lane == 0) frame_policy_decide(sh.verdict, tail.in);
+        __syncwarp();
+        frame_verdict_publish(sh.verdict, tail.dv, tail.hv, lane);
     }
 }
 
@@ -938,8 +998,6 @@ IcpSolver::IcpSolver(cudaStream_t stream) : stream_(stream) {
     CT_CUDA_CHECK(cudaMalloc(&d_acc_, sizeof(double) * kAcc));
     CT_CUDA_CHECK(cudaMalloc(&d_ticket_, sizeof(unsigned int)));
     CT_CUDA_CHECK(cudaMemset(d_ticket_, 0, sizeof(unsigned int)));
-    CT_CUDA_CHECK(cudaMalloc(&d_sync_words_, sizeof(unsigned int) * 128));   // two sets of (arrive, epoch), a 128-byte line each
-    CT_CUDA_CHECK(cudaMemset(d_sync_words_, 0, sizeof(unsigned int) * 128));
     for (int i = 0; i < kMaxEvents; ++i) {
         CT_CUDA_CHECK(cudaEventCreate(&ev_begin_[i]));
         CT_CUDA_CHECK(cudaEventCreate(&ev_end_[i]));
@@ -950,7 +1008,8 @@ IcpSolver::~IcpSolver() {
     cudaFree(d_sys_);
     cudaFree(d_acc_);
     cudaFree(d_ticket_);
-    cudaFree(d_sync_words_);
+    cudaFree(d_loop_rows_);
+    cudaFree(d_loop_pose_);
     cudaFree(d_groups_);
     FreeLmBuffers();
     for (int i = 0; i < kMaxEvents; ++i) {
@@ -1037,40 +1096,31 @@ int IcpSolver::GnCoresident(bool peers) {
     return coresident;
 }
 
-// Loop words: group g, set s at d_sync_words_ + kSyncGroupWords * g + 64 * s (arrive; epoch 32 words further). Launches
-// alternate between the sets, and the solver CTA of every group zeroes its words of the other set, so back-to-back launches
-// of as many groups need no memset. A launch with more groups than the set has clean zeroes the missing groups first.
-static LoopSync LoopSyncOf(unsigned int *words, int set) {
-    LoopSync sync;
-    sync.arrive = words + 64 * set;
-    sync.epoch = sync.arrive + 32;
-    sync.next_arrive = words + 64 * (set ^ 1);
-    sync.next_epoch = sync.next_arrive + 32;
-    return sync;
-}
-int IcpSolver::PrepareLoopWords(int groups) {
-    if (groups > sync_groups_) {
+// The words of the persistent loop (GnLoopWords) for `rows` gather CTAs and `groups` groups, grown on demand and zeroed when
+// allocated, and the tag of iteration 0 of a launch of `num_iters` iterations: the counter advances by num_iters + 1 per
+// launch. Tag 0 is never handed out, so zeroed words never match; when the counter would wrap, both areas are zeroed
+// again (stream order: after every earlier launch) and it restarts at 1.
+unsigned int IcpSolver::ReserveLoopTags(int rows, int groups, int num_iters) {
+    const auto grow = [&](unsigned long long *&buf, int &cap, int want, size_t words_each) {
+        if (want <= cap) return;
         CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(d_sync_words_);
-        d_sync_words_ = nullptr;
-        CT_CUDA_CHECK(cudaMalloc(&d_sync_words_, sizeof(unsigned int) * kSyncGroupWords * groups));
-        CT_CUDA_CHECK(cudaMemset(d_sync_words_, 0, sizeof(unsigned int) * kSyncGroupWords * groups));
-        sync_groups_ = groups;
-        sync_clean_[0] = sync_clean_[1] = groups;
+        cudaFree(buf);
+        buf = nullptr;
+        CT_CUDA_CHECK(cudaMalloc(&buf, sizeof(unsigned long long) * words_each * (size_t) want));
+        CT_CUDA_CHECK(cudaMemsetAsync(buf, 0, sizeof(unsigned long long) * words_each * (size_t) want, stream_));
+        cap = want;
+    };
+    grow(d_loop_rows_, loop_rows_cap_, std::max(rows, 1), kRowWords);
+    grow(d_loop_pose_, loop_groups_cap_, std::max(groups, 1), kPoseGroupWords);
+    const unsigned long long span = (unsigned long long) std::max(num_iters, 0) + 1;
+    if (loop_tag_ + span > 0xffffffffull) {
+        CT_CUDA_CHECK(cudaMemsetAsync(d_loop_rows_, 0, sizeof(unsigned long long) * kRowWords * (size_t) loop_rows_cap_, stream_));
+        CT_CUDA_CHECK(cudaMemsetAsync(d_loop_pose_, 0, sizeof(unsigned long long) * kPoseGroupWords * (size_t) loop_groups_cap_, stream_));
+        loop_tag_ = 1;
     }
-    const int s = sync_set_, c = sync_clean_[s];
-    if (c < groups) {   // both sets of groups [c, groups): idle, as every earlier launch on the stream has ended
-        CT_CUDA_CHECK(cudaMemsetAsync(d_sync_words_ + (size_t) kSyncGroupWords * c, 0,
-                                      sizeof(unsigned int) * kSyncGroupWords * (groups - c), stream_));
-        if (sync_clean_[s ^ 1] >= c) sync_clean_[s ^ 1] = std::max(sync_clean_[s ^ 1], groups);
-        sync_clean_[s] = groups;
-    }
-    return s;
-}
-void IcpSolver::LoopWordsLaunched(int groups) {
-    sync_clean_[sync_set_] = 0;
-    sync_clean_[sync_set_ ^ 1] = std::max(sync_clean_[sync_set_ ^ 1], groups);
-    sync_set_ ^= 1;
+    const unsigned int tag = loop_tag_;
+    loop_tag_ += (unsigned int) span;
+    return tag;
 }
 
 bool IcpSolver::batch_supported() const {
@@ -1119,19 +1169,17 @@ void IcpSolver::EnqueueGaussNewtonBatch(const DeviceMap &map, const cticp_icp_op
         groups_cap_ = (int) h_groups_.size();
     }
     CT_CUDA_CHECK(cudaMemcpyAsync(d_groups_, h_groups_.data(), sizeof(int) * h_groups_.size(), cudaMemcpyHostToDevice, stream_));
-    EnsurePartials(grid);
-    LoopSync sync = LoopSyncOf(d_sync_words_, PrepareLoopWords(batch));
+    const unsigned int tag = ReserveLoopTags(grid - batch, batch, num_iters);
+    GnLoopWords words{d_loop_rows_, d_loop_pose_, tag};
     const float4 *kp = d_keypoints;
     const int *nk = d_groups_ + 2 * batch + 1;
-    double *parts = d_partials_;
     int iters = num_iters;
     PeerLinks links{};
     FrameTailArgs tail_args{};
     GnGroups groups{d_groups_, batch};
-    void *args[] = {&cfg, &kp, &nk, &d_states, &parts, &iters, &links, &sync, &tail_args, &groups};
+    void *args[] = {&cfg, &kp, &nk, &d_states, &iters, &links, &words, &tail_args, &groups};
     CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_gn_persistent<false>, dim3(grid), dim3(kGatherWarps * 32), args,
                                               sizeof(GnShared), stream_));
-    LoopWordsLaunched(batch);
     gather_launches_ += 1;
     launches_ += 1;
 }
@@ -1197,12 +1245,10 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
         void *kernel = peers ? (void *) k_gn_persistent<true> : (void *) k_gn_persistent<false>;
         const int coresident = GnCoresident(peers);
         const int blocks = GatherBlocks(k_share, std::max(1, coresident - 1), kp_per_cta_);
-        EnsurePartials(blocks + 1);
         int grid = std::min(blocks + 1, coresident);
         grid = std::max(grid, 2);
         const float4 *kp = d_keypoints;
         const int *nk = d_num_keypoints;
-        double *parts = d_partials_;
         int iters = num_iters;
         PeerLinks links = peers ? PeerLinksOf(links_host_) : PeerLinks{};
 #ifdef CTICP_DEBUG_TIMERS
@@ -1218,15 +1264,15 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
             cfg.P.dbg_warp = d_dbg_warp_;
         }
 #endif
-        LoopSync sync = LoopSyncOf(d_sync_words_, PrepareLoopWords(1));
+        const unsigned int tag = ReserveLoopTags(grid - 1, 1, num_iters);
+        GnLoopWords words{d_loop_rows_, d_loop_pose_, tag};
         FrameTailArgs tail_args{};
         if (tail) tail_args = *tail;
         GnGroups groups{nullptr, 1};
-        void *args[] = {&cfg, &kp, &nk, &d_state, &parts, &iters, &links, &sync, &tail_args, &groups};
+        void *args[] = {&cfg, &kp, &nk, &d_state, &iters, &links, &words, &tail_args, &groups};
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
         if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
         CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kGatherWarps * 32), args, sizeof(GnShared), stream_));
-        LoopWordsLaunched(1);
         if (timed) cudaEventRecord(ev_end_[ev_used_++], stream_);
         gather_launches_ += 1;
         launches_ += 1;

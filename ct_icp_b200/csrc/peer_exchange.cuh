@@ -20,6 +20,7 @@
 #include <cuda_runtime.h>
 
 #include "icp.h"
+#include "tagged_words.cuh"
 
 namespace cticp {
 
@@ -50,15 +51,6 @@ inline PeerLinks PeerLinksOf(const PeerLinksHost &h) {   // the host-side descri
     return L;
 }
 
-__device__ __forceinline__ void peer_store_u64(unsigned long long *p, unsigned long long v) {
-    asm volatile("st.volatile.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long peer_load_u64(const unsigned long long *p) {
-    unsigned long long v;
-    asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-
 // In-place sum over ranks of acc[0..kAcc) (shared memory of the calling CTA). Called by ALL threads of a CTA (any
 // size that is a multiple of 32); s_half: world * kPeerWords unsigned ints of shared scratch; s_ok: one shared int.
 // `seq` = sequence number of this exchange (uniform, never 0). Returns false on time-out (uniform).
@@ -72,19 +64,19 @@ __device__ __forceinline__ bool peer_allreduce(const PeerLinks &L, unsigned int 
         const unsigned int half = reinterpret_cast<const unsigned int *>(acc)[wd];
         const unsigned long long word = ((unsigned long long) seq << 32) | (unsigned long long) half;
         for (int p = 0; p < L.world; ++p)
-            peer_store_u64(L.inbox[p] + slot + (size_t) L.rank * kPeerWords + wd, word);
+            tagged_store_u64(L.inbox[p] + slot + (size_t) L.rank * kPeerWords + wd, word);
     }
     const unsigned long long *mine = L.inbox[L.rank] + slot;
     const long long t0 = clock64();
     for (int wd = tid; wd < kPeerWords; wd += nthreads) {
         for (int r = 0; r < L.world; ++r) {
-            unsigned long long w = peer_load_u64(mine + (size_t) r * kPeerWords + wd);
+            unsigned long long w = tagged_load_u64(mine + (size_t) r * kPeerWords + wd);
             while ((unsigned int) (w >> 32) != seq) {
                 if (clock64() - t0 > L.timeout_cycles) {
                     *s_ok = 0;
                     break;
                 }
-                w = peer_load_u64(mine + (size_t) r * kPeerWords + wd);
+                w = tagged_load_u64(mine + (size_t) r * kPeerWords + wd);
             }
             s_half[r * kPeerWords + wd] = (unsigned int) w;
         }

@@ -14,7 +14,7 @@
 #   timers      -DCTICP_DEBUG_TIMERS        clock64 stamps in the solver CTA of k_gn_persistent (built here, not benchmarked)
 #   selv1       -DCTICP_SEL_V1              the selection's first cut (owner by binary search over shuffles, separate histogram
 #                                           pass, butterfly sums): what the default path of gather_select.cuh replaced
-#   gridsync    -DCTICP_GN_GRID_BARRIERS    k_gn_persistent with two cg::grid.sync() per iteration instead of the arrive / epoch flags
+#   gridsync    -DCTICP_GN_GRID_BARRIERS    k_gn_persistent with two cg::grid.sync() per iteration around the tagged hand-off words
 #   noprune     -DCTICP_NO_VOXEL_PRUNE      the gather loads every voxel of the stencil (no box-vs-radius prune)
 set -u
 ROOT="$(cd "$(dirname "$0")/.." && pwd)"

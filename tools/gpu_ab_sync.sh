@@ -1,5 +1,5 @@
 #!/bin/bash
-# A/B of the loop synchronisation of k_gn_persistent (arrive / epoch flags = default build, grid barriers = libcticp_b200_gridsync.so),
+# A/B of the loop synchronisation of k_gn_persistent (tagged hand-off words = default build, grid barriers = libcticp_b200_gridsync.so),
 # alternating, same box: does it move the end-to-end numbers (e2e, e2e_dropin)? usage: bash tools/gpu_ab_sync.sh <tag>
 TAG=${1:-x}; mkdir -p gpurun_out
 for round in 1 2; do
