@@ -72,6 +72,8 @@ class Binding:
                                        P(abi.Frame), P(abi.MotionModelOptions), P(abi.IcpSummary)]),
             "icp_register_batch": (C.c_int, [vp, P(abi.IcpOptions), sz, P(vp), P(sz), P(abi.Frame), P(vp),
                                              P(abi.MotionModelOptions), P(abi.IcpSummary)]),
+            "icp_register_batch_ex": (C.c_int, [vp, P(abi.IcpOptions), P(abi.StrategyOptions), sz, P(vp), P(sz),
+                                                P(abi.Frame), P(vp), P(abi.MotionModelOptions), P(abi.IcpSummary)]),
             "icp_gn_normal_equations": (C.c_int, [vp, P(abi.IcpOptions), vp, sz, P(abi.Frame), P(abi.Frame),
                                                   P(abi.MotionModelOptions), vp, vp, P(i32)]),
             "grid_sample_indices": (i64, [C.c_int, vp, sz, sz, dbl, vp, sz]),
@@ -282,6 +284,16 @@ class VoxelMap:
         """B independent registrations (solver GN) in one launch (cticp_icp_register_batch). keypoints_list: B arrays of
         abi.wpoint_dtype() (world rewritten in place); frames: B abi.Frame (updated in place); previous_frames: None or
         B entries, each an abi.Frame or None (no motion prior for that problem). Returns the B abi.IcpSummary."""
+        return self._register_batch(None, icp_options, keypoints_list, frames, previous_frames, motion_options)
+
+    def icp_register_batch_ex(self, icp_options, keypoints_list, frames, previous_frames=None, motion_options=None,
+                              strategy=None):
+        """icp_register_batch for every solver (cticp_icp_register_batch_ex): GN, CERES or ROBUST, with the neighborhood
+        strategy CERES consults (None: icp_register's default). Returns the B abi.IcpSummary."""
+        st = strategy if strategy is not None else abi.StrategyOptions(0, 20, 8, 0)
+        return self._register_batch(st, icp_options, keypoints_list, frames, previous_frames, motion_options)
+
+    def _register_batch(self, strategy, icp_options, keypoints_list, frames, previous_frames, motion_options):
         B = len(keypoints_list)
         if len(frames) != B or (previous_frames is not None and len(previous_frames) != B):
             raise ValueError("keypoints_list, frames and previous_frames must have one entry per problem")
@@ -297,9 +309,12 @@ class VoxelMap:
         if previous_frames is not None:
             prev = (C.c_void_p * m)(*[C.addressof(p) if p is not None else None for p in previous_frames])
         out = (abi.IcpSummary * m)()
-        rc = self.b.fn("icp_register_batch")(
-            self.h, C.byref(icp_options), B, kps, ns, fr, prev,
-            C.byref(motion_options) if motion_options is not None else None, out)
+        mo = C.byref(motion_options) if motion_options is not None else None
+        if strategy is None:
+            rc = self.b.fn("icp_register_batch")(self.h, C.byref(icp_options), B, kps, ns, fr, prev, mo, out)
+        else:
+            rc = self.b.fn("icp_register_batch_ex")(self.h, C.byref(icp_options), C.byref(strategy), B, kps, ns, fr, prev,
+                                                    mo, out)
         if rc >= 0 or rc == abi.ERR_INTERNAL:   # ERR_INTERNAL: a timed-out problem; every output is written all the same
             for b, f in enumerate(frames):
                 C.memmove(C.addressof(f), C.addressof(fr[b]), C.sizeof(abi.Frame))

@@ -782,10 +782,14 @@ int cticp_icp_register(cticp_map *m, const cticp_icp_options *options, const cti
     });
 }
 
-int cticp_icp_register_batch(cticp_map *m, const cticp_icp_options *options, size_t batch,
-                             cticp_wpoint *const *keypoints, const size_t *n, cticp_frame *frames,
-                             const cticp_frame *const *previous_frames, const cticp_motion_model_options *motion_options,
-                             cticp_icp_summary *out_summaries) {
+namespace {
+// cticp_icp_register_batch(_ex): the problems' shared arguments are checked, then every problem's inputs (timestamps) are
+// checked and packed before anything reaches the device; one batched launch of the solver's persistent kernel.
+// gn_only: the entry without a strategy argument, which runs solver GN only.
+int RegisterBatch(cticp_map *m, const cticp_icp_options *options, const cticp_strategy_options *strategy, size_t batch,
+                  cticp_wpoint *const *keypoints, const size_t *n, cticp_frame *frames,
+                  const cticp_frame *const *previous_frames, const cticp_motion_model_options *motion_options,
+                  cticp_icp_summary *out_summaries, bool gn_only) {
     return Guard([&] {
         if (!m || !options || !keypoints || !n || !frames) throw std::invalid_argument("null argument");
         if (batch == 0 || batch > 64) throw std::invalid_argument("batch must be in [1, 64]");
@@ -795,12 +799,24 @@ int cticp_icp_register_batch(cticp_map *m, const cticp_icp_options *options, siz
             total += n[b];
         }
         if (total > (size_t) INT32_MAX) throw std::invalid_argument("too many keypoints in one batch");
-        if (options->solver != CTICP_SOLVER_GN) throw UnsupportedError("cticp_icp_register_batch: solver GN only");
-        if (options->max_number_neighbors > 32 || options->max_number_neighbors < 1)
-            throw UnsupportedError("max_number_neighbors must be in [1, 32]");
+        if (gn_only && options->solver != CTICP_SOLVER_GN) throw UnsupportedError("cticp_icp_register_batch: solver GN only");
+        cticp_strategy_options st{0, 20, 8, 0, 60., 0.1, 2.0, 1.0};   // cticp_icp_register's default
+        if (strategy) st = *strategy;
+        const bool gn = options->solver == CTICP_SOLVER_GN;
+        if (gn) {
+            if (options->max_number_neighbors > 32 || options->max_number_neighbors < 1)
+                throw UnsupportedError("max_number_neighbors must be in [1, 32]");
+        } else if (options->solver != CTICP_SOLVER_CERES && options->solver != CTICP_SOLVER_ROBUST) {
+            throw UnsupportedError("Unsupported Solver Type");
+        }
         CAPI_CUDA(cudaSetDevice(m->device));
-        if (!m->icp->batch_supported())
+        if (gn && !m->icp->batch_supported())
             throw UnsupportedError("cticp_icp_register_batch needs the persistent Gauss-Newton loop with flag synchronisation");
+        if (!gn) {
+            if (!m->icp->use_persistent())
+                throw UnsupportedError("cticp_icp_register_batch_ex needs the persistent LM loop (CTICP_PERSISTENT)");
+            m->icp->CheckCeresOptions(*m->map, *options, st);
+        }
         // every problem's inputs are checked (timestamps) and packed before anything reaches the device
         std::vector<float4> kp(std::max<size_t>(total, 1)), lo(std::max<size_t>(total, 1));
         std::vector<IcpState> S(batch);
@@ -829,7 +845,10 @@ int cticp_icp_register_batch(cticp_map *m, const cticp_icp_options *options, siz
         }
         CAPI_CUDA(cudaMemcpyAsync(D.states, S.data(), sizeof(IcpState) * batch, cudaMemcpyHostToDevice, m->stream));
         m->icp->set_keypoints_lo(D.lo);
-        m->icp->EnqueueGaussNewtonBatch(*m->map, *options, (int) batch, n, D.kp, options->num_iters_icp, D.states);
+        if (gn)
+            m->icp->EnqueueGaussNewtonBatch(*m->map, *options, (int) batch, n, D.kp, options->num_iters_icp, D.states);
+        else
+            m->icp->EnqueueCeresBatch(*m->map, *options, st, (int) batch, n, D.kp, D.states);
         CAPI_CUDA(cudaMemcpyAsync(S.data(), D.states, sizeof(IcpState) * batch, cudaMemcpyDeviceToHost, m->stream));
         CAPI_CUDA(cudaStreamSynchronize(m->stream));
         bool timeout = false, not_enough = false;
@@ -842,6 +861,23 @@ int cticp_icp_register_batch(cticp_map *m, const cticp_icp_options *options, siz
         if (not_enough) g_last_error = "[CT_ICP]Error : not enough keypoints selected in ct-icp !";
         return (int) CTICP_OK;
     });
+}
+}  // namespace
+
+int cticp_icp_register_batch(cticp_map *m, const cticp_icp_options *options, size_t batch,
+                             cticp_wpoint *const *keypoints, const size_t *n, cticp_frame *frames,
+                             const cticp_frame *const *previous_frames, const cticp_motion_model_options *motion_options,
+                             cticp_icp_summary *out_summaries) {
+    return RegisterBatch(m, options, nullptr, batch, keypoints, n, frames, previous_frames, motion_options, out_summaries,
+                         true);
+}
+
+int cticp_icp_register_batch_ex(cticp_map *m, const cticp_icp_options *options, const cticp_strategy_options *strategy,
+                                size_t batch, cticp_wpoint *const *keypoints, const size_t *n, cticp_frame *frames,
+                                const cticp_frame *const *previous_frames,
+                                const cticp_motion_model_options *motion_options, cticp_icp_summary *out_summaries) {
+    return RegisterBatch(m, options, strategy, batch, keypoints, n, frames, previous_frames, motion_options, out_summaries,
+                         false);
 }
 
 int cticp_icp_gn_normal_equations(cticp_map *m, const cticp_icp_options *options, const cticp_wpoint *keypoints,

@@ -83,6 +83,14 @@ struct GnParams {
                                    // interpolates like always (ct_icp.cpp:964-966)
 };
 
+// bound of every wait of the persistent loops on another CTA (k_gn_persistent's hand-off, k_lm_persistent's group barrier)
+constexpr long long kLoopSyncTimeout = 4000000000LL;   // SM cycles (~2 s)
+
+// CTAs of the persistent kernels (icp_batch.cu): GatherBlocks is the worker / gather CTA count of a solo launch for
+// k_hint keypoints; BatchGatherCtas deals the co-resident CTAs of a batched launch over its problems (contract there).
+int GatherBlocks(size_t k_hint, int max_blocks, int kp_per_cta);
+void BatchGatherCtas(const size_t *n, int batch, int coresident, int kp_per_cta, int *gather);
+
 struct FrameTailArgs;   // frame_policy.h
 
 class IcpSolver {
@@ -103,7 +111,7 @@ public:
     // B independent Gauss-Newton registrations against `map` with shared options, in ONE launch of the persistent kernel
     // (k_gn_persistent over groups). Problem b's h_n[b] keypoints are at [kp_base_b, kp_base_b + h_n[b]) of d_keypoints,
     // kp_base_b = h_n[0] + … + h_n[b - 1] (the residual plane, when set_keypoints_lo gave one, alike); its state is
-    // d_states[b]. CTA policy and its bit-identity contract: BatchGatherCtas (icp_gn.cu). Throws CapacityError when
+    // d_states[b]. CTA policy and its bit-identity contract: BatchGatherCtas (icp_batch.cu). Throws CapacityError when
     // the device cannot hold two CTAs per problem; requires batch_supported().
     void EnqueueGaussNewtonBatch(const DeviceMap &map, const cticp_icp_options &opt, int batch, const size_t *h_n,
                                  const float4 *d_keypoints, int num_iters, IcpState *d_states);
@@ -116,6 +124,16 @@ public:
     void EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
                       const float4 *d_keypoints, const int *d_num_keypoints, size_t k_hint, size_t k_capacity,
                       IcpState *d_state, int shard_rank = 0, int shard_world = 1, void *nccl_comm = nullptr);
+    // the option checks of EnqueueCeres, without touching the device: UnsupportedError / std::invalid_argument
+    void CheckCeresOptions(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy) const;
+    // B independent CERES / ROBUST registrations against `map` with shared options and strategy, in ONE launch of the
+    // persistent LM kernel (k_lm_persistent over groups, separated by group barriers). Keypoints and states are laid out as
+    // for EnqueueGaussNewtonBatch; the CTA policy and its bit-identity contract are BatchGatherCtas' with the LM kernel's
+    // co-resident count. A group whose barrier times out ends with failed = 2 without holding up the others. Throws
+    // CapacityError when the device cannot hold two CTAs per problem; requires use_persistent().
+    void EnqueueCeresBatch(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
+                           int batch, const size_t *h_n, const float4 *d_keypoints, IcpState *d_states);
+    bool use_persistent() const { return use_persistent_; }
 
     // single linearisation at the current state → A (12x12, after 1/n and regularisers), b, n_used (debug tap)
     void NormalEquations(const DeviceMap &map, const cticp_icp_options &opt, const float4 *d_keypoints,
@@ -158,11 +176,16 @@ private:
     void EnsurePartials(int blocks);
     void EnsureLmBuffers(size_t k_upper);
     void DebugLmTrace(void *d_lm);
-    int lm_coresident_[6] = {0, 0, 0, 0, 0, 0};   // k_lm_persistent<mode, peers>
+    int lm_coresident_[9] = {};   // k_lm_persistent<mode, peers> at mode * 2 + peers, <mode, false, true> at 6 + mode
     void FreeLmBuffers();
     GnParams MakeParams(const DeviceMap &map, const cticp_icp_options &opt) const;
     int GnCoresident(bool peers);          // co-resident CTAs of k_gn_persistent<peers> on this device
     unsigned int ReserveLoopTags(int rows, int groups, int num_iters);   // k_gn_persistent's words and tags (icp_gn.cu)
+    // group table of a batched launch (first_cta | kp_base | count, BatchGatherCtas) built and uploaded to d_groups_;
+    // returns the grid (icp_batch.cu)
+    int UploadGroupTable(const size_t *h_n, int batch, int coresident);
+    int LmCoresident(int variant, void *kernel);   // co-resident CTAs of a k_lm_persistent instantiation (icp_lm.cu)
+    bool UploadLmStrategy(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy);
 
     cudaStream_t stream_;
     const float4 *kp_lo_ = nullptr;
@@ -186,6 +209,8 @@ private:
     void *d_lm_classes_ = nullptr;   // solver ROBUST: slam::NEIGHBORHOOD_TYPE per keypoint
     void *d_lm_strategy_ = nullptr;  // DistanceBasedStrategy parameters + every map level
     size_t lm_capacity_ = 0;
+    void *d_lm_groups_ = nullptr;    // batched launches: per group an LmState, a stats line and the barrier words (grow-only)
+    int lm_groups_cap_ = 0;
     int launches_ = 0;
     float gather_ms_ = 0.f;
     int gather_launches_ = 0;

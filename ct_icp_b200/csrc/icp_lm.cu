@@ -1096,18 +1096,80 @@ __device__ __forceinline__ void lm_publish(LmState *dst, const LmState *src, int
     }
 }
 
-template <int kMode, bool kPeers>
-__global__ void __launch_bounds__(kLmPWarps * 32, 1)
-k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoints, const int *__restrict__ d_num_keypoints,
-                IcpState *st, LmState *lm_g, ResidualBlock *__restrict__ blocks, int *__restrict__ sel_idx,
-                unsigned char *__restrict__ classes, unsigned long long *stats, const DistanceStrategy *__restrict__ D,
-                double *__restrict__ partials, PeerLinks links) {
+// Groups of a batched launch (EnqueueCeresBatch): group g owns the CTAs [first_cta[g], first_cta[g + 1]) of the grid — the
+// first is g's solver CTA, the others its workers — its keypoints [kp_base[g], kp_base[g] + count[g]) of the launch's
+// keypoint (and residual plane) array, the residual blocks / sel_idx / classes from kp_base[g] · ncn on, the states st[g]
+// and the LmState at kLmStateStride · g, its stats pair, the partial rows [first_cta[g] - g, first_cta[g + 1] - g - 1) and
+// its barrier words. `table` (device) = first_cta[0..B] | kp_base[0..B-1] | count[0..B-1] (the GN batch's table).
+struct LmGroups {
+    const int *table;
+    int num_groups;
+    unsigned int *barrier;   // kLmBarrierWords per group: arrival counter at [0], abort word at [32]; zeroed before each launch
+};
+constexpr int kLmBarrierWords = 64;                                        // two 128-byte lines per group
+constexpr size_t kLmStateStride = (sizeof(LmState) + 127) / 128 * 128;     // LmStates of the groups on separate lines
+constexpr int kLmStatsStride = 16;                                         // one 128-byte line of stats per group
+
+__device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int *p) {
+    unsigned int v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+
+// The grid barrier of cooperative groups, scoped to one group of CTAs: every CTA of the group arrives once per barrier, so
+// the group's barrier k completes when its counter reaches `target` = k · group_ctas. The wait is bounded: a CTA that has
+// waited kLoopSyncTimeout cycles sets the group's abort word; a waiter that finds it set leaves too. Returns false
+// (uniform over the CTA) when the group was aborted. Groups share nothing, so a stalled group never holds up another.
+// Called by all threads of the CTA.
+__device__ __forceinline__ bool lm_group_barrier(unsigned int *bar, unsigned int target) {
+    __syncthreads();
+    int ok = 1;
+    if (threadIdx.x == 0) {
+        unsigned int *count = bar, *abort = bar + 32;
+        __threadfence();
+        atomicAdd(count, 1u);
+        const long long t0 = clock64();
+        while (ld_acquire_u32(count) < target) {
+            if (ld_acquire_u32(abort)) {
+                ok = 0;
+                break;
+            }
+            if (clock64() - t0 > kLoopSyncTimeout) {
+                atomicExch(abort, 1u);
+                ok = 0;
+                break;
+            }
+        }
+    }
+    return __syncthreads_and(ok) != 0;
+}
+
+// The registration of one group: `cta` is this CTA's index in it, `group_ctas` its size, and every pointer is the group's
+// own. Solo (kGrouped false): the whole grid, separated by grid-wide barriers. Grouped: group barriers (lm_group_barrier at
+// `bar`); when one times out every CTA of the group leaves the loop and the solver CTA marks the state failed = 2.
+template <int kMode, bool kPeers, bool kGrouped>
+__device__ __forceinline__ void lm_persistent_body(const GatherConfig &G0, const LmParams &P, const float4 *__restrict__ keypoints,
+                                                   const int *__restrict__ d_num_keypoints, IcpState *st, LmState *lm_g,
+                                                   ResidualBlock *__restrict__ blocks, int *__restrict__ sel_idx,
+                                                   unsigned char *__restrict__ classes, unsigned long long *stats,
+                                                   const DistanceStrategy *__restrict__ D, double *__restrict__ partials,
+                                                   PeerLinks links, int cta, int group_ctas, unsigned int *bar) {
     namespace cg = cooperative_groups;
     cg::grid_group grid = cg::this_grid();
+    unsigned int barriers = 0;   // grouped: barriers taken so far
+    const auto sync = [&]() -> bool {
+        if constexpr (kGrouped) {
+            return lm_group_barrier(bar, ++barriers * (unsigned int) group_ctas);
+        } else {
+            grid.sync();
+            return true;
+        }
+    };
+    bool live = true;   // grouped: false once the group has been aborted
     LmPShared &sh = *reinterpret_cast<LmPShared *>(lm_smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-    const bool solver = blockIdx.x == 0;
-    const int workers = (int) gridDim.x - 1, wi = (int) blockIdx.x - 1;
+    const bool solver = cta == 0;
+    const int workers = group_ctas - 1, wi = cta - 1;
     const int *stencil = kMode == 1 ? nullptr : stencil_table_fill(sh.stencil, G0.r);
     LmState *lm = &sh.solver.lm;   // the solver CTA's working copy (shared memory); lm_g is what the workers see
     unsigned int peer_seq = 0;
@@ -1119,14 +1181,14 @@ k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoint
         lm_publish(lm_g, lm, tid);
         __threadfence();
     }
-    grid.sync();
+    live = sync();
     const int K = *d_num_keypoints;
     CT_STAMP(long long t_mark = clock64(); const long long t_loop = t_mark;)
     CT_STAMP(if (solver && tid < 8) lm->dbg_cycles[tid] = 0;)
 #define LM_STAMP(slot) CT_STAMP(if (solver && tid == 0) { const long long now = clock64(); lm->dbg_cycles[slot] += (unsigned long long) (now - t_mark); t_mark = now; })
 
-    for (int it = 0; it < P.num_iters_icp; ++it) {
-        if (__ldcg(&st->done)) break;   // uniform: written before a grid barrier
+    for (int it = 0; live && it < P.num_iters_icp; ++it) {
+        if (__ldcg(&st->done)) break;   // uniform (over the group): written before a barrier
         // ---- residual assembly (workers)
         if (!solver) {
             // (every warp of this CTA left the previous assembly before the grid barriers in between)
@@ -1139,7 +1201,10 @@ k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoint
             else
                 lm_gather_tiles<false>(G0, P, stencil, keypoints, K, st, blocks, stats, D, sh.tile[w], wi, workers, kLmPWarps, &sh.next, lane);
         }
-        grid.sync();
+        if (!sync()) {
+            live = false;
+            break;
+        }
         LM_STAMP(1)
         // ---- GetProblem (solver): the first max_num_residuals valid blocks in keypoint order, seeds the minimizer
         if (solver) {
@@ -1161,7 +1226,10 @@ k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoint
             __threadfence();
         }
         LM_STAMP(2)
-        grid.sync();
+        if (!sync()) {
+            live = false;
+            break;
+        }
         LM_STAMP(6)
         // ---- ceres::Solve: evaluation 0 at x, then one evaluation per candidate
         for (int ev = 0; ev <= P.ls_max_num_iters; ++ev) {
@@ -1172,7 +1240,10 @@ k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoint
                 lm_eval_device<kLmPWarps * 2>(P, phase, blocks, sel_idx, st, lm_g, sh.eval.u, sh.eval.acc,
                                               hw * workers + wi, workers * kLmPWarps * 2, partials + (size_t) wi * kAcc);
             }
-            grid.sync();
+            if (!sync()) {
+                live = false;
+                break;
+            }
             LM_STAMP(3)
             CT_STAMP(if (solver && tid == 0) lm->dbg_cycles[7] += 1;)
             if (solver) {
@@ -1235,20 +1306,58 @@ k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoint
                 __threadfence();
             }
             LM_STAMP(5)
-            grid.sync();
+            if (!sync()) {
+                live = false;
+                break;
+            }
             LM_STAMP(6)
         }
+        if (!live) break;
     }
     CT_STAMP(if (solver && tid == 0) lm->dbg_cycles[0] = (unsigned long long) (clock64() - t_loop);)
 #undef LM_STAMP
     if (solver) {
         if (kPeers && tid == 0) *links.seq = peer_seq;
+        if (kGrouped && !live && tid == 0) {   // a CTA of the group never arrived: the problem fails, the others go on
+            st->failed = 2;
+            st->done = 1;
+        }
         // the whole state (incl. the debug trace) for the host
         __syncthreads();
         const int words = (int) (sizeof(LmState) / sizeof(int));
         const int *src = reinterpret_cast<const int *>(lm);
         int *dst = reinterpret_cast<int *>(lm_g);
         for (int i = tid; i < words; i += blockDim.x) dst[i] = src[i];
+    }
+}
+
+// kGrouped: one launch runs the groups of `groups` (EnqueueCeresBatch); otherwise the grid is one registration and
+// `groups` is not read.
+template <int kMode, bool kPeers, bool kGrouped = false>
+__global__ void __launch_bounds__(kLmPWarps * 32, 1)
+k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoints, const int *__restrict__ d_num_keypoints,
+                IcpState *st, LmState *lm_g, ResidualBlock *__restrict__ blocks, int *__restrict__ sel_idx,
+                unsigned char *__restrict__ classes, unsigned long long *stats, const DistanceStrategy *__restrict__ D,
+                double *__restrict__ partials, PeerLinks links, LmGroups groups) {
+    if constexpr (kGrouped) {
+        static_assert(!kPeers, "a batched launch is not sharded");
+        const int *first_cta = groups.table;
+        const int B = groups.num_groups;
+        int g = 0;
+        while (first_cta[g + 1] <= (int) blockIdx.x) ++g;
+        const int kp_base = first_cta[B + 1 + g];
+        const size_t block_base = (size_t) P.ncn * kp_base;
+        LmParams Pg = P;
+        if (Pg.kp_lo) Pg.kp_lo += kp_base;
+        lm_persistent_body<kMode, false, true>(
+            G0, Pg, keypoints + kp_base, first_cta + 2 * B + 1 + g, st + g,
+            reinterpret_cast<LmState *>(reinterpret_cast<char *>(lm_g) + kLmStateStride * g), blocks + block_base,
+            sel_idx + block_base, classes + block_base, stats + (size_t) kLmStatsStride * g, D,
+            partials + (size_t) (first_cta[g] - g) * kAcc, links, (int) blockIdx.x - first_cta[g],
+            first_cta[g + 1] - first_cta[g], groups.barrier + (size_t) kLmBarrierWords * g);
+    } else {
+        lm_persistent_body<kMode, kPeers, false>(G0, P, keypoints, d_num_keypoints, st, lm_g, blocks, sel_idx, classes, stats,
+                                                 D, partials, links, (int) blockIdx.x, (int) gridDim.x, nullptr);
     }
 }
 
@@ -1286,11 +1395,101 @@ void IcpSolver::FreeLmBuffers() {
     cudaFree(d_lm_sel_);
     cudaFree(d_lm_classes_);
     cudaFree(d_lm_strategy_);
+    cudaFree(d_lm_groups_);
 }
 
-void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
-                             const float4 *d_keypoints, const int *d_num_keypoints, size_t k_hint, size_t k_capacity,
-                             IcpState *d_state, int shard_rank, int shard_world, void *nccl_comm) {
+// k_lm_persistent<mode, peers, grouped>; mode 0 = CERES nearest neighbor, 1 = CERES distance-based, 2 = ROBUST
+static void *LmPersistentKernel(int mode, bool peers, bool grouped) {
+    if (grouped) return mode == 0 ? (void *) k_lm_persistent<0, false, true>
+                      : mode == 1 ? (void *) k_lm_persistent<1, false, true>
+                                  : (void *) k_lm_persistent<2, false, true>;
+    switch (mode * 2 + (peers ? 1 : 0)) {
+        case 0: return (void *) k_lm_persistent<0, false>;
+        case 1: return (void *) k_lm_persistent<0, true>;
+        case 2: return (void *) k_lm_persistent<1, false>;
+        case 3: return (void *) k_lm_persistent<1, true>;
+        case 4: return (void *) k_lm_persistent<2, false>;
+        default: return (void *) k_lm_persistent<2, true>;
+    }
+}
+int IcpSolver::LmCoresident(int variant, void *kernel) {
+    int &coresident = lm_coresident_[variant];
+    if (coresident == 0) {
+        CT_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(LmPShared)));
+        int per_sm = 0;
+        CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kLmPWarps * 32, sizeof(LmPShared)));
+        coresident = std::max(1, per_sm * num_sms_);
+    }
+    return coresident;
+}
+
+// the DistanceBasedStrategy's parameters and every map level → d_lm_strategy_ when solver CERES uses that strategy
+// (ct_icp.cpp:571; ROBUST does not consult the strategy, :1235). Options checked by CheckCeresOptions. Returns whether it does.
+bool IcpSolver::UploadLmStrategy(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy) {
+    if (opt.solver == CTICP_SOLVER_ROBUST || strategy.type != CTICP_STRATEGY_DISTANCE_BASED) return false;
+    DistanceStrategy D{};
+    D.num_levels = map.NumLevels();
+    D.filter = map.Options().select_valid_normals_direction ? 1 : 0;
+    D.radius_min = strategy.radius_min;
+    D.radius_max = strategy.radius_max;
+    D.exponent = strategy.exponent;
+    for (int i = 0; i < D.num_levels; ++i) D.levels[i] = map.Level(i);
+    if (!d_lm_strategy_) CT_CUDA_CHECK(cudaMalloc(&d_lm_strategy_, sizeof(DistanceStrategy)));
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_lm_strategy_, &D, sizeof(D), cudaMemcpyHostToDevice, stream_));
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));   // D lives on this stack frame
+    return true;
+}
+
+// the parameters of the LM kernels for checked options (CheckCeresOptions)
+static LmParams MakeLmParams(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
+                             const float4 *kp_lo, int shard_rank, int shard_world) {
+    const bool robust = opt.solver == CTICP_SOLVER_ROBUST;
+    const double sum = std::abs(opt.weight_alpha) + std::abs(opt.weight_neighborhood);
+    LmParams P{};
+    P.ncn = robust ? 1 : opt.num_closest_neighbors;
+    map.SearchParams(map.Options().default_radius, &P.level, &P.r);
+    P.radius = map.Options().default_radius;
+    P.bucket_scale = (double) kSelBuckets / (P.radius * P.radius);
+    P.kp_lo = kp_lo;
+    // neighbor count: the strategy's for CERES (neighborhood_strategy.h:81), the ICP options' for ROBUST (:1235)
+    P.kmax = robust ? opt.max_number_neighbors : strategy.max_num_neighbors;
+    P.kmin = opt.min_number_neighbors;            // ct_icp.cpp:574
+    P.lambda_weight = std::abs(opt.weight_alpha) / sum;
+    P.lambda_neighborhood = std::abs(opt.weight_neighborhood) / sum;
+    P.power_planarity = opt.power_planarity;
+    P.max_dist_to_plane = opt.max_dist_to_plane_ct_icp;
+    P.max_num_residuals = opt.max_num_residuals;
+    P.min_number_neighbors = opt.min_number_neighbors;
+    P.num_iters_icp = opt.num_iters_icp;
+    P.threshold_orientation_norm = opt.threshold_orientation_norm;
+    P.threshold_translation_norm = opt.threshold_translation_norm;
+    P.loss = make_loss(opt.loss_function, opt.ls_sigma, opt.ls_tolerant_min_threshold);
+    P.ls_max_num_iters = opt.ls_max_num_iters;
+    P.shard_rank = shard_rank;
+    P.shard_world = shard_world;
+    P.robust = robust ? 1 : 0;
+    // solver ROBUST ignores the parametrization (DoRegisterRobust is CONTINUOUS_TIME only, ct_icp.cpp:1180-1370)
+    P.simple = (!robust && opt.parametrization == CTICP_PARAM_SIMPLE) ? 1 : 0;
+    P.distortion = opt.point_to_plane_with_distortion ? 1 : 0;
+    P.use_lines = opt.use_lines;
+    P.use_barycenter = opt.use_barycenter;
+    P.threshold_linearity = opt.threshold_linearity;
+    P.threshold_planarity = opt.threshold_planarity;
+    P.outlier_distance = opt.outlier_distance;
+    P.weight_neighborhood = opt.weight_neighborhood;
+    return P;
+}
+static GatherConfig LmGatherConfig(const DeviceMap &map, const LmParams &P) {
+    GatherConfig G;
+    G.L = map.Level(P.level);
+    G.r = P.r;
+    G.radius2 = P.radius * P.radius;
+    G.kmax = P.kmax;
+    return G;
+}
+
+void IcpSolver::CheckCeresOptions(const DeviceMap &map, const cticp_icp_options &opt,
+                                  const cticp_strategy_options &strategy) const {
     const bool robust = opt.solver == CTICP_SOLVER_ROBUST;
     if (!robust && opt.distance != CTICP_DIST_POINT_TO_PLANE)
         throw UnsupportedError("solver CERES: only POINT_TO_PLANE is built (SURVEY §8)");
@@ -1305,49 +1504,30 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
     // neighbor count: the strategy's for CERES (neighborhood_strategy.h:81), the ICP options' for ROBUST (:1235)
     const int kmax = robust ? opt.max_number_neighbors : strategy.max_num_neighbors;
     if (kmax > 32 || kmax < 1) throw std::invalid_argument("max_num_neighbors must be in [1, 32]");
-    const bool sharded = nccl_comm != nullptr && shard_world > 1;
     const double sum = std::abs(opt.weight_alpha) + std::abs(opt.weight_neighborhood);
     if (!(sum > 0.0)) throw std::invalid_argument("weight_alpha + weight_neighborhood <= 0");
+    // solver CERES consults the neighborhood strategy (ct_icp.cpp:571); ROBUST does not (:1235)
+    if (!robust && strategy.type == CTICP_STRATEGY_DISTANCE_BASED) {
+        if (!(strategy.radius_max > 0.0)) throw std::invalid_argument("DISTANCE_BASED_STRATEGY: radius_max must be > 0");
+        if (map.Options().select_valid_normals_direction && !map.HasNormals())
+            throw std::invalid_argument("DISTANCE_BASED_STRATEGY with select_valid_normals_direction needs a map that keeps normals");
+    } else if (!robust && strategy.type != CTICP_STRATEGY_NEAREST_NEIGHBOR) {
+        throw std::invalid_argument("unknown neighborhood strategy type");
+    }
+}
+
+
+void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
+                             const float4 *d_keypoints, const int *d_num_keypoints, size_t k_hint, size_t k_capacity,
+                             IcpState *d_state, int shard_rank, int shard_world, void *nccl_comm) {
+    CheckCeresOptions(map, opt, strategy);
+    const bool robust = opt.solver == CTICP_SOLVER_ROBUST;
+    const int ncn = robust ? 1 : opt.num_closest_neighbors;
+    const bool sharded = nccl_comm != nullptr && shard_world > 1;
     EnsureLmBuffers(k_capacity * (size_t) ncn);
-
-    LmParams P{};
-    P.ncn = ncn;
-    map.SearchParams(map.Options().default_radius, &P.level, &P.r);
-    P.radius = map.Options().default_radius;
-    P.bucket_scale = (double) kSelBuckets / (P.radius * P.radius);
-    P.kp_lo = kp_lo_;
-    P.kmax = kmax;
-    P.kmin = opt.min_number_neighbors;            // ct_icp.cpp:574
-    P.lambda_weight = std::abs(opt.weight_alpha) / sum;
-    P.lambda_neighborhood = std::abs(opt.weight_neighborhood) / sum;
-    P.power_planarity = opt.power_planarity;
-    P.max_dist_to_plane = opt.max_dist_to_plane_ct_icp;
-    P.max_num_residuals = opt.max_num_residuals;
-    P.min_number_neighbors = opt.min_number_neighbors;
-    P.num_iters_icp = opt.num_iters_icp;
-    P.threshold_orientation_norm = opt.threshold_orientation_norm;
-    P.threshold_translation_norm = opt.threshold_translation_norm;
-    P.loss = make_loss(opt.loss_function, opt.ls_sigma, opt.ls_tolerant_min_threshold);
-    P.ls_max_num_iters = opt.ls_max_num_iters;
-    P.shard_rank = sharded ? shard_rank : 0;
-    P.shard_world = sharded ? shard_world : 1;
+    LmParams P = MakeLmParams(map, opt, strategy, kp_lo_, sharded ? shard_rank : 0, sharded ? shard_world : 1);
     if (sharded && shard_world > kAcc) throw std::invalid_argument("sharding: world size above 96");
-    P.robust = robust ? 1 : 0;
-    // solver ROBUST ignores the parametrization (DoRegisterRobust is CONTINUOUS_TIME only, ct_icp.cpp:1180-1370)
-    P.simple = (!robust && opt.parametrization == CTICP_PARAM_SIMPLE) ? 1 : 0;
-    P.distortion = opt.point_to_plane_with_distortion ? 1 : 0;
-    P.use_lines = opt.use_lines;
-    P.use_barycenter = opt.use_barycenter;
-    P.threshold_linearity = opt.threshold_linearity;
-    P.threshold_planarity = opt.threshold_planarity;
-    P.outlier_distance = opt.outlier_distance;
-    P.weight_neighborhood = opt.weight_neighborhood;
-
-    GatherConfig G;
-    G.L = map.Level(P.level);
-    G.r = P.r;
-    G.radius2 = P.radius * P.radius;
-    G.kmax = P.kmax;
+    const GatherConfig G = LmGatherConfig(map, P);
 
     auto *lm = static_cast<LmState *>(d_lm_state_);
     auto *blocks_buf = static_cast<ResidualBlock *>(d_lm_blocks_);
@@ -1357,25 +1537,7 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
     const int eval_blocks = (int) std::max<size_t>(1, std::min<size_t>((r_hint + kLmWarps * 2 - 1) / (kLmWarps * 2), (size_t) num_sms_ * 4));
     EnsurePartials(eval_blocks);
 
-    // solver CERES consults the neighborhood strategy (ct_icp.cpp:571); ROBUST does not (:1235)
-    const bool distance_based = !robust && strategy.type == CTICP_STRATEGY_DISTANCE_BASED;
-    if (distance_based) {
-        if (!(strategy.radius_max > 0.0)) throw std::invalid_argument("DISTANCE_BASED_STRATEGY: radius_max must be > 0");
-        DistanceStrategy D{};
-        D.num_levels = map.NumLevels();
-        D.filter = map.Options().select_valid_normals_direction ? 1 : 0;
-        if (D.filter && !map.HasNormals())
-            throw std::invalid_argument("DISTANCE_BASED_STRATEGY with select_valid_normals_direction needs a map that keeps normals");
-        D.radius_min = strategy.radius_min;
-        D.radius_max = strategy.radius_max;
-        D.exponent = strategy.exponent;
-        for (int i = 0; i < D.num_levels; ++i) D.levels[i] = map.Level(i);
-        if (!d_lm_strategy_) CT_CUDA_CHECK(cudaMalloc(&d_lm_strategy_, sizeof(DistanceStrategy)));
-        CT_CUDA_CHECK(cudaMemcpyAsync(d_lm_strategy_, &D, sizeof(D), cudaMemcpyHostToDevice, stream_));
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));   // D lives on this stack frame
-    } else if (!robust && strategy.type != CTICP_STRATEGY_NEAREST_NEIGHBOR) {
-        throw std::invalid_argument("unknown neighborhood strategy type");
-    }
+    const bool distance_based = UploadLmStrategy(map, opt, strategy);
     auto *classes = static_cast<unsigned char *>(d_lm_classes_);
     if (robust) CT_CUDA_CHECK(cudaMemsetAsync(classes, 0, k_capacity, stream_));   // NEIGHBORHOOD_TYPE::NONE
 
@@ -1383,22 +1545,8 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
         // one cooperative launch for the whole registration (k_lm_persistent); the grid must be co-resident
         const int mode = robust ? 2 : (distance_based ? 1 : 0);
         const bool peers = sharded;
-        void *kernel = nullptr;
-        switch (mode * 2 + (peers ? 1 : 0)) {
-            case 0: kernel = (void *) k_lm_persistent<0, false>; break;
-            case 1: kernel = (void *) k_lm_persistent<0, true>; break;
-            case 2: kernel = (void *) k_lm_persistent<1, false>; break;
-            case 3: kernel = (void *) k_lm_persistent<1, true>; break;
-            case 4: kernel = (void *) k_lm_persistent<2, false>; break;
-            default: kernel = (void *) k_lm_persistent<2, true>; break;
-        }
-        int &coresident = lm_coresident_[mode * 2 + (peers ? 1 : 0)];
-        if (coresident == 0) {
-            CT_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(LmPShared)));
-            int per_sm = 0;
-            CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kLmPWarps * 32, sizeof(LmPShared)));
-            coresident = std::max(1, per_sm * num_sms_);
-        }
+        void *kernel = LmPersistentKernel(mode, peers, false);
+        const int coresident = LmCoresident(mode * 2 + (peers ? 1 : 0), kernel);
         const size_t k_share = (k_hint + (size_t) P.shard_world - 1) / (size_t) P.shard_world + 16;
         int grid = (int) std::min<size_t>((size_t) coresident, 1 + std::max<size_t>(1, (k_share + kp_per_cta_ - 1) / kp_per_cta_));
         grid = std::max(grid, 2);
@@ -1409,7 +1557,9 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
         const DistanceStrategy *dstrat = static_cast<const DistanceStrategy *>(d_lm_strategy_);
         double *parts = d_partials_;
         PeerLinks links = peers ? PeerLinksOf(links_host_) : PeerLinks{};
-        void *args[] = {&G, &P, &kp, &nk, &d_state, &lm, &blocks_buf, &sel, &classes, &stats, &dstrat, &parts, &links};
+        LmGroups groups{};
+        GatherConfig g = G;
+        void *args[] = {&g, &P, &kp, &nk, &d_state, &lm, &blocks_buf, &sel, &classes, &stats, &dstrat, &parts, &links, &groups};
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
         if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
         CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kLmPWarps * 32), args, sizeof(LmPShared), stream_));
@@ -1467,6 +1617,62 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
     }
     CT_CUDA_CHECK(cudaGetLastError());
     DebugLmTrace(lm);
+}
+
+void IcpSolver::EnqueueCeresBatch(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
+                                  int batch, const size_t *h_n, const float4 *d_keypoints, IcpState *d_states) {
+    if (!use_persistent_) throw std::logic_error("batched CERES / ROBUST registration needs the persistent loop");
+    if (batch < 1) throw std::invalid_argument("batch must be at least 1");
+    CheckCeresOptions(map, opt, strategy);
+    const bool robust = opt.solver == CTICP_SOLVER_ROBUST;
+    const int mode = robust ? 2 : (strategy.type == CTICP_STRATEGY_DISTANCE_BASED ? 1 : 0);
+    // one problem: the solo launch (grid barriers, the table is not read), with its count taken from the table
+    const bool grouped = batch > 1;
+    void *kernel = LmPersistentKernel(mode, false, grouped);
+    const int coresident = LmCoresident(grouped ? 6 + mode : mode * 2, kernel);
+    if (2 * batch > coresident)
+        throw CapacityError("batch of " + std::to_string(batch) + " registrations: the device holds " +
+                            std::to_string(coresident) + " CTAs of the LM kernel, two per registration needed");
+    size_t total = 0;
+    for (int b = 0; b < batch; ++b) total += h_n[b];
+    LmParams P = MakeLmParams(map, opt, strategy, kp_lo_, 0, 1);
+    GatherConfig G = LmGatherConfig(map, P);
+    EnsureLmBuffers(std::max<size_t>(total, 1) * (size_t) P.ncn);
+    // per group: its LmState (kLmStateStride), its stats line and its barrier words, each area after the B of the one before
+    constexpr size_t kGroupBytes = kLmStateStride + sizeof(unsigned long long) * kLmStatsStride + sizeof(unsigned int) * kLmBarrierWords;
+    if (batch > lm_groups_cap_) {
+        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+        cudaFree(d_lm_groups_);
+        d_lm_groups_ = nullptr;
+        CT_CUDA_CHECK(cudaMalloc(&d_lm_groups_, kGroupBytes * (size_t) batch));
+        lm_groups_cap_ = batch;
+    }
+    char *area = static_cast<char *>(d_lm_groups_);
+    auto *lm = reinterpret_cast<LmState *>(area);
+    auto *stats = reinterpret_cast<unsigned long long *>(area + kLmStateStride * batch);
+    auto *barrier = reinterpret_cast<unsigned int *>(area + (kLmStateStride + sizeof(unsigned long long) * kLmStatsStride) * batch);
+    UploadLmStrategy(map, opt, strategy);
+    auto *classes = static_cast<unsigned char *>(d_lm_classes_);
+    if (robust) CT_CUDA_CHECK(cudaMemsetAsync(classes, 0, total, stream_));   // NEIGHBORHOOD_TYPE::NONE
+    const int grid = UploadGroupTable(h_n, batch, coresident);
+    EnsurePartials(grid - batch);
+    CT_CUDA_CHECK(cudaMemsetAsync(barrier, 0, sizeof(unsigned int) * kLmBarrierWords * batch, stream_));
+
+    const float4 *kp = d_keypoints;
+    const int *nk = d_groups_ + 2 * batch + 1;   // count[0] (read by the solo launch only)
+    auto *blocks_buf = static_cast<ResidualBlock *>(d_lm_blocks_);
+    int *sel = d_lm_sel_;
+    const DistanceStrategy *dstrat = static_cast<const DistanceStrategy *>(d_lm_strategy_);
+    double *parts = d_partials_;
+    PeerLinks links{};
+    LmGroups groups = grouped ? LmGroups{d_groups_, batch, barrier} : LmGroups{};
+    void *args[] = {&G, &P, &kp, &nk, &d_states, &lm, &blocks_buf, &sel, &classes, &stats, &dstrat, &parts, &links, &groups};
+    const bool timed = time_gather_ && ev_used_ < kMaxEvents;
+    if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
+    CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kLmPWarps * 32), args, sizeof(LmPShared), stream_));
+    if (timed) cudaEventRecord(ev_end_[ev_used_++], stream_);
+    gather_launches_ += 1;
+    launches_ += 1;
 }
 
 void IcpSolver::DebugLmTrace(void *d_lm) {

@@ -526,6 +526,24 @@ int cticp_icp_register_batch(cticp_map *m, const cticp_icp_options *options, siz
                              const cticp_motion_model_options *motion_options,
                              cticp_icp_summary *out_summaries);
 
+/* cticp_icp_register_batch for every solver, with the neighborhood strategy that solver CERES consults (nullable: the
+ * default of cticp_icp_register; GN and ROBUST ignore it, as cticp_icp_register does). GN runs the batch above; CERES and
+ * ROBUST run the B problems in one launch of the persistent Levenberg-Marquardt kernel, each on its own group of CTAs
+ * separated by barriers of that group alone, so problems that stop after different numbers of iterations or evaluations
+ * share the launch. Per-problem semantics, the bit-identity contract, the argument checks and the error codes are those
+ * of cticp_icp_register_batch; in addition the option checks of cticp_icp_register for CERES / ROBUST run once, before
+ * anything is uploaded (CTICP_ERR_UNSUPPORTED: CERES with a distance other than POINT_TO_PLANE, num_closest_neighbors
+ * outside [1, min(4, max(min_number_neighbors, 5))], ROBUST with min_number_neighbors < 5, or an engine without the
+ * persistent loop (CTICP_PERSISTENT=0); CTICP_ERR_INVALID_ARGUMENT: neighbor count outside [1, 32], a DISTANCE_BASED
+ * strategy with radius_max <= 0 or with a normal filter on a map without normals). A problem whose group of CTAs does
+ * not meet at a barrier within ~2 s fails alone: CTICP_ERR_INTERNAL after every output is written. */
+int cticp_icp_register_batch_ex(cticp_map *m, const cticp_icp_options *options,
+                                const cticp_strategy_options *strategy,
+                                size_t batch, cticp_wpoint *const *keypoints, const size_t *n, cticp_frame *frames,
+                                const cticp_frame *const *previous_frames,
+                                const cticp_motion_model_options *motion_options,
+                                cticp_icp_summary *out_summaries);
+
 /* Debug tap for parity tests: normal equations of ONE Gauss-Newton linearisation at `frame`
  * (A 12×12 row-major AFTER the 1/n normalisation and regularisers of ct_icp.cpp:877-910, b 12, n used). */
 int cticp_icp_gn_normal_equations(cticp_map *m, const cticp_icp_options *options,

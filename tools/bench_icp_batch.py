@@ -1,13 +1,16 @@
-"""B solo cticp_icp_register calls against one cticp_icp_register_batch call (solver GN), on one map.
+"""B solo cticp_icp_register calls against one batched call (cticp_icp_register_batch for solver GN,
+cticp_icp_register_batch_ex for CERES and ROBUST), on one map.
 
 The map is built from the HDL-64 synthetic sequence (frames 0..2 registered by the CPU oracle, as the GPU parity tests
 do); the B problems are frame 3's keypoints (1.0 m grid, or its first --small keypoints) at B initial poses perturbed by
 a few centimetres. Reported per (B, K):
   - host-timed end to end, per problem: median over --repeats of B solo calls / one batch call (each synchronising)
-  - device time of the k_gn_persistent launches (torch.profiler, separate run): Σ over the B solo launches / the batch
+  - device time of the persistent launches (torch.profiler, separate run): k_gn_persistent for GN, k_lm_persistent for
+    CERES / ROBUST; Σ over the B solo launches / the batch
 The card name and power limit come from a read-only nvidia-smi query in the same run.
 
-usage: python tools/bench_icp_batch.py [--batches 1,2,4,8,16,32] [--small 500] [--repeats 20] [--warmup 3]
+usage: python tools/bench_icp_batch.py [--solver GN|CERES|ROBUST] [--batches 1,2,4,8,16,32] [--small 500]
+                                       [--repeats 20] [--warmup 3]
 """
 import argparse
 import json
@@ -76,6 +79,7 @@ def main():
     ap.add_argument("--small", type=int, default=500, help="keypoints of the small problems (a truncated set)")
     ap.add_argument("--repeats", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--solver", default="GN", choices=sorted(abi.SOLVER))
     args = ap.parse_args()
     batches = [int(b) for b in args.batches.split(",")]
 
@@ -90,11 +94,26 @@ def main():
     m = eng.voxel_map(mopt)
     m.insert(map_xyz)
     io = eng.default_icp_options()
-    io.solver = abi.SOLVER["GN"]
+    io.solver = abi.SOLVER[args.solver]
     io.min_number_neighbors = 10
     io.num_iters_icp = 8
+    if args.solver == "CERES":   # the reference's default options otherwise: nearest-neighbor strategy
+        io.loss_function = abi.LOSS["CAUCHY"]
+        io.num_iters_icp = 4
+    elif args.solver == "ROBUST":
+        io.num_iters_icp = 4
+        io.max_num_residuals = 1000
+        io.weight_alpha, io.weight_neighborhood = 0.9, 0.1
+        io.min_number_neighbors, io.max_number_neighbors = 8, 20
+        io.loss_function = abi.LOSS["CAUCHY"]
+        io.ls_max_num_iters, io.ls_sigma = 8, 0.1
+        io.max_dist_to_plane_ct_icp, io.outlier_distance = 0.5, 0.8
+        io.threshold_linearity, io.threshold_planarity = 0.9, 0.8
+    kernel = "k_gn_persistent" if args.solver == "GN" else "k_lm_persistent"
     mm = eng.default_odometry_options().default_motion_model
     info = {"card": card(), "map_points": int(m.num_points())}
+    if args.solver != "GN":
+        info["solver"] = args.solver
     print(json.dumps(info), flush=True)
 
     def solo_all(kps, frames):
@@ -102,7 +121,10 @@ def main():
             m.icp_register(io, k, f, prev, mm)
 
     def batch_all(kps, frames):
-        m.icp_register_batch(io, kps, frames, [prev] * len(kps), mm)
+        if args.solver == "GN":
+            m.icp_register_batch(io, kps, frames, [prev] * len(kps), mm)
+        else:
+            m.icp_register_batch_ex(io, kps, frames, [prev] * len(kps), mm)
 
     def host_ms(fn, kps, frames):
         for _ in range(args.warmup):
@@ -121,7 +143,7 @@ def main():
             for _ in range(10):
                 fn([k.copy() for k in kps], [f.copy() for f in frames])
             torch.cuda.synchronize()
-        us = [e.device_time_total for e in prof.events() if "k_gn_persistent" in e.name]
+        us = [e.device_time_total for e in prof.events() if kernel in e.name]
         return sum(us) / 10 / 1e3, len(us) // 10
 
     rows = []
