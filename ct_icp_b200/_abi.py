@@ -131,6 +131,11 @@ class CloudSink(_Struct):
                 ("t_dtype", C.c_int32), ("world", C.c_int32)]
 
 
+class DeviceScan(_Struct):   # cticp_device_scan: a scan in device memory (cticp_odometry_register_device)
+    _fields_ = [("xyz", C.c_void_p), ("xyz_stride_bytes", C.c_uint64), ("t", C.c_void_p), ("t_stride_bytes", C.c_uint64),
+                ("num_points", C.c_uint64), ("xyz_dtype", C.c_int32), ("t_dtype", C.c_int32)]
+
+
 class OdometryOptions(_Struct):
     _fields_ = [
         ("ct_icp_options", IcpOptions), ("map_options", MapOptions),

@@ -17,6 +17,19 @@ class CticpError(RuntimeError):
         self.code = code
 
 
+def _is_cuda_tensor(a):
+    """A torch CUDA tensor, recognised without importing torch."""
+    return type(a).__module__.split(".")[0] == "torch" and bool(getattr(a, "is_cuda", False))
+
+
+def _torch_dtype_codes(torch):
+    codes = {torch.int8: 1, torch.uint8: 2, torch.int16: 3, torch.int32: 5, torch.float32: 7, torch.float64: 8}
+    for name, code in (("uint16", 4), ("uint32", 6)):
+        if hasattr(torch, name):
+            codes[getattr(torch, name)] = code
+    return codes
+
+
 def _as_f64_rows(a, cols):
     a = np.ascontiguousarray(a, dtype=np.float64)
     if a.ndim != 2 or a.shape[1] != cols:
@@ -90,6 +103,9 @@ class Binding:
             "odometry_register_cloud": (C.c_int, [vp, P(abi.CloudView), u32, P(abi.Frame), P(abi.Summary)]),
             "odometry_stage_cloud": (i64, [vp, P(abi.CloudView)]),
             "odometry_write_points": (i64, [vp, C.c_int, P(abi.CloudSink)]),
+            "odometry_register_device": (C.c_int, [vp, P(abi.DeviceScan), vp, u32, P(abi.Frame), P(abi.MotionPrior),
+                                                   P(abi.Summary)]),
+            "odometry_write_points_device": (i64, [vp, C.c_int, P(abi.CloudSink), vp]),
             "odometry_register_staged": (C.c_int, [vp, i64, u32, P(abi.Summary)]),
             "odometry_clear_staged": (C.c_int, [vp]),
             "odometry_timer_start": (C.c_int, [vp]),
@@ -343,6 +359,7 @@ class Odometry:
     def __init__(self, binding, options, device=0):
         self.b = binding
         self.options = options.copy()
+        self.device = device
         self.h = C.c_void_p()
         binding.check(binding.fn("odometry_create")(C.byref(self.options), device, C.byref(self.h)))
 
@@ -373,7 +390,10 @@ class Odometry:
         return summary
 
     def RegisterFrame(self, xyz, timestamps, frame_id, motion_model=None):
-        """motion_model: an abi.MotionPrior — the AMotionModel* of the reference's overloads (odometry.h:231-248)"""
+        """motion_model: an abi.MotionPrior — the AMotionModel* of the reference's overloads (odometry.h:231-248).
+        xyz / timestamps: numpy arrays, or torch CUDA tensors on the handle's device (read in place, see _register_tensors)"""
+        if _is_cuda_tensor(xyz) or _is_cuda_tensor(timestamps):
+            return self._register_tensors(xyz, timestamps, frame_id, None, motion_model)
         if motion_model is not None:
             return self._register_ex(xyz, timestamps, frame_id, None, motion_model)
         return self._register(xyz, timestamps, frame_id, None)
@@ -398,8 +418,68 @@ class Odometry:
         self.options = options.copy()
         self.b.check(self.b.fn("odometry_reset_options")(self.h, C.byref(self.options)))
 
-    def RegisterFrameWithEstimate(self, xyz, timestamps, initial_estimate, frame_id):
+    def RegisterFrameWithEstimate(self, xyz, timestamps, initial_estimate, frame_id, motion_model=None):
+        if _is_cuda_tensor(xyz) or _is_cuda_tensor(timestamps):
+            return self._register_tensors(xyz, timestamps, frame_id, initial_estimate, motion_model)
+        if motion_model is not None:
+            return self._register_ex(xyz, timestamps, frame_id, initial_estimate, motion_model)
         return self._register(xyz, timestamps, frame_id, initial_estimate)
+
+    # ---- device memory in and out (engine only) ----------------------------------------------------------------
+    def _register_tensors(self, xyz, timestamps, frame_id, initial_estimate, motion_model):
+        """xyz: (N, >=3) float32 / float64 CUDA tensor with unit column stride (an (N, 4) xyzi tensor is read in place);
+        timestamps: 1-D CUDA tensor of any supported dtype and stride. Both on the handle's device; the scan is read after
+        the work already queued on torch's current stream of that device."""
+        import torch
+        if not (_is_cuda_tensor(xyz) and _is_cuda_tensor(timestamps)):
+            raise ValueError("xyz and timestamps must both be CUDA tensors (or both host arrays)")
+        if xyz.device.index != self.device or timestamps.device.index != self.device:
+            raise ValueError("xyz and timestamps must be on cuda:%d, the handle's device" % self.device)
+        if xyz.dim() != 2 or xyz.shape[1] < 3 or xyz.stride(1) != 1 or xyz.dtype not in (torch.float32, torch.float64):
+            raise ValueError("xyz must be an (N, >=3) float32 / float64 tensor with unit column stride")
+        codes = _torch_dtype_codes(torch)
+        if timestamps.dim() != 1 or timestamps.dtype not in codes:
+            raise ValueError("timestamps must be a 1-D tensor of a supported dtype")
+        if xyz.shape[0] != timestamps.shape[0]:
+            raise ValueError("xyz and timestamps must have the same length")
+        scan = abi.DeviceScan(xyz.data_ptr(), xyz.stride(0) * xyz.element_size(), timestamps.data_ptr(),
+                              timestamps.stride(0) * timestamps.element_size(), xyz.shape[0], codes[xyz.dtype],
+                              codes[timestamps.dtype])
+        return self.register_device(scan, frame_id, initial_estimate, motion_model,
+                                    stream=torch.cuda.current_stream(self.device).cuda_stream)
+
+    def register_device(self, scan, frame_id, initial_estimate=None, motion_model=None, stream=0):
+        """cticp_odometry_register_device on an abi.DeviceScan (any record layout); stream: the producer's cudaStream_t."""
+        summary = abi.Summary()
+        self.b.check(self.b.fn("odometry_register_device")(
+            self.h, C.byref(scan), C.c_void_p(stream or None), frame_id,
+            C.byref(initial_estimate) if initial_estimate is not None else None,
+            C.byref(motion_model) if motion_model is not None else None, C.byref(summary)))
+        return summary
+
+    def write_points_device(self, which, sink, stream=0):
+        """cticp_odometry_write_points_device on an abi.CloudSink in device memory; returns the count."""
+        return self.b.check(self.b.fn("odometry_write_points_device")(self.h, which, C.byref(sink),
+                                                                      C.c_void_p(stream or None)))
+
+    def points_device(self, which, world=True, dtype=None, with_timestamps=False):
+        """One of the summary's point vectors as an (n, 3) — (n, 4) with the timestamps — CUDA tensor of `dtype`
+        (float64 by default, or float32) on the handle's device, written in order with torch's current stream."""
+        import torch
+        dtype = torch.float64 if dtype is None else dtype
+        if dtype not in (torch.float32, torch.float64):
+            raise ValueError("dtype must be torch.float32 or torch.float64")
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        n = self.write_points_device(which, abi.CloudSink(None, 0, 0, 0, 0, 0, 0, 0), stream)
+        cols = 4 if with_timestamps else 3
+        out = torch.empty((n, cols), dtype=dtype, device=torch.device("cuda", self.device))
+        if n:
+            code = abi.DTYPE["float32" if dtype == torch.float32 else "float64"]
+            size = out.element_size()
+            sink = abi.CloudSink(out.data_ptr(), n, cols * size, 0, code, 3 * size, code if with_timestamps else 0,
+                                 1 if world else 0)
+            self.write_points_device(which, sink, stream)
+        return out
 
     # ---- record buffers (sensor_msgs/PointCloud2-like), zero-copy in and out (engine only) -------------------
     @staticmethod

@@ -91,6 +91,7 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_summary") return sizeof(cticp_summary);
     if (s == "cticp_device_timing") return sizeof(cticp_device_timing);
     if (s == "cticp_adaptive_options") return sizeof(cticp_adaptive_options);
+    if (s == "cticp_device_scan") return sizeof(cticp_device_scan);
     return 0;
 }
 
@@ -398,6 +399,28 @@ int64_t cticp_odometry_write_points(cticp_odometry *h, int which, const cticp_cl
     int rc = Guard([&] {
         if (!sink) throw std::invalid_argument("null sink");
         count = h->engine->WritePoints(which, *sink);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int cticp_odometry_register_device(cticp_odometry *h, const cticp_device_scan *scan, void *stream, uint32_t frame_id,
+                                   const cticp_frame *initial_estimate, const cticp_motion_prior *motion_model,
+                                   cticp_summary *out_summary) {
+    return Guard([&] {
+        if (!h || !scan) throw std::invalid_argument("null argument");
+        cticp::ScanView v;
+        v.xyz = scan->xyz; v.xyz_stride = scan->xyz_stride_bytes; v.xyz_dtype = scan->xyz_dtype;
+        v.t = scan->t; v.t_stride = scan->t_stride_bytes; v.t_dtype = scan->t_dtype;
+        v.n = (size_t) scan->num_points;
+        h->engine->RegisterDevice(v, static_cast<cudaStream_t>(stream), frame_id, initial_estimate, out_summary, motion_model);
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_odometry_write_points_device(cticp_odometry *h, int which, const cticp_cloud_sink *sink, void *stream) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!h || !sink) throw std::invalid_argument("null argument");
+        count = h->engine->WritePointsDevice(which, *sink, static_cast<cudaStream_t>(stream));
         return (int) CTICP_OK;
     });
     return rc < 0 ? rc : count;

@@ -1,5 +1,6 @@
 // engine.cu — host orchestration of the H100-native odometry (see engine.h).
 #include "engine.h"
+#include "scan_pack.cuh"
 
 #include <algorithm>
 #include <atomic>
@@ -12,6 +13,7 @@
 #include <emmintrin.h>
 #include <xmmintrin.h>
 
+#include <cudaTypedefs.h>   // PFN_cuMemGetAddressRange (types only: the driver is reached through cudart)
 #include <nvtx3/nvToolsExt.h>   // header-only: ranges are no-ops unless a profiler injects the NVTX library
 
 namespace cticp {
@@ -151,6 +153,8 @@ Engine::Engine(const cticp_odometry_options &options, int device) : options_(opt
     CT_CUDA_CHECK(cudaMalloc(&d_kp_world_, sizeof(double) * 3 * max_pts));
     for (auto &e : ev_) CT_CUDA_CHECK(cudaEventCreate(&e));
     for (auto &e : timer_ev_) CT_CUDA_CHECK(cudaEventCreate(&e));
+    CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_producer_, cudaEventDisableTiming));
+    CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_device_egress_, cudaEventDisableTiming));
     CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
 }
 
@@ -170,6 +174,8 @@ Engine::~Engine() {
     cudaFree(d_kp_world_);
     for (auto &e : ev_) cudaEventDestroy(e);
     for (auto &e : timer_ev_) cudaEventDestroy(e);
+    if (ev_producer_) cudaEventDestroy(ev_producer_);
+    if (ev_device_egress_) cudaEventDestroy(ev_device_egress_);
     for (auto &sc : staged_) { cudaFree(sc.d_points); cudaFree(sc.d_lo); }
     cudaFree(d_flush_);
     for (int i = 0; i < 3; ++i) {
@@ -507,9 +513,7 @@ template <typename F> void DispatchScanTypes(const ScanView &v, F &&fn) {
     }
 }
 template <typename T> inline T LoadUnaligned(const char *p) {   // PointCloud2 records are packed: no alignment promise
-    T v;
-    memcpy(&v, p, sizeof(T));
-    return v;
+    return scan_pack::load_unaligned<T>(p);
 }
 }  // namespace
 
@@ -519,13 +523,11 @@ namespace {
 // speed); for float64 sources also the residual plane lo = value - hi, and whether any coordinate needs it
 template <typename XT>
 inline void PackPoint(XT x, XT y, XT z, double a, float4 *dst, bool *any_lo) {
-    const float fx = (float) x, fy = (float) y, fz = (float) z, fa = (float) a;
-    _mm_stream_ps(reinterpret_cast<float *>(dst), _mm_set_ps(fa, fz, fy, fx));
-    if constexpr (std::is_same<XT, double>::value) {
-        // does any coordinate need the residual plane? (float64 arrays usually hold float32 values: then nothing more is
-        // computed, stored or uploaded; otherwise PackLoPlane makes a second pass)
-        if ((double) fx != x || (double) fy != y || (double) fz != z) *any_lo = true;
-    }
+    using namespace scan_pack;
+    _mm_stream_ps(reinterpret_cast<float *>(dst), _mm_set_ps(hi_of(a), hi_of(z), hi_of(y), hi_of(x)));
+    // does any coordinate need the residual plane? (float64 arrays usually hold float32 values: then nothing more is
+    // computed, stored or uploaded; otherwise PackLoPlane makes a second pass)
+    if (needs_lo(x) || needs_lo(y) || needs_lo(z)) *any_lo = true;
 }
 // The common layout — contiguous float64 x, y, z and contiguous float64 timestamps (numpy's default) — has an AVX2 packer
 // (host_pack.cpp: a plain C++ translation unit, nvcc's front end does not see the AVX intrinsics)
@@ -539,9 +541,7 @@ inline bool F64FastPath(const ScanView &scan) {
 // The residual plane of a float64 scan (value - (double)(float)value per component, alpha included): second pass, only for
 // scans that need it.
 void Engine::PackLoPlane(const ScanView &scan, double bts, double ets, float4 *dst_lo) {
-    const double mn = std::min(bts, ets), mx = std::max(bts, ets);
-    const bool spans = mx > mn;
-    const double inv = spans ? 1.0 / (mx - mn) : 0.0;
+    const scan_pack::AlphaRange ar = scan_pack::alpha_range(bts, ets);
     const char *px = static_cast<const char *>(scan.xyz), *pt = static_cast<const char *>(scan.t);
     const size_t xs = scan.xyz_stride, ts = scan.t_stride;
     DispatchScanTypes(scan, [&](auto xt, auto tt) {
@@ -552,11 +552,9 @@ void Engine::PackLoPlane(const ScanView &scan, double bts, double ets, float4 *d
                 const char *p = px + i * xs;
                 const double x = (double) LoadUnaligned<XT>(p), y = (double) LoadUnaligned<XT>(p + sizeof(XT)),
                              z = (double) LoadUnaligned<XT>(p + 2 * sizeof(XT));
-                const double ti = (double) LoadUnaligned<TT>(pt + i * ts);
-                const double a = spans ? (ti - mn) * inv : 1.0;
-                _mm_stream_ps(reinterpret_cast<float *>(dst_lo + i),
-                              _mm_set_ps((float) (a - (double) (float) a), (float) (z - (double) (float) z),
-                                         (float) (y - (double) (float) y), (float) (x - (double) (float) x)));
+                const double a = scan_pack::alpha_of((double) LoadUnaligned<TT>(pt + i * ts), ar);
+                using scan_pack::lo_of;
+                _mm_stream_ps(reinterpret_cast<float *>(dst_lo + i), _mm_set_ps(lo_of(a), lo_of(z), lo_of(y), lo_of(x)));
             }
             _mm_sfence();
         });
@@ -566,11 +564,11 @@ void Engine::PackLoPlane(const ScanView &scan, double bts, double ets, float4 *d
 // returns whether the scan needs its residual plane (float64 coordinates that are not float32-representable)
 bool Engine::PackScan(const ScanView &scan, double bts, double ets, float4 *dst) {
     std::atomic<bool> needs_lo{false};
-    const double mn = std::min(bts, ets), mx = std::max(bts, ets);
-    const double inv = (mx > mn) ? 1.0 / (mx - mn) : 0.0;
+    const scan_pack::AlphaRange ar = scan_pack::alpha_range(bts, ets);
+    const double mn = ar.mn, inv = ar.inv;
     const char *px = static_cast<const char *>(scan.xyz), *pt = static_cast<const char *>(scan.t);
     const size_t xs = scan.xyz_stride, ts = scan.t_stride;
-    const bool spans = mx > mn;
+    const bool spans = ar.spans;
     const bool fast = F64FastPath(scan);
     DispatchScanTypes(scan, [&](auto xt, auto tt) {
         using XT = typename decltype(xt)::type;
@@ -586,8 +584,7 @@ bool Engine::PackScan(const ScanView &scan, double bts, double ets, float4 *dst)
             for (size_t i = b; i < e && !fast; ++i) {
                 const char *p = px + i * xs;
                 const XT x = LoadUnaligned<XT>(p), y = LoadUnaligned<XT>(p + sizeof(XT)), z = LoadUnaligned<XT>(p + 2 * sizeof(XT));
-                const double ti = (double) LoadUnaligned<TT>(pt + i * ts);
-                const double a = spans ? (ti - mn) * inv : 1.0;
+                const double a = scan_pack::alpha_of((double) LoadUnaligned<TT>(pt + i * ts), ar);
                 PackPoint<XT>(x, y, z, a, dst + i, &any);
             }
             _mm_sfence();
@@ -641,8 +638,8 @@ void Engine::PackAndUpload(const ScanView &scan, const double *pose_timestamps, 
                 double mn = INFINITY, mx = -INFINITY;
                 for (size_t i = b; i < e; ++i) {
                     const double ti = (double) LoadUnaligned<TT>(pt + i * ts);
-                    mn = ti < mn ? ti : mn;
-                    mx = ti > mx ? ti : mx;
+                    mn = scan_pack::min_step(mn, ti);
+                    mx = scan_pack::max_step(mx, ti);
                 }
                 mns[part] = mn;
                 mxs[part] = mx;
@@ -658,9 +655,9 @@ void Engine::PackAndUpload(const ScanView &scan, const double *pose_timestamps, 
             if (part == 0) { *mn_out = smn; *mx_out = smx; }
             if (part == 0 && debug) dbg_barrier_ms = ms_since(t_region);
             const double bts = pose_timestamps ? pose_timestamps[0] : smn, ets = pose_timestamps ? pose_timestamps[1] : smx;
-            const double mn = std::min(bts, ets), mx = std::max(bts, ets);
-            const bool spans = mx > mn;
-            const double inv = spans ? 1.0 / (mx - mn) : 0.0;
+            const scan_pack::AlphaRange ar = scan_pack::alpha_range(bts, ets);
+            const double mn = ar.mn, inv = ar.inv;
+            const bool spans = ar.spans;
             // 3. packing in rounds; alpha = GetAlphaTimestamp(t) (types.h:192-219; the caller range-checks)
             int issued = 0;
             auto issue_ready = [&](bool wait_all) {   // part 0 only
@@ -689,8 +686,7 @@ void Engine::PackAndUpload(const ScanView &scan, const double *pose_timestamps, 
                 for (size_t i = b; i < e && !fast; ++i) {
                     const char *p = px + i * xs;
                     const XT x = LoadUnaligned<XT>(p), y = LoadUnaligned<XT>(p + sizeof(XT)), z = LoadUnaligned<XT>(p + 2 * sizeof(XT));
-                    const double ti = (double) LoadUnaligned<TT>(pt + i * ts);
-                    const double a = spans ? (ti - mn) * inv : 1.0;
+                    const double a = scan_pack::alpha_of((double) LoadUnaligned<TT>(pt + i * ts), ar);
                     PackPoint<XT>(x, y, z, a, dst + i, &any);
                 }
                 _mm_sfence();
@@ -729,8 +725,8 @@ void Engine::MinMaxTimestamps(const ScanView &scan, double *mn_out, double *mx_o
             double mn = INFINITY, mx = -INFINITY;
             for (size_t i = b; i < e; ++i) {
                 const double ti = (double) LoadUnaligned<TT>(pt + i * ts);
-                mn = ti < mn ? ti : mn;
-                mx = ti > mx ? ti : mx;
+                mn = scan_pack::min_step(mn, ti);
+                mx = scan_pack::max_step(mx, ti);
             }
             mns[part] = mn;
             mxs[part] = mx;
@@ -1187,7 +1183,7 @@ void Engine::RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp
         CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_egress_done_, 0));
         egress_pending_ = false;
     }
-    scan_in_staging_ = staged_slot < 0;
+    scan_in_staging_ = staged_slot < 0 && !scan.on_device;
 
     // compute_frame_info, odometry.cpp:186-196
     FrameInfo info;
@@ -1195,6 +1191,20 @@ void Engine::RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp
     if (staged_slot >= 0) {
         info.begin_timestamp = staged_[staged_slot].t_min;
         info.end_timestamp = staged_[staged_slot].t_max;
+    } else if (scan.on_device) {
+        // Device memory: the reduce and the pack run on the stream behind the producer's work (and behind the previous
+        // frame's map update and egress); the host needs min / max only, the pack runs while it initialises the motion
+        CT_CUDA_CHECK(cudaEventRecord(ev_producer_, scan.producer));
+        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_producer_, 0));
+        CT_CUDA_CHECK(cudaEventRecord(ev_[0], stream_));
+        double pose_ts[2];
+        if (initial_estimate) {
+            pose_ts[0] = initial_estimate->begin_pose.dest_timestamp;
+            pose_ts[1] = initial_estimate->end_pose.dest_timestamp;
+        }
+        pipe_->PackFromDevice(scan.xyz, scan.xyz_stride, scan.xyz_dtype, scan.t, scan.t_stride, scan.t_dtype, n,
+                              initial_estimate ? pose_ts : nullptr);
+        pipe_->WaitScanReduce(&info.begin_timestamp, &info.end_timestamp);
     } else {
         // Host buffers: timestamp min/max, packing and the H2D copy, pipelined (PackAndUpload). The copy is enqueued
         // behind the previous frame's map update, which may still be running: the stream keeps the order, and the
@@ -1396,11 +1406,108 @@ cticp_device_timing Engine::LastTiming() {
     return timing_;
 }
 
+// ---- a scan in device memory / point vectors into device memory ------------------------------------------------------
+namespace {
+// [p, p + bytes) must be device (or managed) memory of `device`, inside one allocation: a short buffer is an error here,
+// not a fault in a kernel. The library links cudart statically: the driver's cuMemGetAddressRange comes through the
+// runtime's entry-point query.
+void RequireDeviceRange(const void *p, uint64_t bytes, int device, const char *what) {
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+        cudaGetLastError();
+        throw std::invalid_argument(std::string(what) + ": not a CUDA pointer");
+    }
+    if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != device)
+        throw std::invalid_argument(std::string(what) + ": not device memory of the handle's device");
+    static PFN_cuMemGetAddressRange get_range = [] {
+        void *fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            fn = nullptr;
+        return reinterpret_cast<PFN_cuMemGetAddressRange>(fn);
+    }();
+    if (!get_range) throw CudaError("cuMemGetAddressRange is not available");
+    CUdeviceptr base = 0;
+    size_t size = 0;
+    if (get_range(&base, &size, (CUdeviceptr) reinterpret_cast<uintptr_t>(p)) != CUDA_SUCCESS)
+        throw std::invalid_argument(std::string(what) + ": not inside a device allocation");
+    const uint64_t off = (uint64_t) reinterpret_cast<uintptr_t>(p) - (uint64_t) base;
+    if (bytes > size || off > size - bytes)
+        throw std::invalid_argument(std::string(what) + ": the described buffer extends past the end of its allocation");
+}
+// bytes spanned by n records of `width` bytes every `stride` bytes
+uint64_t SpanBytes(uint64_t n, uint64_t stride, uint64_t width, const char *what) {
+    uint64_t span = 0;
+    if (__builtin_mul_overflow(n - 1, stride, &span) || __builtin_add_overflow(span, width, &span))
+        throw std::invalid_argument(std::string(what) + ": the described buffer overflows the address space");
+    return span;
+}
+}  // namespace
+
+void Engine::RegisterDevice(ScanView scan, cudaStream_t producer, uint32_t frame_id, const cticp_frame *initial_estimate,
+                            cticp_summary *out, const cticp_motion_prior *motion_model) {
+    CT_CUDA_CHECK(cudaSetDevice(device_));
+    if (scan.n == 0 || !scan.xyz || !scan.t) throw std::invalid_argument("The registered frame cannot be empty");
+    if (scan.xyz_dtype != CTICP_DTYPE_FLOAT32 && scan.xyz_dtype != CTICP_DTYPE_FLOAT64)
+        throw std::invalid_argument("x/y/z must be FLOAT32 or FLOAT64");
+    const unsigned tsz = scan_pack::dtype_size(scan.t_dtype);
+    if (!tsz) throw std::invalid_argument("unknown timestamp dtype");
+    if (scan.n > pipe_->MaxPoints()) throw CapacityError("scan has more points than max_points_per_frame");
+    const uint64_t xsz = scan.xyz_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8;
+    RequireDeviceRange(scan.xyz, SpanBytes(scan.n, scan.xyz_stride, 3 * xsz, "xyz"), device_, "xyz");
+    RequireDeviceRange(scan.t, SpanBytes(scan.n, scan.t_stride, tsz, "t"), device_, "t");
+    scan.on_device = true;
+    scan.producer = producer;
+    RegisterCommon(scan, frame_id, initial_estimate, -1, out, motion_model);
+}
+
+void Engine::CheckSink(const cticp_cloud_sink &sink) const {
+    const size_t xs = sink.xyz_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8;
+    if (sink.xyz_dtype != CTICP_DTYPE_FLOAT32 && sink.xyz_dtype != CTICP_DTYPE_FLOAT64)
+        throw std::invalid_argument("sink: x/y/z must be FLOAT32 or FLOAT64");
+    if (sink.t_dtype != 0 && sink.t_dtype != CTICP_DTYPE_FLOAT32 && sink.t_dtype != CTICP_DTYPE_FLOAT64)
+        throw std::invalid_argument("sink: timestamp must be FLOAT32 or FLOAT64");
+    if ((size_t) sink.xyz_offset + 3 * xs > sink.point_step ||
+        (sink.t_dtype && (size_t) sink.t_offset + (sink.t_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8) > sink.point_step))
+        throw std::invalid_argument("sink: a field lies outside the record (point_step)");
+}
+
+int64_t Engine::WritePointsDevice(int which, const cticp_cloud_sink &sink, cudaStream_t consumer) {
+    const float4 *d_pts = nullptr, *d_lo = nullptr;
+    const double *d_world = nullptr;
+    size_t count = 0;
+    ResolvePoints(which, &d_pts, &d_lo, &d_world, &count);
+    const size_t m = std::min((size_t) sink.capacity_points, count);
+    if (m == 0 || !sink.data) return (int64_t) count;
+    CheckSink(sink);
+    // the records' last byte: the later of the two fields of the last record
+    const uint64_t x_end = (uint64_t) sink.xyz_offset + 3 * (sink.xyz_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8);
+    const uint64_t t_end = sink.t_dtype ? (uint64_t) sink.t_offset + (sink.t_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8) : 0;
+    RequireDeviceRange(sink.data, SpanBytes(m, sink.point_step, std::max(x_end, t_end), "sink"), device_, "sink");
+    const auto &f = last_frame_;
+    const scan_pack::AlphaRange ar = scan_pack::alpha_range(f.begin_pose.dest_timestamp, f.end_pose.dest_timestamp);
+    // ordered both ways with the consumer's stream: behind what it queued before (e.g. the sink's allocation), ahead of
+    // what it queues next
+    CT_CUDA_CHECK(cudaEventRecord(ev_producer_, consumer));
+    CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_producer_, 0));
+    pipe_->WritePointsDevice(d_pts, d_lo, d_world, m, sink, ar.mn, ar.mx);
+    CT_CUDA_CHECK(cudaEventRecord(ev_device_egress_, stream_));
+    CT_CUDA_CHECK(cudaStreamWaitEvent(consumer, ev_device_egress_, 0));
+    return (int64_t) count;
+}
+
 // RegistrationSummary::{corrected_points, all_corrected_points, keypoints} on demand
 // the device arrays behind RegistrationSummary::{corrected_points, all_corrected_points, keypoints}
 void Engine::ResolvePoints(int which, const float4 **out_pts, const float4 **out_lo, const double **out_world,
                            size_t *out_count) {
     CT_CUDA_CHECK(cudaSetDevice(device_));
+    // the eager egress (EnqueueEgress) writes d_all_world / the keypoints' world coordinates on its own stream: whatever
+    // reads them on the main stream from here on is ordered behind it
+    if (egress_pending_) {
+        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_egress_done_, 0));
+        egress_pending_ = false;
+    }
     const float4 *d_pts = nullptr, *d_lo = nullptr;
     const double *d_world = nullptr;
     size_t count = 0;
@@ -1535,14 +1642,7 @@ int64_t Engine::WritePoints(int which, const cticp_cloud_sink &sink) {
     ResolvePoints(which, &d_pts, &d_lo, &d_world, &count);
     const size_t m = std::min((size_t) sink.capacity_points, count);
     if (m == 0 || !sink.data) return (int64_t) count;
-    const size_t xs = sink.xyz_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8;
-    if (sink.xyz_dtype != CTICP_DTYPE_FLOAT32 && sink.xyz_dtype != CTICP_DTYPE_FLOAT64)
-        throw std::invalid_argument("sink: x/y/z must be FLOAT32 or FLOAT64");
-    if (sink.t_dtype != 0 && sink.t_dtype != CTICP_DTYPE_FLOAT32 && sink.t_dtype != CTICP_DTYPE_FLOAT64)
-        throw std::invalid_argument("sink: timestamp must be FLOAT32 or FLOAT64");
-    if ((size_t) sink.xyz_offset + 3 * xs > sink.point_step ||
-        (sink.t_dtype && (size_t) sink.t_offset + (sink.t_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8) > sink.point_step))
-        throw std::invalid_argument("sink: a field lies outside the record (point_step)");
+    CheckSink(sink);
     std::vector<float4> hp(m), hl(d_lo ? m : 0);
     std::vector<double> hw(sink.world ? 3 * m : 0);
     CT_CUDA_CHECK(cudaMemcpyAsync(hp.data(), d_pts, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_));
@@ -1560,8 +1660,9 @@ int64_t Engine::WritePoints(int which, const cticp_cloud_sink &sink) {
             double p[3];
             if (sink.world) { p[0] = hw[3 * i]; p[1] = hw[3 * i + 1]; p[2] = hw[3 * i + 2]; }
             else {
-                p[0] = hp[i].x; p[1] = hp[i].y; p[2] = hp[i].z;
-                if (d_lo) { p[0] += (double) hl[i].x; p[1] += (double) hl[i].y; p[2] += (double) hl[i].z; }
+                const float4 l = d_lo ? hl[i] : float4{0, 0, 0, 0};
+                p[0] = scan_pack::rebuild(hp[i].x, l.x, d_lo); p[1] = scan_pack::rebuild(hp[i].y, l.y, d_lo);
+                p[2] = scan_pack::rebuild(hp[i].z, l.z, d_lo);
             }
             if (sink.xyz_dtype == CTICP_DTYPE_FLOAT32) {
                 const float q[3] = {(float) p[0], (float) p[1], (float) p[2]};
@@ -1570,7 +1671,7 @@ int64_t Engine::WritePoints(int which, const cticp_cloud_sink &sink) {
                 memcpy(rec + sink.xyz_offset, p, sizeof(p));
             }
             if (sink.t_dtype) {
-                const double t = mn + ((double) hp[i].w + (d_lo ? (double) hl[i].w : 0.0)) * (mx - mn);
+                const double t = scan_pack::timestamp_of(hp[i].w, d_lo ? hl[i].w : 0.0f, d_lo, mn, mx);
                 if (sink.t_dtype == CTICP_DTYPE_FLOAT32) { const float tf = (float) t; memcpy(rec + sink.t_offset, &tf, 4); }
                 else memcpy(rec + sink.t_offset, &t, 8);
             }

@@ -49,6 +49,10 @@ struct ScanView {
     size_t t_stride = 0;
     int t_dtype = CTICP_DTYPE_FLOAT64;     // any CTICP_DTYPE_*
     size_t n = 0;
+    // in device memory of the engine's device (cticp_odometry_register_device): packed on the device after `producer`'s
+    // work, instead of on the host
+    bool on_device = false;
+    cudaStream_t producer = nullptr;
 };
 
 // host_pack.cpp: (x, y, z, alpha) packing of points [b, e) of a contiguous float64 scan with AVX2; b a multiple of 4.
@@ -97,6 +101,11 @@ public:
 
     void RegisterFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate, cticp_summary *out,
                        const cticp_motion_prior *motion_model = nullptr);
+    // RegisterFrame on a scan in device memory; producer: the stream whose work wrote it (nullptr = legacy default stream)
+    void RegisterDevice(ScanView scan, cudaStream_t producer, uint32_t frame_id, const cticp_frame *initial_estimate,
+                        cticp_summary *out, const cticp_motion_prior *motion_model);
+    // WritePoints into a sink in device memory, enqueued on the engine's stream; `consumer` is made to wait for it
+    int64_t WritePointsDevice(int which, const cticp_cloud_sink &sink, cudaStream_t consumer);
     void SetCallback(cticp_event_fn fn, void *user) { callback_ = fn; callback_user_ = user; }
     const cticp_odometry_options &Options() const { return options_; }
     // device-resident input: pack + copy a scan to HBM now, register it later
@@ -148,6 +157,8 @@ private:
 
     void InitializeMotion(const FrameInfo &info, const cticp_frame *initial_estimate);
     void ResolvePoints(int which, const float4 **out_pts, const float4 **out_lo, const double **out_world, size_t *out_count);
+    void CheckSink(const cticp_cloud_sink &sink) const;
+    cudaEvent_t ev_producer_ = nullptr, ev_device_egress_ = nullptr;   // device input / output: the caller's stream order
     void IngestImpl(const ScanView &scan,
                     const FrameInfo &info, int64_t staged_slot);
     bool PackScan(const ScanView &scan, double bts, double ets, float4 *dst);

@@ -9,11 +9,13 @@
 //   output order  = ascending perm(i) of the winners                   [flag array in permuted index space + scan]
 // and the second shuffle is one scatter through a second permutation — no sort anywhere.
 #include "frame_pipeline.h"
+#include "scan_pack.cuh"
 
 #include <cooperative_groups.h>
 #include <cstdlib>
 
 #include <algorithm>
+#include <atomic>
 #include <cstring>
 
 namespace cticp {
@@ -508,6 +510,155 @@ __global__ void k_distort_frame(float4 *__restrict__ pts, float4 *__restrict__ l
     }
 }
 
+// ---- a scan in device memory: reduce, pack (scan_pack.cuh holds the formulas the host loops use) ----------------------
+constexpr int kScanThreads = 256, kScanMaxCtas = 2 * 132;
+struct ScanPartial {
+    double mn, mx;
+    int lo, pad;
+};
+// x, y, z of one record: byte-assembled (any address), natural scalar loads, or one 16-byte load (float32, 16-aligned)
+enum { kLoadBytes = 0, kLoadNatural = 1, kLoadVec4 = 2 };
+template <typename XT, int LOAD>
+__device__ __forceinline__ void load_xyz(const unsigned char *p, XT &x, XT &y, XT &z) {
+    if constexpr (LOAD == kLoadVec4) {
+        const float4 v = __ldg(reinterpret_cast<const float4 *>(p));
+        x = v.x; y = v.y; z = v.z;
+    } else if constexpr (LOAD == kLoadNatural) {
+        const XT *q = reinterpret_cast<const XT *>(p);
+        x = __ldg(q); y = __ldg(q + 1); z = __ldg(q + 2);
+    } else {
+        x = scan_pack::load_unaligned<XT>(p);
+        y = scan_pack::load_unaligned<XT>(p + sizeof(XT));
+        z = scan_pack::load_unaligned<XT>(p + 2 * sizeof(XT));
+    }
+}
+__device__ __forceinline__ double load_timestamp(const unsigned char *p, int dtype, bool aligned) {
+    if (!aligned) return scan_pack::decode_timestamp(p, dtype);
+    switch (dtype) {
+        case CTICP_DTYPE_INT8: return (double) *reinterpret_cast<const int8_t *>(p);
+        case CTICP_DTYPE_UINT8: return (double) *p;
+        case CTICP_DTYPE_INT16: return (double) __ldg(reinterpret_cast<const short *>(p));
+        case CTICP_DTYPE_UINT16: return (double) __ldg(reinterpret_cast<const unsigned short *>(p));
+        case CTICP_DTYPE_INT32: return (double) __ldg(reinterpret_cast<const int *>(p));
+        case CTICP_DTYPE_UINT32: return (double) __ldg(reinterpret_cast<const unsigned *>(p));
+        case CTICP_DTYPE_FLOAT32: return (double) __ldg(reinterpret_cast<const float *>(p));
+        default: return __ldg(reinterpret_cast<const double *>(p));
+    }
+}
+// timestamp min / max (NaN skipped, as by the host's comparisons) and, for float64 x, y, z, whether some coordinate is not
+// float32-representable. Per-CTA partials; the last CTA combines them in CTA order and publishes the result to device
+// memory (read by k_scan_pack) and to mapped pinned memory, sequence number last (read by the host).
+template <bool XYZ_F64, int LOAD>
+__global__ void __launch_bounds__(kScanThreads) k_scan_reduce(const unsigned char *__restrict__ xyz, size_t xs,
+                                                              const unsigned char *__restrict__ t, size_t ts, int t_dtype,
+                                                              int t_aligned, int n, ScanPartial *__restrict__ part,
+                                                              unsigned *ticket, ScanReduceOut *dout,
+                                                              ScanReduceOut *hout, unsigned seq) {
+    using namespace scan_pack;
+    double mn = INFINITY, mx = -INFINITY;
+    int lo = 0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const double ti = load_timestamp(t + (size_t) i * ts, t_dtype, t_aligned);
+        mn = min_step(mn, ti);
+        mx = max_step(mx, ti);
+        if constexpr (XYZ_F64) {
+            double x, y, z;
+            load_xyz<double, LOAD>(xyz + (size_t) i * xs, x, y, z);
+            lo |= (needs_lo(x) || needs_lo(y) || needs_lo(z)) ? 1 : 0;
+        }
+    }
+    for (int o = 16; o; o >>= 1) {
+        mn = min_step(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+        mx = max_step(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        lo |= __shfl_xor_sync(0xffffffffu, lo, o);
+    }
+    __shared__ ScanPartial warp_part[kScanThreads / 32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (lane == 0) warp_part[warp] = ScanPartial{mn, mx, lo, 0};
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    ScanPartial b = warp_part[0];
+    for (int w = 1; w < kScanThreads / 32; ++w) {
+        b.mn = min_step(b.mn, warp_part[w].mn);
+        b.mx = max_step(b.mx, warp_part[w].mx);
+        b.lo |= warp_part[w].lo;
+    }
+    part[blockIdx.x] = b;
+    __threadfence();
+    if (atomicAdd(ticket, 1u) != gridDim.x - 1) return;
+    __threadfence();
+    ScanPartial r{INFINITY, -INFINITY, 0, 0};
+    for (unsigned c = 0; c < gridDim.x; ++c) {
+        const double cmn = __ldcg(&part[c].mn), cmx = __ldcg(&part[c].mx);
+        r.mn = min_step(r.mn, cmn);
+        r.mx = max_step(r.mx, cmx);
+        r.lo |= __ldcg(&part[c].lo);
+    }
+    *ticket = 0;
+    dout->t_min = r.mn; dout->t_max = r.mx; dout->needs_lo = r.lo;
+    volatile ScanReduceOut *h = hout;
+    h->t_min = r.mn; h->t_max = r.mx; h->needs_lo = r.lo;
+    __threadfence_system();
+    h->seq = seq;
+}
+// (x, y, z, alpha) → hi into raw and, when the reduce found a coordinate float32 cannot hold, lo into raw_lo.
+// use_reduce: the pose pair's timestamps are the reduce's min / max; else (bts, ets) = the initial estimate's.
+template <typename XT, int LOAD>
+__global__ void __launch_bounds__(kScanThreads) k_scan_pack(const unsigned char *__restrict__ xyz, size_t xs,
+                                                            const unsigned char *__restrict__ t, size_t ts, int t_dtype,
+                                                            int t_aligned, int n, const ScanReduceOut *red,
+                                                            int use_reduce, double bts, double ets, float4 *__restrict__ raw,
+                                                            float4 *__restrict__ raw_lo) {
+    using namespace scan_pack;
+    const AlphaRange ar = use_reduce ? alpha_range(red->t_min, red->t_max) : alpha_range(bts, ets);
+    bool write_lo = false;
+    if constexpr (sizeof(XT) == 8) write_lo = red->needs_lo != 0;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        XT x, y, z;
+        if (LOAD == kLoadVec4 && i == n - 1)   // the last record: 12 bytes (a 16-byte load may pass the described buffer)
+            load_xyz<XT, kLoadNatural>(xyz + (size_t) i * xs, x, y, z);
+        else
+            load_xyz<XT, LOAD>(xyz + (size_t) i * xs, x, y, z);
+        const double a = alpha_of(load_timestamp(t + (size_t) i * ts, t_dtype, t_aligned), ar);
+        raw[i] = make_float4(hi_of(x), hi_of(y), hi_of(z), hi_of(a));
+        if (write_lo) raw_lo[i] = make_float4(lo_of((double) x), lo_of((double) y), lo_of((double) z), lo_of(a));
+    }
+}
+// one of the summary's vectors into the caller's record layout: the fields of cticp_odometry_write_points, nothing else
+template <typename T> __device__ __forceinline__ void store_field(unsigned char *p, T v, bool aligned) {
+    if (aligned) *reinterpret_cast<T *>(p) = v;
+    else scan_pack::store_unaligned<T>(p, v);
+}
+__global__ void __launch_bounds__(kScanThreads) k_write_points(const float4 *__restrict__ pts, const float4 *__restrict__ lo,
+                                                               const double *__restrict__ world, int m,
+                                                               unsigned char *__restrict__ data, uint32_t step,
+                                                               uint32_t xoff, int xdt, int x_aligned, uint32_t toff, int tdt,
+                                                               int t_aligned, int use_world, double mn, double mx) {
+    using namespace scan_pack;
+    const bool has_lo = lo != nullptr;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+        unsigned char *rec = data + (size_t) i * step;
+        const float4 p = pts[i];
+        const float4 l = has_lo ? lo[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+        double v[3];
+        if (use_world) {
+            v[0] = world[3 * (size_t) i]; v[1] = world[3 * (size_t) i + 1]; v[2] = world[3 * (size_t) i + 2];
+        } else {
+            v[0] = rebuild(p.x, l.x, has_lo); v[1] = rebuild(p.y, l.y, has_lo); v[2] = rebuild(p.z, l.z, has_lo);
+        }
+        if (xdt == CTICP_DTYPE_FLOAT32) {
+            for (int k = 0; k < 3; ++k) store_field<float>(rec + xoff + 4 * k, hi_of(v[k]), x_aligned);
+        } else {
+            for (int k = 0; k < 3; ++k) store_field<double>(rec + xoff + 8 * k, v[k], x_aligned);
+        }
+        if (tdt) {
+            const double ts = timestamp_of(p.w, l.w, has_lo, mn, mx);
+            if (tdt == CTICP_DTYPE_FLOAT32) store_field<float>(rec + toff, hi_of(ts), t_aligned);
+            else store_field<double>(rec + toff, ts, t_aligned);
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 static uint32_t NextPow2(uint64_t v) {
     uint64_t p = 1;
@@ -550,14 +701,18 @@ FramePipeline::~FramePipeline() {
     cudaFree(d_grid_); cudaFree(d_slot_of_); cudaFree(d_win_); cudaFree(d_desc_); cudaFree(d_src_);
     cudaFree(d_counts_); cudaFree(d_frame_world_); cudaFree(d_all_world_); cudaFree(d_adaptive_);
     cudaFree(d_grid2_);
+    cudaFree(d_scan_partials_); cudaFree(d_scan_ticket_); cudaFree(d_scan_reduce_); cudaFreeHost(h_scan_reduce_);
 }
 
 int FramePipeline::Blocks(size_t n) const { return (int) std::max<size_t>(1, std::min<size_t>((n + 255) / 256, 132 * 8)); }
 
 void FramePipeline::EnsureLo() {
-    if (d_raw_lo_) return;
-    CT_CUDA_CHECK(cudaMallocHost(&h_stage_lo_, sizeof(float4) * max_points_));
-    CT_CUDA_CHECK(cudaMalloc(&d_raw_lo_, sizeof(float4) * max_points_));
+    if (!h_stage_lo_) CT_CUDA_CHECK(cudaMallocHost(&h_stage_lo_, sizeof(float4) * max_points_));
+    EnsureDeviceLo();
+}
+void FramePipeline::EnsureDeviceLo() {
+    if (d_frame_lo_) return;
+    if (!d_raw_lo_) CT_CUDA_CHECK(cudaMalloc(&d_raw_lo_, sizeof(float4) * max_points_));
     CT_CUDA_CHECK(cudaMalloc(&d_frame_lo_, sizeof(float4) * max_points_));
     CT_CUDA_CHECK(cudaMalloc(&d_kp_lo_, sizeof(float4) * max_points_));
     CT_CUDA_CHECK(cudaMalloc(&d_tmp_lo_, sizeof(float4) * max_points_));
@@ -804,6 +959,101 @@ void FramePipeline::TransformAll(const Q4 &qb, const V3 &tb, const Q4 &qe, const
 void FramePipeline::TransformInto(const float4 *pts, const float4 *lo, const int *d_n, const Q4 &qb, const V3 &tb,
                                   const Q4 &qe, const V3 &te, double *d_world, cudaStream_t stream) {
     k_transform_points<<<Blocks(n_), 256, 0, stream ? stream : stream_>>>(pts, lo, d_n, 0, qb, tb, qe, te, slerp_consts(qb, qe), d_world);
+    launches_ += 1;
+    CT_CUDA_CHECK(cudaGetLastError());
+}
+
+void FramePipeline::EnsureScanReduce() {
+    if (d_scan_reduce_) return;
+    CT_CUDA_CHECK(cudaMalloc(&d_scan_partials_, sizeof(ScanPartial) * kScanMaxCtas));
+    CT_CUDA_CHECK(cudaMalloc(&d_scan_ticket_, sizeof(unsigned)));
+    CT_CUDA_CHECK(cudaMemsetAsync(d_scan_ticket_, 0, sizeof(unsigned), stream_));
+    CT_CUDA_CHECK(cudaMalloc(&d_scan_reduce_, sizeof(ScanReduceOut)));
+    CT_CUDA_CHECK(cudaHostAlloc(&h_scan_reduce_, sizeof(ScanReduceOut), cudaHostAllocMapped));
+    memset(h_scan_reduce_, 0, sizeof(ScanReduceOut));
+    CT_CUDA_CHECK(cudaHostGetDevicePointer((void **) &h_scan_reduce_dev_, h_scan_reduce_, 0));
+}
+
+void FramePipeline::PackFromDevice(const void *xyz, size_t xyz_stride, int xyz_dtype, const void *t, size_t t_stride,
+                                   int t_dtype, size_t n, const double *pose_ts) {
+    EnsureScanReduce();
+    scan_xyz_f64_ = xyz_dtype == CTICP_DTYPE_FLOAT64;
+    // the raw lo plane exists before the launches (the pack decides on the device whether to write it); the other lo
+    // planes follow only once the reduce reports a scan that needs them (WaitScanReduce)
+    if (scan_xyz_f64_ && !d_raw_lo_) CT_CUDA_CHECK(cudaMalloc(&d_raw_lo_, sizeof(float4) * max_points_));
+    BeginScan(n);
+    h2d_bytes_ = 0;
+    const auto *px = static_cast<const unsigned char *>(xyz), *pt = static_cast<const unsigned char *>(t);
+    const size_t xsz = scan_xyz_f64_ ? 8 : 4, tsz = scan_pack::dtype_size(t_dtype);
+    // natural loads when every record's field is aligned to its scalar; one 16-byte load for (N, 4)-like float32 rows
+    const bool x_nat = (reinterpret_cast<uintptr_t>(px) % xsz) == 0 && xyz_stride % xsz == 0;
+    const bool x_vec4 = !scan_xyz_f64_ && (reinterpret_cast<uintptr_t>(px) % 16) == 0 && xyz_stride % 16 == 0;
+    const int t_al = ((reinterpret_cast<uintptr_t>(pt) % tsz) == 0 && t_stride % tsz == 0) ? 1 : 0;
+    const int load = x_vec4 ? kLoadVec4 : x_nat ? kLoadNatural : kLoadBytes;
+    const int ni = (int) n;
+    const int blocks = std::min(Blocks(n), kScanMaxCtas);
+    const unsigned seq = ++scan_reduce_seq_;
+    ScanPartial *part = static_cast<ScanPartial *>(d_scan_partials_);
+    if (scan_xyz_f64_) {
+        auto k = load == kLoadNatural ? k_scan_reduce<true, kLoadNatural> : k_scan_reduce<true, kLoadBytes>;
+        k<<<blocks, kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, part, d_scan_ticket_,
+                                                d_scan_reduce_, h_scan_reduce_dev_, seq);
+    } else {
+        k_scan_reduce<false, kLoadBytes><<<blocks, kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni,
+                                                                              part, d_scan_ticket_, d_scan_reduce_,
+                                                                              h_scan_reduce_dev_, seq);
+    }
+    CT_CUDA_CHECK(cudaGetLastError());
+    const int use_reduce = pose_ts ? 0 : 1;
+    const double bts = pose_ts ? pose_ts[0] : 0.0, ets = pose_ts ? pose_ts[1] : 0.0;
+    if (scan_xyz_f64_) {
+        auto k = load == kLoadNatural ? k_scan_pack<double, kLoadNatural> : k_scan_pack<double, kLoadBytes>;
+        k<<<Blocks(n), kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, d_scan_reduce_, use_reduce,
+                                                   bts, ets, d_raw_, d_raw_lo_);
+    } else {
+        auto k = load == kLoadVec4 ? k_scan_pack<float, kLoadVec4>
+                 : load == kLoadNatural ? k_scan_pack<float, kLoadNatural> : k_scan_pack<float, kLoadBytes>;
+        k<<<Blocks(n), kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, d_scan_reduce_, use_reduce,
+                                                   bts, ets, d_raw_, nullptr);
+    }
+    CT_CUDA_CHECK(cudaGetLastError());
+    launches_ += 2;
+}
+
+// Spin on the reduce's sequence number; the stream is polled now and then, so that a faulted kernel surfaces as an error
+void FramePipeline::WaitScanReduce(double *t_min, double *t_max) {
+    volatile unsigned *flag = &h_scan_reduce_->seq;
+    for (unsigned long spins = 1;; ++spins) {
+        if (*flag == scan_reduce_seq_) break;
+        if ((spins & 0xfffu) == 0) {
+            const cudaError_t q = cudaStreamQuery(stream_);
+            if (q == cudaSuccess) {
+                if (*flag == scan_reduce_seq_) break;
+                throw std::runtime_error("the scan reduce never arrived although the stream is idle");
+            }
+            if (q != cudaErrorNotReady) CT_CUDA_CHECK(q);
+        }
+    }
+    std::atomic_thread_fence(std::memory_order_acquire);
+    const volatile ScanReduceOut *r = h_scan_reduce_;
+    *t_min = r->t_min;
+    *t_max = r->t_max;
+    // what the host packer would report: a float64 scan with a coordinate float32 cannot hold carries its residual plane
+    raw_lo_ = scan_xyz_f64_ && r->needs_lo != 0;
+    raw_lo_ptr_ = d_raw_lo_;
+    if (raw_lo_) EnsureDeviceLo();   // before the sampler that writes the frame's lo plane is enqueued
+}
+
+void FramePipeline::WritePointsDevice(const float4 *pts, const float4 *lo, const double *world, size_t m,
+                                      const cticp_cloud_sink &sink, double mn, double mx) {
+    if (m == 0) return;
+    auto *data = static_cast<unsigned char *>(sink.data);
+    const size_t xsz = sink.xyz_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8, tsz = sink.t_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8;
+    const int x_al = ((reinterpret_cast<uintptr_t>(data) + sink.xyz_offset) % xsz == 0 && sink.point_step % xsz == 0) ? 1 : 0;
+    const int t_al = ((reinterpret_cast<uintptr_t>(data) + sink.t_offset) % tsz == 0 && sink.point_step % tsz == 0) ? 1 : 0;
+    k_write_points<<<Blocks(m), kScanThreads, 0, stream_>>>(pts, lo, sink.world ? world : nullptr, (int) m, data,
+                                                             sink.point_step, sink.xyz_offset, sink.xyz_dtype, x_al,
+                                                             sink.t_offset, sink.t_dtype, t_al, sink.world ? 1 : 0, mn, mx);
     launches_ += 1;
     CT_CUDA_CHECK(cudaGetLastError());
 }

@@ -10,6 +10,13 @@
 
 namespace cticp {
 
+// what k_scan_reduce leaves in device memory and in mapped pinned memory (FramePipeline::PackFromDevice)
+struct ScanReduceOut {
+    double t_min, t_max;
+    int needs_lo;
+    unsigned seq;
+};
+
 class FramePipeline {
 public:
     FramePipeline(size_t max_points, cudaStream_t stream);
@@ -23,6 +30,8 @@ public:
     // what LiDAR drivers emit, never need them. raw_lo: the scan as uploaded; frame_lo: the sub-sampled frame and the
     // keypoints drawn from it (also set by DistortFrame, whose output is not float32-representable).
     void EnsureLo();
+    // the device lo planes only (raw, frame, keypoints, scratch): what a scan packed on the device needs
+    void EnsureDeviceLo();
     float4 *StagingLo() { EnsureLo(); return h_stage_lo_; }
     const float4 *StagingLoIfAny() const { return raw_lo_ ? h_stage_lo_ : nullptr; }
     void UploadLo(size_t n);                                  // after Upload*/UploadBegin of the same scan
@@ -43,6 +52,19 @@ public:
     void UploadFromDevice(const float4 *d_src, const float4 *d_src_lo, size_t n);
     // copy a scan read in place into the pipeline's own buffers (before the caller frees it); stream-ordered
     void DetachRaw();
+    // A scan in device memory (x, y, z of xyz_dtype at xyz, one t_dtype timestamp at t, both strided in bytes; the caller
+    // validated the layout): two launches on the pipeline's stream. k_scan_reduce: timestamp min / max and, for float64
+    // x, y, z, whether the scan needs its residual plane, to device memory and to mapped pinned memory. k_scan_pack: the
+    // (x, y, z, alpha) planes into the pipeline's own raw buffers, alpha w.r.t. pose_ts = the initial estimate's {begin,
+    // end} dest_timestamp, or (nullptr) the reduce's min / max read on the device.
+    void PackFromDevice(const void *xyz, size_t xyz_stride, int xyz_dtype, const void *t, size_t t_stride, int t_dtype,
+                        size_t n, const double *pose_ts);
+    // the reduce's min / max (waits for k_scan_reduce only; the pack may still run)
+    void WaitScanReduce(double *t_min, double *t_max);
+    // m points of one of the summary's vectors into records in device memory (cticp_odometry_write_points_device), on
+    // the pipeline's stream; mn / mx: the pose pair's timestamps ordered
+    void WritePointsDevice(const float4 *pts, const float4 *lo, const double *world, size_t m, const cticp_cloud_sink &sink,
+                           double mn, double mx);
 
     // Odometry::InitializeFrame: shuffle → sub_sample_frame → (frames 0,1: timestamp := end) → shuffle
     void SubSampleFrame(double voxel_size, uint64_t seed, uint64_t counter1, uint64_t counter2, bool override_alpha,
@@ -129,6 +151,13 @@ private:
     bool preclear_ = true;
     uint32_t clean_cap_ = 0;
     uint32_t *d_adaptive_ = nullptr;   // tile counters + flags + src of the band-major position space
+    // k_scan_reduce: per-CTA partials, the last CTA's ticket, the result (device / mapped pinned, sequence number last)
+    void *d_scan_partials_ = nullptr;
+    unsigned *d_scan_ticket_ = nullptr;
+    ScanReduceOut *d_scan_reduce_ = nullptr, *h_scan_reduce_ = nullptr, *h_scan_reduce_dev_ = nullptr;
+    unsigned scan_reduce_seq_ = 0;
+    bool scan_xyz_f64_ = false;
+    void EnsureScanReduce();
     size_t adaptive_capacity_ = 0;
     int launches_ = 0;
 };

@@ -405,6 +405,34 @@ int64_t cticp_odometry_get_points(cticp_odometry *h, int which, cticp_wpoint *ds
  * cticp_odometry_get_points that follows only assembles the 64-byte records. 0 (default) = on demand. */
 int cticp_odometry_set_summary_points(cticp_odometry *h, int mask);
 
+/* Device input and output (new). A scan in device memory of the handle's device (cudaMalloc, cudaMallocManaged, a torch
+ * CUDA tensor): x, y, z contiguous of one scalar type at xyz and one timestamp scalar at t, each strided in bytes. Records
+ * need no alignment (PointCloud2 layouts: xyz = data + x_offset, t = data + t_offset, both strides = point_step). */
+typedef struct cticp_device_scan {
+    const void *xyz;
+    uint64_t xyz_stride_bytes;
+    const void *t;
+    uint64_t t_stride_bytes;
+    uint64_t num_points;
+    int32_t xyz_dtype;             /* CTICP_DTYPE_FLOAT32 or CTICP_DTYPE_FLOAT64 */
+    int32_t t_dtype;               /* any CTICP_DTYPE_* */
+} cticp_device_scan;
+/* cticp_odometry_register_frame_ex on a device scan: the same results, byte for byte, as on a host copy of the same values
+ * and scalar types. The scan is packed on the device (no host round trip for the points). stream (a cudaStream_t; NULL =
+ * the legacy default stream) is the producer's stream: the engine waits for its work through an event before reading. The
+ * buffers may be overwritten once the call returns. Checked before anything is enqueued: pointers that are not device
+ * memory of the handle's device, or a described buffer that extends past its allocation (CTICP_ERR_INVALID_ARGUMENT),
+ * unknown dtypes (CTICP_ERR_INVALID_ARGUMENT), more than max_points_per_frame points (CTICP_ERR_CAPACITY). */
+int cticp_odometry_register_device(cticp_odometry *h, const cticp_device_scan *scan, void *stream, uint32_t frame_id,
+                                   const cticp_frame *initial_estimate,      /* nullable */
+                                   const cticp_motion_prior *motion_model,   /* nullable */
+                                   cticp_summary *out_summary);
+/* cticp_odometry_write_points into a sink in device memory of the handle's device: the same bytes, the same
+ * min(capacity_points, count) rule and the same return value. Enqueued on the handle's stream after the work already
+ * queued on `stream` (NULL = the legacy default stream), and `stream` is made to wait for it. Returns the count without
+ * a host synchronisation. */
+int64_t cticp_odometry_write_points_device(cticp_odometry *h, int which, const cticp_cloud_sink *sink, void *stream);
+
 /* ct_icp::Odometry::Trajectory(), src/ct_icp/odometry.cpp:687-689 */
 int64_t cticp_odometry_trajectory(cticp_odometry *h, cticp_frame *dst, size_t cap);
 /* ct_icp::Odometry::MapSize(), src/ct_icp/odometry.cpp:156-158 */
@@ -446,8 +474,9 @@ typedef struct cticp_device_timing {
 } cticp_device_timing;
 int cticp_odometry_last_timing(cticp_odometry *h, cticp_device_timing *out);
 
-/* Device-resident input (new): a scan can be packed and copied to HBM ahead of time (e.g. by a decoder that
- * already runs on the GPU) and registered later without any host→device traffic for the points.
+/* Staged input (new): a scan in host memory can be packed and copied to HBM ahead of time and registered later
+ * without any host→device traffic for the points. A scan that is already in device memory (e.g. written by a decoder
+ * that runs on the GPU) goes to cticp_odometry_register_device instead.
  * cticp_odometry_stage_frame returns a slot id >= 0; slots live until cticp_odometry_clear_staged. */
 int64_t cticp_odometry_stage_frame(cticp_odometry *h, const double *xyz, size_t xyz_stride_bytes, const double *t,
                                    size_t t_stride_bytes, size_t n);
