@@ -74,7 +74,8 @@ struct GnParams {
     double max_dist_to_plane;   // max_dist_to_plane_ct_icp
     double threshold_norm;      // threshold_orientation_norm (GN stop criterion on ‖x‖, ct_icp.cpp:978)
     int shard_rank, shard_world;   // keypoint sharding (multi-GPU); 0/1 when single
-    int debug_flags;               // profiling only (env CTICP_DEBUG_FLAGS): 1 = skip the solve, 2 = skip the gather work
+    int debug_flags;               // profiling only (env CTICP_DEBUG_FLAGS): 1 = skip the solve, 2 = skip the gather work,
+                                   // 8 = no paired tile schedule in k_gn_persistent (bit-identity tests)
     double bucket_scale;           // 32 / radius^2: d2 → histogram bucket of the k-nearest selection (gather_select.cuh)
     const float4 *kp_lo;           // residual plane of the keypoints (nullptr: float32-representable; load_raw, se3.cuh)
     unsigned long long *dbg_warp;  // -DCTICP_DEBUG_TIMERS builds with CTICP_DEBUG_TIMERS set: per-warp phase stamps (icp_gn.cu)

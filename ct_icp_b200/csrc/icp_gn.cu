@@ -168,7 +168,9 @@ __device__ __noinline__ void warp_gn_solve(const double *acc, SolveScratch &S, I
 // dynamically — a warp whose keypoint has a sparse stencil takes the next one while a neighbour is still busy with a
 // dense one — and the registration stays bit-reproducible. Per-warp clock64 stamps of the static tiles of
 // two that came before showed a long tail of slow tiles, and every iteration waited for the slowest while half of the
-// warps had no tile at all.
+// warps had no tile at all. The exception (gn_pair_schedule): in k_gn_persistent, from the second iteration on, a range of
+// more keypoints than warps but at most two per warp gets one tile per warp from the last iteration's costs — the
+// heaviest keypoints alone, the others in pairs — instead of a few warps running a second whole chain after their first.
 struct GnPose {
     Q4 qb, qe;
     V3 tb, te;
@@ -178,9 +180,9 @@ struct GnWarpAcc {
     double sum_sq = 0;               // (unused: Σ scalar² comes out of the CTA's row reduction, accumulator kAccSumSq)
     unsigned n_stencil = 0;          // per-lane partial counters
     int n_used = 0, n_kp = 0, n_valid = 0;
-    CT_STAMP(long long dbg[4] = {0, 0, 0, 0};)   // cycles in phases A, B, C, D
+    CT_STAMP(long long dbg[5] = {0, 0, 0, 0, 0};)   // cycles in phases A, B, C; end of the warp's last tile; longest tile
 };
-constexpr int kDbgIters = 8, kDbgSlots = 6;
+constexpr int kDbgIters = 8, kDbgSlots = 8;
 
 constexpr int kTileMax = 16;   // keypoints per warp tile (phases A / C cost 1/W per keypoint: 16 is deep in the flat part)
 constexpr int kRowCap = 256;   // rows of a CTA's range held in shared memory at a time (longer ranges go in chunks)
@@ -198,7 +200,12 @@ struct __align__(16) CtaRows {
     unsigned char used[kRowCap];
     double red[kRowParts][kAcc];
     int next;                    // tile counter of the chunk
+    // the paired schedule (gn_pair_schedule): stencil points of keypoint r in the last iteration (written for every range:
+    // no bound check in phase C), and this iteration's tiles — warp w takes pair[w][0] and pair[w][1] (kNoKeypoint: none)
+    unsigned cost[kRowCap];
+    unsigned char pair[kGatherWarps][2];
 };
+constexpr unsigned char kNoKeypoint = 0xff;
 
 // keypoints per tile for a CTA range of `span` keypoints
 __device__ __forceinline__ int gn_tile_width(int span) {
@@ -210,30 +217,72 @@ __device__ __forceinline__ int gn_tile_width(int span) {
     return W < kTileMax ? W : kTileMax;
 }
 
+// ranges that take the paired schedule once the last iteration's costs are known: more keypoints than warps, at most two
+// per warp (one keypoint per lane of the warp that builds the schedule: CTAs of at most 16 warps)
+__device__ __forceinline__ bool gn_pairs_apply(int span) {
+    return kGatherWarps > 1 && 2 * kGatherWarps <= 32 && span > kGatherWarps && span <= 2 * kGatherWarps;
+}
+
+// The static schedule of a range of kGatherWarps < n <= 2 kGatherWarps keypoints from the costs of the last iteration
+// (R.cost[0..n), written by every keypoint's phase C): one tile per warp, S = 2 kGatherWarps - n single tiles and
+// n - kGatherWarps pairs. The S heaviest keypoints (most stencil points; ties: lower index first) get a warp each and the
+// remaining ones are paired heaviest with lightest, which makes the largest pair cost as small as it can be. A pair runs
+// phases A and C once for both keypoints (lanes 0 and 1) instead of a second whole chain on the warp that grabbed it.
+// The schedule is a function of the costs alone; the rows go to R.u by keypoint as before, so the result does not depend
+// on it. One warp; writes R.pair.
+__device__ __noinline__ void gn_pair_schedule(CtaRows &R, int n, int lane) {
+    const unsigned c = lane < n ? R.cost[lane] : 0u;
+    int rank = 0;   // position in the order heaviest first, lower index first among equals
+    for (int j = 0; j < n; ++j) {
+        const unsigned cj = __shfl_sync(0xffffffffu, c, j);
+        rank += (cj > c || (cj == c && j < lane)) ? 1 : 0;
+    }
+    const int singles = 2 * kGatherWarps - n, pairs = n - kGatherWarps;
+    if (lane < n) {
+        if (rank < singles) {
+            R.pair[rank][0] = (unsigned char) lane;
+            R.pair[rank][1] = kNoKeypoint;
+        } else if (rank < singles + pairs) {
+            R.pair[rank][0] = (unsigned char) lane;
+        } else {
+            R.pair[singles + (n - 1 - rank)][1] = (unsigned char) lane;
+        }
+    }
+}
+
 // The tiles of the chunk [lo, hi) of this CTA's range (hi - lo <= kRowCap); R.next must be 0 and visible (barrier) on entry.
+// `pair` (nullptr: tiles of W keypoints grabbed from R.next): this warp's one tile of the paired schedule (R.pair).
 __device__ __forceinline__ void gn_gather_tiles(const GatherLaunch &cfg, const int *stencil,
                                                 const float4 *__restrict__ keypoints, int lo, int hi, int W,
-                                                const GnPose &pose, TileScratch &T, CtaRows &R, int lane,
-                                                GnWarpAcc &A, void *bulk = nullptr, bool rigid = false) {
+                                                const unsigned char *pair, const GnPose &pose, TileScratch &T,
+                                                CtaRows &R, int lane, GnWarpAcc &A, void *bulk = nullptr,
+                                                bool rigid = false) {
     const GatherConfig &G = cfg.G;
     const GnParams &P = cfg.P;
     if (hi <= lo) return;
     const int need = P.kmin > 5 ? P.kmin : 5;   // ct_icp.cpp:769 ; neighborhood.h:227
     const double inv_res = 1.0 / G.L.res;
 
-    while (true) {
-        int j0 = 0;
-        if (lane == 0) j0 = atomicAdd(&R.next, W);
-        j0 = __shfl_sync(0xffffffffu, j0, 0);
-        const int t0 = lo + j0;
-        if (t0 >= hi) break;
-        const int wt = (hi - t0) < W ? (hi - t0) : W;
+    for (bool first = true;; first = false) {
+        int wt, r;   // keypoints of the tile; lane < wt: the row (keypoint lo + r) of lane's keypoint
+        if (pair) {
+            if (!first) break;
+            wt = pair[1] == kNoKeypoint ? 1 : 2;
+            r = pair[lane == 0 ? 0 : 1];
+        } else {
+            int j0 = 0;
+            if (lane == 0) j0 = atomicAdd(&R.next, W);
+            j0 = __shfl_sync(0xffffffffu, j0, 0);
+            if (lo + j0 >= hi) break;
+            wt = (hi - lo - j0) < W ? (hi - lo - j0) : W;
+            r = j0 + lane;
+        }
         CT_STAMP(const long long t_a = clock64();)
         // ---- A: world_kpts[i] = InterpolatePose(begin, end, t_i) * raw_i  (ct_icp.cpp:964-966, types.h:361-366)
         V3 p{0, 0, 0};
         int kx = 0, ky = 0, kz = 0;
         if (lane < wt) {
-            const RawPoint kraw = load_raw(keypoints, P.kp_lo, t0 + lane);   // raw xyz (sensor frame) + alpha timestamp
+            const RawPoint kraw = load_raw(keypoints, P.kp_lo, lo + r);   // raw xyz (sensor frame) + alpha timestamp
             const V3 raw{kraw.x, kraw.y, kraw.z};
             p = rigid ? qrot(qnormalized(pose.qe), raw) + pose.te
                       : ct_transform_c(pose.qb, pose.tb, pose.qe, pose.te, kraw.alpha, raw, pose.sc);
@@ -269,7 +318,9 @@ __device__ __forceinline__ void gn_gather_tiles(const GatherLaunch &cfg, const i
             NeighborSums mine;
             mine.n = __double2loint(o[0]);
             A.n_kp += 1;
-            A.n_stencil += (unsigned) __double2hiint(o[0]);
+            const unsigned spts = (unsigned) __double2hiint(o[0]);
+            A.n_stencil += spts;
+            R.cost[r] = spts;   // the next iteration's schedule (gn_pair_schedule)
             if (mine.n >= need) {
                 A.n_valid += 1;
                 mine.sx = o[2]; mine.sy = o[3]; mine.sz = o[4];
@@ -286,12 +337,12 @@ __device__ __forceinline__ void gn_gather_tiles(const GatherLaunch &cfg, const i
                 if (fabs(dist_to_plane) < P.max_dist_to_plane) {              // :803
                     const V3 nw = weight * normal;
                     const double scalar = dot(nw, diff);
-                    const RawPoint kraw = load_raw(keypoints, P.kp_lo, t0 + lane);
+                    const RawPoint kraw = load_raw(keypoints, P.kp_lo, lo + r);
                     const V3 raw{kraw.x, kraw.y, kraw.z};
                     const V3 ob = qrot(pose.qb, raw), oe = qrot(pose.qe, raw);   // :813-816
                     const double a = kraw.alpha, am = 1.0 - a;
                     const V3 cb = cross(ob, nw), ce = cross(oe, nw);
-                    double *u = R.u[j0 + lane];
+                    double *u = R.u[r];
                     u[0] = am * cb.x; u[1] = am * cb.y; u[2] = am * cb.z;
                     u[3] = am * nw.x; u[4] = am * nw.y; u[5] = am * nw.z;
                     u[6] = a * ce.x;  u[7] = a * ce.y;  u[8] = a * ce.z;
@@ -301,11 +352,12 @@ __device__ __forceinline__ void gn_gather_tiles(const GatherLaunch &cfg, const i
                     A.n_used += 1;
                 }
             }
-            R.used[j0 + lane] = used ? 1 : 0;
+            R.used[r] = used ? 1 : 0;
         }
         __syncwarp();   // the moments are consumed before the next tile rewrites them
         CT_STAMP(const long long t_e = clock64();
-                 A.dbg[0] += t_b - t_a; A.dbg[1] += t_c - t_b; A.dbg[2] += t_e - t_c;)
+                 A.dbg[0] += t_b - t_a; A.dbg[1] += t_c - t_b; A.dbg[2] += t_e - t_c;
+                 A.dbg[3] = t_e; if (t_e - t_a > A.dbg[4]) A.dbg[4] = t_e - t_a;)
     }
 }
 
@@ -424,15 +476,17 @@ __device__ __forceinline__ void gn_reduce_rows(GnShared &sh, const double *__res
 
 // The gather half of an iteration for one CTA: its range [c_lo, c_hi) of the keypoints, in chunks of kRowCap rows →
 // the CTA's partial row (kAcc doubles): thread t < kAcc returns entry t. On entry sh.pose is valid and sh.rows.next == 0,
-// both visible to the CTA (the thread that fetched the pose set them before a barrier). All threads call.
+// both visible to the CTA (the thread that fetched the pose set them before a barrier). `paired`: sh.rows.pair holds the
+// schedule of this range (gn_pair_schedule; only for gn_pairs_apply ranges, which are one chunk). All threads call.
 __device__ __forceinline__ double gn_cta_gather(const GatherLaunch &cfg, const int *stencil, const float4 *__restrict__ keypoints,
                                                 int c_lo, int c_hi, GnShared &sh, int lane, int w, GnWarpAcc &A, void *bulk,
-                                                bool rigid) {
+                                                bool rigid, bool paired = false) {
     const int W = gn_tile_width(c_hi - c_lo);
+    const unsigned char *pair = paired ? sh.rows.pair[w] : nullptr;
     double carry = 0;
     for (int base = c_lo;; base += kRowCap) {
         const int top = (c_hi - base) > kRowCap ? base + kRowCap : c_hi;
-        gn_gather_tiles(cfg, stencil, keypoints, base, top, W, sh.pose, sh.tile[w], sh.rows, lane, A, bulk, rigid);
+        gn_gather_tiles(cfg, stencil, keypoints, base, top, W, pair, sh.pose, sh.tile[w], sh.rows, lane, A, bulk, rigid);
         gn_cta_reduce_rows(sh.rows, top > base ? top - base : 0, carry);
         if (top >= c_hi) break;
         if (threadIdx.x == 0) sh.rows.next = 0;
@@ -742,6 +796,12 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
         } else {
             GnWarpAcc A;
             CT_STAMP(const long long t_it = clock64();)
+            // from the second iteration on, a range of more keypoints than warps but at most two per warp takes the paired
+            // schedule, built from the last iteration's costs by warp 1 while warp 0 waits for the pose (the first iteration,
+            // and every one with CTICP_DEBUG_FLAGS & 8, a debug switch for bit-identity tests: tiles of one keypoint grabbed
+            // from the counter)
+            const bool paired = it > 0 && !(P.debug_flags & (2 | 8)) && gn_pairs_apply(c_hi - c_lo);
+            if (w == 1 && paired) gn_pair_schedule(sh.rows, c_hi - c_lo, lane);
             if (w == 0) {   // phases A / C read the pose from shared memory: 34 registers less to keep live
                 if (it == 0) {   // the state the host uploaded
                     if (lane == 0) {
@@ -762,9 +822,10 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
             // (CTICP_DEBUG_FLAGS & 2, timing only: an empty range — the hand-off and the reduction without the gather work)
             const bool skip = (P.debug_flags & 2) != 0;
             const double s = gn_cta_gather(cfg, stencil, keypoints, skip ? 0 : c_lo, skip ? 0 : c_hi, sh, lane, w, A, bulk_ptr,
-                                           P.rigid_first && it == 0);
+                                           P.rigid_first && it == 0, paired);
             if (threadIdx.x < kAcc) tagged_store_double(sh.grp.rows + 2 * threadIdx.x, tag, s);
             CT_STAMP(const long long t_g = clock64();)
+            CT_STAMP(const int dbg_kp = __reduce_add_sync(0xffffffffu, A.n_kp);)
             CT_STAMP(if (P.dbg_warp && lane == 0 && it < kDbgIters) {
                 unsigned long long *o = P.dbg_warp + ((size_t) it * (gather_ctas * kGatherWarps) + (w * gather_ctas + (cta - 1))) * kDbgSlots;
                 o[0] = (unsigned long long) A.dbg[0]; o[1] = (unsigned long long) A.dbg[1];
@@ -772,6 +833,8 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
                 o[3] = (unsigned long long) (t_g0 - t_it);         // pose fetch + barrier
                 o[4] = (unsigned long long) (t_g - t_it);          // pose fetch + tiles + CTA row reduction
                 o[5] = 0;
+                o[6] = A.dbg[3] ? (unsigned long long) (A.dbg[3] - t_g0) : 0;   // end of the warp's last tile
+                o[7] = (unsigned long long) dbg_kp | ((unsigned long long) A.dbg[4] << 8);   // keypoints | longest tile << 8
             })
 #ifdef CTICP_GN_FLAG_SYNC
             if (it == num_iters - 1) break;   // nothing left to wait for: the solver CTA finishes the registration alone
@@ -1124,10 +1187,42 @@ void IcpSolver::PrintWarpStamps(int iters) {
     const int W = dbg_warps_;
     std::vector<unsigned long long> h((size_t) kDbgIters * W * kDbgSlots);
     CT_CUDA_CHECK(cudaMemcpy(h.data(), d_dbg_warp_, sizeof(unsigned long long) * h.size(), cudaMemcpyDeviceToHost));
-    static const char *names[kDbgSlots] = {"A pose+voxel", "B gather+select", "C epilogue", "pose fetch", "fetch+tiles+row reduction", "barrier wait (per CTA)"};
+    static const char *names[kDbgSlots - 1] = {"A pose+voxel", "B gather+select", "C epilogue", "pose fetch", "fetch+tiles+row reduction",
+                                               "barrier wait (per CTA)", "end of last tile"};
+    const auto pct = [](std::vector<unsigned long long> v, int p) { std::sort(v.begin(), v.end()); return v.empty() ? 0ull : v[v.size() * p / 100]; };
     for (int it = 0; it < std::min(iters, kDbgIters); ++it) {
+        const unsigned long long *h_it = h.data() + (size_t) it * W * kDbgSlots;
+        // per CTA: the warp whose last tile ends last, the keypoints it took, the CTA's longest single tile
+        const int ctas = W / kGatherWarps;
+        int last_two = 0, ctas_seen = 0, slowest_cta = -1;
+        unsigned long long slowest_end = 0, a = 0, b = 0, c = 0, kps = 0;
+        std::vector<unsigned long long> cta_end, cta_tile, excess;
+        for (int ct = 0; ct < ctas; ++ct) {
+            unsigned long long end = 0, tile = 0;
+            int last_kp = 0;
+            for (int w = 0; w < kGatherWarps; ++w) {
+                const unsigned long long *o = h_it + ((size_t) w * ctas + ct) * kDbgSlots;
+                if (o[4] == 0) continue;
+                a += o[0]; b += o[1]; c += o[2]; kps += o[7] & 0xff;
+                tile = std::max(tile, o[7] >> 8);
+                if (o[6] >= end) { end = o[6]; last_kp = (int) (o[7] & 0xff); }
+            }
+            if (end == 0) continue;
+            ++ctas_seen;
+            last_two += last_kp >= 2;
+            cta_end.push_back(end);
+            cta_tile.push_back(tile);
+            excess.push_back(end > tile ? end - tile : 0);
+            if (end > slowest_end) { slowest_end = end; slowest_cta = last_kp; }
+        }
+        if (ctas_seen > 0 && kps > 0)
+            fprintf(stderr, "[cticp] GN gather CTAs, iteration %d: %d CTAs; last warp held >= 2 keypoints in %d; slowest CTA %llu "
+                    "(its last warp %d keypoints); CTA tiles end p50 %llu p90 %llu; longest single tile p50 %llu p90 %llu; "
+                    "end - longest tile p50 %llu p90 %llu; per keypoint A %.0f B %.0f C %.0f\n", it, ctas_seen, last_two,
+                    slowest_end, slowest_cta, pct(cta_end, 50), pct(cta_end, 90), pct(cta_tile, 50), pct(cta_tile, 90),
+                    pct(excess, 50), pct(excess, 90), (double) a / kps, (double) b / kps, (double) c / kps);
         fprintf(stderr, "[cticp] GN gather warps, iteration %d (SM cycles; %d warps):", it, W);
-        for (int sl = 0; sl < kDbgSlots; ++sl) {
+        for (int sl = 0; sl < kDbgSlots - 1; ++sl) {
             std::vector<unsigned long long> v;
             for (int w = 0; w < W; ++w) {
                 const unsigned long long x = h[((size_t) it * W + w) * kDbgSlots + sl];
