@@ -217,8 +217,20 @@ class DeviceTiming(_Struct):
         ("map_update_ms", C.c_double), ("icp_iterations", C.c_int32), ("kernel_launches", C.c_int32),
         ("gather_keypoint_iterations", C.c_uint64), ("gather_stencil_points", C.c_uint64),
         ("gather_stencil_voxels", C.c_uint64), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64),
-        ("gather_launches", C.c_int32), ("_pad0", C.c_int32),
+        ("gather_launches", C.c_int32), ("icp_batch_groups", C.c_int32),
     ]
+
+
+# cticp_batch_frame kinds
+BATCH_HOST, BATCH_DEVICE, BATCH_STAGED = 0, 1, 2
+
+
+class BatchFrame(_Struct):   # cticp_batch_frame: one item of cticp_odometry_register_batch
+    _fields_ = [("handle", C.c_void_p), ("kind", C.c_int32), ("frame_id", C.c_uint32),
+                ("xyz", C.c_void_p), ("xyz_stride_bytes", C.c_size_t), ("t", C.c_void_p), ("t_stride_bytes", C.c_size_t),
+                ("n", C.c_size_t), ("device_scan", C.c_void_p), ("stream", C.c_void_p), ("staged_slot", C.c_int64),
+                ("initial_estimate", C.c_void_p), ("motion_model", C.c_void_p), ("out", C.c_void_p),
+                ("status", C.c_int32), ("_pad0", C.c_int32)]
 
 
 # numpy dtype of cticp_wpoint (64 bytes, same as slam::WPoint3D)

@@ -12,9 +12,10 @@ from . import _abi as abi
 
 
 class CticpError(RuntimeError):
-    def __init__(self, code, message):
+    def __init__(self, code, message, statuses=None):
         super().__init__(f"[{code}] {message}")
         self.code = code
+        self.statuses = statuses   # register_batch: every item's status (0 = registered)
 
 
 def _is_cuda_tensor(a):
@@ -108,6 +109,7 @@ class Binding:
             "odometry_write_points_device": (i64, [vp, C.c_int, P(abi.CloudSink), vp]),
             "odometry_register_staged": (C.c_int, [vp, i64, u32, P(abi.Summary)]),
             "odometry_clear_staged": (C.c_int, [vp]),
+            "odometry_register_batch": (C.c_int, [P(abi.BatchFrame), sz]),
             "odometry_timer_start": (C.c_int, [vp]),
             "odometry_timer_stop": (C.c_int, [vp, P(dbl)]),
             "odometry_flush_l2": (C.c_int, [vp, sz]),
@@ -182,6 +184,60 @@ class Binding:
 
     def voxel_map(self, options, device=0):
         return VoxelMap(self, options=options, device=device)
+
+    # ---- many handles, one frame each ------------------------------------------------------------------------
+    def register_batch(self, odometries, scans, frame_ids, initial_estimates=None, motion_models=None):
+        """One frame on each Odometry of `odometries` in one call (cticp_odometry_register_batch): the eligible
+        Gauss-Newton loops run in one grouped launch, every result is that of the single-frame call.
+        scans[i]: (xyz, timestamps) NumPy arrays (RegisterFrame's host path), (xyz, timestamps) torch CUDA tensors (read
+        after the work queued on torch's current stream, as RegisterFrame), or an int staged slot (RegisterStaged).
+        initial_estimates / motion_models: None or one entry (abi.Frame / abi.MotionPrior or None) per item.
+        Returns the summaries; raises CticpError after the call when an item fails (.statuses: every item's status)."""
+        B = len(odometries)
+        for name, lst in (("scans", scans), ("frame_ids", frame_ids), ("initial_estimates", initial_estimates),
+                          ("motion_models", motion_models)):
+            if lst is not None and len(lst) != B:
+                raise ValueError(f"{name} has {len(lst)} entries for {B} odometries")
+        items = (abi.BatchFrame * max(B, 1))()
+        outs = [abi.Summary() for _ in range(B)]
+        keep = []   # every buffer the items point to, alive until the call returns
+        for i, (od, scan) in enumerate(zip(odometries, scans)):
+            it = items[i]
+            it.handle = od.h.value if od.h else None
+            it.frame_id = int(frame_ids[i])
+            it.staged_slot = -1
+            if isinstance(scan, (int, np.integer)):
+                it.kind = abi.BATCH_STAGED
+                it.staged_slot = int(scan)
+            else:
+                xyz, ts = scan
+                if _is_cuda_tensor(xyz) or _is_cuda_tensor(ts):
+                    dscan, stream = od._device_scan(xyz, ts)
+                    keep.append(dscan)
+                    it.kind = abi.BATCH_DEVICE
+                    it.device_scan = C.addressof(dscan)
+                    it.stream = stream or None
+                else:
+                    xyz = np.asarray(xyz)
+                    if xyz.dtype != np.float64 or xyz.ndim != 2 or xyz.shape[1] < 3 or xyz.strides[1] != 8:
+                        xyz = np.ascontiguousarray(xyz[:, :3], dtype=np.float64)
+                    ts = np.ascontiguousarray(ts, dtype=np.float64).reshape(-1)
+                    if len(xyz) != len(ts):
+                        raise ValueError("xyz and timestamps must have the same length")
+                    keep += [xyz, ts]
+                    it.kind = abi.BATCH_HOST
+                    it.xyz, it.xyz_stride_bytes = xyz.ctypes.data, xyz.strides[0]
+                    it.t, it.t_stride_bytes, it.n = ts.ctypes.data, ts.strides[0], len(xyz)
+            if initial_estimates is not None and initial_estimates[i] is not None:
+                it.initial_estimate = C.addressof(initial_estimates[i])
+            if motion_models is not None and motion_models[i] is not None:
+                it.motion_model = C.addressof(motion_models[i])
+            it.out = C.addressof(outs[i])
+        rc = self.fn("odometry_register_batch")(items, B)
+        if rc < 0:
+            msg = self.fn("last_error")()
+            raise CticpError(rc, msg.decode("utf-8", "replace") if msg else "", [items[i].status for i in range(B)])
+        return outs
 
     # ---- sampling ------------------------------------------------------------------------------------------
     def grid_sample_indices(self, xyz, voxel_size, device=0):
@@ -427,8 +483,12 @@ class Odometry:
 
     # ---- device memory in and out (engine only) ----------------------------------------------------------------
     def _register_tensors(self, xyz, timestamps, frame_id, initial_estimate, motion_model):
-        """xyz: (N, >=3) float32 / float64 CUDA tensor with unit column stride (an (N, 4) xyzi tensor is read in place);
-        timestamps: 1-D CUDA tensor of any supported dtype and stride. Both on the handle's device; the scan is read after
+        scan, stream = self._device_scan(xyz, timestamps)
+        return self.register_device(scan, frame_id, initial_estimate, motion_model, stream=stream)
+
+    def _device_scan(self, xyz, timestamps):
+        """(abi.DeviceScan, producer stream) of a tensor scan. xyz: (N, >=3) float32 / float64 CUDA tensor with unit
+        column stride (an (N, 4) xyzi tensor is read in place); timestamps: 1-D CUDA tensor of any supported dtype and stride. Both on the handle's device; the scan is read after
         the work already queued on torch's current stream of that device."""
         import torch
         if not (_is_cuda_tensor(xyz) and _is_cuda_tensor(timestamps)):
@@ -445,8 +505,7 @@ class Odometry:
         scan = abi.DeviceScan(xyz.data_ptr(), xyz.stride(0) * xyz.element_size(), timestamps.data_ptr(),
                               timestamps.stride(0) * timestamps.element_size(), xyz.shape[0], codes[xyz.dtype],
                               codes[timestamps.dtype])
-        return self.register_device(scan, frame_id, initial_estimate, motion_model,
-                                    stream=torch.cuda.current_stream(self.device).cuda_stream)
+        return scan, torch.cuda.current_stream(self.device).cuda_stream
 
     def register_device(self, scan, frame_id, initial_estimate=None, motion_model=None, stream=0):
         """cticp_odometry_register_device on an abi.DeviceScan (any record layout); stream: the producer's cudaStream_t."""

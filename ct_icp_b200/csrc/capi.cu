@@ -92,6 +92,7 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_device_timing") return sizeof(cticp_device_timing);
     if (s == "cticp_adaptive_options") return sizeof(cticp_adaptive_options);
     if (s == "cticp_device_scan") return sizeof(cticp_device_scan);
+    if (s == "cticp_batch_frame") return sizeof(cticp_batch_frame);
     return 0;
 }
 
@@ -485,6 +486,69 @@ int cticp_odometry_register_staged(cticp_odometry *h, int64_t slot, uint32_t fra
         h->engine->RegisterStaged(slot, frame_id, out_summary);
         return (int) CTICP_OK;
     });
+}
+int cticp_odometry_register_batch(cticp_batch_frame *items, size_t batch) {
+    std::vector<BatchItem> work;
+    int rc = Guard([&] {
+        if (!items || batch < 1 || batch > 64) throw std::invalid_argument("batch must hold 1 to 64 items");
+        for (size_t i = 0; i < batch; ++i) {
+            const cticp_batch_frame &it = items[i];
+            const std::string at = "batch item " + std::to_string(i) + ": ";
+            if (!it.handle || !it.handle->engine || !it.out) throw std::invalid_argument(at + "null handle or summary");
+            if (it.kind == CTICP_BATCH_HOST) {
+                if (!it.xyz || !it.t) throw std::invalid_argument(at + "null scan pointer");
+            } else if (it.kind == CTICP_BATCH_DEVICE) {
+                if (!it.device_scan) throw std::invalid_argument(at + "null device scan");
+            } else if (it.kind == CTICP_BATCH_STAGED) {
+                if (it.initial_estimate || it.motion_model)
+                    throw std::invalid_argument(at + "a staged slot takes no initial estimate and no motion model");
+            } else
+                throw std::invalid_argument(at + "unknown kind");
+            for (size_t j = 0; j < i; ++j)
+                if (items[j].handle == it.handle) throw std::invalid_argument(at + "the same handle twice");
+            if (it.handle->engine->Device() != items[0].handle->engine->Device())
+                throw std::invalid_argument(at + "handles on different devices");
+        }
+        for (size_t i = 0; i < batch; ++i)
+            if (items[i].handle->engine->ShardingMode() != 0)
+                throw UnsupportedError("batch item " + std::to_string(i) + ": a sharded handle cannot join a batch");
+        work.resize(batch);
+        for (size_t i = 0; i < batch; ++i) {
+            const cticp_batch_frame &it = items[i];
+            BatchItem &w = work[i];
+            w.engine = it.handle->engine;
+            w.kind = it.kind;
+            if (it.kind == CTICP_BATCH_HOST) {
+                w.scan.xyz = it.xyz; w.scan.xyz_stride = it.xyz_stride_bytes; w.scan.t = it.t; w.scan.t_stride = it.t_stride_bytes;
+                w.scan.n = it.n;
+            } else if (it.kind == CTICP_BATCH_DEVICE) {
+                const cticp_device_scan *d = it.device_scan;
+                w.scan.xyz = d->xyz; w.scan.xyz_stride = d->xyz_stride_bytes; w.scan.xyz_dtype = d->xyz_dtype;
+                w.scan.t = d->t; w.scan.t_stride = d->t_stride_bytes; w.scan.t_dtype = d->t_dtype;
+                w.scan.n = (size_t) d->num_points;
+                w.producer = static_cast<cudaStream_t>(it.stream);
+            }
+            w.slot = it.staged_slot;
+            w.frame_id = it.frame_id;
+            w.initial_estimate = it.initial_estimate;
+            w.motion_model = it.motion_model;
+            w.out = it.out;
+        }
+        return (int) CTICP_OK;
+    });
+    if (rc < 0) return rc;
+    RegisterBatch(work);
+    // every item's status; the message of the first failing one is left in cticp_last_error (set last)
+    int first = CTICP_OK;
+    for (size_t i = batch; i-- > 0;) {
+        items[i].status = CTICP_OK;
+        if (work[i].error) {
+            const std::exception_ptr e = work[i].error;
+            items[i].status = Guard([&]() -> int { std::rethrow_exception(e); });
+            first = items[i].status;
+        }
+    }
+    return first;
 }
 int cticp_odometry_clear_staged(cticp_odometry *h) {
     return Guard([&] {

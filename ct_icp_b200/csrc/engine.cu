@@ -150,6 +150,7 @@ Engine::Engine(const cticp_odometry_options &options, int device) : options_(opt
     CT_CUDA_CHECK(cudaHostGetDevicePointer((void **) &h_verdict_dev_, h_verdict_, 0));
     CT_CUDA_CHECK(cudaStreamCreateWithFlags(&aux_stream_, cudaStreamNonBlocking));
     CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_state_up_, cudaEventDisableTiming));
+    CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_group_done_, cudaEventDisableTiming));
     CT_CUDA_CHECK(cudaMalloc(&d_kp_world_, sizeof(double) * 3 * max_pts));
     for (auto &e : ev_) CT_CUDA_CHECK(cudaEventCreate(&e));
     for (auto &e : timer_ev_) CT_CUDA_CHECK(cudaEventCreate(&e));
@@ -170,6 +171,7 @@ Engine::~Engine() {
     cudaFree(d_verdict_);
     cudaFreeHost(h_verdict_);
     if (ev_state_up_) cudaEventDestroy(ev_state_up_);
+    if (ev_group_done_) cudaEventDestroy(ev_group_done_);
     if (aux_stream_) cudaStreamDestroy(aux_stream_);
     cudaFree(d_kp_world_);
     for (auto &e : ev_) cudaEventDestroy(e);
@@ -342,7 +344,7 @@ void Engine::IngestImpl(const ScanView &scan, const FrameInfo &info, int64_t sta
     }
     if (n > pipe_->MaxPoints()) throw CapacityError("scan has more points than max_points_per_frame");
 
-    // host buffers were packed and their H2D copy enqueued by PackAndUpload (RegisterCommon) before the pose pair existed
+    // host buffers were packed and their H2D copy enqueued by PackAndUpload (PrepareFrame) before the pose pair existed
     if (staged_slot >= 0) pipe_->UploadFromDevice(staged_[staged_slot].d_points, staged_[staged_slot].d_lo, n);   // already packed, already in HBM: read in place
     timing_.h2d_bytes += pipe_->h2d_bytes();
     const double sample_size = k < options_.init_num_frames ? options_.init_voxel_size : options_.voxel_size;
@@ -792,10 +794,18 @@ void Engine::FlushL2(size_t bytes) {
     CT_CUDA_CHECK(cudaMemsetAsync(d_flush_, 0x5A, bytes, stream_));
 }
 
-// TryRegister, odometry.cpp:525-601
+// TryRegister, odometry.cpp:525-601, in three parts: the work up to the ICP launch, the launch, the work after it
 void Engine::TryRegister(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
                          const MotionModel *mm, int attempt_idx) {
     NvtxRange range("cticp.icp");
+    TryRegisterBegin(info, options, rs, sample_voxel_size, mm, attempt_idx);
+    LaunchIcp(options);
+    TryRegisterEnd(info, options, rs);
+}
+
+// sampling, the registration state to the device, ev_[1]
+void Engine::TryRegisterBegin(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
+                              const MotionModel *mm, int attempt_idx) {
     const int k = info.registered_fid;
     const bool at_startup = k < options_.init_num_frames;
     auto t0 = hclock::now();
@@ -848,11 +858,16 @@ void Engine::TryRegister(const FrameInfo &info, cticp_icp_options &options, Summ
     } else
         CT_CUDA_CHECK(cudaMemcpyAsync(d_state_, h_state_, sizeof(IcpState), cudaMemcpyHostToDevice, stream_));
     CT_CUDA_CHECK(cudaEventRecord(ev_[1], stream_));
+    if (tail_armed_) tail_in_.seq = ++verdict_seq_;
+}
+
+// the solo ICP launch between ev_[1] and ev_[2]
+void Engine::LaunchIcp(const cticp_icp_options &options) {
     icp_->set_keypoints_lo(pipe_->d_keypoints_lo());
     FrameTailArgs tail{};
-    bool verdict_by_icp_kernel = false;
+    verdict_by_icp_kernel_ = false;
+    timing_.icp_batch_groups = 1;
     if (tail_armed_) {
-        tail_in_.seq = ++verdict_seq_;
         tail.in = tail_in_;
         tail.counts = pipe_->d_counts();
         tail.dv = d_verdict_;
@@ -861,7 +876,7 @@ void Engine::TryRegister(const FrameInfo &info, cticp_icp_options &options, Summ
     }
     switch (options.solver) {
         case CTICP_SOLVER_GN:
-            verdict_by_icp_kernel =
+            verdict_by_icp_kernel_ =
                 icp_->EnqueueGaussNewton(*map_, options, pipe_->d_keypoints(), pipe_->d_count_keypoints(), KeypointHint(),
                                          options.num_iters_icp, d_state_, shard_rank_, shard_world_, nccl_comm_,
                                          (tail_armed_ && tail_in_kernel_) ? &tail : nullptr);
@@ -876,11 +891,29 @@ void Engine::TryRegister(const FrameInfo &info, cticp_icp_options &options, Summ
             throw UnsupportedError("Unsupported Solver Type");
     }
     CT_CUDA_CHECK(cudaEventRecord(ev_[2], stream_));
+}
+
+GnProblem Engine::IcpProblem(const PendingFrame &f) const {
+    return GnProblem{map_.get(), &f.icp_options, pipe_->d_keypoints(), pipe_->d_keypoints_lo(), pipe_->d_count_keypoints(),
+                     KeypointHint(), f.icp_options.num_iters_icp, d_state_};
+}
+
+void Engine::AdoptGroupedIcp(PendingFrame &f, cudaEvent_t launched, int groups) {
+    CT_CUDA_CHECK(cudaSetDevice(device_));
+    CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, launched, 0));
+    CT_CUDA_CHECK(cudaEventRecord(ev_[2], stream_));
+    verdict_by_icp_kernel_ = false;
+    timing_.icp_batch_groups = groups;
+    f.icp_launched = true;
+}
+
+// the verdict or the state back to the host, the registration summary
+void Engine::TryRegisterEnd(const FrameInfo &info, const cticp_icp_options &options, Summary &rs) {
     if (tail_armed_) {
         // device tail (frame_policy.h): verdict + speculative map update behind the ICP kernel; the host waits for the
         // verdict's sequence number in mapped pinned memory, not for the stream
         tail_armed_ = false;
-        if (!verdict_by_icp_kernel) {   // (k_gn_persistent's solver CTA writes the verdict itself)
+        if (!verdict_by_icp_kernel_) {   // (k_gn_persistent's solver CTA writes the verdict itself)
             k_frame_policy<<<1, 32, 0, stream_>>>(d_state_, pipe_->d_counts(), tail_in_, d_verdict_, h_verdict_dev_);
             CT_CUDA_CHECK(cudaGetLastError());
             tail_launches_ += 1;
@@ -905,6 +938,7 @@ void Engine::TryRegister(const FrameInfo &info, cticp_icp_options &options, Summ
     staging_in_flight_ = false;
     icp_->CollectGatherTiming();
     timing_.h2d_bytes += sizeof(IcpState);
+    const IcpState &S = *h_state_;
 
     if (getenv("CTICP_DEBUG_TIMERS"))
         fprintf(stderr, "[cticp] GN loop, solver CTA (SM cycles over %d iterations, needs a -DCTICP_DEBUG_TIMERS build): loop %llu, "
@@ -1145,8 +1179,14 @@ void Engine::UpdateMap(Summary &s, int registered_fid) {
 // RegisterFrame / RegisterFrameWithEstimate (odometry.cpp:199-236) → DoRegister (:386-501)
 void Engine::RegisterFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate,
                            cticp_summary *out, const cticp_motion_prior *motion_model) {
+    PendingFrame f;
+    BeginFrame(scan, frame_id, initial_estimate, out, motion_model, f);
+    CompleteFrame(f);
+}
+void Engine::BeginFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate, cticp_summary *out,
+                        const cticp_motion_prior *motion_model, PendingFrame &f) {
     if (scan.n == 0 || !scan.xyz || !scan.t) throw std::invalid_argument("The registered frame cannot be empty");
-    RegisterCommon(scan, frame_id, initial_estimate, -1, out, motion_model);
+    PrepareFrame(scan, frame_id, initial_estimate, -1, out, motion_model, f);
 }
 
 // IterateOverCallbacks, odometry.cpp:742-750. The hook may fetch the frame / the keypoints (GetPoints) under the pose pair
@@ -1160,21 +1200,44 @@ void Engine::FireEvent(int event, const Summary &rs, const FrameInfo &info) {
     if (!callback_(event, callback_user_)) throw CallbackError("Callback returned false");
 }
 void Engine::RegisterStaged(int64_t slot, uint32_t frame_id, cticp_summary *out) {
+    PendingFrame f;
+    BeginStaged(slot, frame_id, out, f);
+    CompleteFrame(f);
+}
+void Engine::BeginStaged(int64_t slot, uint32_t frame_id, cticp_summary *out, PendingFrame &f) {
     if (slot < 0 || slot >= (int64_t) staged_.size()) throw std::invalid_argument("unknown staged slot");
     ScanView none;
     none.n = staged_[slot].n;
-    RegisterCommon(none, frame_id, nullptr, slot, out);
+    PrepareFrame(none, frame_id, nullptr, slot, out, nullptr, f);
 }
 
-void Engine::RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate,
-                            int64_t staged_slot, cticp_summary *out, const cticp_motion_prior *motion_model) {
+void Engine::CompleteFrame(PendingFrame &f) {
+    if (f.icp_pending && !f.icp_launched) {
+        LaunchIcp(f.icp_options);
+        f.icp_launched = true;
+    }
+    FinishFrame(f);
+}
+
+const Engine::MotionModel *Engine::ModelOf(const PendingFrame &f) const {
+    return f.caller_model.present ? &f.caller_model : f.default_model ? &default_motion_model_ : nullptr;
+}
+
+// Phase 1 of a frame: ingest, motion initialisation, arming the device tail, sampling, the state upload. A plain
+// registration stops before its ICP launch (f.icp_pending); a robust one runs its attempts here.
+void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate,
+                          int64_t staged_slot, cticp_summary *out, const cticp_motion_prior *motion_model, PendingFrame &f) {
     const size_t n = scan.n;
-    auto t_start = hclock::now();
+    f = PendingFrame{};
+    f.n = n;
+    f.out = out;
+    f.t_start = hclock::now();
+    const auto t_start = f.t_start;
     CT_CUDA_CHECK(cudaSetDevice(device_));
     if (n > pipe_->MaxPoints()) throw CapacityError("scan has more points than max_points_per_frame");
     memset(&timing_, 0, sizeof(timing_));
     icp_->reset_timing();
-    const int launches0 = map_->launches() + pipe_->launches() + icp_->launches() + tail_launches_;
+    f.launches0 = map_->launches() + pipe_->launches() + icp_->launches() + tail_launches_;
     tail_armed_ = tail_launched_ = false;
     keypoints_in_summary_ = false;
     last_all_world_valid_ = last_kp_world_valid_ = frame_world_valid_ = false;
@@ -1186,7 +1249,7 @@ void Engine::RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp
     scan_in_staging_ = staged_slot < 0 && !scan.on_device;
 
     // compute_frame_info, odometry.cpp:186-196
-    FrameInfo info;
+    FrameInfo &info = f.info;
     double t_pack = 0;
     if (staged_slot >= 0) {
         info.begin_timestamp = staged_[staged_slot].t_min;
@@ -1236,35 +1299,32 @@ void Engine::RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp
 
     if (staged_slot >= 0) CT_CUDA_CHECK(cudaEventRecord(ev_[0], stream_));
     IngestImpl(scan, info, staged_slot);
-    const double t_initialization = ms_since(t_start);
+    f.t_initialization = ms_since(t_start);
 
-    Summary summary;
+    Summary &summary = f.summary;
     summary.frame = trajectory_.back();
     summary.initial_frame = summary.frame;
-    bool early_return = false;
-    bool ran_icp = false;
     if (k > 0) {
-        const MotionModel *mm = nullptr;
-        MotionModel caller_model;
         if (motion_model) {   // the caller's AMotionModel* (a PreviousFrameMotionModel in its current state)
-            caller_model.present = true;
-            caller_model.options = motion_model->options;
-            caller_model.previous_frame = FrameFromC(motion_model->previous_frame);
-            mm = &caller_model;
+            f.caller_model.present = true;
+            f.caller_model.options = motion_model->options;
+            f.caller_model.previous_frame = FrameFromC(motion_model->previous_frame);
         } else if (options_.with_default_motion_model) {   // odometry.cpp:412-417
             default_motion_model_.present = true;
             default_motion_model_.options = options_.default_motion_model;
             default_motion_model_.previous_frame = trajectory_[k - 1];
-            mm = &default_motion_model_;
+            f.default_model = true;
         }
-        ran_icp = true;
+        const MotionModel *mm = ModelOf(f);
+        f.ran_icp = true;
         if (options_.robust_registration) {
             RobustRegistration(info, summary, mm);
         } else {
-            cticp_icp_options ct_icp_options = options_.ct_icp_options;
+            cticp_icp_options &ct_icp_options = f.icp_options;
+            ct_icp_options = options_.ct_icp_options;
             const double sample_voxel_size = k < options_.init_num_frames ? options_.init_sample_voxel_size
                                                                           : options_.sample_voxel_size;
-            auto t0 = hclock::now();
+            f.t_try = hclock::now();
             // NB trajectory_[k] is still the INITIAL estimate here (odometry.cpp:429-431)
             const double relative_orientation =
                 angular_distance_deg(trajectory_[k - 1].end_pose.pose.q, trajectory_[k].end_pose.pose.q);
@@ -1291,9 +1351,38 @@ void Engine::RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp
                 in.room_for = (int) room;
                 tail_armed_ = true;
             }
-            TryRegister(info, ct_icp_options, summary, sample_voxel_size, mm, 0);
-            summary.t_try_register = ms_since(t0);
-            summary.relative_orientation = relative_orientation;
+            f.relative_orientation = relative_orientation;
+            NvtxRange range("cticp.icp");
+            TryRegisterBegin(info, ct_icp_options, summary, sample_voxel_size, mm, 0);
+            f.icp_pending = true;
+            // the frames whose ICP can run in a grouped launch (RegisterBatch): exactly those the solo launch would run
+            // through the persistent GN loop with the armed device tail
+            f.joins = tail_armed_ && ct_icp_options.solver == CTICP_SOLVER_GN && icp_->batch_supported() && !nccl_comm_ &&
+                      shard_world_ <= 1 && ct_icp_options.max_number_neighbors >= 1 && ct_icp_options.max_number_neighbors <= 32;
+        }
+    } else {
+        CT_CUDA_CHECK(cudaEventRecord(ev_[1], stream_));
+        CT_CUDA_CHECK(cudaEventRecord(ev_[2], stream_));
+        pipe_->QueueCountsReadback();
+    }
+}
+
+// Phase 3 of a frame, after its ICP launch: the verdict, the assessment, the map update, the summary.
+void Engine::FinishFrame(PendingFrame &f) {
+    CT_CUDA_CHECK(cudaSetDevice(device_));
+    const size_t n = f.n;
+    const auto t_start = f.t_start;
+    const FrameInfo &info = f.info;
+    const int k = info.registered_fid;
+    Summary &summary = f.summary;
+    bool &early_return = f.early_return;
+    const bool ran_icp = f.ran_icp;
+    cticp_summary *out = f.out;
+    if (k > 0) {
+        if (f.icp_pending) {
+            TryRegisterEnd(info, f.icp_options, summary);
+            summary.t_try_register = ms_since(f.t_try);
+            summary.relative_orientation = f.relative_orientation;
             summary.ego_orientation = EgoAngularDistance(summary.frame);
             summary.relative_distance = norm(summary.frame.end_pose.pose.t - summary.frame.begin_pose.pose.t);
             bool assessed = AssessRegistration(summary);
@@ -1304,10 +1393,6 @@ void Engine::RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp
             }
         }
         if (!early_return) trajectory_[k] = summary.frame;
-    } else {
-        CT_CUDA_CHECK(cudaEventRecord(ev_[1], stream_));
-        CT_CUDA_CHECK(cudaEventRecord(ev_[2], stream_));
-        pipe_->QueueCountsReadback();
     }
     last_frame_ = summary.frame;
     last_info_ = info;
@@ -1346,14 +1431,14 @@ void Engine::RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp
         staging_in_flight_ = false;
     }
 
-    timing_.kernel_launches = map_->launches() + pipe_->launches() + icp_->launches() + tail_launches_ - launches0;
+    timing_.kernel_launches = map_->launches() + pipe_->launches() + icp_->launches() + tail_launches_ - f.launches0;
     if (out) {
         FillSummary(summary, out);
         out->num_all_corrected_points = n;
         out->num_corrected_points = (uint64_t) pipe_->h_counts()[1];
         out->num_keypoints = (ran_icp && keypoints_in_summary_) ? (uint64_t) pipe_->h_counts()[2] : 0;
         out->odometry_total = ms_since(t_start);
-        out->odometry_initialization = t_initialization;
+        out->odometry_initialization = f.t_initialization;
         out->odometry_try_register = summary.t_try_register;
         out->odometry_duration_sampling = summary.t_sampling;
         out->odometry_map_update = ms_since(t_before_map);
@@ -1447,6 +1532,12 @@ uint64_t SpanBytes(uint64_t n, uint64_t stride, uint64_t width, const char *what
 
 void Engine::RegisterDevice(ScanView scan, cudaStream_t producer, uint32_t frame_id, const cticp_frame *initial_estimate,
                             cticp_summary *out, const cticp_motion_prior *motion_model) {
+    PendingFrame f;
+    BeginDevice(scan, producer, frame_id, initial_estimate, out, motion_model, f);
+    CompleteFrame(f);
+}
+void Engine::BeginDevice(ScanView scan, cudaStream_t producer, uint32_t frame_id, const cticp_frame *initial_estimate,
+                         cticp_summary *out, const cticp_motion_prior *motion_model, PendingFrame &f) {
     CT_CUDA_CHECK(cudaSetDevice(device_));
     if (scan.n == 0 || !scan.xyz || !scan.t) throw std::invalid_argument("The registered frame cannot be empty");
     if (scan.xyz_dtype != CTICP_DTYPE_FLOAT32 && scan.xyz_dtype != CTICP_DTYPE_FLOAT64)
@@ -1459,7 +1550,7 @@ void Engine::RegisterDevice(ScanView scan, cudaStream_t producer, uint32_t frame
     RequireDeviceRange(scan.t, SpanBytes(scan.n, scan.t_stride, tsz, "t"), device_, "t");
     scan.on_device = true;
     scan.producer = producer;
-    RegisterCommon(scan, frame_id, initial_estimate, -1, out, motion_model);
+    PrepareFrame(scan, frame_id, initial_estimate, -1, out, motion_model, f);
 }
 
 void Engine::CheckSink(const cticp_cloud_sink &sink) const {

@@ -6,7 +6,9 @@
 #pragma once
 #include <algorithm>
 #include <atomic>
+#include <chrono>
 #include <condition_variable>
+#include <exception>
 #include <functional>
 #include <memory>
 #include <mutex>
@@ -95,9 +97,67 @@ private:
 };
 
 class Engine {
+    struct FrameInfo {
+        int registered_fid = -1;
+        uint32_t frame_id = uint32_t(-1);
+        double begin_timestamp = -1, end_timestamp = -1;
+    };
+    struct Summary {   // RegistrationSummary minus the point vectors
+        HostFrame frame, initial_frame;
+        int sample_size = 0, number_of_residuals = 0, robust_level = 0;
+        double distance_correction = 0, relative_distance = 0, relative_orientation = 0, ego_orientation = 0;
+        bool success = true, points_added = false;
+        int number_of_attempts = 0;
+        std::string error_message;
+        cticp_icp_summary icp{};
+        double t_try_register = 0, t_sampling = 0;
+    };
+    struct MotionModel {
+        bool present = false;
+        cticp_motion_model_options options{};
+        HostFrame previous_frame;
+    };
+
 public:
     Engine(const cticp_odometry_options &options, int device);
     ~Engine();
+
+    // A frame between the three phases every registration goes through: Begin* (ingest, motion initialisation, arming
+    // the device tail, sampling, the state upload; a robust registration runs its attempts here), the ICP launch (solo:
+    // LaunchIcp; or a grouped launch shared with other handles, RegisterBatch), FinishFrame (verdict, map update,
+    // summary). RegisterFrame / RegisterDevice / RegisterStaged run them back to back.
+    struct PendingFrame {
+        size_t n = 0;
+        cticp_summary *out = nullptr;
+        std::chrono::steady_clock::time_point t_start, t_try;
+        double t_initialization = 0, relative_orientation = 0;
+        FrameInfo info;
+        Summary summary;
+        MotionModel caller_model;
+        bool default_model = false;   // the handle's default motion model applies (caller_model absent)
+        int launches0 = 0;
+        cticp_icp_options icp_options{};
+        bool ran_icp = false, early_return = false;
+        bool icp_pending = false;     // a plain registration waits for its ICP launch and its TryRegisterEnd
+        bool icp_launched = false;
+        bool joins = false;           // its ICP may run in a grouped launch (solver GN, persistent loop, armed device tail)
+    };
+    void BeginFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate, cticp_summary *out,
+                    const cticp_motion_prior *motion_model, PendingFrame &f);
+    void BeginDevice(ScanView scan, cudaStream_t producer, uint32_t frame_id, const cticp_frame *initial_estimate,
+                     cticp_summary *out, const cticp_motion_prior *motion_model, PendingFrame &f);
+    void BeginStaged(int64_t slot, uint32_t frame_id, cticp_summary *out, PendingFrame &f);
+    // the solo launch when still pending, then FinishFrame
+    void CompleteFrame(PendingFrame &f);
+    // a joining frame's registration in a grouped launch (valid until FinishFrame)
+    GnProblem IcpProblem(const PendingFrame &f) const;
+    // recorded on the engine's stream after the state upload and the sampling of the pending frame
+    cudaEvent_t IcpReadyEvent() const { return ev_[1]; }
+    // the grouped launch that ran the pending frame's ICP is enqueued, `launched` recorded behind it; `groups` problems
+    void AdoptGroupedIcp(PendingFrame &f, cudaEvent_t launched, int groups);
+    void FinishFrame(PendingFrame &f);
+    // recorded behind a grouped launch this engine's stream carried (RegisterBatch)
+    cudaEvent_t GroupDoneEvent() const { return ev_group_done_; }
 
     void RegisterFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate, cticp_summary *out,
                        const cticp_motion_prior *motion_model = nullptr);
@@ -134,27 +194,6 @@ public:
     int ShardingMode() const { return shard_world_ <= 1 ? 0 : (icp_ && icp_->peers_ready() ? 2 : 1); }
 
 private:
-    struct FrameInfo {
-        int registered_fid = -1;
-        uint32_t frame_id = uint32_t(-1);
-        double begin_timestamp = -1, end_timestamp = -1;
-    };
-    struct Summary {   // RegistrationSummary minus the point vectors
-        HostFrame frame, initial_frame;
-        int sample_size = 0, number_of_residuals = 0, robust_level = 0;
-        double distance_correction = 0, relative_distance = 0, relative_orientation = 0, ego_orientation = 0;
-        bool success = true, points_added = false;
-        int number_of_attempts = 0;
-        std::string error_message;
-        cticp_icp_summary icp{};
-        double t_try_register = 0, t_sampling = 0;
-    };
-    struct MotionModel {
-        bool present = false;
-        cticp_motion_model_options options{};
-        HostFrame previous_frame;
-    };
-
     void InitializeMotion(const FrameInfo &info, const cticp_frame *initial_estimate);
     void ResolvePoints(int which, const float4 **out_pts, const float4 **out_lo, const double **out_world, size_t *out_count);
     void CheckSink(const cticp_cloud_sink &sink) const;
@@ -169,8 +208,9 @@ private:
     void MinMaxTimestamps(const ScanView &scan, double *mn_out, double *mx_out);
     std::unique_ptr<HostPool> pool_;
     static int HostTeamSize(int ranks_on_node);
-    void RegisterCommon(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate,
-                        int64_t staged_slot, cticp_summary *out, const cticp_motion_prior *motion_model = nullptr);
+    void PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate, int64_t staged_slot,
+                      cticp_summary *out, const cticp_motion_prior *motion_model, PendingFrame &f);
+    const MotionModel *ModelOf(const PendingFrame &f) const;
     void FireEvent(int event, const Summary &rs, const FrameInfo &info);
     cticp_event_fn callback_ = nullptr;
     void *callback_user_ = nullptr;
@@ -190,6 +230,11 @@ private:
     size_t flush_bytes_ = 0;
     void TryRegister(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
                      const MotionModel *mm, int attempt_idx);
+    void TryRegisterBegin(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
+                          const MotionModel *mm, int attempt_idx);
+    void LaunchIcp(const cticp_icp_options &options);
+    void TryRegisterEnd(const FrameInfo &info, const cticp_icp_options &options, Summary &rs);
+    bool verdict_by_icp_kernel_ = false;   // the last ICP launch decided the frame's tail itself (CTICP_TAIL_IN_KERNEL)
     bool AssessRegistration(Summary &s) const;
     void RobustRegistration(const FrameInfo &info, Summary &rs, const MotionModel *mm);
     void ComputeSummaryMetrics(Summary &s, int k);
@@ -214,6 +259,7 @@ private:
     // the registration state goes up on a second stream while the sampler runs (the ICP kernel waits for its event)
     cudaStream_t aux_stream_ = nullptr;
     cudaEvent_t ev_state_up_ = nullptr;
+    cudaEvent_t ev_group_done_ = nullptr;
     void FillSummary(const Summary &s, cticp_summary *out) const;
     // grid-size hint for the ICP kernels: the keypoint count is only known on the device when they are enqueued, so
     // the host sizes the grid from the previous registration (keypoint counts change slowly) with 25% head-room;
@@ -279,6 +325,23 @@ private:
     void *d_mailbox_ = nullptr;
     std::vector<void *> peer_mapped_;
 };
+
+// One frame of RegisterBatch (odometry_batch.cu): the arguments of the single-frame entry `kind` (CTICP_BATCH_*) names
+struct BatchItem {
+    Engine *engine = nullptr;
+    int kind = CTICP_BATCH_HOST;
+    ScanView scan;                 // HOST, DEVICE (scan.n: the staged slot's size is looked up by the engine)
+    cudaStream_t producer = nullptr;
+    int64_t slot = -1;
+    uint32_t frame_id = 0;
+    const cticp_frame *initial_estimate = nullptr;
+    const cticp_motion_prior *motion_model = nullptr;
+    cticp_summary *out = nullptr;
+    std::exception_ptr error;      // out: what the item's single-frame call would have thrown
+};
+// One frame on each engine (all distinct, one device, none sharded), their eligible GN loops in one grouped launch
+// (cticp_odometry_register_batch has the contract). A failing item ends alone with its exception in `error`.
+void RegisterBatch(std::vector<BatchItem> &items);
 
 // conversions shared with capi.cu
 HostPose PoseFromC(const cticp_pose &c);

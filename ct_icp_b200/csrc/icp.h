@@ -94,6 +94,19 @@ void BatchGatherCtas(const size_t *n, int batch, int coresident, int kp_per_cta,
 
 struct FrameTailArgs;   // frame_policy.h
 
+// One registration of a grouped Gauss-Newton launch (IcpSolver::EnqueueGaussNewtonGroups)
+struct GnProblem {
+    const DeviceMap *map;
+    const cticp_icp_options *opt;
+    const float4 *keypoints;
+    const float4 *keypoints_lo;     // residual plane of the keypoints (nullptr: none; se3.cuh load_raw)
+    const int *d_num_keypoints;     // device keypoint count; nullptr: exactly n keypoints
+    size_t n;                       // the keypoint count, or with d_num_keypoints the estimate a solo launch sizes its grid
+                                    // from (EnqueueGaussNewton's k_upper)
+    int num_iters;
+    IcpState *d_state;
+};
+
 class IcpSolver {
 public:
     explicit IcpSolver(cudaStream_t stream);
@@ -110,12 +123,17 @@ public:
                             const FrameTailArgs *tail = nullptr);
 
     // B independent Gauss-Newton registrations against `map` with shared options, in ONE launch of the persistent kernel
-    // (k_gn_persistent over groups). Problem b's h_n[b] keypoints are at [kp_base_b, kp_base_b + h_n[b]) of d_keypoints,
-    // kp_base_b = h_n[0] + … + h_n[b - 1] (the residual plane, when set_keypoints_lo gave one, alike); its state is
-    // d_states[b]. CTA policy and its bit-identity contract: BatchGatherCtas (icp_batch.cu). Throws CapacityError when
-    // the device cannot hold two CTAs per problem; requires batch_supported().
+    // (EnqueueGaussNewtonGroups, every group on the same map). Problem b's h_n[b] keypoints are at
+    // [kp_base_b, kp_base_b + h_n[b]) of d_keypoints, kp_base_b = h_n[0] + … + h_n[b - 1] (the residual plane, when
+    // set_keypoints_lo gave one, alike); its state is d_states[b].
     void EnqueueGaussNewtonBatch(const DeviceMap &map, const cticp_icp_options &opt, int batch, const size_t *h_n,
                                  const float4 *d_keypoints, int num_iters, IcpState *d_states);
+    // B independent Gauss-Newton registrations, each with its own map, options, keypoints and iteration count, in ONE
+    // launch of the grouped persistent kernel (k_gn_persistent<false, true>) on this solver's stream, with this solver's
+    // loop words and group table. CTA policy and its bit-identity contract with the solo launch: BatchGatherCtas
+    // (icp_batch.cu) on the problems' n. Throws CapacityError when the device cannot hold two CTAs per problem;
+    // requires batch_supported(). The table is built on the host before this returns: `problems` may go afterwards.
+    void EnqueueGaussNewtonGroups(const GnProblem *problems, int batch);
     // the batch has no launch-per-iteration form (CTICP_PERSISTENT=0) and cannot use grid-wide barriers, which would
     // couple groups with different iteration counts (-DCTICP_GN_GRID_BARRIERS builds)
     bool batch_supported() const;
@@ -182,7 +200,7 @@ private:
     GnParams MakeParams(const DeviceMap &map, const cticp_icp_options &opt) const;
     int GnCoresident(bool peers);          // co-resident CTAs of k_gn_persistent<peers> on this device
     unsigned int ReserveLoopTags(int rows, int groups, int num_iters);   // k_gn_persistent's words and tags (icp_gn.cu)
-    // group table of a batched launch (first_cta | kp_base | count, BatchGatherCtas) built and uploaded to d_groups_;
+    // group table of a batched LM launch (first_cta | kp_base | count, BatchGatherCtas) built and uploaded to d_groups_;
     // returns the grid (icp_batch.cu)
     int UploadGroupTable(const size_t *h_n, int batch, int coresident);
     int LmCoresident(int variant, void *kernel);   // co-resident CTAs of a k_lm_persistent instantiation (icp_lm.cu)
@@ -201,9 +219,12 @@ private:
     unsigned long long *d_loop_pose_ = nullptr;   // k_gn_persistent: tagged pose words, one block per group (grow-only)
     int loop_rows_cap_ = 0, loop_groups_cap_ = 0;
     unsigned int loop_tag_ = 1;                   // next tag to hand out (never 0)
-    int *d_groups_ = nullptr;                // batched launches: first_cta | kp_base | keypoint counts (grow-only)
+    int *d_groups_ = nullptr;                // batched LM launches: first_cta | kp_base | keypoint counts (grow-only)
     int groups_cap_ = 0;                     // ints d_groups_ holds
     std::vector<int> h_groups_;
+    unsigned char *d_gn_table_ = nullptr;    // grouped GN launches: GnGroup table | first_cta | counts (grow-only)
+    size_t gn_table_cap_ = 0;
+    std::vector<unsigned char> h_gn_table_;
     // solver CERES (icp_lm.cu)
     void *d_lm_state_ = nullptr, *d_lm_stats_ = nullptr, *d_lm_blocks_ = nullptr;
     int *d_lm_sel_ = nullptr;

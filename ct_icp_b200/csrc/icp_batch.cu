@@ -1,5 +1,5 @@
-// icp_batch.cu — CTA policy of the persistent registration kernels and the group table of their batched launches
-// (EnqueueGaussNewtonBatch, icp_gn.cu; EnqueueCeresBatch, icp_lm.cu). Host code only.
+// icp_batch.cu — CTA policy of the persistent registration kernels (EnqueueGaussNewtonGroups, icp_gn.cu;
+// EnqueueCeresBatch, icp_lm.cu) and the group table of the batched LM launch. Host code only.
 #include <algorithm>
 #include <cstdint>
 #include <string>
@@ -30,7 +30,7 @@ int GatherBlocks(size_t k_hint, int max_blocks, int kp_per_cta) {
 // CTA policy of a batched persistent launch: gather[b] = the gather (GN) / worker (LM) CTAs of problem b (each problem also
 // has its solver CTA). Contract:
 //  - When every problem fits with what a solo call would give it — solo_b = GatherBlocks(n_b + 16, coresident - 1), the
-//    grid of EnqueueGaussNewton and of EnqueueCeres's persistent launch — and Σ (1 + solo_b) <= coresident,
+//    grid of EnqueueGaussNewton and of EnqueueCeres's persistent launch for n_b = k_upper / k_hint — and Σ (1 + solo_b) <= coresident,
 //    gather[b] = solo_b. Keypoint ranges, tiles and the order of every reduction are then those of the solo call: each
 //    problem's result is bit-identical to it.
 //  - Otherwise the coresident - batch CTAs left for gathering are dealt one at a time to the problem with the most keypoints

@@ -46,6 +46,16 @@ struct GatherLaunch {
     GnParams P;
 };
 
+// One registration of a grouped k_gn_persistent launch (GnGroups): everything a solo launch takes as kernel parameters.
+// Groups may search different maps with different options (the odometry's batch: one handle per group).
+struct GnGroup {
+    GatherLaunch cfg;            // map level, search and GN parameters; cfg.P.kp_lo: the group's residual plane
+    const float4 *keypoints;
+    const int *num_keypoints;    // device count
+    IcpState *st;
+    int num_iters;
+};
+
 __device__ __forceinline__ M3 euler_from_sincos(double sa, double ca, double sb, double cb, double sg, double cg) {
     M3 R;   // ct_icp.cpp:916-932
     R.m[0][0] = cg * cb; R.m[0][1] = -sg * ca + cg * sb * sa; R.m[0][2] = sg * sa + cg * sb * ca;
@@ -423,6 +433,7 @@ struct GnShared {
         unsigned long long *pose;   // the group's tagged pose words
         int gather_ctas;
     } grp;
+    GnGroup group;    // grouped k_gn_persistent: this CTA's entry of the group table
     unsigned long long mbar[kGatherWarps];   // -DCTICP_SEL_BULK: one mbarrier per warp for the bulk copies
 };
 
@@ -603,13 +614,13 @@ struct GnLoopWords {
     unsigned int tag;           // tag of iteration 0's rows; iteration it's rows and pose words carry tag + it
 };
 
-// The groups of one k_gn_persistent launch. Group g owns the CTAs [first_cta[g], first_cta[g + 1]) of the grid — the first
-// is g's solver CTA, the others gather g's keypoints — its keypoints [kp_base[g], kp_base[g] + count[g]) of the launch's
-// keypoint (and residual plane) array, the state st[g], the partial rows [first_cta[g] - g, first_cta[g + 1] - g - 1) and
-// its own pose words. Groups never wait on each other. `table` (device) = first_cta[0..B] | kp_base[0..B-1];
-// num_groups == 1: the whole grid is one group with its keypoints at index 0, and `table` is not read.
+// The groups of one grouped k_gn_persistent launch (k_gn_persistent<false, true>). Group g owns the CTAs
+// [first_cta[g], first_cta[g + 1]) of the grid — the first is g's solver CTA, the others gather g's keypoints — the
+// registration table[g], the partial rows [first_cta[g] - g, first_cta[g + 1] - g - 1) and its own pose words. Groups
+// never wait on each other. Both arrays are in device memory (IcpSolver::EnqueueGaussNewtonGroups).
 struct GnGroups {
-    const int *table;
+    const GnGroup *table;        // [num_groups]
+    const int *first_cta;        // [num_groups + 1]
     int num_groups;
 };
 
@@ -700,38 +711,46 @@ __device__ __forceinline__ void gn_fetch_pose(GnShared &sh, unsigned int tag, lo
 // into the instruction cache. With `tail.enabled` the solver CTA also decides the frame's tail after the loop
 // (frame_policy.h).
 //
-// Groups (GnGroups): one launch can run B independent registrations against the same map, each on its own contiguous range
-// of CTAs with its own solver CTA, state, partial rows and pose words; everything above holds per group. A group that
-// converges or fails leaves the loop alone while the others go on, and one group's serial tail overlaps the others'
-// gathers. The single registration (solo L3 call, odometry) is the one-group case; kPeers and the frame tail are single-group.
+// Groups (kGrouped, GnGroups): one launch runs B independent registrations, each on its own contiguous range of CTAs with
+// its own map, options, keypoints, iteration count, solver CTA, state, partial rows and pose words; everything above holds
+// per group. A group that converges or fails leaves the loop alone while the others go on, and one group's serial tail
+// overlaps the others' gathers. Each CTA copies its group's entry to shared memory and reads it from there; the solo
+// instantiation reads the same values from its kernel parameters and never the table. kPeers and the frame tail are solo.
 //
 // kPeers (multi-GPU, keypoints sharded): between its reduction and its solve the solver CTA exchanges the accumulator
 // with the other ranks' solver CTAs through NVLink peer memory (peer_exchange.cuh) — the all-reduce of SURVEY §8e
 // happens INSIDE the loop, so the sharded loop is still one launch and costs one NVLink round trip per iteration.
-template <bool kPeers>
+template <bool kPeers, bool kGrouped>
 __global__ void __launch_bounds__(kGatherWarps * 32, 1)
-k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const int *__restrict__ d_num_keypoints,
-                IcpState *st, int num_iters, PeerLinks links, GnLoopWords words, FrameTailArgs tail, GnGroups groups) {
+k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints, const int *__restrict__ d_num_keypoints,
+                IcpState *st, int solo_iters, PeerLinks links, GnLoopWords words, FrameTailArgs tail, GnGroups groups) {
+    static_assert(!(kPeers && kGrouped), "the sharded loop is single-group");
 #ifndef CTICP_GN_FLAG_SYNC
     cg::grid_group grid = cg::this_grid();
 #endif
     GnShared &sh = *reinterpret_cast<GnShared *>(gn_smem_raw);
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const GnParams &P = cfg.P;
     // this CTA's group (GnGroups): from here on the group is the whole registration — `cta` is the index within the
-    // group, `group_ctas` its size, and st / rows / pose words / the keypoint count are the group's own
-    int g = 0, cta = blockIdx.x, group_ctas = gridDim.x, kp_base = 0;
+    // group, `group_ctas` its size, and the state / rows / pose words / keypoints are the group's own
+    int g = 0, cta = blockIdx.x, group_ctas = gridDim.x;
     unsigned long long *rows = words.rows, *pose_words = words.pose;
-    if (groups.num_groups > 1) {
-        const int *first_cta = groups.table;
+    if constexpr (kGrouped) {
+        const int *first_cta = groups.first_cta;
         while (first_cta[g + 1] <= (int) blockIdx.x) ++g;
         cta = (int) blockIdx.x - first_cta[g];
         group_ctas = first_cta[g + 1] - first_cta[g];
-        kp_base = groups.table[groups.num_groups + 1 + g];
-        st += g;
         rows += (size_t) (first_cta[g] - g) * kRowWords;   // the gather CTAs of the groups before this one
         pose_words += (size_t) kPoseGroupWords * g;
+        const int *src = reinterpret_cast<const int *>(groups.table + g);
+        int *dst = reinterpret_cast<int *>(&sh.group);
+        for (int i = threadIdx.x; i < (int) (sizeof(GnGroup) / sizeof(int)); i += blockDim.x) dst[i] = src[i];
+        __syncthreads();
+        st = sh.group.st;
     }
+    const GatherLaunch &cfg = kGrouped ? sh.group.cfg : solo_cfg;
+    const float4 *__restrict__ keypoints = kGrouped ? sh.group.keypoints : solo_keypoints;
+    const GnParams &P = cfg.P;
+    const int num_iters = kGrouped ? sh.group.num_iters : solo_iters;
     const bool solver_cta = cta == 0;
     unsigned int peer_seq = 0;   // sequence number of the last exchange (solver CTA only)
     if (kPeers && solver_cta) peer_seq = *links.seq;
@@ -777,7 +796,7 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
     long long t_loop = 0, t_solve = 0;
     if (solver_cta && threadIdx.x == 0) t_loop = clock64();
     // this rank's keypoint range and the tile width: constant over the iterations (integer divisions)
-    const int K = d_num_keypoints[g];
+    const int K = kGrouped ? *sh.group.num_keypoints : *d_num_keypoints;
     int kp_lo = 0, kp_hi = K;
     if (P.shard_world > 1) {
         kp_lo = (int) ((long long) K * P.shard_rank / P.shard_world);
@@ -786,8 +805,8 @@ k_gn_persistent(GatherLaunch cfg, const float4 *__restrict__ keypoints, const in
     // this CTA's balanced share of the range
     int c_lo = 0, c_hi = 0;
     if (!solver_cta) {
-        c_lo = kp_base + kp_lo + (int) ((long long) (kp_hi - kp_lo) * (cta - 1) / gather_ctas);
-        c_hi = kp_base + kp_lo + (int) ((long long) (kp_hi - kp_lo) * cta / gather_ctas);
+        c_lo = kp_lo + (int) ((long long) (kp_hi - kp_lo) * (cta - 1) / gather_ctas);
+        c_hi = kp_lo + (int) ((long long) (kp_hi - kp_lo) * cta / gather_ctas);
     }
     for (int it = 0; it < num_iters; ++it) {
         const unsigned int tag = words.tag + (unsigned int) it;
@@ -1030,8 +1049,8 @@ void IcpSolver::SetPeerLinks(const PeerLinksHost &links) {
 }
 void IcpSolver::PreloadShardedKernels() {
     cudaFuncAttributes a;
-    cudaFuncGetAttributes(&a, k_gn_persistent<true>);
-    cudaFuncGetAttributes(&a, k_gn_persistent<false>);
+    cudaFuncGetAttributes(&a, k_gn_persistent<true, false>);
+    cudaFuncGetAttributes(&a, k_gn_persistent<false, false>);
     cudaFuncGetAttributes(&a, k_gn_iterate);
     cudaFuncGetAttributes(&a, k_peer_allreduce);
     cudaFuncGetAttributes(&a, k_gn_solve_acc);
@@ -1053,8 +1072,9 @@ IcpSolver::IcpSolver(cudaStream_t stream) : stream_(stream) {
     int dev = 0;
     cudaGetDevice(&dev);
     CT_CUDA_CHECK(cudaFuncSetAttribute(k_gn_iterate, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(GnShared)));
-    CT_CUDA_CHECK(cudaFuncSetAttribute(k_gn_persistent<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(GnShared)));
-    CT_CUDA_CHECK(cudaFuncSetAttribute(k_gn_persistent<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(GnShared)));
+    CT_CUDA_CHECK(cudaFuncSetAttribute(k_gn_persistent<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(GnShared)));
+    CT_CUDA_CHECK(cudaFuncSetAttribute(k_gn_persistent<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(GnShared)));
+    CT_CUDA_CHECK(cudaFuncSetAttribute(k_gn_persistent<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(GnShared)));
     cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, dev);
     CT_CUDA_CHECK(cudaMalloc(&d_sys_, sizeof(double) * 160));
     CT_CUDA_CHECK(cudaMalloc(&d_acc_, sizeof(double) * kAcc));
@@ -1073,6 +1093,7 @@ IcpSolver::~IcpSolver() {
     cudaFree(d_loop_rows_);
     cudaFree(d_loop_pose_);
     cudaFree(d_groups_);
+    cudaFree(d_gn_table_);
     FreeLmBuffers();
     for (int i = 0; i < kMaxEvents; ++i) {
         cudaEventDestroy(ev_begin_[i]);
@@ -1106,7 +1127,7 @@ GnParams IcpSolver::MakeParams(const DeviceMap &map, const cticp_icp_options &op
 int IcpSolver::GnCoresident(bool peers) {
     int &coresident = max_coresident_[peers ? 1 : 0];
     if (coresident == 0) {
-        void *kernel = peers ? (void *) k_gn_persistent<true> : (void *) k_gn_persistent<false>;
+        void *kernel = peers ? (void *) k_gn_persistent<true, false> : (void *) k_gn_persistent<false, false>;
         int per_sm = 0;
         CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGatherWarps * 32, sizeof(GnShared)));
         coresident = std::max(1, per_sm * num_sms_);
@@ -1151,31 +1172,80 @@ bool IcpSolver::batch_supported() const {
 
 void IcpSolver::EnqueueGaussNewtonBatch(const DeviceMap &map, const cticp_icp_options &opt, int batch, const size_t *h_n,
                                         const float4 *d_keypoints, int num_iters, IcpState *d_states) {
-    if (!batch_supported()) throw std::logic_error("batched Gauss-Newton needs the persistent flag-synchronised loop");
-    if (opt.max_number_neighbors > 32 || opt.max_number_neighbors < 1)
-        throw std::invalid_argument("max_number_neighbors must be in [1, 32]");
     if (batch < 1) throw std::invalid_argument("batch must be at least 1");
-    GatherLaunch cfg;
-    cfg.P = MakeParams(map, opt);
-    cfg.G.L = map.Level(cfg.P.level);
-    cfg.G.r = cfg.P.r;
-    cfg.G.radius2 = cfg.P.radius * cfg.P.radius;
-    cfg.G.kmax = cfg.P.kmax;
+    std::vector<GnProblem> problems(batch);
+    size_t base = 0;
+    for (int b = 0; b < batch; ++b) {
+        problems[b] = GnProblem{&map, &opt, d_keypoints + base, kp_lo_ ? kp_lo_ + base : nullptr, nullptr, h_n[b], num_iters,
+                                d_states + b};
+        base += h_n[b];
+    }
+    EnqueueGaussNewtonGroups(problems.data(), batch);
+}
+
+void IcpSolver::EnqueueGaussNewtonGroups(const GnProblem *problems, int batch) {
+    if (!batch_supported()) throw std::logic_error("batched Gauss-Newton needs the persistent flag-synchronised loop");
+    if (batch < 1) throw std::invalid_argument("batch must be at least 1");
+    for (int b = 0; b < batch; ++b)
+        if (problems[b].opt->max_number_neighbors > 32 || problems[b].opt->max_number_neighbors < 1)
+            throw std::invalid_argument("max_number_neighbors must be in [1, 32]");
+    // (k_gn_persistent<false, true> has the launch bounds and the shared memory of the solo kernel: the same occupancy)
     const int coresident = GnCoresident(false);
     if (2 * batch > coresident)
         throw CapacityError("batch of " + std::to_string(batch) + " registrations: the device holds " +
                                 std::to_string(coresident) + " CTAs of the Gauss-Newton kernel, two per registration needed");
-    const int grid = UploadGroupTable(h_n, batch, coresident);
-    const unsigned int tag = ReserveLoopTags(grid - batch, batch, num_iters);
+    // table: GnGroup[B] | first_cta[0..B] | the counts of the problems without a device count
+    std::vector<size_t> n(batch);
+    for (int b = 0; b < batch; ++b) n[b] = problems[b].n;
+    std::vector<int> gather(batch);
+    BatchGatherCtas(n.data(), batch, coresident, kp_per_cta_, gather.data());
+    const size_t cta_off = sizeof(GnGroup) * (size_t) batch, count_off = cta_off + sizeof(int) * (size_t) (batch + 1);
+    const size_t bytes = count_off + sizeof(int) * (size_t) batch;
+    if (bytes > gn_table_cap_) {
+        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+        cudaFree(d_gn_table_);
+        d_gn_table_ = nullptr;
+        CT_CUDA_CHECK(cudaMalloc(&d_gn_table_, bytes));
+        gn_table_cap_ = bytes;
+    }
+    h_gn_table_.assign(bytes, 0);
+    GnGroup *table = reinterpret_cast<GnGroup *>(h_gn_table_.data());
+    int *first_cta = reinterpret_cast<int *>(h_gn_table_.data() + cta_off);
+    int *count = reinterpret_cast<int *>(h_gn_table_.data() + count_off);
+    const int *d_count = reinterpret_cast<const int *>(d_gn_table_ + count_off);
+    int max_iters = 0;
+    for (int b = 0; b < batch; ++b) {
+        const GnProblem &p = problems[b];
+        if (p.n > (size_t) INT32_MAX) throw std::invalid_argument("too many keypoints in one problem");
+        GnGroup &e = table[b];
+        e.cfg.P = MakeParams(*p.map, *p.opt);
+        e.cfg.P.kp_lo = p.keypoints_lo;
+        e.cfg.G.L = p.map->Level(e.cfg.P.level);
+        e.cfg.G.r = e.cfg.P.r;
+        e.cfg.G.radius2 = e.cfg.P.radius * e.cfg.P.radius;
+        e.cfg.G.kmax = e.cfg.P.kmax;
+        e.keypoints = p.keypoints;
+        count[b] = (int) p.n;
+        e.num_keypoints = p.d_num_keypoints ? p.d_num_keypoints : d_count + b;
+        e.st = p.d_state;
+        e.num_iters = p.num_iters;
+        max_iters = std::max(max_iters, p.num_iters);
+        first_cta[b + 1] = first_cta[b] + 1 + gather[b];
+    }
+    const int grid = first_cta[batch];
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_gn_table_, h_gn_table_.data(), bytes, cudaMemcpyHostToDevice, stream_));
+    const unsigned int tag = ReserveLoopTags(grid - batch, batch, max_iters);
     GnLoopWords words{d_loop_rows_, d_loop_pose_, tag};
-    const float4 *kp = d_keypoints;
-    const int *nk = d_groups_ + 2 * batch + 1;
-    int iters = num_iters;
+    GatherLaunch cfg{};
+    const float4 *kp = nullptr;
+    const int *nk = nullptr;
+    IcpState *st = nullptr;
+    int iters = 0;
     PeerLinks links{};
     FrameTailArgs tail_args{};
-    GnGroups groups{d_groups_, batch};
-    void *args[] = {&cfg, &kp, &nk, &d_states, &iters, &links, &words, &tail_args, &groups};
-    CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_gn_persistent<false>, dim3(grid), dim3(kGatherWarps * 32), args,
+    GnGroups groups{reinterpret_cast<const GnGroup *>(d_gn_table_), reinterpret_cast<const int *>(d_gn_table_ + cta_off), batch};
+    void *args[] = {&cfg, &kp, &nk, &st, &iters, &links, &words, &tail_args, &groups};
+    CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_gn_persistent<false, true>, dim3(grid), dim3(kGatherWarps * 32), args,
                                               sizeof(GnShared), stream_));
     gather_launches_ += 1;
     launches_ += 1;
@@ -1271,7 +1341,7 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
     const size_t k_share = (k_upper + shard_world - 1) / shard_world + 16;
     if (use_persistent_ && (!nccl_comm || peers)) {
         // one cooperative launch for the whole loop; the grid must be co-resident (grid-wide barriers)
-        void *kernel = peers ? (void *) k_gn_persistent<true> : (void *) k_gn_persistent<false>;
+        void *kernel = peers ? (void *) k_gn_persistent<true, false> : (void *) k_gn_persistent<false, false>;
         const int coresident = GnCoresident(peers);
         const int blocks = GatherBlocks(k_share, std::max(1, coresident - 1), kp_per_cta_);
         int grid = std::min(blocks + 1, coresident);
@@ -1297,7 +1367,7 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
         GnLoopWords words{d_loop_rows_, d_loop_pose_, tag};
         FrameTailArgs tail_args{};
         if (tail) tail_args = *tail;
-        GnGroups groups{nullptr, 1};
+        GnGroups groups{nullptr, nullptr, 1};
         void *args[] = {&cfg, &kp, &nk, &d_state, &iters, &links, &words, &tail_args, &groups};
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
         if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);

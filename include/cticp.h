@@ -470,7 +470,8 @@ typedef struct cticp_device_timing {
     uint64_t h2d_bytes;                    /* host→device bytes copied by the call (scan + state) */
     uint64_t d2h_bytes;                    /* device→host bytes copied by the call (poses, counters) */
     int32_t gather_launches;               /* launches of the neighbor-gather kernel */
-    int32_t _pad0;
+    int32_t icp_batch_groups;              /* problems in the ICP launch of the last frame: 1 solo, B in a grouped launch of
+                                              cticp_odometry_register_batch, 0 without an ICP */
 } cticp_device_timing;
 int cticp_odometry_last_timing(cticp_odometry *h, cticp_device_timing *out);
 
@@ -481,6 +482,46 @@ int cticp_odometry_last_timing(cticp_odometry *h, cticp_device_timing *out);
 int64_t cticp_odometry_stage_frame(cticp_odometry *h, const double *xyz, size_t xyz_stride_bytes, const double *t,
                                    size_t t_stride_bytes, size_t n);
 int cticp_odometry_register_staged(cticp_odometry *h, int64_t slot, uint32_t frame_id, cticp_summary *out_summary);
+
+/* ---- one frame on each of many handles in one call ------------------------------------------------------------------
+ * Each item registers one frame on its own handle, with the semantics of the single-frame entry its kind names:
+ *   CTICP_BATCH_HOST    xyz / t / n with strides in host memory (cticp_odometry_register_frame_ex)
+ *   CTICP_BATCH_DEVICE  device_scan + producer stream (cticp_odometry_register_device)
+ *   CTICP_BATCH_STAGED  staged_slot (cticp_odometry_register_staged; initial_estimate and motion_model must be NULL)
+ * The frames whose single-frame call would run the Gauss-Newton loop through the persistent kernel with the device tail
+ * (solver GN, k > 0, no robust_registration, motion compensation CONTINUOUS, no callback, not sharded, a non-empty scan)
+ * run their GN loops in ONE grouped launch, each against its own handle's map; every other frame takes its single-frame
+ * path inside the call. Each item's summary, trajectory entry, map and point vectors are those of the single-frame call,
+ * byte for byte when the joining problems fit on the device together (each gets its solo grid); otherwise they differ by
+ * the GN summation order only and are reproducible from run to run.
+ * Errors: CTICP_ERR_INVALID_ARGUMENT before any handle is touched for batch outside [1, 64], a null item, handle, out or
+ * scan pointer, an unknown kind, the same handle twice, or handles on different devices; CTICP_ERR_UNSUPPORTED for a
+ * sharded handle. Per-item errors (timestamp, capacity, internal, ...) go to that item's status, the other items complete;
+ * the call then returns the first failing item's status and cticp_last_error() carries its message.
+ * The handles must not be used from other threads during the call. */
+enum { CTICP_BATCH_HOST = 0, CTICP_BATCH_DEVICE = 1, CTICP_BATCH_STAGED = 2 };
+typedef struct cticp_batch_frame {
+    cticp_odometry *handle;
+    int32_t kind;                       /* CTICP_BATCH_* */
+    uint32_t frame_id;
+    /* CTICP_BATCH_HOST */
+    const double *xyz;
+    size_t xyz_stride_bytes;
+    const double *t;
+    size_t t_stride_bytes;
+    size_t n;
+    /* CTICP_BATCH_DEVICE */
+    const cticp_device_scan *device_scan;
+    void *stream;                       /* the producer's cudaStream_t (NULL: legacy default stream) */
+    /* CTICP_BATCH_STAGED */
+    int64_t staged_slot;
+    const cticp_frame *initial_estimate;        /* nullable */
+    const cticp_motion_prior *motion_model;     /* nullable */
+    cticp_summary *out;
+    int32_t status;                     /* out: CTICP_OK or the item's error */
+    int32_t _pad0;
+} cticp_batch_frame;
+int cticp_odometry_register_batch(cticp_batch_frame *items, size_t batch);
 int cticp_odometry_clear_staged(cticp_odometry *h);
 /* CUDA-event stopwatch on the handle's stream (the stream every kernel of this handle is launched on) */
 int cticp_odometry_timer_start(cticp_odometry *h);
