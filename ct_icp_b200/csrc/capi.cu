@@ -2,6 +2,7 @@
 // returns a cticp_status and records its message for cticp_last_error().
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -42,24 +43,22 @@ int Guard(F &&f) {
         return Fail(CTICP_ERR_INTERNAL, e.what());
     }
 }
-#define CAPI_CUDA(expr)                                                                          \
-    do {                                                                                         \
-        cudaError_t _e = (expr);                                                                 \
-        if (_e != cudaSuccess) throw CudaError(std::string(#expr) + ": " + cudaGetErrorString(_e)); \
-    } while (0)
-
 void RequireDevice(int device) {
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count)
         throw std::runtime_error("NO_DEVICE: no usable CUDA device (this engine has no CPU fallback)");
-    CAPI_CUDA(cudaSetDevice(device));
+    CT_CUDA_CHECK(cudaSetDevice(device));
     cudaDeviceProp prop;
-    CAPI_CUDA(cudaGetDeviceProperties(&prop, device));
+    CT_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9 || prop.minor != 0) throw std::runtime_error("NO_DEVICE: this build targets sm_90a (Hopper H100) only");
 }
 }  // namespace
 
 struct cticp_map {
+    // a handle of cticp_map_create owns its stream, map and solver; an odometry's view borrows its engine's
+    cticp::Stream owned_stream;
+    std::unique_ptr<DeviceMap> owned_map;
+    std::unique_ptr<IcpSolver> owned_icp;
     DeviceMap *map = nullptr;
     IcpSolver *icp = nullptr;
     cudaStream_t stream = nullptr;
@@ -67,7 +66,7 @@ struct cticp_map {
     bool owned = false;
 };
 struct cticp_odometry {
-    Engine *engine = nullptr;
+    std::unique_ptr<Engine> engine;
     cticp_map map_view;
 };
 
@@ -298,25 +297,18 @@ int cticp_odometry_create(const cticp_odometry_options *options, int device, cti
     return Guard([&] {
         if (!options || !out) throw std::invalid_argument("null argument");
         RequireDevice(device);
-        auto *h = new cticp_odometry();
-        try {
-            h->engine = new Engine(*options, device);
-        } catch (...) {
-            delete h;
-            throw;
-        }
+        auto h = std::make_unique<cticp_odometry>();
+        h->engine = std::make_unique<Engine>(*options, device);
         h->map_view.map = &h->engine->Map();
         h->map_view.icp = &h->engine->Solver();
         h->map_view.stream = h->engine->Stream();
         h->map_view.device = device;
         h->map_view.owned = false;
-        *out = h;
+        *out = h.release();
         return (int) CTICP_OK;
     });
 }
 void cticp_odometry_destroy(cticp_odometry *h) {
-    if (!h) return;
-    delete h->engine;
     delete h;
 }
 int cticp_odometry_register_frame(cticp_odometry *h, const double *xyz, size_t xyz_stride_bytes, const double *t,
@@ -353,9 +345,8 @@ int cticp_odometry_reset_options(cticp_odometry *h, const cticp_odometry_options
     return Guard([&] {
         if (!h || !options) throw std::invalid_argument("null argument");
         const int device = h->engine->Device();
-        Engine *fresh = new Engine(*options, device);   // throws before the old engine is touched
-        delete h->engine;
-        h->engine = fresh;
+        auto fresh = std::make_unique<Engine>(*options, device);   // throws before the old engine is touched
+        h->engine = std::move(fresh);
         h->map_view.map = &h->engine->Map();
         h->map_view.icp = &h->engine->Solver();
         h->map_view.stream = h->engine->Stream();
@@ -516,7 +507,7 @@ int cticp_odometry_register_batch(cticp_batch_frame *items, size_t batch) {
         for (size_t i = 0; i < batch; ++i) {
             const cticp_batch_frame &it = items[i];
             BatchItem &w = work[i];
-            w.engine = it.handle->engine;
+            w.engine = it.handle->engine.get();
             w.kind = it.kind;
             if (it.kind == CTICP_BATCH_HOST) {
                 w.scan.xyz = it.xyz; w.scan.xyz_stride = it.xyz_stride_bytes; w.scan.t = it.t; w.scan.t_stride = it.t_stride_bytes;
@@ -591,14 +582,17 @@ int cticp_map_create(const cticp_map_options *options, int device, cticp_map **o
     return Guard([&] {
         if (!options || !out) throw std::invalid_argument("null argument");
         RequireDevice(device);
-        auto *m = new cticp_map();
+        auto m = std::make_unique<cticp_map>();
         m->device = device;
         m->owned = true;
-        CAPI_CUDA(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
-        m->map = new DeviceMap(*options, m->stream, options->select_valid_normals_direction != 0);
-        m->icp = new IcpSolver(m->stream);
-        CAPI_CUDA(cudaStreamSynchronize(m->stream));
-        *out = m;
+        m->owned_stream = cticp::Stream(cudaStreamNonBlocking);
+        m->stream = m->owned_stream.get();
+        m->owned_map = std::make_unique<DeviceMap>(*options, m->stream, options->select_valid_normals_direction != 0);
+        m->map = m->owned_map.get();
+        m->owned_icp = std::make_unique<IcpSolver>(m->stream);
+        m->icp = m->owned_icp.get();
+        CT_CUDA_CHECK(cudaStreamSynchronize(m->stream));
+        *out = m.release();
         return (int) CTICP_OK;
     });
 }
@@ -606,17 +600,14 @@ void cticp_map_destroy(cticp_map *m) {
     if (!m || !m->owned) return;
     cudaSetDevice(m->device);
     cudaStreamSynchronize(m->stream);
-    delete m->icp;
-    delete m->map;
-    cudaStreamDestroy(m->stream);
-    delete m;
+    delete m;   // the solver and the map go before the stream (reverse declaration order)
 }
 int cticp_map_insert(cticp_map *m, const double *xyz, size_t stride_bytes, size_t n) {
     return cticp_map_insert_from(m, xyz, stride_bytes, n, nullptr);
 }
 int cticp_map_insert_from(cticp_map *m, const double *xyz, size_t stride_bytes, size_t n, const double origin[3]) {
     return Guard([&] {
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         m->map->InsertHost(xyz, stride_bytes, n, origin ? V3{origin[0], origin[1], origin[2]} : V3{0, 0, 0});
         m->map->SyncCounters();
         m->map->MaintainTables();
@@ -625,7 +616,7 @@ int cticp_map_insert_from(cticp_map *m, const double *xyz, size_t stride_bytes, 
 }
 int cticp_map_remove_far(cticp_map *m, const double location[3], double distance) {
     return Guard([&] {
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         m->map->RemoveFar(V3{location[0], location[1], location[2]}, distance);
         m->map->SyncCounters();
         m->map->MaintainTables();
@@ -635,7 +626,7 @@ int cticp_map_remove_far(cticp_map *m, const double location[3], double distance
 int64_t cticp_map_num_points(cticp_map *m, int map_idx) {
     int64_t v = 0;
     int rc = Guard([&] {
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         if (map_idx < 0 || map_idx >= m->map->NumLevels()) throw std::invalid_argument("map_idx");
         v = (int64_t) m->map->SyncCounters()[map_idx].num_points;
         return (int) CTICP_OK;
@@ -645,7 +636,7 @@ int64_t cticp_map_num_points(cticp_map *m, int map_idx) {
 int64_t cticp_map_num_voxels(cticp_map *m, int map_idx) {
     int64_t v = 0;
     int rc = Guard([&] {
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         if (map_idx < 0 || map_idx >= m->map->NumLevels()) throw std::invalid_argument("map_idx");
         v = (int64_t) m->map->SyncCounters()[map_idx].num_voxels;
         return (int) CTICP_OK;
@@ -655,7 +646,7 @@ int64_t cticp_map_num_voxels(cticp_map *m, int map_idx) {
 int64_t cticp_map_export(cticp_map *m, int map_idx, double *dst_xyz, int32_t *dst_voxel, size_t cap_points) {
     int64_t v = 0;
     int rc = Guard([&] {
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         if (map_idx < 0 || map_idx >= m->map->NumLevels()) throw std::invalid_argument("map_idx");
         std::vector<double> xyz;
         std::vector<int> vox;
@@ -671,20 +662,19 @@ int64_t cticp_map_export(cticp_map *m, int map_idx, double *dst_xyz, int32_t *ds
 int cticp_map_compute_neighborhoods(cticp_map *m, const double *queries_xyz, size_t n, int max_num_neighbors,
                                     double *out_points, int32_t *out_counts) {
     return Guard([&] {
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         if (n == 0) return (int) CTICP_OK;
-        double *d_q, *d_out;
-        int *d_cnt;
-        CAPI_CUDA(cudaMalloc(&d_q, sizeof(double) * 3 * n));
-        CAPI_CUDA(cudaMalloc(&d_out, sizeof(double) * 3 * n * max_num_neighbors));
-        CAPI_CUDA(cudaMalloc(&d_cnt, sizeof(int) * n));
-        CAPI_CUDA(cudaMemcpyAsync(d_q, queries_xyz, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, m->stream));
-        CAPI_CUDA(cudaMemsetAsync(d_out, 0, sizeof(double) * 3 * n * max_num_neighbors, m->stream));
-        m->icp->Neighborhoods(*m->map, d_q, n, max_num_neighbors, d_out, d_cnt);
-        CAPI_CUDA(cudaMemcpyAsync(out_points, d_out, sizeof(double) * 3 * n * max_num_neighbors, cudaMemcpyDeviceToHost, m->stream));
-        CAPI_CUDA(cudaMemcpyAsync(out_counts, d_cnt, sizeof(int) * n, cudaMemcpyDeviceToHost, m->stream));
-        CAPI_CUDA(cudaStreamSynchronize(m->stream));
-        cudaFree(d_q); cudaFree(d_out); cudaFree(d_cnt);
+        DeviceArray<double> d_q, d_out;
+        DeviceArray<int> d_cnt;
+        d_q.reserve(3 * n, m->stream);
+        d_out.reserve(3 * n * max_num_neighbors, m->stream);
+        d_cnt.reserve(n, m->stream);
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_q.data(), queries_xyz, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, m->stream));
+        CT_CUDA_CHECK(cudaMemsetAsync(d_out.data(), 0, sizeof(double) * 3 * n * max_num_neighbors, m->stream));
+        m->icp->Neighborhoods(*m->map, d_q.data(), n, max_num_neighbors, d_out.data(), d_cnt.data());
+        CT_CUDA_CHECK(cudaMemcpyAsync(out_points, d_out.data(), sizeof(double) * 3 * n * max_num_neighbors, cudaMemcpyDeviceToHost, m->stream));
+        CT_CUDA_CHECK(cudaMemcpyAsync(out_counts, d_cnt.data(), sizeof(int) * n, cudaMemcpyDeviceToHost, m->stream));
+        CT_CUDA_CHECK(cudaStreamSynchronize(m->stream));
         return (int) CTICP_OK;
     });
 }
@@ -692,29 +682,28 @@ int cticp_map_radius_search(cticp_map *m, const double *queries_xyz, const doubl
                             int max_num_neighbors, const double *sensor_location, double *out_points,
                             int32_t *out_counts) {
     return Guard([&] {
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         if (n == 0) return (int) CTICP_OK;
         if (!queries_xyz || !radiuses || !out_points || !out_counts) throw std::invalid_argument("null argument");
-        double *d_q, *d_r, *d_out;
-        int *d_cnt;
-        CAPI_CUDA(cudaMalloc(&d_q, sizeof(double) * 3 * n));
-        CAPI_CUDA(cudaMalloc(&d_r, sizeof(double) * n));
-        CAPI_CUDA(cudaMalloc(&d_out, sizeof(double) * 3 * n * max_num_neighbors));
-        CAPI_CUDA(cudaMalloc(&d_cnt, sizeof(int) * n));
-        CAPI_CUDA(cudaMemcpyAsync(d_q, queries_xyz, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, m->stream));
-        CAPI_CUDA(cudaMemcpyAsync(d_r, radiuses, sizeof(double) * n, cudaMemcpyHostToDevice, m->stream));
-        CAPI_CUDA(cudaMemsetAsync(d_out, 0, sizeof(double) * 3 * n * max_num_neighbors, m->stream));
-        m->icp->RadiusSearch(*m->map, d_q, d_r, n, max_num_neighbors, sensor_location, d_out, d_cnt);
-        CAPI_CUDA(cudaMemcpyAsync(out_points, d_out, sizeof(double) * 3 * n * max_num_neighbors, cudaMemcpyDeviceToHost, m->stream));
-        CAPI_CUDA(cudaMemcpyAsync(out_counts, d_cnt, sizeof(int) * n, cudaMemcpyDeviceToHost, m->stream));
-        CAPI_CUDA(cudaStreamSynchronize(m->stream));
-        cudaFree(d_q); cudaFree(d_r); cudaFree(d_out); cudaFree(d_cnt);
+        DeviceArray<double> d_q, d_r, d_out;
+        DeviceArray<int> d_cnt;
+        d_q.reserve(3 * n, m->stream);
+        d_r.reserve(n, m->stream);
+        d_out.reserve(3 * n * max_num_neighbors, m->stream);
+        d_cnt.reserve(n, m->stream);
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_q.data(), queries_xyz, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, m->stream));
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_r.data(), radiuses, sizeof(double) * n, cudaMemcpyHostToDevice, m->stream));
+        CT_CUDA_CHECK(cudaMemsetAsync(d_out.data(), 0, sizeof(double) * 3 * n * max_num_neighbors, m->stream));
+        m->icp->RadiusSearch(*m->map, d_q.data(), d_r.data(), n, max_num_neighbors, sensor_location, d_out.data(), d_cnt.data());
+        CT_CUDA_CHECK(cudaMemcpyAsync(out_points, d_out.data(), sizeof(double) * 3 * n * max_num_neighbors, cudaMemcpyDeviceToHost, m->stream));
+        CT_CUDA_CHECK(cudaMemcpyAsync(out_counts, d_cnt.data(), sizeof(int) * n, cudaMemcpyDeviceToHost, m->stream));
+        CT_CUDA_CHECK(cudaStreamSynchronize(m->stream));
         return (int) CTICP_OK;
     });
 }
 int cticp_map_clear(cticp_map *m) {
     return Guard([&] {
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         m->map->Clear();
         m->map->SyncCounters();
         return (int) CTICP_OK;
@@ -731,18 +720,12 @@ double AlphaOf(double t, double bts, double ets) {
     return (t - mn) / (mx - mn);
 }
 struct DeviceKeypoints {
-    float4 *d_kp = nullptr;
-    float4 *d_lo = nullptr;   // residual plane (se3.cuh load_raw); has_lo: some coordinate is not float32-representable
+    DeviceArray<float4> d_kp;
+    DeviceArray<float4> d_lo;   // residual plane (se3.cuh load_raw); has_lo: some coordinate is not float32-representable
     bool has_lo = false;
-    int *d_n = nullptr;
-    IcpState *d_state = nullptr;
-    const float4 *lo() const { return has_lo ? d_lo : nullptr; }
-    ~DeviceKeypoints() {
-        cudaFree(d_kp);
-        cudaFree(d_lo);
-        cudaFree(d_n);
-        cudaFree(d_state);
-    }
+    DeviceArray<int> d_n;
+    DeviceArray<IcpState> d_state;
+    const float4 *lo() const { return has_lo ? d_lo.data() : nullptr; }
 };
 // keypoints → (fp32 raw xyz, alpha) in kp[0..n) and its residual plane in lo[0..n); returns whether some value is not
 // float32-representable. Throws TimestampError for a timestamp outside the frame, before writing anything else.
@@ -771,17 +754,17 @@ void UploadRegistrationInputs(cticp_map *m, const cticp_wpoint *keypoints, size_
                               DeviceKeypoints &D, IcpState &S) {
     std::vector<float4> kp(n), lo(n);
     D.has_lo = PackKeypoints(keypoints, n, frame, kp.data(), lo.data());
-    CAPI_CUDA(cudaMalloc(&D.d_kp, sizeof(float4) * std::max<size_t>(n, 1)));
-    CAPI_CUDA(cudaMalloc(&D.d_lo, sizeof(float4) * std::max<size_t>(n, 1)));
-    CAPI_CUDA(cudaMemcpyAsync(D.d_lo, lo.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, m->stream));
-    CAPI_CUDA(cudaMalloc(&D.d_n, sizeof(int)));
-    CAPI_CUDA(cudaMalloc(&D.d_state, sizeof(IcpState)));
+    D.d_kp.reserve(std::max<size_t>(n, 1), m->stream);
+    D.d_lo.reserve(std::max<size_t>(n, 1), m->stream);
+    CT_CUDA_CHECK(cudaMemcpyAsync(D.d_lo.data(), lo.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, m->stream));
+    D.d_n.reserve(1, m->stream);
+    D.d_state.reserve(1, m->stream);
     const int ni = (int) n;
     InitialState(frame, previous_frame, mo, S);
-    CAPI_CUDA(cudaMemcpyAsync(D.d_kp, kp.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, m->stream));
-    CAPI_CUDA(cudaMemcpyAsync(D.d_n, &ni, sizeof(int), cudaMemcpyHostToDevice, m->stream));
-    CAPI_CUDA(cudaMemcpyAsync(D.d_state, &S, sizeof(IcpState), cudaMemcpyHostToDevice, m->stream));
-    CAPI_CUDA(cudaStreamSynchronize(m->stream));
+    CT_CUDA_CHECK(cudaMemcpyAsync(D.d_kp.data(), kp.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, m->stream));
+    CT_CUDA_CHECK(cudaMemcpyAsync(D.d_n.data(), &ni, sizeof(int), cudaMemcpyHostToDevice, m->stream));
+    CT_CUDA_CHECK(cudaMemcpyAsync(D.d_state.data(), &S, sizeof(IcpState), cudaMemcpyHostToDevice, m->stream));
+    CT_CUDA_CHECK(cudaStreamSynchronize(m->stream));
 }
 void InitialState(const cticp_frame *frame, const cticp_frame *previous_frame, const cticp_motion_model_options *mo,
                   IcpState &S) {
@@ -842,7 +825,7 @@ int cticp_icp_register(cticp_map *m, const cticp_icp_options *options, const cti
                        const cticp_motion_model_options *motion_options, cticp_icp_summary *out_summary) {
     return Guard([&] {
         if (!m || !options || !keypoints || !frame) throw std::invalid_argument("null argument");
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         DeviceKeypoints D;
         IcpState S;
         UploadRegistrationInputs(m, keypoints, n, frame, previous_frame, motion_options, D, S);
@@ -851,17 +834,17 @@ int cticp_icp_register(cticp_map *m, const cticp_icp_options *options, const cti
         m->icp->set_keypoints_lo(D.lo());
         switch (options->solver) {
             case CTICP_SOLVER_GN:
-                m->icp->EnqueueGaussNewton(*m->map, *options, D.d_kp, D.d_n, n, options->num_iters_icp, D.d_state);
+                m->icp->EnqueueGaussNewton(*m->map, *options, D.d_kp.data(), D.d_n.data(), n, options->num_iters_icp, D.d_state.data());
                 break;
             case CTICP_SOLVER_CERES:
             case CTICP_SOLVER_ROBUST:
-                m->icp->EnqueueCeres(*m->map, *options, st, D.d_kp, D.d_n, n, n, D.d_state);
+                m->icp->EnqueueCeres(*m->map, *options, st, D.d_kp.data(), D.d_n.data(), n, n, D.d_state.data());
                 break;
             default:
                 throw UnsupportedError("Unsupported Solver Type");
         }
-        CAPI_CUDA(cudaMemcpyAsync(&S, D.d_state, sizeof(IcpState), cudaMemcpyDeviceToHost, m->stream));
-        CAPI_CUDA(cudaStreamSynchronize(m->stream));
+        CT_CUDA_CHECK(cudaMemcpyAsync(&S, D.d_state.data(), sizeof(IcpState), cudaMemcpyDeviceToHost, m->stream));
+        CT_CUDA_CHECK(cudaStreamSynchronize(m->stream));
         WriteRegistrationOutputs(S, keypoints, n, frame, out_summary);
         if (S.failed == 2) throw std::runtime_error("Error During Optimization");
         if (S.failed) g_last_error = "[CT_ICP]Error : not enough keypoints selected in ct-icp !";
@@ -896,7 +879,7 @@ int RegisterBatch(cticp_map *m, const cticp_icp_options *options, const cticp_st
         } else if (options->solver != CTICP_SOLVER_CERES && options->solver != CTICP_SOLVER_ROBUST) {
             throw UnsupportedError("Unsupported Solver Type");
         }
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         if (gn && !m->icp->batch_supported())
             throw UnsupportedError("cticp_icp_register_batch needs the persistent Gauss-Newton loop with flag synchronisation");
         if (!gn) {
@@ -918,26 +901,23 @@ int RegisterBatch(cticp_map *m, const cticp_icp_options *options, const cticp_st
             for (size_t b = 0, base = 0; b < batch; base += n[b], ++b)
                 if (!has_lo[b])
                     for (size_t i = 0; i < n[b]; ++i) lo[base + i] = make_float4(-0.f, -0.f, -0.f, -0.f);
-        struct Buffers {
-            float4 *kp = nullptr, *lo = nullptr;
-            IcpState *states = nullptr;
-            ~Buffers() { cudaFree(kp); cudaFree(lo); cudaFree(states); }
-        } D;
-        CAPI_CUDA(cudaMalloc(&D.kp, sizeof(float4) * kp.size()));
-        CAPI_CUDA(cudaMalloc(&D.states, sizeof(IcpState) * batch));
-        CAPI_CUDA(cudaMemcpyAsync(D.kp, kp.data(), sizeof(float4) * total, cudaMemcpyHostToDevice, m->stream));
+        DeviceArray<float4> d_kp, d_lo;
+        DeviceArray<IcpState> d_states;
+        d_kp.reserve(kp.size(), m->stream);
+        d_states.reserve(batch, m->stream);
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_kp.data(), kp.data(), sizeof(float4) * total, cudaMemcpyHostToDevice, m->stream));
         if (any_lo) {
-            CAPI_CUDA(cudaMalloc(&D.lo, sizeof(float4) * lo.size()));
-            CAPI_CUDA(cudaMemcpyAsync(D.lo, lo.data(), sizeof(float4) * total, cudaMemcpyHostToDevice, m->stream));
+            d_lo.reserve(lo.size(), m->stream);
+            CT_CUDA_CHECK(cudaMemcpyAsync(d_lo.data(), lo.data(), sizeof(float4) * total, cudaMemcpyHostToDevice, m->stream));
         }
-        CAPI_CUDA(cudaMemcpyAsync(D.states, S.data(), sizeof(IcpState) * batch, cudaMemcpyHostToDevice, m->stream));
-        m->icp->set_keypoints_lo(D.lo);
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_states.data(), S.data(), sizeof(IcpState) * batch, cudaMemcpyHostToDevice, m->stream));
+        m->icp->set_keypoints_lo(d_lo.data());
         if (gn)
-            m->icp->EnqueueGaussNewtonBatch(*m->map, *options, (int) batch, n, D.kp, options->num_iters_icp, D.states);
+            m->icp->EnqueueGaussNewtonBatch(*m->map, *options, (int) batch, n, d_kp.data(), options->num_iters_icp, d_states.data());
         else
-            m->icp->EnqueueCeresBatch(*m->map, *options, st, (int) batch, n, D.kp, D.states);
-        CAPI_CUDA(cudaMemcpyAsync(S.data(), D.states, sizeof(IcpState) * batch, cudaMemcpyDeviceToHost, m->stream));
-        CAPI_CUDA(cudaStreamSynchronize(m->stream));
+            m->icp->EnqueueCeresBatch(*m->map, *options, st, (int) batch, n, d_kp.data(), d_states.data());
+        CT_CUDA_CHECK(cudaMemcpyAsync(S.data(), d_states.data(), sizeof(IcpState) * batch, cudaMemcpyDeviceToHost, m->stream));
+        CT_CUDA_CHECK(cudaStreamSynchronize(m->stream));
         bool timeout = false, not_enough = false;
         for (size_t b = 0; b < batch; ++b) {
             WriteRegistrationOutputs(S[b], keypoints[b], n[b], &frames[b], out_summaries ? &out_summaries[b] : nullptr);
@@ -973,13 +953,13 @@ int cticp_icp_gn_normal_equations(cticp_map *m, const cticp_icp_options *options
                                   int32_t *out_num_used) {
     return Guard([&] {
         if (!m || !options || !keypoints || !frame) throw std::invalid_argument("null argument");
-        CAPI_CUDA(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
         DeviceKeypoints D;
         IcpState S;
         UploadRegistrationInputs(m, keypoints, n, frame, previous_frame, motion_options, D, S);
         int n_used = 0;
         m->icp->set_keypoints_lo(D.lo());
-        m->icp->NormalEquations(*m->map, *options, D.d_kp, D.d_n, n, D.d_state, out_A144, out_b12, &n_used);
+        m->icp->NormalEquations(*m->map, *options, D.d_kp.data(), D.d_n.data(), n, D.d_state.data(), out_A144, out_b12, &n_used);
         *out_num_used = n_used;
         return (int) CTICP_OK;
     });
@@ -992,10 +972,9 @@ int64_t cticp_grid_sample_indices(int device, const double *xyz, size_t stride_b
     int rc = Guard([&] {
         RequireDevice(device);
         if (n == 0) return (int) CTICP_OK;
-        cudaStream_t stream;
-        CAPI_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+        const cticp::Stream stream(cudaStreamNonBlocking);
         {
-            FramePipeline pipe(n, stream);
+            FramePipeline pipe(n, stream.get());
             float4 *stage = pipe.Staging(), *stage_lo = pipe.StagingLo();
             for (size_t i = 0; i < n; ++i) {
                 const double *p = reinterpret_cast<const double *>(reinterpret_cast<const char *>(xyz) + stride_bytes * i);
@@ -1008,12 +987,11 @@ int64_t cticp_grid_sample_indices(int device, const double *xyz, size_t stride_b
             pipe.GridSelect(pipe.d_raw(), pipe.d_raw_lo(), nullptr, pipe.d_count_n(), n, voxel_size, 0, 0, 0, 0, 0, 0, 0.f,
                             pipe.d_frame_mut(), pipe.d_frame_lo_mut(), pipe.d_frame_src_mut(), pipe.d_count_frame());
             pipe.QueueCountsReadback();
-            CAPI_CUDA(cudaStreamSynchronize(stream));
+            CT_CUDA_CHECK(cudaStreamSynchronize(stream.get()));
             total = pipe.h_counts()[1];
             const size_t k = std::min<size_t>(cap, (size_t) total);
-            CAPI_CUDA(cudaMemcpy(out_indices, pipe.d_frame_src(), sizeof(uint32_t) * k, cudaMemcpyDeviceToHost));
+            CT_CUDA_CHECK(cudaMemcpy(out_indices, pipe.d_frame_src(), sizeof(uint32_t) * k, cudaMemcpyDeviceToHost));
         }
-        cudaStreamDestroy(stream);
         return (int) CTICP_OK;
     });
     return rc < 0 ? rc : total;
@@ -1024,10 +1002,9 @@ int64_t cticp_adaptive_sample_indices(int device, const cticp_adaptive_options *
     int rc = Guard([&] {
         RequireDevice(device);
         if (n == 0 || !options) return (int) CTICP_OK;
-        cudaStream_t stream;
-        CAPI_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+        const cticp::Stream stream(cudaStreamNonBlocking);
         {
-            FramePipeline pipe(n, stream);
+            FramePipeline pipe(n, stream.get());
             float4 *stage = pipe.Staging(), *stage_lo = pipe.StagingLo();
             for (size_t i = 0; i < n; ++i) {
                 const double *p = reinterpret_cast<const double *>(reinterpret_cast<const char *>(xyz) + stride_bytes * i);
@@ -1040,12 +1017,11 @@ int64_t cticp_adaptive_sample_indices(int device, const cticp_adaptive_options *
             pipe.AdaptiveSelect(*options, pipe.d_raw(), pipe.d_raw_lo(), nullptr, pipe.d_count_n(), n, pipe.d_frame_mut(),
                                 pipe.d_frame_lo_mut(), pipe.d_frame_src_mut(), pipe.d_count_frame());
             pipe.QueueCountsReadback();
-            CAPI_CUDA(cudaStreamSynchronize(stream));
+            CT_CUDA_CHECK(cudaStreamSynchronize(stream.get()));
             total = pipe.h_counts()[1];
             const size_t k = std::min<size_t>(cap, (size_t) total);
-            CAPI_CUDA(cudaMemcpy(out_indices, pipe.d_frame_src(), sizeof(uint32_t) * k, cudaMemcpyDeviceToHost));
+            CT_CUDA_CHECK(cudaMemcpy(out_indices, pipe.d_frame_src(), sizeof(uint32_t) * k, cudaMemcpyDeviceToHost));
         }
-        cudaStreamDestroy(stream);
         return (int) CTICP_OK;
     });
     return rc < 0 ? rc : total;

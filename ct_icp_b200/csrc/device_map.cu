@@ -19,14 +19,6 @@
 
 namespace cticp {
 
-#define CT_CUDA_CHECK(expr)                                                                              \
-    do {                                                                                                 \
-        cudaError_t _e = (expr);                                                                         \
-        if (_e != cudaSuccess)                                                                           \
-            throw CudaError(std::string(#expr) + ": " + cudaGetErrorString(_e) + " @" + __FILE__ + ":" + \
-                            std::to_string(__LINE__));                                                   \
-    } while (0)
-
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void k_clear_level(MapLevel L) {
     const uint32_t cap = L.cap_mask + 1;
@@ -435,119 +427,86 @@ DeviceMap::DeviceMap(const cticp_map_options &options, cudaStream_t stream, bool
     if (options.num_resolutions < 1 || options.num_resolutions > CTICP_MAX_RESOLUTIONS)
         throw std::invalid_argument("map_options.num_resolutions out of range");
     levels_.resize(options.num_resolutions);
+    storage_.reserve(options.num_resolutions);
     for (int i = 0; i < options.num_resolutions; ++i) {
         const auto &rp = options.resolutions[i];
         if (!(rp.resolution > 0) || rp.max_num_points < 1 || rp.max_num_points > kMaxB)
             throw std::invalid_argument("map resolution / max_num_points out of the supported range (1..64)");
         // default capacity: enough for a 100 m local map at load <= 0.5; tables double on demand (MaintainTables)
         uint64_t cap = options.capacity_voxels ? options.capacity_voxels : (rp.resolution < 0.5 ? (1ull << 20) : (1ull << 18));
-        AllocLevel(levels_[i], NextPow2(std::max<uint64_t>(cap, 1024)), rp);
+        storage_.push_back(AllocLevel(levels_[i], NextPow2(std::max<uint64_t>(cap, 1024)), rp));
     }
-    CT_CUDA_CHECK(cudaMalloc(&d_counters_, sizeof(MapCounters) * levels_.size()));
-    CT_CUDA_CHECK(cudaMemsetAsync(d_counters_, 0, sizeof(MapCounters) * levels_.size(), stream_));
-    CT_CUDA_CHECK(cudaMalloc(&d_scalar_, 64));
-    CT_CUDA_CHECK(cudaMallocHost(&h_counters_, sizeof(MapCounters) * CTICP_MAX_RESOLUTIONS));
-    memset(h_counters_, 0, sizeof(MapCounters) * CTICP_MAX_RESOLUTIONS);
+    d_counters_.reserve(levels_.size(), stream_);
+    CT_CUDA_CHECK(cudaMemsetAsync(d_counters_.data(), 0, sizeof(MapCounters) * levels_.size(), stream_));
+    d_scalar_.reserve(16, stream_);
+    h_counters_.reserve(CTICP_MAX_RESOLUTIONS, stream_);
+    memset(h_counters_.data(), 0, sizeof(MapCounters) * CTICP_MAX_RESOLUTIONS);
 }
 
-DeviceMap::~DeviceMap() {
-    for (auto &L : levels_) FreeLevel(L);
-    cudaFree(d_counters_);
-    cudaFree(d_scalar_);
-    cudaFree(d_next_);
-    cudaFree(d_touched_);
-    cudaFree(d_world_tmp_);
-    cudaFree(d_frame_origins_);
-    cudaFreeHost(h_counters_);
-}
-
-void DeviceMap::AllocLevel(MapLevel &L, uint32_t cap, const cticp_resolution_param &rp) {
+DeviceMap::LevelStorage DeviceMap::AllocLevel(MapLevel &L, uint32_t cap, const cticp_resolution_param &rp) {
+    LevelStorage s;
     L.cap_mask = cap - 1;
     L.B = rp.max_num_points;
     L.res = rp.resolution;
     L.min_dist2 = rp.min_distance_between_points * rp.min_distance_between_points;
-    CT_CUDA_CHECK(cudaMalloc(&L.slots, sizeof(MapSlot) * (size_t) cap));
-    CT_CUDA_CHECK(cudaMalloc(&L.points, sizeof(float4) * (size_t) cap * L.B));
-    CT_CUDA_CHECK(cudaMalloc(&L.head, sizeof(int) * (size_t) cap));
-    L.normals = nullptr;
-    if (with_normals_) CT_CUDA_CHECK(cudaMalloc(&L.normals, sizeof(double) * 4 * (size_t) cap));
+    s.slots.reserve(cap, stream_);
+    s.points.reserve((size_t) cap * L.B, stream_);
+    s.head.reserve(cap, stream_);
+    if (with_normals_) s.normals.reserve(4 * (size_t) cap, stream_);
+    L.slots = s.slots.data();
+    L.points = s.points.data();
+    L.head = s.head.data();
+    L.normals = s.normals.data();
     k_clear_level<<<592, 256, 0, stream_>>>(L);
     CT_CUDA_CHECK(cudaGetLastError());
-}
-void DeviceMap::FreeLevel(MapLevel &L) {
-    cudaFree(L.slots);
-    cudaFree(L.points);
-    cudaFree(L.head);
-    cudaFree(L.normals);
-    L.normals = nullptr;
-    L.slots = nullptr;
-    L.points = nullptr;
-    L.head = nullptr;
+    return s;
 }
 
 void DeviceMap::EnsureScratch(size_t n_upper) {
-    if (n_upper <= scratch_n_) return;
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    cudaFree(d_next_);
-    cudaFree(d_touched_);
-    size_t n = std::max<size_t>(n_upper, 1024);
-    CT_CUDA_CHECK(cudaMalloc(&d_next_, sizeof(int) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_touched_, sizeof(uint32_t) * n));
-    scratch_n_ = n;
+    const size_t n = std::max<size_t>(n_upper, 1024);
+    d_next_.reserve(n, stream_);
+    d_touched_.reserve(n, stream_);
 }
 
 void DeviceMap::InsertDevice(const double *d_world_xyz, const int *d_n, size_t n_upper, V3 origin) {
     if (n_upper == 0) return;
     EnsureScratch(n_upper);
-    // frame_id_to_frame[fidx].poses.front() (map.h:158-160): one begin position per inserted frame, never erased
-    if (frame_count_ >= (1u << 24) - 2) throw CapacityError("more than 2^24 frames inserted into one map");
+    EnsureFrameOrigin();
     if (with_normals_) {
-        if (frame_count_ >= frame_capacity_) {
-            const size_t cap = std::max<size_t>(4096, frame_capacity_ * 2);
-            double *fresh = nullptr;
-            CT_CUDA_CHECK(cudaMalloc(&fresh, sizeof(double) * 3 * cap));
-            if (frame_count_)
-                CT_CUDA_CHECK(cudaMemcpyAsync(fresh, d_frame_origins_, sizeof(double) * 3 * frame_count_,
-                                              cudaMemcpyDeviceToDevice, stream_));
-            CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-            cudaFree(d_frame_origins_);
-            d_frame_origins_ = fresh;
-            frame_capacity_ = cap;
-        }
         // 24 bytes by value through a kernel-free path: cudaMemcpyAsync from pageable memory copies the source before
         // returning, so the stack variable may go out of scope
         const double o[3] = {origin.x, origin.y, origin.z};
-        CT_CUDA_CHECK(cudaMemcpyAsync(d_frame_origins_ + 3 * frame_count_, o, sizeof(o), cudaMemcpyHostToDevice, stream_));
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_frame_origins_.data() + 3 * frame_count_, o, sizeof(o), cudaMemcpyHostToDevice, stream_));
     }
     const int frame_ordinal = (int) frame_count_++;
     const int threads = 256;
     const int blocks = (int) std::min<size_t>((n_upper + threads - 1) / threads, 132 * 8);
     for (size_t i = 0; i < levels_.size(); ++i) {
-        MapCounters *ctr = d_counters_ + i;
+        MapCounters *ctr = d_counters_.data() + i;
         CT_CUDA_CHECK(cudaMemsetAsync(&ctr->num_touched, 0, sizeof(unsigned), stream_));
-        k_insert_claim<<<blocks, threads, 0, stream_>>>(levels_[i], ctr, d_world_xyz, d_n, d_next_, d_touched_);
+        k_insert_claim<<<blocks, threads, 0, stream_>>>(levels_[i], ctr, d_world_xyz, d_n, d_next_.data(), d_touched_.data());
         const int cblocks = (int) std::min<size_t>((n_upper + kInsertWarps - 1) / kInsertWarps, 132 * 8);
-        k_insert_commit<<<cblocks, kInsertWarps * 32, 0, stream_>>>(levels_[i], ctr, d_world_xyz, d_next_, d_touched_,
-                                                                     d_frame_origins_, frame_ordinal);
+        k_insert_commit<<<cblocks, kInsertWarps * 32, 0, stream_>>>(levels_[i], ctr, d_world_xyz, d_next_.data(), d_touched_.data(),
+                                                                     d_frame_origins_.data(), frame_ordinal);
         launches_ += 2;
     }
     CT_CUDA_CHECK(cudaGetLastError());
     dirty_ = true;
 }
 
+// frame_id_to_frame[fidx].poses.front() (map.h:158-160): room for one more begin position per inserted frame (never
+// erased); the table doubles with its contents copied over
 void DeviceMap::EnsureFrameOrigin() {
     if (frame_count_ >= (1u << 24) - 2) throw CapacityError("more than 2^24 frames inserted into one map");
-    if (with_normals_ && frame_count_ >= frame_capacity_) {
-        const size_t cap = std::max<size_t>(4096, frame_capacity_ * 2);
-        double *fresh = nullptr;
-        CT_CUDA_CHECK(cudaMalloc(&fresh, sizeof(double) * 3 * cap));
+    const size_t frame_capacity = d_frame_origins_.capacity() / 3;
+    if (with_normals_ && frame_count_ >= frame_capacity) {
+        DeviceArray<double> fresh;
+        fresh.reserve(3 * std::max<size_t>(4096, frame_capacity * 2), stream_);
         if (frame_count_)
-            CT_CUDA_CHECK(cudaMemcpyAsync(fresh, d_frame_origins_, sizeof(double) * 3 * frame_count_,
+            CT_CUDA_CHECK(cudaMemcpyAsync(fresh.data(), d_frame_origins_.data(), sizeof(double) * 3 * frame_count_,
                                           cudaMemcpyDeviceToDevice, stream_));
         CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(d_frame_origins_);
-        d_frame_origins_ = fresh;
-        frame_capacity_ = cap;
+        d_frame_origins_ = std::move(fresh);
     }
 }
 
@@ -566,7 +525,7 @@ void DeviceMap::UpdateFused(const float4 *d_frame, const float4 *d_frame_lo, con
         EnsureFrameOrigin();
         if (with_normals_) {
             const double o[3] = {origin.x, origin.y, origin.z};
-            CT_CUDA_CHECK(cudaMemcpyAsync(d_frame_origins_ + 3 * frame_count_, o, sizeof(o), cudaMemcpyHostToDevice, stream_));
+            CT_CUDA_CHECK(cudaMemcpyAsync(d_frame_origins_.data() + 3 * frame_count_, o, sizeof(o), cudaMemcpyHostToDevice, stream_));
         }
         frame_ordinal = (int) frame_count_++;
     }
@@ -582,7 +541,7 @@ void DeviceMap::UpdateFused(const float4 *d_frame, const float4 *d_frame_lo, con
     FusedUpdateArgs a{};
     a.num_levels = (int) levels_.size();
     for (int l = 0; l < a.num_levels; ++l) a.levels[l] = levels_[l];
-    a.counters = d_counters_;
+    a.counters = d_counters_.data();
     a.frame = d_frame;
     a.frame_lo = d_frame_lo;
     a.d_n = d_n;
@@ -593,12 +552,12 @@ void DeviceMap::UpdateFused(const float4 *d_frame, const float4 *d_frame_lo, con
     a.max_distance = max_distance;
     a.do_remove = do_remove ? 1 : 0;
     a.do_insert = do_insert ? 1 : 0;
-    a.next = d_next_;
-    a.touched = d_touched_;
-    a.frame_origins = d_frame_origins_;
+    a.next = d_next_.data();
+    a.touched = d_touched_.data();
+    a.frame_origins = d_frame_origins_.data();
     a.frame_ordinal = frame_ordinal;
     a.verdict = d_verdict;
-    a.frame_origins_mut = with_normals_ ? d_frame_origins_ : nullptr;
+    a.frame_origins_mut = with_normals_ ? d_frame_origins_.data() : nullptr;
     void *args[] = {&a};
     CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_map_update_fused, dim3(fused_grid_), dim3(kInsertWarps * 32), args, 0, stream_));
     launches_ += 1;
@@ -614,23 +573,18 @@ void DeviceMap::InsertHost(const double *xyz, size_t stride_bytes, size_t n, V3 
     }
     SyncCounters();
     EnsureRoomFor(n);
-    if (n > world_tmp_n_) {
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(d_world_tmp_);
-        CT_CUDA_CHECK(cudaMalloc(&d_world_tmp_, sizeof(double) * 3 * n));
-        world_tmp_n_ = n;
-    }
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_world_tmp_, packed.data(), sizeof(double) * 3 * n, cudaMemcpyHostToDevice, stream_));
+    d_world_tmp_.reserve(3 * n, stream_);
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_world_tmp_.data(), packed.data(), sizeof(double) * 3 * n, cudaMemcpyHostToDevice, stream_));
     int ni = (int) n;
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_scalar_, &ni, sizeof(int), cudaMemcpyHostToDevice, stream_));
-    InsertDevice(d_world_tmp_, reinterpret_cast<int *>(d_scalar_), n, origin);
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_scalar_.data(), &ni, sizeof(int), cudaMemcpyHostToDevice, stream_));
+    InsertDevice(d_world_tmp_.data(), d_scalar_.data(), n, origin);
     CT_CUDA_CHECK(cudaStreamSynchronize(stream_));   // `packed` / `ni` go out of scope
     CheckOverflow();
 }
 
 void DeviceMap::RemoveFar(V3 location, double distance) {
     for (size_t i = 0; i < levels_.size(); ++i) {
-        k_remove_far<<<592, 256, 0, stream_>>>(levels_[i], d_counters_ + i, location, distance);
+        k_remove_far<<<592, 256, 0, stream_>>>(levels_[i], d_counters_.data() + i, location, distance);
         launches_ += 1;
     }
     CT_CUDA_CHECK(cudaGetLastError());
@@ -639,7 +593,7 @@ void DeviceMap::RemoveFar(V3 location, double distance) {
 
 void DeviceMap::Clear() {
     for (auto &L : levels_) k_clear_level<<<592, 256, 0, stream_>>>(L);
-    CT_CUDA_CHECK(cudaMemsetAsync(d_counters_, 0, sizeof(MapCounters) * levels_.size(), stream_));
+    CT_CUDA_CHECK(cudaMemsetAsync(d_counters_.data(), 0, sizeof(MapCounters) * levels_.size(), stream_));
     CT_CUDA_CHECK(cudaGetLastError());
     frame_count_ = 0;
     dirty_ = true;
@@ -647,7 +601,7 @@ void DeviceMap::Clear() {
 
 const MapCounters *DeviceMap::SyncCounters() {
     if (dirty_) {
-        CT_CUDA_CHECK(cudaMemcpyAsync(h_counters_, d_counters_, sizeof(MapCounters) * levels_.size(),
+        CT_CUDA_CHECK(cudaMemcpyAsync(h_counters_.data(), d_counters_.data(), sizeof(MapCounters) * levels_.size(),
                                       cudaMemcpyDeviceToHost, stream_));
         CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
         dirty_ = false;
@@ -656,11 +610,11 @@ const MapCounters *DeviceMap::SyncCounters() {
         CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
         readback_pending_ = false;
     }
-    return h_counters_;
+    return h_counters_.data();
 }
 
 void DeviceMap::QueueCounterReadback() {
-    CT_CUDA_CHECK(cudaMemcpyAsync(h_counters_, d_counters_, sizeof(MapCounters) * levels_.size(),
+    CT_CUDA_CHECK(cudaMemcpyAsync(h_counters_.data(), d_counters_.data(), sizeof(MapCounters) * levels_.size(),
                                   cudaMemcpyDeviceToHost, stream_));
     dirty_ = false;   // valid after the next stream synchronisation
     readback_pending_ = true;
@@ -676,20 +630,20 @@ void DeviceMap::CheckOverflow() {
 void DeviceMap::RebuildLevel(size_t i, uint64_t new_cap) {
     MapLevel fresh{};
     cticp_resolution_param rp = options_.resolutions[i];
-    AllocLevel(fresh, (uint32_t) new_cap, rp);
-    k_rebuild<<<592, 256, 0, stream_>>>(levels_[i], fresh, d_counters_ + i);
-    CT_CUDA_CHECK(cudaMemsetAsync(&(d_counters_ + i)->num_tombs, 0, sizeof(unsigned), stream_));
-    CT_CUDA_CHECK(cudaMemsetAsync(&(d_counters_ + i)->overflow, 0, sizeof(unsigned), stream_));
+    LevelStorage storage = AllocLevel(fresh, (uint32_t) new_cap, rp);
+    k_rebuild<<<592, 256, 0, stream_>>>(levels_[i], fresh, d_counters_.data() + i);
+    CT_CUDA_CHECK(cudaMemsetAsync(&(d_counters_.data() + i)->num_tombs, 0, sizeof(unsigned), stream_));
+    CT_CUDA_CHECK(cudaMemsetAsync(&(d_counters_.data() + i)->overflow, 0, sizeof(unsigned), stream_));
     CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    FreeLevel(levels_[i]);
     levels_[i] = fresh;
-    h_counters_[i].num_tombs = 0;
-    h_counters_[i].overflow = 0;
+    storage_[i] = std::move(storage);
+    h_counters_.data()[i].num_tombs = 0;
+    h_counters_.data()[i].overflow = 0;
     ++rebuilds_;
 }
 
 void DeviceMap::MaintainTables() {
-    const MapCounters *c = h_counters_;
+    const MapCounters *c = h_counters_.data();
     for (size_t i = 0; i < levels_.size(); ++i) {
         const uint64_t cap = (uint64_t) levels_[i].cap_mask + 1;
         const uint64_t used = (uint64_t) c[i].num_voxels + c[i].num_tombs;
@@ -711,7 +665,7 @@ void DeviceMap::MaintainTables() {
 // Before an insert of up to n_new points (every one of them may open a new voxel): make sure no probe sequence can wrap.
 // Uses the host copy of the counters (the previous frame's read-back), so it costs nothing unless a table must grow.
 void DeviceMap::EnsureRoomFor(size_t n_new) {
-    const MapCounters *c = h_counters_;
+    const MapCounters *c = h_counters_.data();
     for (size_t i = 0; i < levels_.size(); ++i) {
         uint64_t cap = (uint64_t) levels_[i].cap_mask + 1;
         const uint64_t live = (uint64_t) c[i].num_voxels + n_new, used = live + c[i].num_tombs;
@@ -736,22 +690,21 @@ size_t DeviceMap::Export(int level, std::vector<double> &xyz, std::vector<int> &
     xyz.assign(3 * n, 0.0);
     voxels.assign(3 * n, 0);
     if (n == 0) return 0;
-    double *d_xyz;
-    int *d_vox, *d_idx;
-    unsigned long long *d_cursor;
-    CT_CUDA_CHECK(cudaMalloc(&d_xyz, sizeof(double) * 3 * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_vox, sizeof(int) * 3 * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_idx, sizeof(int) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_cursor, sizeof(unsigned long long)));
-    CT_CUDA_CHECK(cudaMemsetAsync(d_cursor, 0, sizeof(unsigned long long), stream_));
-    k_export<<<592, 256, 0, stream_>>>(levels_[level], d_cursor, d_xyz, d_vox, d_idx, n);
+    DeviceArray<double> d_xyz;
+    DeviceArray<int> d_vox, d_idx;
+    DeviceArray<unsigned long long> d_cursor;
+    d_xyz.reserve(3 * n, stream_);
+    d_vox.reserve(3 * n, stream_);
+    d_idx.reserve(n, stream_);
+    d_cursor.reserve(1, stream_);
+    CT_CUDA_CHECK(cudaMemsetAsync(d_cursor.data(), 0, sizeof(unsigned long long), stream_));
+    k_export<<<592, 256, 0, stream_>>>(levels_[level], d_cursor.data(), d_xyz.data(), d_vox.data(), d_idx.data(), n);
     std::vector<double> hx(3 * n);
     std::vector<int> hv(3 * n), hi(n);
-    CT_CUDA_CHECK(cudaMemcpyAsync(hx.data(), d_xyz, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, stream_));
-    CT_CUDA_CHECK(cudaMemcpyAsync(hv.data(), d_vox, sizeof(int) * 3 * n, cudaMemcpyDeviceToHost, stream_));
-    CT_CUDA_CHECK(cudaMemcpyAsync(hi.data(), d_idx, sizeof(int) * n, cudaMemcpyDeviceToHost, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(hx.data(), d_xyz.data(), sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(hv.data(), d_vox.data(), sizeof(int) * 3 * n, cudaMemcpyDeviceToHost, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(hi.data(), d_idx.data(), sizeof(int) * n, cudaMemcpyDeviceToHost, stream_));
     CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    cudaFree(d_xyz); cudaFree(d_vox); cudaFree(d_idx); cudaFree(d_cursor);
     // deterministic order: (voxel x, y, z, index in voxel) — same as the oracle's sorted export
     std::vector<size_t> order(n);
     std::iota(order.begin(), order.end(), 0);

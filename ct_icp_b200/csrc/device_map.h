@@ -6,13 +6,11 @@
 #include <vector>
 
 #include "../../include/cticp.h"
+#include "cuda_owner.h"
 #include "device_map.cuh"
 
 namespace cticp {
 
-struct CudaError : std::runtime_error {
-    using std::runtime_error::runtime_error;
-};
 struct CapacityError : std::runtime_error {
     using std::runtime_error::runtime_error;
 };
@@ -23,9 +21,6 @@ class DeviceMap {
 public:
     // with_normals: maintain the per-voxel normals that RadiusSearchInPlace's sensor_location filter reads (map.h:482-490)
     DeviceMap(const cticp_map_options &options, cudaStream_t stream, bool with_normals = false);
-    ~DeviceMap();
-    DeviceMap(const DeviceMap &) = delete;
-    DeviceMap &operator=(const DeviceMap &) = delete;
 
     // InsertPointCloud (map.h:153-254): world points (fp64 xyz triples) already on the device, count on the device
     // `origin` = frame_poses.front().tr of the inserted frame (orients the normals, :222-226)
@@ -51,7 +46,7 @@ public:
     const MapCounters *SyncCounters();
     // enqueue the D2H of the counters; they are valid after the caller's next stream synchronisation
     void QueueCounterReadback();
-    const MapCounters *HostCounters() const { return h_counters_; }
+    const MapCounters *HostCounters() const { return h_counters_.data(); }
     void NotifyStreamSynchronized() { readback_pending_ = false; }
     void CheckOverflow();
     // tombstone purge / growth, driven by HostCounters(); call between frames
@@ -73,28 +68,33 @@ public:
     int rebuilds() const { return rebuilds_; }
 
 private:
-    void AllocLevel(MapLevel &L, uint32_t cap, const cticp_resolution_param &rp);
+    // the tables a MapLevel points into
+    struct LevelStorage {
+        DeviceArray<MapSlot> slots;
+        DeviceArray<float4> points;
+        DeviceArray<int> head;
+        DeviceArray<double> normals;
+    };
+    LevelStorage AllocLevel(MapLevel &L, uint32_t cap, const cticp_resolution_param &rp);
     void RebuildLevel(size_t i, uint64_t new_cap);
-    void FreeLevel(MapLevel &L);
     void EnsureScratch(size_t n_upper);
     void EnsureFrameOrigin();
 
     cticp_map_options options_;
     cudaStream_t stream_;
     std::vector<MapLevel> levels_;
-    MapCounters *d_counters_ = nullptr;
-    MapCounters *h_counters_ = nullptr;   // pinned
-    void *d_scalar_ = nullptr;
-    int *d_next_ = nullptr;
-    uint32_t *d_touched_ = nullptr;
-    size_t scratch_n_ = 0;
-    double *d_world_tmp_ = nullptr;
-    size_t world_tmp_n_ = 0;
+    std::vector<LevelStorage> storage_;   // storage_[i] owns what levels_[i] points to
+    DeviceArray<MapCounters> d_counters_;
+    PinnedArray<MapCounters> h_counters_;
+    DeviceArray<int> d_scalar_;
+    DeviceArray<int> d_next_;
+    DeviceArray<uint32_t> d_touched_;
+    DeviceArray<double> d_world_tmp_;
     bool dirty_ = true;
     bool readback_pending_ = false;
     bool with_normals_ = false;
-    double *d_frame_origins_ = nullptr;   // [3 * frame_capacity_] begin position of every inserted frame
-    size_t frame_capacity_ = 0, frame_count_ = 0;
+    DeviceArray<double> d_frame_origins_;   // 3 doubles per frame: begin position of every inserted frame
+    size_t frame_count_ = 0;
     int launches_ = 0;
     int rebuilds_ = 0;
     int fused_grid_ = 0;

@@ -18,14 +18,6 @@
 
 namespace cticp {
 
-#define CT_CUDA_CHECK(expr)                                                                              \
-    do {                                                                                                 \
-        cudaError_t _e = (expr);                                                                         \
-        if (_e != cudaSuccess)                                                                           \
-            throw CudaError(std::string(#expr) + ": " + cudaGetErrorString(_e) + " @" + __FILE__ + ":" + \
-                            std::to_string(__LINE__));                                                   \
-    } while (0)
-
 // NVTX range of one stage of RegisterFrame (ingest / sample / icp / map_update / egress): timelines of ncu / nsys-less tools
 // attribute the launches to the stage that enqueued them
 struct NvtxRange {
@@ -133,63 +125,36 @@ Engine::Engine(const cticp_odometry_options &options, int device) : options_(opt
     {
         pool_ = std::make_unique<HostPool>(HostTeamSize(1));
     }
-    CT_CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+    stream_ = cticp::Stream(cudaStreamNonBlocking);
     // per-voxel normals are only read by the DistanceBasedStrategy's sensor-side filter (map.h:482-490)
     const bool with_normals = options_.map_options.select_valid_normals_direction &&
                               options_.neighborhood_strategy.type == CTICP_STRATEGY_DISTANCE_BASED;
-    map_ = std::make_unique<DeviceMap>(options_.map_options, stream_, with_normals);
+    map_ = std::make_unique<DeviceMap>(options_.map_options, stream_.get(), with_normals);
     const size_t max_pts = options_.max_points_per_frame ? (size_t) options_.max_points_per_frame : (size_t) 524288;
-    pipe_ = std::make_unique<FramePipeline>(max_pts, stream_);
-    icp_ = std::make_unique<IcpSolver>(stream_);
-    CT_CUDA_CHECK(cudaMalloc(&d_state_, sizeof(IcpState)));
-    CT_CUDA_CHECK(cudaMallocHost(&h_state_, sizeof(IcpState)));
-    CT_CUDA_CHECK(cudaMalloc(&d_verdict_, sizeof(FrameVerdict)));
-    CT_CUDA_CHECK(cudaMemsetAsync(d_verdict_, 0, sizeof(FrameVerdict), stream_));
-    CT_CUDA_CHECK(cudaHostAlloc(&h_verdict_, sizeof(FrameVerdict), cudaHostAllocMapped));
-    memset(h_verdict_, 0, sizeof(FrameVerdict));
-    CT_CUDA_CHECK(cudaHostGetDevicePointer((void **) &h_verdict_dev_, h_verdict_, 0));
-    CT_CUDA_CHECK(cudaStreamCreateWithFlags(&aux_stream_, cudaStreamNonBlocking));
-    CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_state_up_, cudaEventDisableTiming));
-    CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_group_done_, cudaEventDisableTiming));
-    CT_CUDA_CHECK(cudaMalloc(&d_kp_world_, sizeof(double) * 3 * max_pts));
-    for (auto &e : ev_) CT_CUDA_CHECK(cudaEventCreate(&e));
-    for (auto &e : timer_ev_) CT_CUDA_CHECK(cudaEventCreate(&e));
-    CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_producer_, cudaEventDisableTiming));
-    CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_device_egress_, cudaEventDisableTiming));
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    pipe_ = std::make_unique<FramePipeline>(max_pts, stream_.get());
+    icp_ = std::make_unique<IcpSolver>(stream_.get());
+    d_state_.reserve(1, stream_.get());
+    h_state_.reserve(1, stream_.get());
+    d_verdict_.reserve(1, stream_.get());
+    CT_CUDA_CHECK(cudaMemsetAsync(d_verdict_.data(), 0, sizeof(FrameVerdict), stream_.get()));
+    h_verdict_.reserve(1, stream_.get());
+    memset(h_verdict_.data(), 0, sizeof(FrameVerdict));
+    CT_CUDA_CHECK(cudaHostGetDevicePointer((void **) &h_verdict_dev_, h_verdict_.data(), 0));
+    aux_stream_ = cticp::Stream(cudaStreamNonBlocking);
+    ev_state_up_ = Event(cudaEventDisableTiming);
+    ev_group_done_ = Event(cudaEventDisableTiming);
+    d_kp_world_.reserve(3 * max_pts, stream_.get());
+    for (auto &e : ev_) e = Event(cudaEventDefault);
+    for (auto &e : timer_ev_) e = Event(cudaEventDefault);
+    ev_producer_ = Event(cudaEventDisableTiming);
+    ev_device_egress_ = Event(cudaEventDisableTiming);
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
 }
 
 Engine::~Engine() {
     cudaSetDevice(device_);
-    if (stream_) cudaStreamSynchronize(stream_);
+    if (stream_.get()) cudaStreamSynchronize(stream_.get());
     DestroySharding();
-    icp_.reset();
-    pipe_.reset();
-    map_.reset();
-    cudaFree(d_state_);
-    cudaFreeHost(h_state_);
-    cudaFree(d_verdict_);
-    cudaFreeHost(h_verdict_);
-    if (ev_state_up_) cudaEventDestroy(ev_state_up_);
-    if (ev_group_done_) cudaEventDestroy(ev_group_done_);
-    if (aux_stream_) cudaStreamDestroy(aux_stream_);
-    cudaFree(d_kp_world_);
-    for (auto &e : ev_) cudaEventDestroy(e);
-    for (auto &e : timer_ev_) cudaEventDestroy(e);
-    if (ev_producer_) cudaEventDestroy(ev_producer_);
-    if (ev_device_egress_) cudaEventDestroy(ev_device_egress_);
-    for (auto &sc : staged_) { cudaFree(sc.d_points); cudaFree(sc.d_lo); }
-    cudaFree(d_flush_);
-    for (int i = 0; i < 3; ++i) {
-        cudaFreeHost(h_world_[i]);
-        cudaFreeHost(h_src_[i]);
-    }
-    if (ev_egress_main_) cudaEventDestroy(ev_egress_main_);
-    if (ev_egress_done_) cudaEventDestroy(ev_egress_done_);
-    for (auto &e : ev_egress_chunk_)
-        if (e) cudaEventDestroy(e);
-    if (egress_stream_) cudaStreamDestroy(egress_stream_);
-    if (stream_) cudaStreamDestroy(stream_);
 }
 
 void Engine::Reset() {   // odometry.cpp:956-965
@@ -204,8 +169,8 @@ void Engine::Reset() {   // odometry.cpp:956-965
     default_motion_model_ = MotionModel();
     last_num_keypoints_ = 0;   // grid-size hint: keeps a reset run bit-identical to a fresh one
     last_all_world_valid_ = last_kp_world_valid_ = false;
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    if (egress_stream_) CT_CUDA_CHECK(cudaStreamSynchronize(egress_stream_));
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
+    if (egress_stream_.get()) CT_CUDA_CHECK(cudaStreamSynchronize(egress_stream_.get()));
     egress_pending_ = false;
     egress_valid_[0] = egress_valid_[1] = egress_valid_[2] = false;
     tail_event_valid_ = false;
@@ -218,17 +183,17 @@ void Engine::SetSummaryPoints(int mask) {
     if (summary_points_mask_) AllocEgress();
 }
 void Engine::AllocEgress() {
-    if (!egress_stream_) {
-        CT_CUDA_CHECK(cudaStreamCreateWithFlags(&egress_stream_, cudaStreamNonBlocking));
-        CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_egress_main_, cudaEventDisableTiming));
-        CT_CUDA_CHECK(cudaEventCreateWithFlags(&ev_egress_done_, cudaEventDisableTiming));
-        for (auto &e : ev_egress_chunk_) CT_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    if (!ev_egress_chunk_[kEgressChunks - 1].get()) {   // created last: a set that failed part way is created again
+        egress_stream_ = cticp::Stream(cudaStreamNonBlocking);
+        ev_egress_main_ = Event(cudaEventDisableTiming);
+        ev_egress_done_ = Event(cudaEventDisableTiming);
+        for (auto &e : ev_egress_chunk_) e = Event(cudaEventDisableTiming);
     }
     const size_t cap = pipe_->MaxPoints();
     for (int i = 0; i < 3; ++i) {
         if (!(summary_points_mask_ & (1 << i))) continue;
-        if (!h_world_[i]) CT_CUDA_CHECK(cudaMallocHost(&h_world_[i], sizeof(double) * 3 * cap));
-        if (i != CTICP_POINTS_ALL_CORRECTED && !h_src_[i]) CT_CUDA_CHECK(cudaMallocHost(&h_src_[i], sizeof(uint32_t) * cap));
+        h_world_[i].reserve(3 * cap, stream_.get());
+        if (i != CTICP_POINTS_ALL_CORRECTED) h_src_[i].reserve(cap, stream_.get());
     }
     if (summary_points_mask_ & (1 << CTICP_POINTS_ALL_CORRECTED)) pipe_->EnsureAllWorld();
 }
@@ -243,15 +208,15 @@ void Engine::EnqueueEgress(const HostFrame &f, bool ran_icp) {
     const V3 tb = f.begin_pose.pose.t, te = f.end_pose.pose.t;
     const size_t n_all = pipe_->n(), n_frame = (size_t) pipe_->h_counts()[1];
     const size_t n_kp = (ran_icp && keypoints_in_summary_) ? (size_t) pipe_->h_counts()[2] : 0;
-    cudaStream_t es = egress_stream_;
+    cudaStream_t es = egress_stream_.get();
     if (summary_points_mask_ & (1 << CTICP_POINTS_ALL_CORRECTED)) {
         pipe_->TransformAll(qb, tb, qe, te, es);
         for (int c = 0; c < kEgressChunks; ++c) {
             const size_t b = n_all * (size_t) c / kEgressChunks, e = n_all * (size_t) (c + 1) / kEgressChunks;
             if (e > b)
-                CT_CUDA_CHECK(cudaMemcpyAsync(h_world_[1] + 3 * b, pipe_->d_all_world() + 3 * b, sizeof(double) * 3 * (e - b),
+                CT_CUDA_CHECK(cudaMemcpyAsync(h_world_[1].data() + 3 * b, pipe_->d_all_world() + 3 * b, sizeof(double) * 3 * (e - b),
                                               cudaMemcpyDeviceToHost, es));
-            CT_CUDA_CHECK(cudaEventRecord(ev_egress_chunk_[c], es));
+            CT_CUDA_CHECK(cudaEventRecord(ev_egress_chunk_[c].get(), es));
         }
         last_all_world_valid_ = true;
         egress_valid_[1] = true;
@@ -261,9 +226,9 @@ void Engine::EnqueueEgress(const HostFrame &f, bool ran_icp) {
     if ((summary_points_mask_ & (1 << CTICP_POINTS_KEYPOINTS))) {
         if (n_kp) {
             pipe_->TransformInto(pipe_->d_keypoints(), pipe_->d_keypoints_lo(), pipe_->d_count_keypoints(), qb, tb, qe, te,
-                                 d_kp_world_, es);
-            CT_CUDA_CHECK(cudaMemcpyAsync(h_world_[2], d_kp_world_, sizeof(double) * 3 * n_kp, cudaMemcpyDeviceToHost, es));
-            CT_CUDA_CHECK(cudaMemcpyAsync(h_src_[2], pipe_->d_keypoints_src(), sizeof(uint32_t) * n_kp, cudaMemcpyDeviceToHost, es));
+                                 d_kp_world_.data(), es);
+            CT_CUDA_CHECK(cudaMemcpyAsync(h_world_[2].data(), d_kp_world_.data(), sizeof(double) * 3 * n_kp, cudaMemcpyDeviceToHost, es));
+            CT_CUDA_CHECK(cudaMemcpyAsync(h_src_[2].data(), pipe_->d_keypoints_src(), sizeof(uint32_t) * n_kp, cudaMemcpyDeviceToHost, es));
             last_kp_world_valid_ = true;
         }
         egress_valid_[2] = true;
@@ -271,15 +236,15 @@ void Engine::EnqueueEgress(const HostFrame &f, bool ran_icp) {
         timing_.d2h_bytes += (sizeof(double) * 3 + sizeof(uint32_t)) * n_kp;
     }
     if (summary_points_mask_ & (1 << CTICP_POINTS_CORRECTED)) {
-        CT_CUDA_CHECK(cudaEventRecord(ev_egress_main_, stream_));          // d_frame_world is written by the main stream
-        CT_CUDA_CHECK(cudaStreamWaitEvent(es, ev_egress_main_, 0));
-        CT_CUDA_CHECK(cudaMemcpyAsync(h_world_[0], pipe_->d_frame_world(), sizeof(double) * 3 * n_frame, cudaMemcpyDeviceToHost, es));
-        CT_CUDA_CHECK(cudaMemcpyAsync(h_src_[0], pipe_->d_frame_src(), sizeof(uint32_t) * n_frame, cudaMemcpyDeviceToHost, es));
+        CT_CUDA_CHECK(cudaEventRecord(ev_egress_main_.get(), stream_.get()));          // d_frame_world is written by the main stream
+        CT_CUDA_CHECK(cudaStreamWaitEvent(es, ev_egress_main_.get(), 0));
+        CT_CUDA_CHECK(cudaMemcpyAsync(h_world_[0].data(), pipe_->d_frame_world(), sizeof(double) * 3 * n_frame, cudaMemcpyDeviceToHost, es));
+        CT_CUDA_CHECK(cudaMemcpyAsync(h_src_[0].data(), pipe_->d_frame_src(), sizeof(uint32_t) * n_frame, cudaMemcpyDeviceToHost, es));
         egress_valid_[0] = true;
         egress_count_[0] = n_frame;
         timing_.d2h_bytes += (sizeof(double) * 3 + sizeof(uint32_t)) * n_frame;
     }
-    CT_CUDA_CHECK(cudaEventRecord(ev_egress_done_, es));
+    CT_CUDA_CHECK(cudaEventRecord(ev_egress_done_.get(), es));
     egress_pending_ = true;
 }
 
@@ -338,14 +303,14 @@ void Engine::IngestImpl(const ScanView &scan, const FrameInfo &info, int64_t sta
     // TPose::InterpolatePose CHECK (types.h:456): begin <= t <= end for every timestamp that gets interpolated
     const double t_lo = (k <= 1) ? info.end_timestamp : info.begin_timestamp, t_hi = info.end_timestamp;
     if (!(bts <= t_lo && t_hi <= ets)) {
-        cudaStreamSynchronize(stream_);   // the scan's H2D copy may be in flight: leave the staging buffer quiescent
+        cudaStreamSynchronize(stream_.get());   // the scan's H2D copy may be in flight: leave the staging buffer quiescent
         staging_in_flight_ = false;
         throw TimestampError("The timestamp cannot be interpolated between the two poses");
     }
     if (n > pipe_->MaxPoints()) throw CapacityError("scan has more points than max_points_per_frame");
 
     // host buffers were packed and their H2D copy enqueued by PackAndUpload (PrepareFrame) before the pose pair existed
-    if (staged_slot >= 0) pipe_->UploadFromDevice(staged_[staged_slot].d_points, staged_[staged_slot].d_lo, n);   // already packed, already in HBM: read in place
+    if (staged_slot >= 0) pipe_->UploadFromDevice(staged_[staged_slot].d_points.data(), staged_[staged_slot].d_lo.data(), n);   // already packed, already in HBM: read in place
     timing_.h2d_bytes += pipe_->h2d_bytes();
     const double sample_size = k < options_.init_num_frames ? options_.init_voxel_size : options_.voxel_size;
     // frames 0 and 1: every timestamp := end_timestamp (odometry.cpp:355-359)
@@ -625,7 +590,7 @@ void Engine::PackAndUpload(const ScanView &scan, const double *pose_timestamps, 
     // piece boundaries on multiples of 4 points (= one 64-byte line of the staging buffer per 4 NT stores)
     auto piece_begin = [&](size_t piece) { return piece >= pieces ? n : (n * piece / pieces) & ~size_t(3); };
     pipe_->UploadBegin(n);
-    if (debug) cudaEventRecord(ev_[4], stream_);
+    if (debug) cudaEventRecord(ev_[4].get(), stream_.get());
     const bool fast = F64FastPath(scan);
     const auto t_region = hclock::now();
     double dbg_barrier_ms = 0, dbg_round_ms[kRounds] = {0, 0, 0, 0};   // part 0's view (CTICP_DEBUG_TIMERS)
@@ -707,7 +672,7 @@ void Engine::PackAndUpload(const ScanView &scan, const double *pose_timestamps, 
         pipe_->UploadLo(n);
     }
     if (debug) {
-        cudaEventRecord(ev_[5], stream_);
+        cudaEventRecord(ev_[5].get(), stream_.get());
         fprintf(stderr, "[cticp] pack region (%d parts, %d packers): min/max + barrier at %.3f ms, rounds complete at %.3f %.3f %.3f %.3f, "
                 "region end %.3f ms\n", parts, packers, dbg_barrier_ms, dbg_round_ms[0], dbg_round_ms[1], dbg_round_ms[2],
                 dbg_round_ms[3], ms_since(t_region));
@@ -748,50 +713,45 @@ int64_t Engine::StageFrame(const ScanView &scan) {
     StagedScan sc;
     sc.n = n;
     MinMaxTimestamps(scan, &sc.t_min, &sc.t_max);
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));   // the pinned staging buffer may still feed a previous copy
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));   // the pinned staging buffer may still feed a previous copy
     const bool needs_lo = PackScan(scan, sc.t_min, sc.t_max, pipe_->Staging());
     float4 *stage_lo = needs_lo ? pipe_->StagingLo() : nullptr;
     if (needs_lo) PackLoPlane(scan, sc.t_min, sc.t_max, stage_lo);
-    CT_CUDA_CHECK(cudaMalloc(&sc.d_points, sizeof(float4) * n));
-    CT_CUDA_CHECK(cudaMemcpyAsync(sc.d_points, pipe_->Staging(), sizeof(float4) * n, cudaMemcpyHostToDevice, stream_));
+    sc.d_points.reserve(n, stream_.get());
+    CT_CUDA_CHECK(cudaMemcpyAsync(sc.d_points.data(), pipe_->Staging(), sizeof(float4) * n, cudaMemcpyHostToDevice, stream_.get()));
     if (needs_lo) {
-        CT_CUDA_CHECK(cudaMalloc(&sc.d_lo, sizeof(float4) * n));
-        CT_CUDA_CHECK(cudaMemcpyAsync(sc.d_lo, stage_lo, sizeof(float4) * n, cudaMemcpyHostToDevice, stream_));
+        sc.d_lo.reserve(n, stream_.get());
+        CT_CUDA_CHECK(cudaMemcpyAsync(sc.d_lo.data(), stage_lo, sizeof(float4) * n, cudaMemcpyHostToDevice, stream_.get()));
     }
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    staged_.push_back(sc);
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
+    staged_.push_back(std::move(sc));
     return (int64_t) staged_.size() - 1;
 }
 void Engine::ClearStaged() {
     CT_CUDA_CHECK(cudaSetDevice(device_));
     // the last registered scan may be a staged one, read in place: the pipeline keeps its own copy (points() of that frame
     // stay valid), and the egress of that frame must be done reading it
-    if (egress_stream_) CT_CUDA_CHECK(cudaStreamSynchronize(egress_stream_));
+    if (egress_stream_.get()) CT_CUDA_CHECK(cudaStreamSynchronize(egress_stream_.get()));
     pipe_->DetachRaw();
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    for (auto &sc : staged_) { cudaFree(sc.d_points); cudaFree(sc.d_lo); }
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
     staged_.clear();
 }
 void Engine::TimerStart() {
     CT_CUDA_CHECK(cudaSetDevice(device_));
-    CT_CUDA_CHECK(cudaEventRecord(timer_ev_[0], stream_));
+    CT_CUDA_CHECK(cudaEventRecord(timer_ev_[0].get(), stream_.get()));
 }
 double Engine::TimerStop() {
     CT_CUDA_CHECK(cudaSetDevice(device_));
-    CT_CUDA_CHECK(cudaEventRecord(timer_ev_[1], stream_));
-    CT_CUDA_CHECK(cudaEventSynchronize(timer_ev_[1]));
+    CT_CUDA_CHECK(cudaEventRecord(timer_ev_[1].get(), stream_.get()));
+    CT_CUDA_CHECK(cudaEventSynchronize(timer_ev_[1].get()));
     float ms = 0.f;
-    CT_CUDA_CHECK(cudaEventElapsedTime(&ms, timer_ev_[0], timer_ev_[1]));
+    CT_CUDA_CHECK(cudaEventElapsedTime(&ms, timer_ev_[0].get(), timer_ev_[1].get()));
     return (double) ms;
 }
 void Engine::FlushL2(size_t bytes) {
     CT_CUDA_CHECK(cudaSetDevice(device_));
-    if (bytes > flush_bytes_) {
-        cudaFree(d_flush_);
-        CT_CUDA_CHECK(cudaMalloc(&d_flush_, bytes));
-        flush_bytes_ = bytes;
-    }
-    CT_CUDA_CHECK(cudaMemsetAsync(d_flush_, 0x5A, bytes, stream_));
+    d_flush_.reserve(bytes, stream_.get());
+    CT_CUDA_CHECK(cudaMemsetAsync(d_flush_.data(), 0x5A, bytes, stream_.get()));
 }
 
 // TryRegister, odometry.cpp:525-601, in three parts: the work up to the ICP launch, the launch, the work after it
@@ -817,7 +777,7 @@ void Engine::TryRegisterBegin(const FrameInfo &info, cticp_icp_options &options,
     rs.t_sampling = ms_since(t0);
     if (callback_) {   // odometry.cpp:568: the keypoint count is needed on the host for the hook's GetPoints
         pipe_->QueueCountsReadback();
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+        CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
         staging_in_flight_ = false;
         keypoints_in_summary_ = true;   // the hook receives the sampled keypoints (odometry.cpp:568)
         FireEvent(CTICP_EVENT_BEFORE_ITERATION, rs, info);
@@ -827,7 +787,7 @@ void Engine::TryRegisterBegin(const FrameInfo &info, cticp_icp_options &options,
         options.num_iters_icp = std::max(options.num_iters_icp, 15);
     }
     // registration state → device
-    IcpState &S = *h_state_;
+    IcpState &S = *h_state_.data();
     memset(&S, 0, sizeof(S));
     const Q4 qb = qnormalized(rs.frame.begin_pose.pose.q), qe = qnormalized(rs.frame.end_pose.pose.q);
     S.qb[0] = qb.x; S.qb[1] = qb.y; S.qb[2] = qb.z; S.qb[3] = qb.w;
@@ -852,12 +812,12 @@ void Engine::TryRegisterBegin(const FrameInfo &info, cticp_icp_options &options,
     if (tail_armed_) {
         // nothing on stream_ touches d_state_ until the ICP kernel (the previous frame's readers completed before its verdict
         // arrived): the state goes up on the second stream while the sampler is still running
-        CT_CUDA_CHECK(cudaMemcpyAsync(d_state_, h_state_, sizeof(IcpState), cudaMemcpyHostToDevice, aux_stream_));
-        CT_CUDA_CHECK(cudaEventRecord(ev_state_up_, aux_stream_));
-        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_state_up_, 0));
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_state_.data(), h_state_.data(), sizeof(IcpState), cudaMemcpyHostToDevice, aux_stream_.get()));
+        CT_CUDA_CHECK(cudaEventRecord(ev_state_up_.get(), aux_stream_.get()));
+        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_.get(), ev_state_up_.get(), 0));
     } else
-        CT_CUDA_CHECK(cudaMemcpyAsync(d_state_, h_state_, sizeof(IcpState), cudaMemcpyHostToDevice, stream_));
-    CT_CUDA_CHECK(cudaEventRecord(ev_[1], stream_));
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_state_.data(), h_state_.data(), sizeof(IcpState), cudaMemcpyHostToDevice, stream_.get()));
+    CT_CUDA_CHECK(cudaEventRecord(ev_[1].get(), stream_.get()));
     if (tail_armed_) tail_in_.seq = ++verdict_seq_;
 }
 
@@ -870,7 +830,7 @@ void Engine::LaunchIcp(const cticp_icp_options &options) {
     if (tail_armed_) {
         tail.in = tail_in_;
         tail.counts = pipe_->d_counts();
-        tail.dv = d_verdict_;
+        tail.dv = d_verdict_.data();
         tail.hv = h_verdict_dev_;
         tail.enabled = 1;
     }
@@ -878,30 +838,30 @@ void Engine::LaunchIcp(const cticp_icp_options &options) {
         case CTICP_SOLVER_GN:
             verdict_by_icp_kernel_ =
                 icp_->EnqueueGaussNewton(*map_, options, pipe_->d_keypoints(), pipe_->d_count_keypoints(), KeypointHint(),
-                                         options.num_iters_icp, d_state_, shard_rank_, shard_world_, nccl_comm_,
+                                         options.num_iters_icp, d_state_.data(), shard_rank_, shard_world_, nccl_comm_,
                                          (tail_armed_ && tail_in_kernel_) ? &tail : nullptr);
             break;
         case CTICP_SOLVER_CERES:
         case CTICP_SOLVER_ROBUST:
             icp_->EnqueueCeres(*map_, options, options_.neighborhood_strategy, pipe_->d_keypoints(),
-                               pipe_->d_count_keypoints(), KeypointHint(), pipe_->n(), d_state_, shard_rank_, shard_world_,
+                               pipe_->d_count_keypoints(), KeypointHint(), pipe_->n(), d_state_.data(), shard_rank_, shard_world_,
                                nccl_comm_);
             break;
         default:
             throw UnsupportedError("Unsupported Solver Type");
     }
-    CT_CUDA_CHECK(cudaEventRecord(ev_[2], stream_));
+    CT_CUDA_CHECK(cudaEventRecord(ev_[2].get(), stream_.get()));
 }
 
 GnProblem Engine::IcpProblem(const PendingFrame &f) const {
     return GnProblem{map_.get(), &f.icp_options, pipe_->d_keypoints(), pipe_->d_keypoints_lo(), pipe_->d_count_keypoints(),
-                     KeypointHint(), f.icp_options.num_iters_icp, d_state_};
+                     KeypointHint(), f.icp_options.num_iters_icp, d_state_.data()};
 }
 
 void Engine::AdoptGroupedIcp(PendingFrame &f, cudaEvent_t launched, int groups) {
     CT_CUDA_CHECK(cudaSetDevice(device_));
-    CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, launched, 0));
-    CT_CUDA_CHECK(cudaEventRecord(ev_[2], stream_));
+    CT_CUDA_CHECK(cudaStreamWaitEvent(stream_.get(), launched, 0));
+    CT_CUDA_CHECK(cudaEventRecord(ev_[2].get(), stream_.get()));
     verdict_by_icp_kernel_ = false;
     timing_.icp_batch_groups = groups;
     f.icp_launched = true;
@@ -914,7 +874,7 @@ void Engine::TryRegisterEnd(const FrameInfo &info, const cticp_icp_options &opti
         // verdict's sequence number in mapped pinned memory, not for the stream
         tail_armed_ = false;
         if (!verdict_by_icp_kernel_) {   // (k_gn_persistent's solver CTA writes the verdict itself)
-            k_frame_policy<<<1, 32, 0, stream_>>>(d_state_, pipe_->d_counts(), tail_in_, d_verdict_, h_verdict_dev_);
+            k_frame_policy<<<1, 32, 0, stream_.get()>>>(d_state_.data(), pipe_->d_counts(), tail_in_, d_verdict_.data(), h_verdict_dev_);
             CT_CUDA_CHECK(cudaGetLastError());
             tail_launches_ += 1;
         }
@@ -922,23 +882,23 @@ void Engine::TryRegisterEnd(const FrameInfo &info, const cticp_icp_options &opti
             NvtxRange range_map("cticp.map_update");
             map_->UpdateFused(pipe_->d_frame(), pipe_->d_frame_lo(), pipe_->d_count_frame(), pipe_->n(), pipe_->d_frame_world_mut(),
                               Q4{0, 0, 0, 1}, V3{0, 0, 0}, Q4{0, 0, 0, 1}, V3{0, 0, 0}, true, V3{0, 0, 0}, options_.max_distance,
-                              true, V3{0, 0, 0}, d_verdict_);
+                              true, V3{0, 0, 0}, d_verdict_.data());
         }
         tail_launched_ = true;
         WaitVerdict(tail_in_.seq);
-        memcpy(h_state_, &h_verdict_->state, sizeof(IcpState));
-        pipe_->SetHostCounts(h_verdict_->counts);
+        memcpy(h_state_.data(), &h_verdict_.data()->state, sizeof(IcpState));
+        pipe_->SetHostCounts(h_verdict_.data()->counts);
         timing_.d2h_bytes += sizeof(FrameVerdict);
     } else {
-        CT_CUDA_CHECK(cudaMemcpyAsync(h_state_, d_state_, sizeof(IcpState), cudaMemcpyDeviceToHost, stream_));
+        CT_CUDA_CHECK(cudaMemcpyAsync(h_state_.data(), d_state_.data(), sizeof(IcpState), cudaMemcpyDeviceToHost, stream_.get()));
         pipe_->QueueCountsReadback();
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+        CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
         timing_.d2h_bytes += sizeof(IcpState) + sizeof(int) * 4;
     }
     staging_in_flight_ = false;
     icp_->CollectGatherTiming();
     timing_.h2d_bytes += sizeof(IcpState);
-    const IcpState &S = *h_state_;
+    const IcpState &S = *h_state_.data();
 
     if (getenv("CTICP_DEBUG_TIMERS"))
         fprintf(stderr, "[cticp] GN loop, solver CTA (SM cycles over %d iterations, needs a -DCTICP_DEBUG_TIMERS build): loop %llu, "
@@ -977,8 +937,8 @@ void Engine::TryRegisterEnd(const FrameInfo &info, const cticp_icp_options &opti
     // persistent launch (solver GN), else the whole iteration is reported as neighborhood time
     {
         float icp_ms = 0.f;
-        if (tail_launched_) cudaEventSynchronize(ev_[2]);   // (complete: the verdict's kernel ran behind it)
-        if (cudaEventElapsedTime(&icp_ms, ev_[1], ev_[2]) != cudaSuccess) {
+        if (tail_launched_) cudaEventSynchronize(ev_[2].get());   // (complete: the verdict's kernel ran behind it)
+        if (cudaEventElapsedTime(&icp_ms, ev_[1].get(), ev_[2].get()) != cudaSuccess) {
             cudaGetLastError();
             icp_ms = 0.f;
         }
@@ -996,11 +956,11 @@ void Engine::TryRegisterEnd(const FrameInfo &info, const cticp_icp_options &opti
 // Spin on the verdict's sequence number (written by k_frame_policy after a system-wide fence). The stream is polled now
 // and then: a faulted kernel must surface as an error, not as a hang.
 void Engine::WaitVerdict(unsigned seq) {
-    volatile unsigned *flag = &h_verdict_->seq;
+    volatile unsigned *flag = &h_verdict_.data()->seq;
     for (unsigned long spins = 1;; ++spins) {
         if (*flag == seq) break;
         if ((spins & 0xfffu) == 0) {
-            const cudaError_t q = cudaStreamQuery(stream_);
+            const cudaError_t q = cudaStreamQuery(stream_.get());
             if (q == cudaSuccess) {
                 if (*flag == seq) break;
                 throw std::runtime_error("the frame verdict never arrived although the stream is idle");
@@ -1014,7 +974,7 @@ void Engine::WaitVerdict(unsigned seq) {
 
 // What UpdateMap (below) does on the host around its launch, for a map update the device has already decided and run.
 void Engine::AdoptDeviceMapUpdate(Summary &s) {
-    const FrameVerdict &v = *h_verdict_;
+    const FrameVerdict &v = *h_verdict_.data();
     const bool inserted = v.action == kFrameInsert;
     tracker_.cum_orientation += s.relative_orientation;
     tracker_.cum_distance += s.relative_distance;
@@ -1243,7 +1203,7 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
     last_all_world_valid_ = last_kp_world_valid_ = frame_world_valid_ = false;
     egress_valid_[0] = egress_valid_[1] = egress_valid_[2] = false;
     if (egress_pending_) {   // the previous frame's egress still reads d_raw / d_frame_world / the keypoints
-        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_egress_done_, 0));
+        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_.get(), ev_egress_done_.get(), 0));
         egress_pending_ = false;
     }
     scan_in_staging_ = staged_slot < 0 && !scan.on_device;
@@ -1257,9 +1217,9 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
     } else if (scan.on_device) {
         // Device memory: the reduce and the pack run on the stream behind the producer's work (and behind the previous
         // frame's map update and egress); the host needs min / max only, the pack runs while it initialises the motion
-        CT_CUDA_CHECK(cudaEventRecord(ev_producer_, scan.producer));
-        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_producer_, 0));
-        CT_CUDA_CHECK(cudaEventRecord(ev_[0], stream_));
+        CT_CUDA_CHECK(cudaEventRecord(ev_producer_.get(), scan.producer));
+        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_.get(), ev_producer_.get(), 0));
+        CT_CUDA_CHECK(cudaEventRecord(ev_[0].get(), stream_.get()));
         double pose_ts[2];
         if (initial_estimate) {
             pose_ts[0] = initial_estimate->begin_pose.dest_timestamp;
@@ -1272,9 +1232,9 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
         // Host buffers: timestamp min/max, packing and the H2D copy, pipelined (PackAndUpload). The copy is enqueued
         // behind the previous frame's map update, which may still be running: the stream keeps the order, and the
         // pinned staging buffer is free (its previous copy completed before that frame's ICP state was read back).
-        if (staging_in_flight_) CT_CUDA_CHECK(cudaStreamSynchronize(stream_));   // only after a call that threw midway
+        if (staging_in_flight_) CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));   // only after a call that threw midway
         staging_in_flight_ = true;
-        CT_CUDA_CHECK(cudaEventRecord(ev_[0], stream_));
+        CT_CUDA_CHECK(cudaEventRecord(ev_[0].get(), stream_.get()));
         double pose_ts[2];
         if (initial_estimate) {
             pose_ts[0] = initial_estimate->begin_pose.dest_timestamp;
@@ -1291,13 +1251,13 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
 
     // the previous frame's map update: its counters tell whether the tables need maintenance. Waits on that frame's
     // last event, NOT on the stream — this frame's H2D copy is already in flight behind it.
-    if (tail_event_valid_) CT_CUDA_CHECK(cudaEventSynchronize(ev_[3]));
-    else CT_CUDA_CHECK(cudaStreamSynchronize(stream_));   // first frame, after Reset(), or after a call that threw
+    if (tail_event_valid_) CT_CUDA_CHECK(cudaEventSynchronize(ev_[3].get()));
+    else CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));   // first frame, after Reset(), or after a call that threw
     tail_event_valid_ = false;
     map_->NotifyStreamSynchronized();
     map_->MaintainTables();
 
-    if (staged_slot >= 0) CT_CUDA_CHECK(cudaEventRecord(ev_[0], stream_));
+    if (staged_slot >= 0) CT_CUDA_CHECK(cudaEventRecord(ev_[0].get(), stream_.get()));
     IngestImpl(scan, info, staged_slot);
     f.t_initialization = ms_since(t_start);
 
@@ -1361,8 +1321,8 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
                       shard_world_ <= 1 && ct_icp_options.max_number_neighbors >= 1 && ct_icp_options.max_number_neighbors <= 32;
         }
     } else {
-        CT_CUDA_CHECK(cudaEventRecord(ev_[1], stream_));
-        CT_CUDA_CHECK(cudaEventRecord(ev_[2], stream_));
+        CT_CUDA_CHECK(cudaEventRecord(ev_[1].get(), stream_.get()));
+        CT_CUDA_CHECK(cudaEventRecord(ev_[2].get(), stream_.get()));
         pipe_->QueueCountsReadback();
     }
 }
@@ -1386,7 +1346,7 @@ void Engine::FinishFrame(PendingFrame &f) {
             summary.ego_orientation = EgoAngularDistance(summary.frame);
             summary.relative_distance = norm(summary.frame.end_pose.pose.t - summary.frame.begin_pose.pose.t);
             bool assessed = AssessRegistration(summary);
-            if (tail_launched_) assessed = h_verdict_->assess_ok != 0;   // the device acted on ITS evaluation of the same formulas
+            if (tail_launched_) assessed = h_verdict_.data()->assess_ok != 0;   // the device acted on ITS evaluation of the same formulas
             if (!assessed) {
                 summary.success = false;
                 if (options_.quit_on_error) early_return = true;
@@ -1402,7 +1362,7 @@ void Engine::FinishFrame(PendingFrame &f) {
         const auto &f = summary.frame;
         if (!ran_icp) {   // frame 0: no pose read-back has synchronised the stream yet; F sizes the map tables / the egress
             pipe_->QueueCountsReadback();
-            CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+            CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
             staging_in_flight_ = false;
         }
         if (!fused_map_update_) {
@@ -1411,7 +1371,7 @@ void Engine::FinishFrame(PendingFrame &f) {
             if (summary_points_mask_) EnqueueEgress(f, ran_icp);
         }
         ComputeSummaryMetrics(summary, k);
-        if (tail_launched_ && h_verdict_->action != kFrameDeferred)
+        if (tail_launched_ && h_verdict_.data()->action != kFrameDeferred)
             AdoptDeviceMapUpdate(summary);   // evicted / inserted already, behind the ICP kernel
         else
             UpdateMap(summary, k);
@@ -1424,10 +1384,10 @@ void Engine::FinishFrame(PendingFrame &f) {
             egress_valid_[0] = e0; egress_valid_[1] = e1; egress_valid_[2] = e2;
         }
     }
-    CT_CUDA_CHECK(cudaEventRecord(ev_[3], stream_));
+    CT_CUDA_CHECK(cudaEventRecord(ev_[3].get(), stream_.get()));
     tail_event_valid_ = true;
     if (!ran_icp) {   // frame 0: counts for the summary
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+        CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
         staging_in_flight_ = false;
     }
 
@@ -1467,15 +1427,15 @@ void Engine::FillSummary(const Summary &s, cticp_summary *out) const {
 cticp_device_timing Engine::LastTiming() {
     cudaSetDevice(device_);
     if (registered_frames_ == 0) {   // nothing recorded yet: querying the events would leave a sticky CUDA error
-        cudaStreamSynchronize(stream_);
+        cudaStreamSynchronize(stream_.get());
         return timing_;
     }
-    cudaEventSynchronize(ev_[3]);
+    cudaEventSynchronize(ev_[3].get());
     float a = 0, b = 0, c = 0, d = 0;
-    cudaEventElapsedTime(&a, ev_[0], ev_[1]);
-    cudaEventElapsedTime(&b, ev_[1], ev_[2]);
-    cudaEventElapsedTime(&c, ev_[2], ev_[3]);
-    cudaEventElapsedTime(&d, ev_[0], ev_[3]);
+    cudaEventElapsedTime(&a, ev_[0].get(), ev_[1].get());
+    cudaEventElapsedTime(&b, ev_[1].get(), ev_[2].get());
+    cudaEventElapsedTime(&c, ev_[2].get(), ev_[3].get());
+    cudaEventElapsedTime(&d, ev_[0].get(), ev_[3].get());
     timing_.ingest_ms = a;
     timing_.icp_ms = b;
     timing_.map_update_ms = c;
@@ -1484,7 +1444,7 @@ cticp_device_timing Engine::LastTiming() {
     timing_.gather_launches = icp_->gather_launches();
     if (getenv("CTICP_DEBUG_TIMERS")) {
         float h = 0, g = 0;
-        if (cudaEventElapsedTime(&h, ev_[4], ev_[5]) == cudaSuccess && cudaEventElapsedTime(&g, ev_[0], ev_[4]) == cudaSuccess)
+        if (cudaEventElapsedTime(&h, ev_[4].get(), ev_[5].get()) == cudaSuccess && cudaEventElapsedTime(&g, ev_[0].get(), ev_[4].get()) == cudaSuccess)
             fprintf(stderr, "[cticp] device: ev0->upload start %.3f ms, H2D %.3f ms\n", g, h);
         cudaGetLastError();
     }
@@ -1580,11 +1540,11 @@ int64_t Engine::WritePointsDevice(int which, const cticp_cloud_sink &sink, cudaS
     const scan_pack::AlphaRange ar = scan_pack::alpha_range(f.begin_pose.dest_timestamp, f.end_pose.dest_timestamp);
     // ordered both ways with the consumer's stream: behind what it queued before (e.g. the sink's allocation), ahead of
     // what it queues next
-    CT_CUDA_CHECK(cudaEventRecord(ev_producer_, consumer));
-    CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_producer_, 0));
+    CT_CUDA_CHECK(cudaEventRecord(ev_producer_.get(), consumer));
+    CT_CUDA_CHECK(cudaStreamWaitEvent(stream_.get(), ev_producer_.get(), 0));
     pipe_->WritePointsDevice(d_pts, d_lo, d_world, m, sink, ar.mn, ar.mx);
-    CT_CUDA_CHECK(cudaEventRecord(ev_device_egress_, stream_));
-    CT_CUDA_CHECK(cudaStreamWaitEvent(consumer, ev_device_egress_, 0));
+    CT_CUDA_CHECK(cudaEventRecord(ev_device_egress_.get(), stream_.get()));
+    CT_CUDA_CHECK(cudaStreamWaitEvent(consumer, ev_device_egress_.get(), 0));
     return (int64_t) count;
 }
 
@@ -1596,7 +1556,7 @@ void Engine::ResolvePoints(int which, const float4 **out_pts, const float4 **out
     // the eager egress (EnqueueEgress) writes d_all_world / the keypoints' world coordinates on its own stream: whatever
     // reads them on the main stream from here on is ordered behind it
     if (egress_pending_) {
-        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_, ev_egress_done_, 0));
+        CT_CUDA_CHECK(cudaStreamWaitEvent(stream_.get(), ev_egress_done_.get(), 0));
         egress_pending_ = false;
     }
     const float4 *d_pts = nullptr, *d_lo = nullptr;
@@ -1628,12 +1588,12 @@ void Engine::ResolvePoints(int which, const float4 **out_pts, const float4 **out
             count = (last_info_.registered_fid > 0 && keypoints_in_summary_) ? (size_t) pipe_->h_counts()[2] : 0;
             if (count && !last_kp_world_valid_) {
                 pipe_->TransformInto(pipe_->d_keypoints(), pipe_->d_keypoints_lo(), pipe_->d_count_keypoints(), f.begin_pose.pose.q,
-                                     f.begin_pose.pose.t, f.end_pose.pose.q, f.end_pose.pose.t, d_kp_world_);
+                                     f.begin_pose.pose.t, f.end_pose.pose.q, f.end_pose.pose.t, d_kp_world_.data());
                 last_kp_world_valid_ = true;
             }
             d_pts = pipe_->d_keypoints();
             d_lo = pipe_->d_keypoints_lo();
-            d_world = d_kp_world_;
+            d_world = d_kp_world_.data();
             break;
         default:
             throw std::invalid_argument("which");
@@ -1655,14 +1615,14 @@ int64_t Engine::GetPoints(int which, cticp_wpoint *dst, size_t cap) {
         const size_t m = std::min(cap, count);
         if (m == 0 || !dst) return (int64_t) count;
         const bool chunked = which == CTICP_POINTS_ALL_CORRECTED;   // copied first and in pieces (EnqueueEgress)
-        if (!chunked) CT_CUDA_CHECK(cudaEventSynchronize(ev_egress_done_));
+        if (!chunked) CT_CUDA_CHECK(cudaEventSynchronize(ev_egress_done_.get()));
         const auto &f = last_frame_;
         const double bts = f.begin_pose.dest_timestamp, ets = f.end_pose.dest_timestamp;
         const double mn = std::min(bts, ets), mx = std::max(bts, ets);
         const float4 *stage = pipe_->Staging();
         const float4 *stage_lo = pipe_->StagingLoIfAny();
-        const double *w = h_world_[which];
-        const uint32_t *src = which == CTICP_POINTS_ALL_CORRECTED ? nullptr : h_src_[which];
+        const double *w = h_world_[which].data();
+        const uint32_t *src = which == CTICP_POINTS_ALL_CORRECTED ? nullptr : h_src_[which].data();
         // frames 0 and 1: the sub-sampled frame (and its keypoints) carry timestamp := end_timestamp (odometry.cpp:355-359)
         const bool override_t = src && last_info_.registered_fid <= 1;
         const double t_override = mn + (double) (float) AlphaTimestamp(last_info_.end_timestamp, bts, ets) * (mx - mn);
@@ -1671,7 +1631,7 @@ int64_t Engine::GetPoints(int which, cticp_wpoint *dst, size_t cap) {
         for (int c = 0; c < pieces; ++c) {
         const size_t pb = chunked ? count * (size_t) c / kEgressChunks : 0;
         const size_t pe = std::min(m, chunked ? count * (size_t) (c + 1) / kEgressChunks : m);
-        if (chunked) CT_CUDA_CHECK(cudaEventSynchronize(ev_egress_chunk_[c]));
+        if (chunked) CT_CUDA_CHECK(cudaEventSynchronize(ev_egress_chunk_[c].get()));
         if (pe <= pb) continue;
         pool_->ParallelFor(pe - pb, [&](size_t b0, size_t e0, int) {
             for (size_t i = pb + b0; i < pb + e0; ++i) {
@@ -1703,10 +1663,10 @@ int64_t Engine::GetPoints(int which, cticp_wpoint *dst, size_t cap) {
     if (m == 0 || !dst) return (int64_t) count;
     std::vector<float4> hp(m), hl(d_lo ? m : 0);
     std::vector<double> hw(3 * m);
-    CT_CUDA_CHECK(cudaMemcpyAsync(hp.data(), d_pts, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_));
-    if (d_lo) CT_CUDA_CHECK(cudaMemcpyAsync(hl.data(), d_lo, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_));
-    CT_CUDA_CHECK(cudaMemcpyAsync(hw.data(), d_world, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost, stream_));
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(hp.data(), d_pts, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_.get()));
+    if (d_lo) CT_CUDA_CHECK(cudaMemcpyAsync(hl.data(), d_lo, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_.get()));
+    CT_CUDA_CHECK(cudaMemcpyAsync(hw.data(), d_world, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost, stream_.get()));
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
     const double bts = f.begin_pose.dest_timestamp, ets = f.end_pose.dest_timestamp;
     const double mn = std::min(bts, ets), mx = std::max(bts, ets);
     for (size_t i = 0; i < m; ++i) {
@@ -1736,11 +1696,11 @@ int64_t Engine::WritePoints(int which, const cticp_cloud_sink &sink) {
     CheckSink(sink);
     std::vector<float4> hp(m), hl(d_lo ? m : 0);
     std::vector<double> hw(sink.world ? 3 * m : 0);
-    CT_CUDA_CHECK(cudaMemcpyAsync(hp.data(), d_pts, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_));
-    if (d_lo) CT_CUDA_CHECK(cudaMemcpyAsync(hl.data(), d_lo, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(hp.data(), d_pts, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_.get()));
+    if (d_lo) CT_CUDA_CHECK(cudaMemcpyAsync(hl.data(), d_lo, sizeof(float4) * m, cudaMemcpyDeviceToHost, stream_.get()));
     if (sink.world)
-        CT_CUDA_CHECK(cudaMemcpyAsync(hw.data(), d_world, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost, stream_));
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
+        CT_CUDA_CHECK(cudaMemcpyAsync(hw.data(), d_world, sizeof(double) * 3 * m, cudaMemcpyDeviceToHost, stream_.get()));
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream_.get()));
     const auto &f = last_frame_;
     const double bts = f.begin_pose.dest_timestamp, ets = f.end_pose.dest_timestamp;
     const double mn = std::min(bts, ets), mx = std::max(bts, ets);

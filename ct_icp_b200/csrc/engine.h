@@ -152,12 +152,12 @@ public:
     // a joining frame's registration in a grouped launch (valid until FinishFrame)
     GnProblem IcpProblem(const PendingFrame &f) const;
     // recorded on the engine's stream after the state upload and the sampling of the pending frame
-    cudaEvent_t IcpReadyEvent() const { return ev_[1]; }
+    cudaEvent_t IcpReadyEvent() const { return ev_[1].get(); }
     // the grouped launch that ran the pending frame's ICP is enqueued, `launched` recorded behind it; `groups` problems
     void AdoptGroupedIcp(PendingFrame &f, cudaEvent_t launched, int groups);
     void FinishFrame(PendingFrame &f);
     // recorded behind a grouped launch this engine's stream carried (RegisterBatch)
-    cudaEvent_t GroupDoneEvent() const { return ev_group_done_; }
+    cudaEvent_t GroupDoneEvent() const { return ev_group_done_.get(); }
 
     void RegisterFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate, cticp_summary *out,
                        const cticp_motion_prior *motion_model = nullptr);
@@ -185,7 +185,7 @@ public:
     void Reset();
     DeviceMap &Map() { return *map_; }
     IcpSolver &Solver() { return *icp_; }
-    cudaStream_t Stream() const { return stream_; }
+    cudaStream_t Stream() const { return stream_.get(); }
     int Device() const { return device_; }
     cticp_device_timing LastTiming();   // synchronises on the last frame's final event
     void SetTimeGather(bool on) { icp_->set_time_gather(on); }
@@ -197,7 +197,11 @@ private:
     void InitializeMotion(const FrameInfo &info, const cticp_frame *initial_estimate);
     void ResolvePoints(int which, const float4 **out_pts, const float4 **out_lo, const double **out_world, size_t *out_count);
     void CheckSink(const cticp_cloud_sink &sink) const;
-    cudaEvent_t ev_producer_ = nullptr, ev_device_egress_ = nullptr;   // device input / output: the caller's stream order
+    // The owning members below are released in reverse declaration order once the destructor has synchronised stream_:
+    // stream_ comes first so that it is destroyed after everything that was enqueued on it, the egress stream after its
+    // events and buffers.
+    cticp::Stream stream_;
+    Event ev_producer_, ev_device_egress_;   // device input / output: the caller's stream order
     void IngestImpl(const ScanView &scan,
                     const FrameInfo &info, int64_t staged_slot);
     bool PackScan(const ScanView &scan, double bts, double ets, float4 *dst);
@@ -219,15 +223,14 @@ private:
     bool fused_sampling_ = true;       // CTICP_FUSED_SAMPLING=0: the two grid selections as separate launches
     bool keypoints_sampled_ = false;   // the keypoints of the coming first attempt were sampled with the frame   // d_frame_world holds the sub-sampled frame under last_frame_
     struct StagedScan {
-        float4 *d_points = nullptr;
-        float4 *d_lo = nullptr;   // residual plane, float64 scans only (se3.cuh load_raw)
+        DeviceArray<float4> d_points;
+        DeviceArray<float4> d_lo;   // residual plane, float64 scans only (se3.cuh load_raw)
         size_t n = 0;
         double t_min = 0, t_max = 0;
     };
     std::vector<StagedScan> staged_;
-    cudaEvent_t timer_ev_[2];
-    void *d_flush_ = nullptr;
-    size_t flush_bytes_ = 0;
+    Event timer_ev_[2];
+    DeviceArray<unsigned char> d_flush_;
     void TryRegister(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
                      const MotionModel *mm, int attempt_idx);
     void TryRegisterBegin(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
@@ -249,17 +252,17 @@ private:
     bool tail_armed_ = false;      // the coming TryRegister enqueues the device tail (tail_in_ is filled)
     bool tail_launched_ = false;   // the last TryRegister did: h_verdict_ holds this frame's verdict
     FramePolicyIn tail_in_{};
-    FrameVerdict *d_verdict_ = nullptr;
-    FrameVerdict *h_verdict_ = nullptr;       // mapped pinned memory
+    DeviceArray<FrameVerdict> d_verdict_;
+    PinnedArray<FrameVerdict> h_verdict_{cudaHostAllocMapped};
     FrameVerdict *h_verdict_dev_ = nullptr;   // its device address
     unsigned verdict_seq_ = 0;
     int tail_launches_ = 0;
     void WaitVerdict(unsigned seq);
     void AdoptDeviceMapUpdate(Summary &s);
     // the registration state goes up on a second stream while the sampler runs (the ICP kernel waits for its event)
-    cudaStream_t aux_stream_ = nullptr;
-    cudaEvent_t ev_state_up_ = nullptr;
-    cudaEvent_t ev_group_done_ = nullptr;
+    cticp::Stream aux_stream_;
+    Event ev_state_up_;
+    Event ev_group_done_;
     void FillSummary(const Summary &s, cticp_summary *out) const;
     // grid-size hint for the ICP kernels: the keypoint count is only known on the device when they are enqueued, so
     // the host sizes the grid from the previous registration (keypoint counts change slowly) with 25% head-room;
@@ -275,12 +278,11 @@ private:
 
     cticp_odometry_options options_;
     int device_;
-    cudaStream_t stream_ = nullptr;
     std::unique_ptr<DeviceMap> map_;
     std::unique_ptr<FramePipeline> pipe_;
     std::unique_ptr<IcpSolver> icp_;
-    IcpState *d_state_ = nullptr;
-    IcpState *h_state_ = nullptr;   // pinned
+    DeviceArray<IcpState> d_state_;
+    PinnedArray<IcpState> h_state_;
     std::vector<HostFrame> trajectory_;
     MotionModel default_motion_model_;
     int registered_frames_ = 0;
@@ -295,25 +297,25 @@ private:
     HostFrame last_frame_;
     FrameInfo last_info_;
     bool last_all_world_valid_ = false, last_kp_world_valid_ = false;
-    double *d_kp_world_ = nullptr;
+    DeviceArray<double> d_kp_world_;
     // eager egress of the summary vectors: world coordinates (+ source indices) to pinned host memory on a second
     // stream, overlapped with the map update; GetPoints assembles the 64-byte records on the host team
     void EnqueueEgress(const HostFrame &f, bool ran_icp);
     void AllocEgress();
     int summary_points_mask_ = 0;
-    cudaStream_t egress_stream_ = nullptr;
-    cudaEvent_t ev_egress_main_ = nullptr, ev_egress_done_ = nullptr;
-    static constexpr int kEgressChunks = 4;            // the N world points go back in pieces: the host assembles the
-    cudaEvent_t ev_egress_chunk_[kEgressChunks] = {};  // records of piece i while piece i + 1 is still on the bus
+    cticp::Stream egress_stream_;
+    Event ev_egress_main_, ev_egress_done_;
+    static constexpr int kEgressChunks = 4;   // the N world points go back in pieces: the host assembles the
+    Event ev_egress_chunk_[kEgressChunks];    // records of piece i while piece i + 1 is still on the bus
     bool egress_pending_ = false;           // ev_egress_done_ recorded, next frame's upload must wait for it
     bool egress_valid_[3] = {false, false, false};
     size_t egress_count_[3] = {0, 0, 0};
-    double *h_world_[3] = {nullptr, nullptr, nullptr};   // pinned: corrected / all corrected / keypoints, xyz triples
-    uint32_t *h_src_[3] = {nullptr, nullptr, nullptr};   // pinned: index into the scan (corrected, keypoints)
+    PinnedArray<double> h_world_[3];     // corrected / all corrected / keypoints, xyz triples
+    PinnedArray<uint32_t> h_src_[3];     // index into the scan (corrected, keypoints)
     bool scan_in_staging_ = false;          // the pinned staging buffer holds the last registered scan
     // timing
     cticp_device_timing timing_{};
-    cudaEvent_t ev_[6];
+    Event ev_[6];
     bool tail_event_valid_ = false;    // ev_[3] (end of the last frame's map update) has been recorded and not yet waited on
     bool staging_in_flight_ = false;   // the pinned staging buffer may still feed an H2D copy
     // multi-GPU

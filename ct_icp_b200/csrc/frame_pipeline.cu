@@ -20,14 +20,6 @@
 
 namespace cticp {
 
-#define CT_CUDA_CHECK(expr)                                                                              \
-    do {                                                                                                 \
-        cudaError_t _e = (expr);                                                                         \
-        if (_e != cudaSuccess)                                                                           \
-            throw CudaError(std::string(#expr) + ": " + cudaGetErrorString(_e) + " @" + __FILE__ + ":" + \
-                            std::to_string(__LINE__));                                                   \
-    } while (0)
-
 constexpr unsigned long long kGridEmpty = ~0ull;
 constexpr size_t kMaxTiles = 4096;   // up to 4M points per scan
 constexpr int kTileShift = 10, kTile = 1 << kTileShift, kTileThreads = kTile / 4;   // 1024 positions per CTA
@@ -669,60 +661,38 @@ static uint32_t NextPow2(uint64_t v) {
 FramePipeline::FramePipeline(size_t max_points, cudaStream_t stream) : stream_(stream), max_points_(max_points) {
     const size_t n = max_points_;
     if (const char *e = getenv("CTICP_SAMPLE_PRECLEAR")) preclear_ = atoi(e) != 0;
-    grid_cap_ = std::max<uint32_t>(NextPow2(2 * n), 1024);
-    CT_CUDA_CHECK(cudaMallocHost(&h_stage_, sizeof(float4) * n));
-    CT_CUDA_CHECK(cudaMallocHost(&h_counts_, sizeof(int) * 8));
-    CT_CUDA_CHECK(cudaMalloc(&d_raw_, sizeof(float4) * n));
-    raw_ptr_ = d_raw_;
-    CT_CUDA_CHECK(cudaMalloc(&d_frame_, sizeof(float4) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_keypoints_, sizeof(float4) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_tmp_points_, sizeof(float4) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_frame_src_, sizeof(uint32_t) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_kp_src_, sizeof(uint32_t) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_tmp_src_, sizeof(uint32_t) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_grid_, sizeof(unsigned long long) * 2 * (size_t) grid_cap_));
-    CT_CUDA_CHECK(cudaMalloc(&d_slot_of_, sizeof(int) * n));
     if ((n + kTile - 1) / kTile > kMaxTiles) throw std::invalid_argument("max_points_per_frame too large");
-    CT_CUDA_CHECK(cudaMalloc(&d_win_, sizeof(uint32_t) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_desc_, sizeof(unsigned long long) * kDescWords));
-    CT_CUDA_CHECK(cudaMemsetAsync(d_desc_, 0, sizeof(unsigned long long) * kDescWords, stream_));
-    CT_CUDA_CHECK(cudaMalloc(&d_src_, sizeof(uint32_t) * n));
-    CT_CUDA_CHECK(cudaMalloc(&d_counts_, sizeof(int) * 8));
-    CT_CUDA_CHECK(cudaMalloc(&d_frame_world_, sizeof(double) * 3 * n));
-    CT_CUDA_CHECK(cudaMemsetAsync(d_counts_, 0, sizeof(int) * 8, stream_));
-    memset(h_counts_, 0, sizeof(int) * 8);
-}
-FramePipeline::~FramePipeline() {
-    cudaFreeHost(h_stage_); cudaFreeHost(h_counts_);
-    cudaFree(d_raw_); cudaFree(d_frame_); cudaFree(d_keypoints_); cudaFree(d_tmp_points_);
-    cudaFreeHost(h_stage_lo_);
-    cudaFree(d_raw_lo_); cudaFree(d_frame_lo_); cudaFree(d_kp_lo_); cudaFree(d_tmp_lo_);
-    cudaFree(d_frame_src_); cudaFree(d_kp_src_); cudaFree(d_tmp_src_);
-    cudaFree(d_grid_); cudaFree(d_slot_of_); cudaFree(d_win_); cudaFree(d_desc_); cudaFree(d_src_);
-    cudaFree(d_counts_); cudaFree(d_frame_world_); cudaFree(d_all_world_); cudaFree(d_adaptive_);
-    cudaFree(d_grid2_);
-    cudaFree(d_scan_partials_); cudaFree(d_scan_ticket_); cudaFree(d_scan_reduce_); cudaFreeHost(h_scan_reduce_);
+    grid_cap_ = std::max<uint32_t>(NextPow2(2 * n), 1024);
+    h_stage_.reserve(n, stream_);
+    h_counts_.reserve(8, stream_);
+    for (auto *a : {&d_raw_, &d_frame_, &d_keypoints_, &d_tmp_points_}) a->reserve(n, stream_);
+    raw_ptr_ = d_raw_.data();
+    for (auto *a : {&d_frame_src_, &d_kp_src_, &d_tmp_src_, &d_win_, &d_src_}) a->reserve(n, stream_);
+    d_grid_.reserve(2 * (size_t) grid_cap_, stream_);
+    d_slot_of_.reserve(n, stream_);
+    d_desc_.reserve(kDescWords, stream_);
+    CT_CUDA_CHECK(cudaMemsetAsync(d_desc_.data(), 0, sizeof(unsigned long long) * kDescWords, stream_));
+    d_counts_.reserve(8, stream_);
+    d_frame_world_.reserve(3 * n, stream_);
+    CT_CUDA_CHECK(cudaMemsetAsync(d_counts_.data(), 0, sizeof(int) * 8, stream_));
+    memset(h_counts_.data(), 0, sizeof(int) * 8);
 }
 
 int FramePipeline::Blocks(size_t n) const { return (int) std::max<size_t>(1, std::min<size_t>((n + 255) / 256, 132 * 8)); }
 
 void FramePipeline::EnsureLo() {
-    if (!h_stage_lo_) CT_CUDA_CHECK(cudaMallocHost(&h_stage_lo_, sizeof(float4) * max_points_));
+    h_stage_lo_.reserve(max_points_, stream_);
     EnsureDeviceLo();
 }
 void FramePipeline::EnsureDeviceLo() {
-    if (d_frame_lo_) return;
-    if (!d_raw_lo_) CT_CUDA_CHECK(cudaMalloc(&d_raw_lo_, sizeof(float4) * max_points_));
-    CT_CUDA_CHECK(cudaMalloc(&d_frame_lo_, sizeof(float4) * max_points_));
-    CT_CUDA_CHECK(cudaMalloc(&d_kp_lo_, sizeof(float4) * max_points_));
-    CT_CUDA_CHECK(cudaMalloc(&d_tmp_lo_, sizeof(float4) * max_points_));
+    for (auto *a : {&d_raw_lo_, &d_frame_lo_, &d_kp_lo_, &d_tmp_lo_}) a->reserve(max_points_, stream_);
 }
 
 void FramePipeline::UploadLo(size_t n) {
     EnsureLo();
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_lo_, h_stage_lo_, sizeof(float4) * n, cudaMemcpyHostToDevice, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_lo_.data(), h_stage_lo_.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, stream_));
     raw_lo_ = true;
-    raw_lo_ptr_ = d_raw_lo_;
+    raw_lo_ptr_ = d_raw_lo_.data();
     h2d_bytes_ += sizeof(float4) * n;
 }
 
@@ -730,21 +700,21 @@ void FramePipeline::BeginScan(size_t n) {
     if (n > max_points_) throw CapacityError("scan has more points than max_points_per_frame");
     raw_lo_ = frame_lo_ = distorted_ = false;
     n_ = n;
-    h_counts_[0] = (int) n;
+    h_counts_.data()[0] = (int) n;
     n_on_device_ = false;
-    raw_ptr_ = d_raw_;
-    raw_lo_ptr_ = d_raw_lo_;
+    raw_ptr_ = d_raw_.data();
+    raw_lo_ptr_ = d_raw_lo_.data();
 }
 
 int FramePipeline::TakeHostN(const int *d_n) {
-    if (d_n != d_counts_ || n_on_device_) return -1;
+    if (d_n != d_counts_.data() || n_on_device_) return -1;
     n_on_device_ = true;
     return (int) n_;
 }
 
 void FramePipeline::Upload(size_t n) {
     BeginScan(n);
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_, h_stage_, sizeof(float4) * n, cudaMemcpyHostToDevice, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_.data(), h_stage_.data(), sizeof(float4) * n, cudaMemcpyHostToDevice, stream_));
     h2d_bytes_ = sizeof(float4) * n;
 }
 
@@ -754,7 +724,7 @@ void FramePipeline::UploadBegin(size_t n) {
 }
 void FramePipeline::UploadRange(size_t begin, size_t end) {
     if (end <= begin) return;
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_ + begin, h_stage_ + begin, sizeof(float4) * (end - begin), cudaMemcpyHostToDevice, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_.data() + begin, h_stage_.data() + begin, sizeof(float4) * (end - begin), cudaMemcpyHostToDevice, stream_));
 }
 
 void FramePipeline::UploadFromDevice(const float4 *d_src, const float4 *d_src_lo, size_t n) {
@@ -766,14 +736,14 @@ void FramePipeline::UploadFromDevice(const float4 *d_src, const float4 *d_src_lo
 }
 
 void FramePipeline::DetachRaw() {
-    if (raw_ptr_ == d_raw_) return;
-    if (n_) CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_, raw_ptr_, sizeof(float4) * n_, cudaMemcpyDeviceToDevice, stream_));
+    if (raw_ptr_ == d_raw_.data()) return;
+    if (n_) CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_.data(), raw_ptr_, sizeof(float4) * n_, cudaMemcpyDeviceToDevice, stream_));
     if (raw_lo_) {
         EnsureLo();
-        CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_lo_, raw_lo_ptr_, sizeof(float4) * n_, cudaMemcpyDeviceToDevice, stream_));
+        CT_CUDA_CHECK(cudaMemcpyAsync(d_raw_lo_.data(), raw_lo_ptr_, sizeof(float4) * n_, cudaMemcpyDeviceToDevice, stream_));
     }
-    raw_ptr_ = d_raw_;
-    raw_lo_ptr_ = d_raw_lo_;
+    raw_ptr_ = d_raw_.data();
+    raw_lo_ptr_ = d_raw_lo_.data();
 }
 
 void FramePipeline::GridSelect(const float4 *in, const float4 *in_lo, const uint32_t *in_src, const int *d_n_in,
@@ -784,22 +754,22 @@ void FramePipeline::GridSelect(const float4 *in, const float4 *in_lo, const uint
     clean_cap_ = 0;   // (this selection dirties what the fused sampler may have left clean)
     // scratch hash grid: only the prefix that can be touched is cleared; keys and vals are adjacent → one memset
     const uint32_t cap = std::max<uint32_t>(NextPow2(2 * n_upper), 1024);
-    unsigned long long *keys = d_grid_, *vals = d_grid_ + cap;
+    unsigned long long *keys = d_grid_.data(), *vals = d_grid_.data() + cap;
     CT_CUDA_CHECK(cudaMemsetAsync(keys, 0xFF, sizeof(unsigned long long) * 2 * (size_t) cap, stream_));
     // look-back descriptors + ticket of the standalone selection (the fused sampler's are kept apart: it relies on finding
     // its own clean)
     const size_t num_tiles = (n_upper + kTile - 1) / kTile;
-    unsigned long long *desc = d_desc_ + kFusedDescWords;
+    unsigned long long *desc = d_desc_.data() + kFusedDescWords;
     CT_CUDA_CHECK(cudaMemsetAsync(desc, 0, sizeof(unsigned long long) * (kMaxTiles + 1), stream_));
     const int n_host = TakeHostN(d_n_in);
-    k_grid_claim<<<Blocks(n_upper), 256, 0, stream_>>>(in, in_lo, d_n_in, n_host, d_counts_, voxel_size, use_perm1, seed, c1,
-                                                       keys, vals, cap - 1, d_slot_of_, d_src_);
+    k_grid_claim<<<Blocks(n_upper), 256, 0, stream_>>>(in, in_lo, d_n_in, n_host, d_counts_.data(), voxel_size, use_perm1, seed, c1,
+                                                       keys, vals, cap - 1, d_slot_of_.data(), d_src_.data());
     k_grid_select<<<(int) std::max<size_t>(1, num_tiles), kTileThreads, 0, stream_>>>(
-        d_n_in, use_perm1 ? d_src_ : nullptr, d_slot_of_, vals, desc, d_n_out, use_perm2 ? d_win_ : nullptr, in, in_lo, in_src,
+        d_n_in, use_perm1 ? d_src_.data() : nullptr, d_slot_of_.data(), vals, desc, d_n_out, use_perm2 ? d_win_.data() : nullptr, in, in_lo, in_src,
         out, out_lo, out_src);
     launches_ += 2;
     if (use_perm2) {
-        k_grid_scatter<<<Blocks(n_upper), 256, 0, stream_>>>(d_n_out, d_win_, in, in_lo, in_src, seed, c2, override_alpha,
+        k_grid_scatter<<<Blocks(n_upper), 256, 0, stream_>>>(d_n_out, d_win_.data(), in, in_lo, in_src, seed, c2, override_alpha,
                                                              alpha_value, out, out_lo, out_src);
         launches_ += 1;
     }
@@ -821,22 +791,17 @@ void FramePipeline::AdaptiveSelect(const cticp_adaptive_options &o, const float4
     }
     const size_t positions = n_upper * (size_t) o.num_bands;
     if ((positions + kTile - 1) / kTile > kMaxTiles) throw CapacityError("adaptive sampling: scan too large");
-    if (positions > adaptive_capacity_) {
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(d_adaptive_);
-        CT_CUDA_CHECK(cudaMalloc(&d_adaptive_, sizeof(uint32_t) * (kMaxTiles + 2 * positions)));
-        adaptive_capacity_ = positions;
-    }
-    uint32_t *tile_count = d_adaptive_, *flags = d_adaptive_ + kMaxTiles, *src = flags + positions;
+    d_adaptive_.reserve(kMaxTiles + 2 * positions, stream_);
+    uint32_t *tile_count = d_adaptive_.data(), *flags = d_adaptive_.data() + kMaxTiles, *src = flags + positions;
     const uint32_t cap = std::max<uint32_t>(NextPow2(2 * n_upper), 1024);
-    unsigned long long *keys = d_grid_, *vals = d_grid_ + cap;
+    unsigned long long *keys = d_grid_.data(), *vals = d_grid_.data() + cap;
     CT_CUDA_CHECK(cudaMemsetAsync(keys, 0xFF, sizeof(unsigned long long) * 2 * (size_t) cap, stream_));
     CT_CUDA_CHECK(cudaMemsetAsync(tile_count, 0, sizeof(uint32_t) * (kMaxTiles + positions), stream_));
     const int blocks = Blocks(n_upper);
-    int *d_positions = d_counts_ + 3;
-    k_adaptive_claim<<<blocks, 256, 0, stream_>>>(in, in_lo, d_n_in, TakeHostN(d_n_in), d_counts_, B, keys, vals, cap - 1,
-                                                  d_slot_of_, d_positions);
-    k_adaptive_mark<<<blocks, 256, 0, stream_>>>(in, in_lo, d_n_in, B, vals, d_slot_of_, flags, src, tile_count);
+    int *d_positions = d_counts_.data() + 3;
+    k_adaptive_claim<<<blocks, 256, 0, stream_>>>(in, in_lo, d_n_in, TakeHostN(d_n_in), d_counts_.data(), B, keys, vals, cap - 1,
+                                                  d_slot_of_.data(), d_positions);
+    k_adaptive_mark<<<blocks, 256, 0, stream_>>>(in, in_lo, d_n_in, B, vals, d_slot_of_.data(), flags, src, tile_count);
     const size_t num_tiles = (positions + kTile - 1) / kTile;
     k_grid_emit<<<(int) std::min<size_t>(std::max<size_t>(1, num_tiles), 1184), kTileThreads, 0, stream_>>>(
         in, in_lo, in_src, d_positions, flags, src, tile_count, 0, 0, 0, 0, 0.f, out, out_lo, out_src, d_n_out);
@@ -852,9 +817,9 @@ void FramePipeline::AdaptiveSelect(const cticp_adaptive_options &o, const float4
 // sampling's parameters must be known when the frame arrives: true for the first registration attempt of a frame.
 void FramePipeline::SampleFused(double voxel_size, double sample_voxel_size, uint64_t seed, uint64_t counter1,
                                 uint64_t counter2, bool override_alpha, float alpha_value) {
-    if (!d_grid2_) {
-        CT_CUDA_CHECK(cudaMalloc(&d_grid2_, sizeof(unsigned long long) * 2 * (size_t) grid_cap_));
-        CT_CUDA_CHECK(cudaMemsetAsync(d_grid2_, 0xFF, sizeof(unsigned long long) * 2 * (size_t) grid_cap_, stream_));
+    if (!d_grid2_.data()) {
+        d_grid2_.reserve(2 * (size_t) grid_cap_, stream_);
+        CT_CUDA_CHECK(cudaMemsetAsync(d_grid2_.data(), 0xFF, sizeof(unsigned long long) * 2 * (size_t) grid_cap_, stream_));
         int per_sm = 0;
         CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_sample_fused, kTileThreads, 0));
         int dev = 0, sms = 132;
@@ -869,25 +834,25 @@ void FramePipeline::SampleFused(double voxel_size, double sample_voxel_size, uin
     a.raw_lo = d_raw_lo();
     a.n = (int) n_;
     n_on_device_ = true;
-    a.frame_lo = d_frame_lo_; a.kp_lo = d_kp_lo_;
+    a.frame_lo = d_frame_lo_.data(); a.kp_lo = d_kp_lo_.data();
     frame_lo_ = raw_lo_;
-    a.counts = d_counts_;
+    a.counts = d_counts_.data();
     a.voxel1 = voxel_size;
     a.voxel2 = sample_voxel_size;
     a.seed = seed; a.c1 = counter1; a.c2 = counter2;
     a.override_alpha = override_alpha ? 1 : 0;
     a.alpha_value = alpha_value;
-    a.grid = d_grid_;
+    a.grid = d_grid_.data();
     a.cap1 = std::max<uint32_t>(NextPow2(2 * n_), 1024);
     a.pre_cleared = (preclear_ && clean_cap_ >= a.cap1) ? 1 : 0;
     a.clear_after = preclear_ ? 1 : 0;
     clean_cap_ = preclear_ ? a.cap1 : 0;        // what this launch leaves behind
-    a.grid2 = d_grid2_;
-    a.desc = d_desc_;
-    a.slot_at = d_slot_of_;
-    a.src = d_src_; a.win = d_win_;
-    a.frame = d_frame_; a.keypoints = d_keypoints_;
-    a.frame_src = d_frame_src_; a.kp_src = d_kp_src_;
+    a.grid2 = d_grid2_.data();
+    a.desc = d_desc_.data();
+    a.slot_at = d_slot_of_.data();
+    a.src = d_src_.data(); a.win = d_win_.data();
+    a.frame = d_frame_.data(); a.keypoints = d_keypoints_.data();
+    a.frame_src = d_frame_src_.data(); a.kp_src = d_kp_src_.data();
     void *args[] = {&a};
     CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_sample_fused, dim3(fused_grid_), dim3(kTileThreads), args, 0, stream_));
     launches_ += 1;
@@ -895,8 +860,8 @@ void FramePipeline::SampleFused(double voxel_size, double sample_voxel_size, uin
 
 void FramePipeline::SubSampleFrame(double voxel_size, uint64_t seed, uint64_t counter1, uint64_t counter2,
                                    bool override_alpha, float alpha_value) {
-    GridSelect(raw_ptr_, d_raw_lo(), nullptr, d_counts_ + 0, n_, voxel_size, 1, seed, counter1, 1, counter2,
-               override_alpha ? 1 : 0, alpha_value, d_frame_, d_frame_lo_, d_frame_src_, d_counts_ + 1);
+    GridSelect(raw_ptr_, d_raw_lo(), nullptr, d_counts_.data() + 0, n_, voxel_size, 1, seed, counter1, 1, counter2,
+               override_alpha ? 1 : 0, alpha_value, d_frame_.data(), d_frame_lo_.data(), d_frame_src_.data(), d_counts_.data() + 1);
     frame_lo_ = raw_lo_;
 }
 
@@ -904,21 +869,21 @@ void FramePipeline::SampleKeypoints(int sampling, double sample_voxel_size, int 
                                     uint64_t counter, const cticp_adaptive_options *adaptive) {
     if (sampling == CTICP_SAMPLING_ADAPTIVE) {
         if (!adaptive) throw std::invalid_argument("adaptive options missing");
-        AdaptiveSelect(*adaptive, d_frame_, d_frame_lo(), d_frame_src_, d_counts_ + 1, n_, d_keypoints_, d_kp_lo_, d_kp_src_,
-                       d_counts_ + 2);
+        AdaptiveSelect(*adaptive, d_frame_.data(), d_frame_lo(), d_frame_src_.data(), d_counts_.data() + 1, n_, d_keypoints_.data(), d_kp_lo_.data(), d_kp_src_.data(),
+                       d_counts_.data() + 2);
     } else if (sampling == CTICP_SAMPLING_GRID) {
-        GridSelect(d_frame_, d_frame_lo(), d_frame_src_, d_counts_ + 1, n_, sample_voxel_size, 0, 0, 0, 0, 0, 0, 0.f,
-                   d_keypoints_, d_kp_lo_, d_kp_src_, d_counts_ + 2);
+        GridSelect(d_frame_.data(), d_frame_lo(), d_frame_src_.data(), d_counts_.data() + 1, n_, sample_voxel_size, 0, 0, 0, 0, 0, 0, 0.f,
+                   d_keypoints_.data(), d_kp_lo_.data(), d_kp_src_.data(), d_counts_.data() + 2);
     } else {
-        k_copy_points<<<Blocks(n_), 256, 0, stream_>>>(d_frame_, d_frame_lo(), d_frame_src_, d_counts_ + 1, d_keypoints_,
-                                                       d_kp_lo_, d_kp_src_, d_counts_ + 2);
+        k_copy_points<<<Blocks(n_), 256, 0, stream_>>>(d_frame_.data(), d_frame_lo(), d_frame_src_.data(), d_counts_.data() + 1, d_keypoints_.data(),
+                                                       d_kp_lo_.data(), d_kp_src_.data(), d_counts_.data() + 2);
         launches_ += 1;
     }
     if (max_num_keypoints > 0) {
-        k_truncate_shuffle<<<Blocks(n_), 256, 0, stream_>>>(d_keypoints_, d_keypoints_lo(), d_kp_src_, d_counts_ + 2,
-                                                            max_num_keypoints, seed, counter, d_tmp_points_, d_tmp_lo_,
-                                                            d_tmp_src_);
-        k_clamp_count<<<1, 1, 0, stream_>>>(d_counts_ + 2, max_num_keypoints);
+        k_truncate_shuffle<<<Blocks(n_), 256, 0, stream_>>>(d_keypoints_.data(), d_keypoints_lo(), d_kp_src_.data(), d_counts_.data() + 2,
+                                                            max_num_keypoints, seed, counter, d_tmp_points_.data(), d_tmp_lo_.data(),
+                                                            d_tmp_src_.data());
+        k_clamp_count<<<1, 1, 0, stream_>>>(d_counts_.data() + 2, max_num_keypoints);
         std::swap(d_keypoints_, d_tmp_points_);
         std::swap(d_kp_lo_, d_tmp_lo_);
         std::swap(d_kp_src_, d_tmp_src_);
@@ -928,12 +893,12 @@ void FramePipeline::SampleKeypoints(int sampling, double sample_voxel_size, int 
 }
 
 void FramePipeline::QueueCountsReadback() {
-    CT_CUDA_CHECK(cudaMemcpyAsync(h_counts_, d_counts_, sizeof(int) * 4, cudaMemcpyDeviceToHost, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(h_counts_.data(), d_counts_.data(), sizeof(int) * 4, cudaMemcpyDeviceToHost, stream_));
 }
 
 void FramePipeline::DistortFrame(const Q4 &qb, const V3 &tb, const Q4 &qe, const V3 &te) {
     EnsureLo();
-    k_distort_frame<<<Blocks(n_), 256, 0, stream_>>>(d_frame_, d_frame_lo_, frame_lo_ ? 1 : 0, d_counts_ + 1, qb, tb, qe, te,
+    k_distort_frame<<<Blocks(n_), 256, 0, stream_>>>(d_frame_.data(), d_frame_lo_.data(), frame_lo_ ? 1 : 0, d_counts_.data() + 1, qb, tb, qe, te,
                                                      slerp_consts(qb, qe));
     frame_lo_ = distorted_ = true;
     launches_ += 1;
@@ -941,17 +906,17 @@ void FramePipeline::DistortFrame(const Q4 &qb, const V3 &tb, const Q4 &qe, const
 }
 
 void FramePipeline::TransformFrame(const Q4 &qb, const V3 &tb, const Q4 &qe, const V3 &te) {
-    k_transform_points<<<Blocks(n_), 256, 0, stream_>>>(d_frame_, d_frame_lo(), d_counts_ + 1, 0, qb, tb, qe, te, slerp_consts(qb, qe), d_frame_world_);
+    k_transform_points<<<Blocks(n_), 256, 0, stream_>>>(d_frame_.data(), d_frame_lo(), d_counts_.data() + 1, 0, qb, tb, qe, te, slerp_consts(qb, qe), d_frame_world_.data());
     launches_ += 1;
     CT_CUDA_CHECK(cudaGetLastError());
 }
 
 void FramePipeline::EnsureAllWorld() {
-    if (!d_all_world_) CT_CUDA_CHECK(cudaMalloc(&d_all_world_, sizeof(double) * 3 * max_points_));
+    d_all_world_.reserve(3 * max_points_, stream_);
 }
 void FramePipeline::TransformAll(const Q4 &qb, const V3 &tb, const Q4 &qe, const V3 &te, cudaStream_t stream) {
     EnsureAllWorld();
-    k_transform_points<<<Blocks(n_), 256, 0, stream ? stream : stream_>>>(raw_ptr_, d_raw_lo(), nullptr, (int) n_, qb, tb, qe, te, slerp_consts(qb, qe), d_all_world_);
+    k_transform_points<<<Blocks(n_), 256, 0, stream ? stream : stream_>>>(raw_ptr_, d_raw_lo(), nullptr, (int) n_, qb, tb, qe, te, slerp_consts(qb, qe), d_all_world_.data());
     launches_ += 1;
     CT_CUDA_CHECK(cudaGetLastError());
 }
@@ -964,14 +929,14 @@ void FramePipeline::TransformInto(const float4 *pts, const float4 *lo, const int
 }
 
 void FramePipeline::EnsureScanReduce() {
-    if (d_scan_reduce_) return;
-    CT_CUDA_CHECK(cudaMalloc(&d_scan_partials_, sizeof(ScanPartial) * kScanMaxCtas));
-    CT_CUDA_CHECK(cudaMalloc(&d_scan_ticket_, sizeof(unsigned)));
-    CT_CUDA_CHECK(cudaMemsetAsync(d_scan_ticket_, 0, sizeof(unsigned), stream_));
-    CT_CUDA_CHECK(cudaMalloc(&d_scan_reduce_, sizeof(ScanReduceOut)));
-    CT_CUDA_CHECK(cudaHostAlloc(&h_scan_reduce_, sizeof(ScanReduceOut), cudaHostAllocMapped));
-    memset(h_scan_reduce_, 0, sizeof(ScanReduceOut));
-    CT_CUDA_CHECK(cudaHostGetDevicePointer((void **) &h_scan_reduce_dev_, h_scan_reduce_, 0));
+    if (h_scan_reduce_dev_) return;
+    d_scan_partials_.reserve(kScanMaxCtas, stream_);
+    d_scan_ticket_.reserve(1, stream_);
+    CT_CUDA_CHECK(cudaMemsetAsync(d_scan_ticket_.data(), 0, sizeof(unsigned), stream_));
+    d_scan_reduce_.reserve(1, stream_);
+    h_scan_reduce_.reserve(1, stream_);
+    memset(h_scan_reduce_.data(), 0, sizeof(ScanReduceOut));
+    CT_CUDA_CHECK(cudaHostGetDevicePointer((void **) &h_scan_reduce_dev_, h_scan_reduce_.data(), 0));
 }
 
 void FramePipeline::PackFromDevice(const void *xyz, size_t xyz_stride, int xyz_dtype, const void *t, size_t t_stride,
@@ -980,7 +945,7 @@ void FramePipeline::PackFromDevice(const void *xyz, size_t xyz_stride, int xyz_d
     scan_xyz_f64_ = xyz_dtype == CTICP_DTYPE_FLOAT64;
     // the raw lo plane exists before the launches (the pack decides on the device whether to write it); the other lo
     // planes follow only once the reduce reports a scan that needs them (WaitScanReduce)
-    if (scan_xyz_f64_ && !d_raw_lo_) CT_CUDA_CHECK(cudaMalloc(&d_raw_lo_, sizeof(float4) * max_points_));
+    if (scan_xyz_f64_) d_raw_lo_.reserve(max_points_, stream_);
     BeginScan(n);
     h2d_bytes_ = 0;
     const auto *px = static_cast<const unsigned char *>(xyz), *pt = static_cast<const unsigned char *>(t);
@@ -993,14 +958,14 @@ void FramePipeline::PackFromDevice(const void *xyz, size_t xyz_stride, int xyz_d
     const int ni = (int) n;
     const int blocks = std::min(Blocks(n), kScanMaxCtas);
     const unsigned seq = ++scan_reduce_seq_;
-    ScanPartial *part = static_cast<ScanPartial *>(d_scan_partials_);
+    ScanPartial *part = d_scan_partials_.data();
     if (scan_xyz_f64_) {
         auto k = load == kLoadNatural ? k_scan_reduce<true, kLoadNatural> : k_scan_reduce<true, kLoadBytes>;
-        k<<<blocks, kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, part, d_scan_ticket_,
-                                                d_scan_reduce_, h_scan_reduce_dev_, seq);
+        k<<<blocks, kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, part, d_scan_ticket_.data(),
+                                                d_scan_reduce_.data(), h_scan_reduce_dev_, seq);
     } else {
         k_scan_reduce<false, kLoadBytes><<<blocks, kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni,
-                                                                              part, d_scan_ticket_, d_scan_reduce_,
+                                                                              part, d_scan_ticket_.data(), d_scan_reduce_.data(),
                                                                               h_scan_reduce_dev_, seq);
     }
     CT_CUDA_CHECK(cudaGetLastError());
@@ -1008,13 +973,13 @@ void FramePipeline::PackFromDevice(const void *xyz, size_t xyz_stride, int xyz_d
     const double bts = pose_ts ? pose_ts[0] : 0.0, ets = pose_ts ? pose_ts[1] : 0.0;
     if (scan_xyz_f64_) {
         auto k = load == kLoadNatural ? k_scan_pack<double, kLoadNatural> : k_scan_pack<double, kLoadBytes>;
-        k<<<Blocks(n), kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, d_scan_reduce_, use_reduce,
-                                                   bts, ets, d_raw_, d_raw_lo_);
+        k<<<Blocks(n), kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, d_scan_reduce_.data(), use_reduce,
+                                                   bts, ets, d_raw_.data(), d_raw_lo_.data());
     } else {
         auto k = load == kLoadVec4 ? k_scan_pack<float, kLoadVec4>
                  : load == kLoadNatural ? k_scan_pack<float, kLoadNatural> : k_scan_pack<float, kLoadBytes>;
-        k<<<Blocks(n), kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, d_scan_reduce_, use_reduce,
-                                                   bts, ets, d_raw_, nullptr);
+        k<<<Blocks(n), kScanThreads, 0, stream_>>>(px, xyz_stride, pt, t_stride, t_dtype, t_al, ni, d_scan_reduce_.data(), use_reduce,
+                                                   bts, ets, d_raw_.data(), nullptr);
     }
     CT_CUDA_CHECK(cudaGetLastError());
     launches_ += 2;
@@ -1022,7 +987,7 @@ void FramePipeline::PackFromDevice(const void *xyz, size_t xyz_stride, int xyz_d
 
 // Spin on the reduce's sequence number; the stream is polled now and then, so that a faulted kernel surfaces as an error
 void FramePipeline::WaitScanReduce(double *t_min, double *t_max) {
-    volatile unsigned *flag = &h_scan_reduce_->seq;
+    volatile unsigned *flag = &h_scan_reduce_.data()->seq;
     for (unsigned long spins = 1;; ++spins) {
         if (*flag == scan_reduce_seq_) break;
         if ((spins & 0xfffu) == 0) {
@@ -1035,12 +1000,12 @@ void FramePipeline::WaitScanReduce(double *t_min, double *t_max) {
         }
     }
     std::atomic_thread_fence(std::memory_order_acquire);
-    const volatile ScanReduceOut *r = h_scan_reduce_;
+    const volatile ScanReduceOut *r = h_scan_reduce_.data();
     *t_min = r->t_min;
     *t_max = r->t_max;
     // what the host packer would report: a float64 scan with a coordinate float32 cannot hold carries its residual plane
     raw_lo_ = scan_xyz_f64_ && r->needs_lo != 0;
-    raw_lo_ptr_ = d_raw_lo_;
+    raw_lo_ptr_ = d_raw_lo_.data();
     if (raw_lo_) EnsureDeviceLo();   // before the sampler that writes the frame's lo plane is enqueued
 }
 

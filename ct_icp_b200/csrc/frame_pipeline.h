@@ -16,31 +16,29 @@ struct ScanReduceOut {
     int needs_lo;
     unsigned seq;
 };
+struct ScanPartial;   // frame_pipeline.cu
 
 class FramePipeline {
 public:
     FramePipeline(size_t max_points, cudaStream_t stream);
-    ~FramePipeline();
-    FramePipeline(const FramePipeline &) = delete;
-    FramePipeline &operator=(const FramePipeline &) = delete;
 
     // pinned staging buffer the host packs (x, y, z, alpha) into, then Upload(n) enqueues the H2D copy
-    float4 *Staging() { return h_stage_; }
+    float4 *Staging() { return h_stage_.data(); }
     // residual planes (value - (double)(float)value, see load_raw in se3.cuh) — allocated on first use: float32 scans,
     // what LiDAR drivers emit, never need them. raw_lo: the scan as uploaded; frame_lo: the sub-sampled frame and the
     // keypoints drawn from it (also set by DistortFrame, whose output is not float32-representable).
     void EnsureLo();
     // the device lo planes only (raw, frame, keypoints, scratch): what a scan packed on the device needs
     void EnsureDeviceLo();
-    float4 *StagingLo() { EnsureLo(); return h_stage_lo_; }
-    const float4 *StagingLoIfAny() const { return raw_lo_ ? h_stage_lo_ : nullptr; }
+    float4 *StagingLo() { EnsureLo(); return h_stage_lo_.data(); }
+    const float4 *StagingLoIfAny() const { return raw_lo_ ? h_stage_lo_.data() : nullptr; }
     void UploadLo(size_t n);                                  // after Upload*/UploadBegin of the same scan
     bool raw_has_lo() const { return raw_lo_; }
     bool frame_has_lo() const { return frame_lo_; }
     bool frame_distorted() const { return distorted_; }
     const float4 *d_raw_lo() const { return raw_lo_ ? raw_lo_ptr_ : nullptr; }
-    const float4 *d_frame_lo() const { return frame_lo_ ? d_frame_lo_ : nullptr; }
-    const float4 *d_keypoints_lo() const { return frame_lo_ ? d_kp_lo_ : nullptr; }
+    const float4 *d_frame_lo() const { return frame_lo_ ? d_frame_lo_.data() : nullptr; }
+    const float4 *d_keypoints_lo() const { return frame_lo_ ? d_kp_lo_.data() : nullptr; }
     size_t MaxPoints() const { return max_points_; }
     void Upload(size_t n);
     // the same copy in pieces, so that it can start while the tail of the scan is still being packed:
@@ -89,24 +87,24 @@ public:
     void EnsureAllWorld();
 
     void QueueCountsReadback();   // h_counts()[0..2] = N, F, K after the next stream sync
-    const int *h_counts() const { return h_counts_; }
+    const int *h_counts() const { return h_counts_.data(); }
     // the same four counters, brought back by another route (the frame verdict, frame_policy.h)
     void SetHostCounts(const int *c) {
-        for (int i = 0; i < 4; ++i) h_counts_[i] = c[i];
+        for (int i = 0; i < 4; ++i) h_counts_.data()[i] = c[i];
     }
-    const int *d_counts() const { return d_counts_; }
+    const int *d_counts() const { return d_counts_.data(); }
 
     const float4 *d_raw() const { return raw_ptr_; }
-    const float4 *d_frame() const { return d_frame_; }
-    const float4 *d_keypoints() const { return d_keypoints_; }
-    float4 *d_keypoints_mut() { return d_keypoints_; }
-    const uint32_t *d_frame_src() const { return d_frame_src_; }
-    const uint32_t *d_keypoints_src() const { return d_kp_src_; }
-    const double *d_frame_world() const { return d_frame_world_; }
-    const double *d_all_world() const { return d_all_world_; }
-    int *d_count_n() { return d_counts_ + 0; }
-    int *d_count_frame() { return d_counts_ + 1; }
-    int *d_count_keypoints() { return d_counts_ + 2; }
+    const float4 *d_frame() const { return d_frame_.data(); }
+    const float4 *d_keypoints() const { return d_keypoints_.data(); }
+    float4 *d_keypoints_mut() { return d_keypoints_.data(); }
+    const uint32_t *d_frame_src() const { return d_frame_src_.data(); }
+    const uint32_t *d_keypoints_src() const { return d_kp_src_.data(); }
+    const double *d_frame_world() const { return d_frame_world_.data(); }
+    const double *d_all_world() const { return d_all_world_.data(); }
+    int *d_count_n() { return d_counts_.data() + 0; }
+    int *d_count_frame() { return d_counts_.data() + 1; }
+    int *d_count_keypoints() { return d_counts_.data() + 2; }
     size_t n() const { return n_; }
     size_t h2d_bytes() const { return h2d_bytes_; }
     int launches() const { return launches_; }
@@ -115,10 +113,10 @@ public:
     void GridSelect(const float4 *in, const float4 *in_lo, const uint32_t *in_src, const int *d_n_in, size_t n_upper,
                     double voxel_size, int use_perm1, uint64_t seed, uint64_t c1, int use_perm2, uint64_t c2,
                     int override_alpha, float alpha_value, float4 *out, float4 *out_lo, uint32_t *out_src, int *d_n_out);
-    float4 *d_frame_lo_mut() { EnsureLo(); return d_frame_lo_; }
-    double *d_frame_world_mut() { return d_frame_world_; }
-    float4 *d_frame_mut() { return d_frame_; }
-    uint32_t *d_frame_src_mut() { return d_frame_src_; }
+    float4 *d_frame_lo_mut() { EnsureLo(); return d_frame_lo_.data(); }
+    double *d_frame_world_mut() { return d_frame_world_.data(); }
+    float4 *d_frame_mut() { return d_frame_.data(); }
+    uint32_t *d_frame_src_mut() { return d_frame_src_.data(); }
 
 private:
     int Blocks(size_t n) const;
@@ -132,33 +130,35 @@ private:
     bool n_on_device_ = true;
     const float4 *raw_ptr_ = nullptr, *raw_lo_ptr_ = nullptr;   // the scan being read: d_raw_ / d_raw_lo_ or a staged scan
     uint32_t grid_cap_ = 0;
-    float4 *h_stage_ = nullptr;
-    int *h_counts_ = nullptr;
-    float4 *d_raw_ = nullptr, *d_frame_ = nullptr, *d_keypoints_ = nullptr, *d_tmp_points_ = nullptr;
-    float4 *h_stage_lo_ = nullptr, *d_raw_lo_ = nullptr, *d_frame_lo_ = nullptr, *d_kp_lo_ = nullptr, *d_tmp_lo_ = nullptr;
+    PinnedArray<float4> h_stage_;
+    PinnedArray<int> h_counts_;
+    DeviceArray<float4> d_raw_, d_frame_, d_keypoints_, d_tmp_points_;
+    PinnedArray<float4> h_stage_lo_;
+    DeviceArray<float4> d_raw_lo_, d_frame_lo_, d_kp_lo_, d_tmp_lo_;
     bool raw_lo_ = false, frame_lo_ = false, distorted_ = false;
-    uint32_t *d_frame_src_ = nullptr, *d_kp_src_ = nullptr, *d_tmp_src_ = nullptr;
-    unsigned long long *d_grid_ = nullptr;
-    int *d_slot_of_ = nullptr;
-    uint32_t *d_src_ = nullptr, *d_win_ = nullptr;   // point of each position / compacted winners before the second shuffle
-    unsigned long long *d_desc_ = nullptr;            // look-back descriptors of the selections (frame_pipeline.cu)
-    int *d_counts_ = nullptr;
-    double *d_frame_world_ = nullptr, *d_all_world_ = nullptr;
-    unsigned long long *d_grid2_ = nullptr;   // hash grid of the fused sampler's second selection
+    DeviceArray<uint32_t> d_frame_src_, d_kp_src_, d_tmp_src_;
+    DeviceArray<unsigned long long> d_grid_;
+    DeviceArray<int> d_slot_of_;
+    DeviceArray<uint32_t> d_src_, d_win_;   // point of each position / compacted winners before the second shuffle
+    DeviceArray<unsigned long long> d_desc_;   // look-back descriptors of the selections (frame_pipeline.cu)
+    DeviceArray<int> d_counts_;
+    DeviceArray<double> d_frame_world_, d_all_world_;
+    DeviceArray<unsigned long long> d_grid2_;   // hash grid of the fused sampler's second selection
     int fused_grid_ = 0;
     // k_sample_fused leaves the hash grid clean for the next frame (CTICP_SAMPLE_PRECLEAR=0: every launch clears it itself):
     // the capacity that is clean right now
     bool preclear_ = true;
     uint32_t clean_cap_ = 0;
-    uint32_t *d_adaptive_ = nullptr;   // tile counters + flags + src of the band-major position space
+    DeviceArray<uint32_t> d_adaptive_;   // tile counters + flags + src of the band-major position space
     // k_scan_reduce: per-CTA partials, the last CTA's ticket, the result (device / mapped pinned, sequence number last)
-    void *d_scan_partials_ = nullptr;
-    unsigned *d_scan_ticket_ = nullptr;
-    ScanReduceOut *d_scan_reduce_ = nullptr, *h_scan_reduce_ = nullptr, *h_scan_reduce_dev_ = nullptr;
+    DeviceArray<ScanPartial> d_scan_partials_;
+    DeviceArray<unsigned> d_scan_ticket_;
+    DeviceArray<ScanReduceOut> d_scan_reduce_;
+    PinnedArray<ScanReduceOut> h_scan_reduce_{cudaHostAllocMapped};
+    ScanReduceOut *h_scan_reduce_dev_ = nullptr;
     unsigned scan_reduce_seq_ = 0;
     bool scan_xyz_f64_ = false;
     void EnsureScanReduce();
-    size_t adaptive_capacity_ = 0;
     int launches_ = 0;
 };
 

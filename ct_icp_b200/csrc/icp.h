@@ -93,6 +93,9 @@ int GatherBlocks(size_t k_hint, int max_blocks, int kp_per_cta);
 void BatchGatherCtas(const size_t *n, int batch, int coresident, int kp_per_cta, int *gather);
 
 struct FrameTailArgs;   // frame_policy.h
+struct LmState;            // icp_lm.cu
+struct DistanceStrategy;   // icp_lm.cu
+struct ResidualBlock;      // lm_functor.cuh
 
 // One registration of a grouped Gauss-Newton launch (IcpSolver::EnqueueGaussNewtonGroups)
 struct GnProblem {
@@ -110,7 +113,6 @@ struct GnProblem {
 class IcpSolver {
 public:
     explicit IcpSolver(cudaStream_t stream);
-    ~IcpSolver();
 
     // d_keypoints: float4 (raw xyz fp32, alpha fp32); d_num_keypoints: device int; upper bound for grid sizing.
     // Enqueues `num_iters` GN iterations on the stream; state is read back by the caller.
@@ -188,7 +190,7 @@ public:
     void PreloadShardedKernels();
     void PreloadLmKernels();   // icp_lm.cu
     void NcclAllReduceAccumulator(void *nccl_comm);   // nccl_shard.cu
-    double *acc_buffer() const { return d_acc_; }
+    double *acc_buffer() const { return d_acc_.data(); }
     bool peers_ready() const { return peers_ready_; }
 
 private:
@@ -196,7 +198,6 @@ private:
     void EnsureLmBuffers(size_t k_upper);
     void DebugLmTrace(void *d_lm);
     int lm_coresident_[9] = {};   // k_lm_persistent<mode, peers> at mode * 2 + peers, <mode, false, true> at 6 + mode
-    void FreeLmBuffers();
     GnParams MakeParams(const DeviceMap &map, const cticp_icp_options &opt) const;
     int GnCoresident(bool peers);          // co-resident CTAs of k_gn_persistent<peers> on this device
     unsigned int ReserveLoopTags(int rows, int groups, int num_iters);   // k_gn_persistent's words and tags (icp_gn.cu)
@@ -208,37 +209,33 @@ private:
 
     cudaStream_t stream_;
     const float4 *kp_lo_ = nullptr;
-    double *d_partials_ = nullptr;
-    unsigned long long *d_dbg_warp_ = nullptr;   // [kDbgIters][warps][kDbgSlots]
+    DeviceArray<double> d_partials_;   // kAcc per CTA (grow-only)
+    DeviceArray<unsigned long long> d_dbg_warp_;   // [kDbgIters][warps][kDbgSlots]
     int dbg_warps_ = 0;
-    int partial_blocks_ = 0;
-    double *d_sys_ = nullptr;      // 12*12 + 12 + 4 debug output of the solve kernel
-    double *d_acc_ = nullptr;      // reduced accumulator (multi-GPU all-reduce buffer)
-    unsigned int *d_ticket_ = nullptr;   // last-CTA-done counter of k_gn_iterate
-    unsigned long long *d_loop_rows_ = nullptr;   // k_gn_persistent: tagged partial rows of the gather CTAs (grow-only)
-    unsigned long long *d_loop_pose_ = nullptr;   // k_gn_persistent: tagged pose words, one block per group (grow-only)
-    int loop_rows_cap_ = 0, loop_groups_cap_ = 0;
-    unsigned int loop_tag_ = 1;                   // next tag to hand out (never 0)
-    int *d_groups_ = nullptr;                // batched LM launches: first_cta | kp_base | keypoint counts (grow-only)
-    int groups_cap_ = 0;                     // ints d_groups_ holds
+    DeviceArray<double> d_sys_;      // 12*12 + 12 + 4 debug output of the solve kernel
+    DeviceArray<double> d_acc_;      // reduced accumulator (multi-GPU all-reduce buffer)
+    DeviceArray<unsigned int> d_ticket_;   // last-CTA-done counter of k_gn_iterate
+    DeviceArray<unsigned long long> d_loop_rows_;   // k_gn_persistent: tagged partial rows of the gather CTAs (grow-only)
+    DeviceArray<unsigned long long> d_loop_pose_;   // k_gn_persistent: tagged pose words, one block per group (grow-only)
+    unsigned int loop_tag_ = 1;                     // next tag to hand out (never 0)
+    DeviceArray<int> d_groups_;                // batched LM launches: first_cta | kp_base | keypoint counts (grow-only)
     std::vector<int> h_groups_;
-    unsigned char *d_gn_table_ = nullptr;    // grouped GN launches: GnGroup table | first_cta | counts (grow-only)
-    size_t gn_table_cap_ = 0;
+    DeviceArray<unsigned char> d_gn_table_;    // grouped GN launches: GnGroup table | first_cta | counts (grow-only)
     std::vector<unsigned char> h_gn_table_;
     // solver CERES (icp_lm.cu)
-    void *d_lm_state_ = nullptr, *d_lm_stats_ = nullptr, *d_lm_blocks_ = nullptr;
-    int *d_lm_sel_ = nullptr;
-    void *d_lm_classes_ = nullptr;   // solver ROBUST: slam::NEIGHBORHOOD_TYPE per keypoint
-    void *d_lm_strategy_ = nullptr;  // DistanceBasedStrategy parameters + every map level
-    size_t lm_capacity_ = 0;
-    void *d_lm_groups_ = nullptr;    // batched launches: per group an LmState, a stats line and the barrier words (grow-only)
-    int lm_groups_cap_ = 0;
+    DeviceArray<LmState> d_lm_state_;
+    DeviceArray<unsigned long long> d_lm_stats_;
+    DeviceArray<ResidualBlock> d_lm_blocks_;
+    DeviceArray<int> d_lm_sel_;
+    DeviceArray<unsigned char> d_lm_classes_;   // solver ROBUST: slam::NEIGHBORHOOD_TYPE per keypoint
+    DeviceArray<DistanceStrategy> d_lm_strategy_;  // DistanceBasedStrategy parameters + every map level
+    DeviceArray<char> d_lm_groups_;             // batched launches: per group an LmState, a stats line and the barrier words (grow-only)
     int launches_ = 0;
     float gather_ms_ = 0.f;
     int gather_launches_ = 0;
     bool time_gather_ = false;
     static constexpr int kMaxEvents = 64;
-    cudaEvent_t ev_begin_[kMaxEvents], ev_end_[kMaxEvents];
+    Event ev_begin_[kMaxEvents], ev_end_[kMaxEvents];
     int ev_used_ = 0;
     int num_sms_ = 132;
     int max_coresident_[2] = {0, 0};   // k_gn_persistent<false / true>

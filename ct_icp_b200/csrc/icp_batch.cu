@@ -9,14 +9,6 @@
 
 namespace cticp {
 
-#define CT_CUDA_CHECK(expr)                                                                              \
-    do {                                                                                                 \
-        cudaError_t _e = (expr);                                                                         \
-        if (_e != cudaSuccess)                                                                           \
-            throw CudaError(std::string(#expr) + ": " + cudaGetErrorString(_e) + " @" + __FILE__ + ":" + \
-                            std::to_string(__LINE__));                                                   \
-    } while (0)
-
 int GatherBlocks(size_t k_hint, int max_blocks, int kp_per_cta) {
     // One CTA (kGatherWarps warps, 128 registers per thread) per SM. A keypoint set smaller than the machine is spread
     // thin — `kp_per_cta` keypoints per CTA, so each keypoint's warp has an SM sub-partition nearly to itself: the loop
@@ -76,14 +68,8 @@ int IcpSolver::UploadGroupTable(const size_t *h_n, int batch, int coresident) {
         base += (long long) h_n[b];
     }
     if (base > (long long) INT32_MAX) throw std::invalid_argument("too many keypoints in one batch");
-    if ((int) h_groups_.size() > groups_cap_) {
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(d_groups_);
-        d_groups_ = nullptr;
-        CT_CUDA_CHECK(cudaMalloc(&d_groups_, sizeof(int) * h_groups_.size()));
-        groups_cap_ = (int) h_groups_.size();
-    }
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_groups_, h_groups_.data(), sizeof(int) * h_groups_.size(), cudaMemcpyHostToDevice, stream_));
+    d_groups_.reserve(h_groups_.size(), stream_);
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_groups_.data(), h_groups_.data(), sizeof(int) * h_groups_.size(), cudaMemcpyHostToDevice, stream_));
     return first_cta[batch];
 }
 

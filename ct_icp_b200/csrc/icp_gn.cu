@@ -22,14 +22,6 @@
 namespace cticp {
 namespace cg = cooperative_groups;
 
-#define CT_CUDA_CHECK(expr)                                                                              \
-    do {                                                                                                 \
-        cudaError_t _e = (expr);                                                                         \
-        if (_e != cudaSuccess)                                                                           \
-            throw CudaError(std::string(#expr) + ": " + cudaGetErrorString(_e) + " @" + __FILE__ + ":" + \
-                            std::to_string(__LINE__));                                                   \
-    } while (0)
-
 // Warps per CTA of the gather kernels (one keypoint per warp at a time). Fewer, fatter CTAs make the grid-wide
 // barriers and the reduction of the per-CTA partial sums cheaper, and more warps share one SM's instruction cache: on
 // config 2 (K ~ 1.2k) the GN loop per frame got faster from 4 to 8 to 16 warps (CTICP_GATHER_WARPS selects it)
@@ -1059,7 +1051,7 @@ void IcpSolver::PreloadShardedKernels() {
 }
 void IcpSolver::AllReduceAccumulator(void *nccl_comm, IcpState *d_state) {
     if (peers_ready_) {
-        k_peer_allreduce<<<1, 256, 0, stream_>>>(PeerLinksOf(links_host_), d_acc_, d_state);
+        k_peer_allreduce<<<1, 256, 0, stream_>>>(PeerLinksOf(links_host_), d_acc_.data(), d_state);
         launches_ += 1;
         return;
     }
@@ -1076,37 +1068,16 @@ IcpSolver::IcpSolver(cudaStream_t stream) : stream_(stream) {
     CT_CUDA_CHECK(cudaFuncSetAttribute(k_gn_persistent<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(GnShared)));
     CT_CUDA_CHECK(cudaFuncSetAttribute(k_gn_persistent<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(GnShared)));
     cudaDeviceGetAttribute(&num_sms_, cudaDevAttrMultiProcessorCount, dev);
-    CT_CUDA_CHECK(cudaMalloc(&d_sys_, sizeof(double) * 160));
-    CT_CUDA_CHECK(cudaMalloc(&d_acc_, sizeof(double) * kAcc));
-    CT_CUDA_CHECK(cudaMalloc(&d_ticket_, sizeof(unsigned int)));
-    CT_CUDA_CHECK(cudaMemset(d_ticket_, 0, sizeof(unsigned int)));
+    d_sys_.reserve(160, stream_);
+    d_acc_.reserve(kAcc, stream_);
+    d_ticket_.reserve(1, stream_);
+    CT_CUDA_CHECK(cudaMemset(d_ticket_.data(), 0, sizeof(unsigned int)));
     for (int i = 0; i < kMaxEvents; ++i) {
-        CT_CUDA_CHECK(cudaEventCreate(&ev_begin_[i]));
-        CT_CUDA_CHECK(cudaEventCreate(&ev_end_[i]));
+        ev_begin_[i] = Event(cudaEventDefault);
+        ev_end_[i] = Event(cudaEventDefault);
     }
 }
-IcpSolver::~IcpSolver() {
-    cudaFree(d_partials_);
-    cudaFree(d_sys_);
-    cudaFree(d_acc_);
-    cudaFree(d_ticket_);
-    cudaFree(d_loop_rows_);
-    cudaFree(d_loop_pose_);
-    cudaFree(d_groups_);
-    cudaFree(d_gn_table_);
-    FreeLmBuffers();
-    for (int i = 0; i < kMaxEvents; ++i) {
-        cudaEventDestroy(ev_begin_[i]);
-        cudaEventDestroy(ev_end_[i]);
-    }
-}
-void IcpSolver::EnsurePartials(int blocks) {
-    if (blocks <= partial_blocks_) return;
-    CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    cudaFree(d_partials_);
-    CT_CUDA_CHECK(cudaMalloc(&d_partials_, sizeof(double) * kAcc * (size_t) blocks));
-    partial_blocks_ = blocks;
-}
+void IcpSolver::EnsurePartials(int blocks) { d_partials_.reserve((size_t) kAcc * blocks, stream_); }
 GnParams IcpSolver::MakeParams(const DeviceMap &map, const cticp_icp_options &opt) const {
     GnParams P{};
     map.SearchParams(map.Options().default_radius, &P.level, &P.r);
@@ -1140,21 +1111,17 @@ int IcpSolver::GnCoresident(bool peers) {
 // launch. Tag 0 is never handed out, so zeroed words never match; when the counter would wrap, both areas are zeroed
 // again (stream order: after every earlier launch) and it restarts at 1.
 unsigned int IcpSolver::ReserveLoopTags(int rows, int groups, int num_iters) {
-    const auto grow = [&](unsigned long long *&buf, int &cap, int want, size_t words_each) {
-        if (want <= cap) return;
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(buf);
-        buf = nullptr;
-        CT_CUDA_CHECK(cudaMalloc(&buf, sizeof(unsigned long long) * words_each * (size_t) want));
-        CT_CUDA_CHECK(cudaMemsetAsync(buf, 0, sizeof(unsigned long long) * words_each * (size_t) want, stream_));
-        cap = want;
+    const auto grow = [&](DeviceArray<unsigned long long> &buf, size_t words) {
+        if (words <= buf.capacity()) return;
+        buf.reserve(words, stream_);
+        CT_CUDA_CHECK(cudaMemsetAsync(buf.data(), 0, sizeof(unsigned long long) * words, stream_));
     };
-    grow(d_loop_rows_, loop_rows_cap_, std::max(rows, 1), kRowWords);
-    grow(d_loop_pose_, loop_groups_cap_, std::max(groups, 1), kPoseGroupWords);
+    grow(d_loop_rows_, kRowWords * (size_t) std::max(rows, 1));
+    grow(d_loop_pose_, kPoseGroupWords * (size_t) std::max(groups, 1));
     const unsigned long long span = (unsigned long long) std::max(num_iters, 0) + 1;
     if (loop_tag_ + span > 0xffffffffull) {
-        CT_CUDA_CHECK(cudaMemsetAsync(d_loop_rows_, 0, sizeof(unsigned long long) * kRowWords * (size_t) loop_rows_cap_, stream_));
-        CT_CUDA_CHECK(cudaMemsetAsync(d_loop_pose_, 0, sizeof(unsigned long long) * kPoseGroupWords * (size_t) loop_groups_cap_, stream_));
+        CT_CUDA_CHECK(cudaMemsetAsync(d_loop_rows_.data(), 0, sizeof(unsigned long long) * d_loop_rows_.capacity(), stream_));
+        CT_CUDA_CHECK(cudaMemsetAsync(d_loop_pose_.data(), 0, sizeof(unsigned long long) * d_loop_pose_.capacity(), stream_));
         loop_tag_ = 1;
     }
     const unsigned int tag = loop_tag_;
@@ -1201,18 +1168,12 @@ void IcpSolver::EnqueueGaussNewtonGroups(const GnProblem *problems, int batch) {
     BatchGatherCtas(n.data(), batch, coresident, kp_per_cta_, gather.data());
     const size_t cta_off = sizeof(GnGroup) * (size_t) batch, count_off = cta_off + sizeof(int) * (size_t) (batch + 1);
     const size_t bytes = count_off + sizeof(int) * (size_t) batch;
-    if (bytes > gn_table_cap_) {
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(d_gn_table_);
-        d_gn_table_ = nullptr;
-        CT_CUDA_CHECK(cudaMalloc(&d_gn_table_, bytes));
-        gn_table_cap_ = bytes;
-    }
+    d_gn_table_.reserve(bytes, stream_);
     h_gn_table_.assign(bytes, 0);
     GnGroup *table = reinterpret_cast<GnGroup *>(h_gn_table_.data());
     int *first_cta = reinterpret_cast<int *>(h_gn_table_.data() + cta_off);
     int *count = reinterpret_cast<int *>(h_gn_table_.data() + count_off);
-    const int *d_count = reinterpret_cast<const int *>(d_gn_table_ + count_off);
+    const int *d_count = reinterpret_cast<const int *>(d_gn_table_.data() + count_off);
     int max_iters = 0;
     for (int b = 0; b < batch; ++b) {
         const GnProblem &p = problems[b];
@@ -1233,9 +1194,9 @@ void IcpSolver::EnqueueGaussNewtonGroups(const GnProblem *problems, int batch) {
         first_cta[b + 1] = first_cta[b] + 1 + gather[b];
     }
     const int grid = first_cta[batch];
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_gn_table_, h_gn_table_.data(), bytes, cudaMemcpyHostToDevice, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_gn_table_.data(), h_gn_table_.data(), bytes, cudaMemcpyHostToDevice, stream_));
     const unsigned int tag = ReserveLoopTags(grid - batch, batch, max_iters);
-    GnLoopWords words{d_loop_rows_, d_loop_pose_, tag};
+    GnLoopWords words{d_loop_rows_.data(), d_loop_pose_.data(), tag};
     GatherLaunch cfg{};
     const float4 *kp = nullptr;
     const int *nk = nullptr;
@@ -1243,7 +1204,7 @@ void IcpSolver::EnqueueGaussNewtonGroups(const GnProblem *problems, int batch) {
     int iters = 0;
     PeerLinks links{};
     FrameTailArgs tail_args{};
-    GnGroups groups{reinterpret_cast<const GnGroup *>(d_gn_table_), reinterpret_cast<const int *>(d_gn_table_ + cta_off), batch};
+    GnGroups groups{reinterpret_cast<const GnGroup *>(d_gn_table_.data()), reinterpret_cast<const int *>(d_gn_table_.data() + cta_off), batch};
     void *args[] = {&cfg, &kp, &nk, &st, &iters, &links, &words, &tail_args, &groups};
     CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_gn_persistent<false, true>, dim3(grid), dim3(kGatherWarps * 32), args,
                                               sizeof(GnShared), stream_));
@@ -1253,10 +1214,10 @@ void IcpSolver::EnqueueGaussNewtonGroups(const GnProblem *problems, int batch) {
 
 void IcpSolver::PrintWarpStamps(int iters) {
 #ifdef CTICP_DEBUG_TIMERS
-    if (!d_dbg_warp_ || dbg_warps_ <= 0) return;
+    if (!d_dbg_warp_.data() || dbg_warps_ <= 0) return;
     const int W = dbg_warps_;
     std::vector<unsigned long long> h((size_t) kDbgIters * W * kDbgSlots);
-    CT_CUDA_CHECK(cudaMemcpy(h.data(), d_dbg_warp_, sizeof(unsigned long long) * h.size(), cudaMemcpyDeviceToHost));
+    CT_CUDA_CHECK(cudaMemcpy(h.data(), d_dbg_warp_.data(), sizeof(unsigned long long) * h.size(), cudaMemcpyDeviceToHost));
     static const char *names[kDbgSlots - 1] = {"A pose+voxel", "B gather+select", "C epilogue", "pose fetch", "fetch+tiles+row reduction",
                                                "barrier wait (per CTA)", "end of last tile"};
     const auto pct = [](std::vector<unsigned long long> v, int p) { std::sort(v.begin(), v.end()); return v.empty() ? 0ull : v[v.size() * p / 100]; };
@@ -1318,8 +1279,8 @@ void IcpSolver::CollectGatherTiming() {
         float ms = 0.f;
         // (the caller may have learnt the result from the frame verdict, which the device writes before — or, with
         // CTICP_TAIL_IN_KERNEL=1, from inside — the kernel this event follows)
-        cudaEventSynchronize(ev_end_[i]);
-        if (cudaEventElapsedTime(&ms, ev_begin_[i], ev_end_[i]) == cudaSuccess) gather_ms_ += ms;
+        cudaEventSynchronize(ev_end_[i].get());
+        if (cudaEventElapsedTime(&ms, ev_begin_[i].get(), ev_end_[i].get()) == cudaSuccess) gather_ms_ += ms;
     }
     ev_used_ = 0;
 }
@@ -1353,26 +1314,22 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
 #ifdef CTICP_DEBUG_TIMERS
         if (getenv("CTICP_DEBUG_TIMERS")) {
             const int warps = (grid - 1) * kGatherWarps;
-            if (warps > dbg_warps_) {
-                CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-                cudaFree(d_dbg_warp_);
-                CT_CUDA_CHECK(cudaMalloc(&d_dbg_warp_, sizeof(unsigned long long) * kDbgIters * warps * kDbgSlots));
-            }
+            d_dbg_warp_.reserve((size_t) kDbgIters * warps * kDbgSlots, stream_);
             dbg_warps_ = warps;
-            CT_CUDA_CHECK(cudaMemsetAsync(d_dbg_warp_, 0, sizeof(unsigned long long) * kDbgIters * warps * kDbgSlots, stream_));
-            cfg.P.dbg_warp = d_dbg_warp_;
+            CT_CUDA_CHECK(cudaMemsetAsync(d_dbg_warp_.data(), 0, sizeof(unsigned long long) * kDbgIters * warps * kDbgSlots, stream_));
+            cfg.P.dbg_warp = d_dbg_warp_.data();
         }
 #endif
         const unsigned int tag = ReserveLoopTags(grid - 1, 1, num_iters);
-        GnLoopWords words{d_loop_rows_, d_loop_pose_, tag};
+        GnLoopWords words{d_loop_rows_.data(), d_loop_pose_.data(), tag};
         FrameTailArgs tail_args{};
         if (tail) tail_args = *tail;
         GnGroups groups{nullptr, nullptr, 1};
         void *args[] = {&cfg, &kp, &nk, &d_state, &iters, &links, &words, &tail_args, &groups};
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
-        if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
+        if (timed) cudaEventRecord(ev_begin_[ev_used_].get(), stream_);
         CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kGatherWarps * 32), args, sizeof(GnShared), stream_));
-        if (timed) cudaEventRecord(ev_end_[ev_used_++], stream_);
+        if (timed) cudaEventRecord(ev_end_[ev_used_++].get(), stream_);
         gather_launches_ += 1;
         launches_ += 1;
         return tail != nullptr;
@@ -1381,15 +1338,15 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
     EnsurePartials(blocks + 1);
     for (int it = 0; it < num_iters; ++it) {
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
-        if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
+        if (timed) cudaEventRecord(ev_begin_[ev_used_].get(), stream_);
         k_gn_iterate<<<blocks, kGatherWarps * 32, sizeof(GnShared), stream_>>>(cfg, d_keypoints, d_num_keypoints, d_state,
-                                                                              d_partials_, d_ticket_, nccl_comm ? 2 : 0, d_acc_, nullptr);
-        if (timed) cudaEventRecord(ev_end_[ev_used_++], stream_);
+                                                                              d_partials_.data(), d_ticket_.data(), nccl_comm ? 2 : 0, d_acc_.data(), nullptr);
+        if (timed) cudaEventRecord(ev_end_[ev_used_++].get(), stream_);
         ++gather_launches_;
         launches_ += 1;
         if (nccl_comm) {
             AllReduceAccumulator(nccl_comm, d_state);   // in-place sum of d_acc_ over ranks (peer mailboxes, else NCCL)
-            k_gn_solve_acc<<<1, 32, 0, stream_>>>(d_acc_, d_state, cfg.P);
+            k_gn_solve_acc<<<1, 32, 0, stream_>>>(d_acc_.data(), d_state, cfg.P);
             launches_ += 1;
         }
     }
@@ -1408,12 +1365,12 @@ void IcpSolver::NormalEquations(const DeviceMap &map, const cticp_icp_options &o
     cfg.G.kmax = cfg.P.kmax;
     const int blocks = GatherBlocks(k_upper, num_sms_, kp_per_cta_);
     EnsurePartials(blocks);
-    CT_CUDA_CHECK(cudaMemsetAsync(d_sys_, 0, sizeof(double) * 160, stream_));
+    CT_CUDA_CHECK(cudaMemsetAsync(d_sys_.data(), 0, sizeof(double) * 160, stream_));
     k_gn_iterate<<<blocks, kGatherWarps * 32, sizeof(GnShared), stream_>>>(cfg, d_keypoints, d_num_keypoints, d_state,
-                                                                          d_partials_, d_ticket_, 1, d_acc_, d_sys_);
+                                                                          d_partials_.data(), d_ticket_.data(), 1, d_acc_.data(), d_sys_.data());
     launches_ += 1;
     double h[160];
-    CT_CUDA_CHECK(cudaMemcpyAsync(h, d_sys_, sizeof(h), cudaMemcpyDeviceToHost, stream_));
+    CT_CUDA_CHECK(cudaMemcpyAsync(h, d_sys_.data(), sizeof(h), cudaMemcpyDeviceToHost, stream_));
     CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
     for (int i = 0; i < 144; ++i) h_A144[i] = h[i];
     for (int i = 0; i < 12; ++i) h_b12[i] = h[144 + i];
@@ -1444,15 +1401,14 @@ void IcpSolver::RadiusSearch(const DeviceMap &map, const double *d_queries, cons
     R.filter = (sensor_location && map.Options().select_valid_normals_direction && map.HasNormals()) ? 1 : 0;
     if (sensor_location) R.sensor = V3{sensor_location[0], sensor_location[1], sensor_location[2]};
     for (int i = 0; i < R.num_levels; ++i) R.levels[i] = map.Level(i);
-    RadiusSearchLevels *d_R = nullptr;
-    CT_CUDA_CHECK(cudaMalloc(&d_R, sizeof(R)));
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_R, &R, sizeof(R), cudaMemcpyHostToDevice, stream_));
+    DeviceArray<RadiusSearchLevels> d_R;
+    d_R.reserve(1, stream_);
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_R.data(), &R, sizeof(R), cudaMemcpyHostToDevice, stream_));
     const int blocks = (int) std::max<size_t>(1, std::min((n + kGatherWarps - 1) / kGatherWarps, (size_t) num_sms_ * 2));
-    k_radius_search<<<blocks, kGatherWarps * 32, 0, stream_>>>(d_R, kmax, d_queries, d_radiuses, (int) n, d_out_points, d_out_counts);
+    k_radius_search<<<blocks, kGatherWarps * 32, 0, stream_>>>(d_R.data(), kmax, d_queries, d_radiuses, (int) n, d_out_points, d_out_counts);
     launches_ += 1;
     CT_CUDA_CHECK(cudaGetLastError());
     CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    cudaFree(d_R);
 }
 
 }  // namespace cticp

@@ -28,14 +28,6 @@
 
 namespace cticp {
 
-#define CT_CUDA_CHECK(expr)                                                                              \
-    do {                                                                                                 \
-        cudaError_t _e = (expr);                                                                         \
-        if (_e != cudaSuccess)                                                                           \
-            throw CudaError(std::string(#expr) + ": " + cudaGetErrorString(_e) + " @" + __FILE__ + ":" + \
-                            std::to_string(__LINE__));                                                   \
-    } while (0)
-
 constexpr int kLmWarps = 4;
 constexpr int kAccCost = 91;   // Σ 1/2 rho(s) in the accumulator
 
@@ -1363,20 +1355,11 @@ k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoint
 
 // ---------------------------------------------------------------------------------------------------------------
 void IcpSolver::EnsureLmBuffers(size_t k_upper) {
-    if (!d_lm_state_) {
-        CT_CUDA_CHECK(cudaMalloc(&d_lm_state_, sizeof(LmState)));
-        CT_CUDA_CHECK(cudaMalloc(&d_lm_stats_, sizeof(unsigned long long) * 2));
-        }
-    if (k_upper > lm_capacity_) {
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(d_lm_blocks_);
-        cudaFree(d_lm_sel_);
-        cudaFree(d_lm_classes_);
-        CT_CUDA_CHECK(cudaMalloc(&d_lm_classes_, k_upper));
-        CT_CUDA_CHECK(cudaMalloc(&d_lm_blocks_, sizeof(ResidualBlock) * k_upper));
-        CT_CUDA_CHECK(cudaMalloc(&d_lm_sel_, sizeof(int) * k_upper));
-        lm_capacity_ = k_upper;
-    }
+    d_lm_state_.reserve(1, stream_);
+    d_lm_stats_.reserve(2, stream_);
+    d_lm_classes_.reserve(k_upper, stream_);
+    d_lm_blocks_.reserve(k_upper, stream_);
+    d_lm_sel_.reserve(k_upper, stream_);
 }
 void IcpSolver::PreloadLmKernels() {
     cudaFuncAttributes a;
@@ -1387,15 +1370,6 @@ void IcpSolver::PreloadLmKernels() {
     cudaFuncGetAttributes(&a, k_lm_gather<true>);
     cudaFuncGetAttributes(&a, k_rb_gather);
     cudaFuncGetAttributes(&a, k_lm_select);
-}
-void IcpSolver::FreeLmBuffers() {
-    cudaFree(d_lm_state_);
-    cudaFree(d_lm_stats_);
-    cudaFree(d_lm_blocks_);
-    cudaFree(d_lm_sel_);
-    cudaFree(d_lm_classes_);
-    cudaFree(d_lm_strategy_);
-    cudaFree(d_lm_groups_);
 }
 
 // k_lm_persistent<mode, peers, grouped>; mode 0 = CERES nearest neighbor, 1 = CERES distance-based, 2 = ROBUST
@@ -1434,8 +1408,8 @@ bool IcpSolver::UploadLmStrategy(const DeviceMap &map, const cticp_icp_options &
     D.radius_max = strategy.radius_max;
     D.exponent = strategy.exponent;
     for (int i = 0; i < D.num_levels; ++i) D.levels[i] = map.Level(i);
-    if (!d_lm_strategy_) CT_CUDA_CHECK(cudaMalloc(&d_lm_strategy_, sizeof(DistanceStrategy)));
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_lm_strategy_, &D, sizeof(D), cudaMemcpyHostToDevice, stream_));
+    d_lm_strategy_.reserve(1, stream_);
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_lm_strategy_.data(), &D, sizeof(D), cudaMemcpyHostToDevice, stream_));
     CT_CUDA_CHECK(cudaStreamSynchronize(stream_));   // D lives on this stack frame
     return true;
 }
@@ -1529,16 +1503,16 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
     if (sharded && shard_world > kAcc) throw std::invalid_argument("sharding: world size above 96");
     const GatherConfig G = LmGatherConfig(map, P);
 
-    auto *lm = static_cast<LmState *>(d_lm_state_);
-    auto *blocks_buf = static_cast<ResidualBlock *>(d_lm_blocks_);
-    auto *stats = static_cast<unsigned long long *>(d_lm_stats_);
+    auto *lm = d_lm_state_.data();
+    auto *blocks_buf = d_lm_blocks_.data();
+    auto *stats = d_lm_stats_.data();
     const int gather_blocks = (int) std::max<size_t>(1, std::min<size_t>((k_hint + kLmWarps - 1) / kLmWarps, (size_t) num_sms_ * 8));
     const size_t r_hint = opt.max_num_residuals > 0 ? std::min<size_t>(k_hint, (size_t) opt.max_num_residuals) : k_hint;
     const int eval_blocks = (int) std::max<size_t>(1, std::min<size_t>((r_hint + kLmWarps * 2 - 1) / (kLmWarps * 2), (size_t) num_sms_ * 4));
     EnsurePartials(eval_blocks);
 
     const bool distance_based = UploadLmStrategy(map, opt, strategy);
-    auto *classes = static_cast<unsigned char *>(d_lm_classes_);
+    auto *classes = d_lm_classes_.data();
     if (robust) CT_CUDA_CHECK(cudaMemsetAsync(classes, 0, k_capacity, stream_));   // NEIGHBORHOOD_TYPE::NONE
 
     if (use_persistent_ && (!sharded || peers_ready_)) {
@@ -1553,17 +1527,17 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
         EnsurePartials(grid);
         const float4 *kp = d_keypoints;
         const int *nk = d_num_keypoints;
-        int *sel = d_lm_sel_;
-        const DistanceStrategy *dstrat = static_cast<const DistanceStrategy *>(d_lm_strategy_);
-        double *parts = d_partials_;
+        int *sel = d_lm_sel_.data();
+        const DistanceStrategy *dstrat = d_lm_strategy_.data();
+        double *parts = d_partials_.data();
         PeerLinks links = peers ? PeerLinksOf(links_host_) : PeerLinks{};
         LmGroups groups{};
         GatherConfig g = G;
         void *args[] = {&g, &P, &kp, &nk, &d_state, &lm, &blocks_buf, &sel, &classes, &stats, &dstrat, &parts, &links, &groups};
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
-        if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
+        if (timed) cudaEventRecord(ev_begin_[ev_used_].get(), stream_);
         CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kLmPWarps * 32), args, sizeof(LmPShared), stream_));
-        if (timed) cudaEventRecord(ev_end_[ev_used_++], stream_);
+        if (timed) cudaEventRecord(ev_end_[ev_used_++].get(), stream_);
         gather_launches_ += 1;
         launches_ += 1;
         DebugLmTrace(lm);
@@ -1574,41 +1548,41 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
     launches_ += 1;
     for (int it = 0; it < opt.num_iters_icp; ++it) {
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
-        if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
+        if (timed) cudaEventRecord(ev_begin_[ev_used_].get(), stream_);
         if (robust)
             k_rb_gather<<<gather_blocks, kLmWarps * 32, 0, stream_>>>(G, P, d_keypoints, d_num_keypoints, d_state, blocks_buf,
                                                                      classes, stats);
         else if (distance_based)
             k_lm_gather<true><<<gather_blocks, kLmWarps * 32, 0, stream_>>>(G, P, d_keypoints, d_num_keypoints, d_state, blocks_buf,
-                                                                           stats, static_cast<const DistanceStrategy *>(d_lm_strategy_));
+                                                                           stats, d_lm_strategy_.data());
         else
             k_lm_gather<false><<<gather_blocks, kLmWarps * 32, 0, stream_>>>(G, P, d_keypoints, d_num_keypoints, d_state, blocks_buf,
                                                                             stats, nullptr);
-        if (timed) cudaEventRecord(ev_end_[ev_used_++], stream_);
+        if (timed) cudaEventRecord(ev_end_[ev_used_++].get(), stream_);
         ++gather_launches_;
         // One evaluation + minimizer step. Sharded: every rank evaluates its share of the residual blocks, the 96-double
         // accumulators are summed over the ranks (ncclAllReduce, bit-identical result everywhere) and every rank takes
         // the same step — the exchange of SURVEY §8e, once per LM evaluation.
         auto eval_and_step = [&](int phase) {
-            k_lm_eval<<<eval_blocks, kLmWarps * 32, 0, stream_>>>(P, phase, blocks_buf, d_lm_sel_, d_state, lm, d_partials_);
+            k_lm_eval<<<eval_blocks, kLmWarps * 32, 0, stream_>>>(P, phase, blocks_buf, d_lm_sel_.data(), d_state, lm, d_partials_.data());
             if (sharded && peers_ready_) {   // exchange inside the step kernel (NVLink peer mailboxes)
-                k_lm_step<true><<<1, 128, 0, stream_>>>(P, phase, d_partials_, eval_blocks, d_state, lm, PeerLinksOf(links_host_));
+                k_lm_step<true><<<1, 128, 0, stream_>>>(P, phase, d_partials_.data(), eval_blocks, d_state, lm, PeerLinksOf(links_host_));
             } else if (sharded) {            // fallback: library collective between two kernels
-                k_lm_reduce<<<1, 128, 0, stream_>>>(d_partials_, eval_blocks, d_acc_);
+                k_lm_reduce<<<1, 128, 0, stream_>>>(d_partials_.data(), eval_blocks, d_acc_.data());
                 AllReduceAccumulator(nccl_comm, d_state);
-                k_lm_step<false><<<1, 128, 0, stream_>>>(P, phase, d_acc_, 1, d_state, lm, PeerLinks{});
+                k_lm_step<false><<<1, 128, 0, stream_>>>(P, phase, d_acc_.data(), 1, d_state, lm, PeerLinks{});
                 launches_ += 1;
             } else {
-                k_lm_step<false><<<1, 128, 0, stream_>>>(P, phase, d_partials_, eval_blocks, d_state, lm, PeerLinks{});
+                k_lm_step<false><<<1, 128, 0, stream_>>>(P, phase, d_partials_.data(), eval_blocks, d_state, lm, PeerLinks{});
             }
             launches_ += 2;
         };
         if (sharded) {   // all-gather of the per-rank valid counts (as a sum of one-hot vectors)
-            k_lm_select<<<1, 1024, 0, stream_>>>(P, 1, d_num_keypoints, blocks_buf, d_lm_sel_, d_state, lm, stats, d_acc_);
+            k_lm_select<<<1, 1024, 0, stream_>>>(P, 1, d_num_keypoints, blocks_buf, d_lm_sel_.data(), d_state, lm, stats, d_acc_.data());
             AllReduceAccumulator(nccl_comm, d_state);
             launches_ += 1;
         }
-        k_lm_select<<<1, 1024, 0, stream_>>>(P, 0, d_num_keypoints, blocks_buf, d_lm_sel_, d_state, lm, stats, d_acc_);
+        k_lm_select<<<1, 1024, 0, stream_>>>(P, 0, d_num_keypoints, blocks_buf, d_lm_sel_.data(), d_state, lm, stats, d_acc_.data());
         launches_ += 2;
         eval_and_step(0);
         for (int ls = 0; ls < opt.ls_max_num_iters; ++ls) eval_and_step(1);
@@ -1640,37 +1614,31 @@ void IcpSolver::EnqueueCeresBatch(const DeviceMap &map, const cticp_icp_options 
     EnsureLmBuffers(std::max<size_t>(total, 1) * (size_t) P.ncn);
     // per group: its LmState (kLmStateStride), its stats line and its barrier words, each area after the B of the one before
     constexpr size_t kGroupBytes = kLmStateStride + sizeof(unsigned long long) * kLmStatsStride + sizeof(unsigned int) * kLmBarrierWords;
-    if (batch > lm_groups_cap_) {
-        CT_CUDA_CHECK(cudaStreamSynchronize(stream_));
-        cudaFree(d_lm_groups_);
-        d_lm_groups_ = nullptr;
-        CT_CUDA_CHECK(cudaMalloc(&d_lm_groups_, kGroupBytes * (size_t) batch));
-        lm_groups_cap_ = batch;
-    }
-    char *area = static_cast<char *>(d_lm_groups_);
+    d_lm_groups_.reserve(kGroupBytes * (size_t) batch, stream_);
+    char *area = d_lm_groups_.data();
     auto *lm = reinterpret_cast<LmState *>(area);
     auto *stats = reinterpret_cast<unsigned long long *>(area + kLmStateStride * batch);
     auto *barrier = reinterpret_cast<unsigned int *>(area + (kLmStateStride + sizeof(unsigned long long) * kLmStatsStride) * batch);
     UploadLmStrategy(map, opt, strategy);
-    auto *classes = static_cast<unsigned char *>(d_lm_classes_);
+    auto *classes = d_lm_classes_.data();
     if (robust) CT_CUDA_CHECK(cudaMemsetAsync(classes, 0, total, stream_));   // NEIGHBORHOOD_TYPE::NONE
     const int grid = UploadGroupTable(h_n, batch, coresident);
     EnsurePartials(grid - batch);
     CT_CUDA_CHECK(cudaMemsetAsync(barrier, 0, sizeof(unsigned int) * kLmBarrierWords * batch, stream_));
 
     const float4 *kp = d_keypoints;
-    const int *nk = d_groups_ + 2 * batch + 1;   // count[0] (read by the solo launch only)
-    auto *blocks_buf = static_cast<ResidualBlock *>(d_lm_blocks_);
-    int *sel = d_lm_sel_;
-    const DistanceStrategy *dstrat = static_cast<const DistanceStrategy *>(d_lm_strategy_);
-    double *parts = d_partials_;
+    const int *nk = d_groups_.data() + 2 * batch + 1;   // count[0] (read by the solo launch only)
+    auto *blocks_buf = d_lm_blocks_.data();
+    int *sel = d_lm_sel_.data();
+    const DistanceStrategy *dstrat = d_lm_strategy_.data();
+    double *parts = d_partials_.data();
     PeerLinks links{};
-    LmGroups groups = grouped ? LmGroups{d_groups_, batch, barrier} : LmGroups{};
+    LmGroups groups = grouped ? LmGroups{d_groups_.data(), batch, barrier} : LmGroups{};
     void *args[] = {&G, &P, &kp, &nk, &d_states, &lm, &blocks_buf, &sel, &classes, &stats, &dstrat, &parts, &links, &groups};
     const bool timed = time_gather_ && ev_used_ < kMaxEvents;
-    if (timed) cudaEventRecord(ev_begin_[ev_used_], stream_);
+    if (timed) cudaEventRecord(ev_begin_[ev_used_].get(), stream_);
     CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kLmPWarps * 32), args, sizeof(LmPShared), stream_));
-    if (timed) cudaEventRecord(ev_end_[ev_used_++], stream_);
+    if (timed) cudaEventRecord(ev_end_[ev_used_++].get(), stream_);
     gather_launches_ += 1;
     launches_ += 1;
 }

@@ -70,7 +70,7 @@ void Check(ncclResult_t r, const char *what) {
 }  // namespace
 
 void IcpSolver::NcclAllReduceAccumulator(void *nccl_comm) {
-    Check(Api().AllReduce(d_acc_, d_acc_, kAcc, ncclDouble, ncclSum, (ncclComm_t) nccl_comm, stream_), "ncclAllReduce");
+    Check(Api().AllReduce(d_acc_.data(), d_acc_.data(), kAcc, ncclDouble, ncclSum, (ncclComm_t) nccl_comm, stream_), "ncclAllReduce");
 }
 
 // ---- peer mailboxes ------------------------------------------------------------------------------------------
@@ -143,8 +143,8 @@ bool Engine::ConnectPeers() {
     mine.pid = (long long) getpid();
     mine.device = device_;
     if (d_mailbox_) {
-        if (cudaMemsetAsync(d_mailbox_, 0, kMailboxBytes + 256, stream_) != cudaSuccess ||
-            cudaStreamSynchronize(stream_) != cudaSuccess)
+        if (cudaMemsetAsync(d_mailbox_, 0, kMailboxBytes + 256, stream_.get()) != cudaSuccess ||
+            cudaStreamSynchronize(stream_.get()) != cudaSuccess)
             my_ok = 0;
         if (cudaIpcGetMemHandle(&mine.handle, d_mailbox_) != cudaSuccess) {
             cudaGetLastError();
@@ -156,17 +156,13 @@ bool Engine::ConnectPeers() {
     // all-gather of the blobs (NCCL is only the bootstrap here)
     std::vector<PeerBlob> all((size_t) world);
     {
-        PeerBlob *d_all = nullptr;
-        if (cudaMalloc(&d_all, sizeof(PeerBlob) * (size_t) world) != cudaSuccess) throw CudaError("cudaMalloc (peer bootstrap)");
-        cudaMemcpyAsync(d_all + rank, &mine, sizeof(PeerBlob), cudaMemcpyHostToDevice, stream_);
+        DeviceArray<PeerBlob> d_all;
+        d_all.reserve(world, stream_.get());
+        cudaMemcpyAsync(d_all.data() + rank, &mine, sizeof(PeerBlob), cudaMemcpyHostToDevice, stream_.get());
         if (api.AllGather)
-            Check(api.AllGather(d_all + rank, d_all, sizeof(PeerBlob), ncclChar, comm, stream_), "ncclAllGather");
-        cudaMemcpyAsync(all.data(), d_all, sizeof(PeerBlob) * (size_t) world, cudaMemcpyDeviceToHost, stream_);
-        if (cudaStreamSynchronize(stream_) != cudaSuccess) {
-            cudaFree(d_all);
-            throw CudaError("peer bootstrap: stream error");
-        }
-        cudaFree(d_all);
+            Check(api.AllGather(d_all.data() + rank, d_all.data(), sizeof(PeerBlob), ncclChar, comm, stream_.get()), "ncclAllGather");
+        cudaMemcpyAsync(all.data(), d_all.data(), sizeof(PeerBlob) * (size_t) world, cudaMemcpyDeviceToHost, stream_.get());
+        if (cudaStreamSynchronize(stream_.get()) != cudaSuccess) throw CudaError("peer bootstrap: stream error");
     }
 
     PeerLinksHost links;
@@ -211,20 +207,14 @@ bool Engine::ConnectPeers() {
     }
     links.seq = d_mailbox_ ? (unsigned int *) ((char *) d_mailbox_ + kMailboxBytes) : nullptr;
 
-    // agreement: min over ranks of my_ok
+    // agreement: min over ranks of my_ok (the flag serves the rendezvous below as well)
     int agreed = 0;
-    {
-        int *d_flag = nullptr;
-        if (cudaMalloc(&d_flag, sizeof(int)) != cudaSuccess) throw CudaError("cudaMalloc (peer bootstrap)");
-        cudaMemcpyAsync(d_flag, &my_ok, sizeof(int), cudaMemcpyHostToDevice, stream_);
-        Check(api.AllReduce(d_flag, d_flag, 1, ncclInt, ncclMin, comm, stream_), "ncclAllReduce (peer agreement)");
-        cudaMemcpyAsync(&agreed, d_flag, sizeof(int), cudaMemcpyDeviceToHost, stream_);
-        if (cudaStreamSynchronize(stream_) != cudaSuccess) {
-            cudaFree(d_flag);
-            throw CudaError("peer bootstrap: stream error");
-        }
-        cudaFree(d_flag);
-    }
+    DeviceArray<int> d_flag;
+    d_flag.reserve(1, stream_.get());
+    cudaMemcpyAsync(d_flag.data(), &my_ok, sizeof(int), cudaMemcpyHostToDevice, stream_.get());
+    Check(api.AllReduce(d_flag.data(), d_flag.data(), 1, ncclInt, ncclMin, comm, stream_.get()), "ncclAllReduce (peer agreement)");
+    cudaMemcpyAsync(&agreed, d_flag.data(), sizeof(int), cudaMemcpyDeviceToHost, stream_.get());
+    if (cudaStreamSynchronize(stream_.get()) != cudaSuccess) throw CudaError("peer bootstrap: stream error");
     if (!agreed) {
         DisconnectPeers();
         return false;
@@ -240,15 +230,9 @@ bool Engine::ConnectPeers() {
     // every rank loads the sharded kernels' modules NOW, then the ranks meet once more: the first exchange finds all peers
     // warm instead of one of them inside a lazy module load
     icp_->PreloadShardedKernels();
-    {
-        int *d_flag = nullptr;
-        if (cudaMalloc(&d_flag, sizeof(int)) == cudaSuccess) {
-            cudaMemsetAsync(d_flag, 0, sizeof(int), stream_);
-            Check(api.AllReduce(d_flag, d_flag, 1, ncclInt, ncclMin, comm, stream_), "ncclAllReduce (peer rendezvous)");
-            cudaStreamSynchronize(stream_);
-            cudaFree(d_flag);
-        }
-    }
+    cudaMemsetAsync(d_flag.data(), 0, sizeof(int), stream_.get());
+    Check(api.AllReduce(d_flag.data(), d_flag.data(), 1, ncclInt, ncclMin, comm, stream_.get()), "ncclAllReduce (peer rendezvous)");
+    cudaStreamSynchronize(stream_.get());
     if (getenv("CTICP_DEBUG_P2P"))
         fprintf(stderr, "[cticp] rank %d/%d: peer mailboxes connected (%zu IPC mappings)\n", rank, world, peer_mapped_.size());
     return true;
@@ -266,7 +250,7 @@ void Engine::DisconnectPeers() {
 void Engine::EnableSharding(const void *unique_id, int rank, int world) {
     if (!unique_id || world < 1 || rank < 0 || rank >= world) throw std::invalid_argument("EnableSharding arguments");
     if (cudaSetDevice(device_) != cudaSuccess) throw CudaError("cudaSetDevice");
-    if (stream_) cudaStreamSynchronize(stream_);
+    if (stream_.get()) cudaStreamSynchronize(stream_.get());
     DisconnectPeers();
     if (nccl_comm_) {
         Api().CommDestroy((ncclComm_t) nccl_comm_);

@@ -7,14 +7,6 @@
 
 namespace cticp {
 
-#define CT_CUDA_CHECK(expr)                                                                              \
-    do {                                                                                                 \
-        cudaError_t _e = (expr);                                                                         \
-        if (_e != cudaSuccess)                                                                           \
-            throw CudaError(std::string(#expr) + ": " + cudaGetErrorString(_e) + " @" + __FILE__ + ":" + \
-                            std::to_string(__LINE__));                                                   \
-    } while (0)
-
 void RegisterBatch(std::vector<BatchItem> &items) {
     std::vector<Engine::PendingFrame> frames(items.size());
     std::vector<size_t> joining;
