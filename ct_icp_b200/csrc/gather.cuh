@@ -405,6 +405,11 @@ __device__ __forceinline__ Eig3 sym_eig3_fast(double a00, double a01, double a02
     const double c00 = b11 * b22 - s12 * s12, c01 = s01 * b22 - s12 * s02, c02 = s01 * s12 - b11 * s02;
     const double det = (b00 * c00 - s01 * c01 + s02 * c02) / (p * p * p);
     const double half_det = fmin(fmax(det * 0.5, -1.0), 1.0);
+    // Two coincident LARGEST eigenvalues (a disc) put half_det at -1, where acos turns the rounding error of half_det
+    // (~u) into an angle error ~sqrt(u) and the pair e1, e2 drifts apart by ~1e-8 relative (the normal, of e0, stays
+    // accurate and passes the check below). Their error is ~u p / sqrt(1 + half_det): within 1e-4 of -1 it exceeds ~100 u
+    // |A|, so such matrices take the Jacobi solver (tests/test_gpu_device_math.py, regime "disc_exact").
+    if (half_det < -1.0 + 1e-4) return sym_eig3(a00, a01, a02, a11, a12, a22);
     const double angle = acos(half_det) * (1.0 / 3.0);
     double ca, sa;   // angle in [0, pi/3]
     cos_sin_upto_third_pi(angle, ca, sa);
