@@ -858,6 +858,15 @@ GnProblem Engine::IcpProblem(const PendingFrame &f) const {
                      KeypointHint(), f.icp_options.num_iters_icp, d_state_.data()};
 }
 
+LmProblem Engine::CeresProblem(const PendingFrame &f) {
+    CT_CUDA_CHECK(cudaSetDevice(device_));
+    icp_->set_keypoints_lo(pipe_->d_keypoints_lo());
+    const LmProblem p = icp_->PrepareCeres(*map_, f.icp_options, options_.neighborhood_strategy, pipe_->d_keypoints(),
+                                           pipe_->d_count_keypoints(), KeypointHint(), pipe_->n(), d_state_.data());
+    CT_CUDA_CHECK(cudaEventRecord(ev_[1].get(), stream_.get()));   // (the grouped launch reads what the preparation wrote)
+    return p;
+}
+
 void Engine::AdoptGroupedIcp(PendingFrame &f, cudaEvent_t launched, int groups) {
     CT_CUDA_CHECK(cudaSetDevice(device_));
     CT_CUDA_CHECK(cudaStreamWaitEvent(stream_.get(), launched, 0));
@@ -1316,9 +1325,26 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
             TryRegisterBegin(info, ct_icp_options, summary, sample_voxel_size, mm, 0);
             f.icp_pending = true;
             // the frames whose ICP can run in a grouped launch (RegisterBatch): exactly those the solo launch would run
-            // through the persistent GN loop with the armed device tail
-            f.joins = tail_armed_ && ct_icp_options.solver == CTICP_SOLVER_GN && icp_->batch_supported() && !nccl_comm_ &&
-                      shard_world_ <= 1 && ct_icp_options.max_number_neighbors >= 1 && ct_icp_options.max_number_neighbors <= 32;
+            // through the persistent GN loop, or the solo launch of k_lm_persistent, with the armed device tail
+            if (tail_armed_ && !nccl_comm_ && shard_world_ <= 1) {
+                const int solver = ct_icp_options.solver;
+                if (solver == CTICP_SOLVER_GN && icp_->batch_supported() && ct_icp_options.max_number_neighbors >= 1 &&
+                    ct_icp_options.max_number_neighbors <= 32) {
+                    f.joins = kJoinsGn;
+                } else if ((solver == CTICP_SOLVER_CERES || solver == CTICP_SOLVER_ROBUST) && icp_->use_persistent()) {
+                    // options the LM path rejects keep the single-frame path, which fails them alone
+                    bool accepted = true;
+                    try {
+                        icp_->CheckCeresOptions(*map_, ct_icp_options, options_.neighborhood_strategy);
+                    } catch (const std::exception &) {
+                        accepted = false;
+                    }
+                    if (accepted)
+                        f.joins = solver == CTICP_SOLVER_ROBUST ? kJoinsRobust
+                                  : options_.neighborhood_strategy.type == CTICP_STRATEGY_DISTANCE_BASED ? kJoinsCeresDistance
+                                                                                                           : kJoinsCeresNearest;
+                }
+            }
         }
     } else {
         CT_CUDA_CHECK(cudaEventRecord(ev_[1].get(), stream_.get()));

@@ -126,6 +126,9 @@ public:
     // the device tail, sampling, the state upload; a robust registration runs its attempts here), the ICP launch (solo:
     // LaunchIcp; or a grouped launch shared with other handles, RegisterBatch), FinishFrame (verdict, map update,
     // summary). RegisterFrame / RegisterDevice / RegisterStaged run them back to back.
+    // The grouped ICP launches of RegisterBatch, one per kind of joining frame: solver GN (k_gn_persistent), and solver
+    // CERES with the nearest-neighbour strategy, CERES with the distance-based strategy and ROBUST (k_lm_persistent's modes).
+    enum { kJoinsNone = -1, kJoinsGn = 0, kJoinsCeresNearest, kJoinsCeresDistance, kJoinsRobust, kJoinKinds };
     struct PendingFrame {
         size_t n = 0;
         cticp_summary *out = nullptr;
@@ -140,7 +143,7 @@ public:
         bool ran_icp = false, early_return = false;
         bool icp_pending = false;     // a plain registration waits for its ICP launch and its TryRegisterEnd
         bool icp_launched = false;
-        bool joins = false;           // its ICP may run in a grouped launch (solver GN, persistent loop, armed device tail)
+        int joins = kJoinsNone;       // the grouped launch its ICP may run in (persistent loop, armed device tail)
     };
     void BeginFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate, cticp_summary *out,
                     const cticp_motion_prior *motion_model, PendingFrame &f);
@@ -151,7 +154,10 @@ public:
     void CompleteFrame(PendingFrame &f);
     // a joining frame's registration in a grouped launch (valid until FinishFrame)
     GnProblem IcpProblem(const PendingFrame &f) const;
-    // recorded on the engine's stream after the state upload and the sampling of the pending frame
+    // the same for a CERES / ROBUST frame: prepares this handle's LM buffers for it (IcpSolver::PrepareCeres) on the
+    // engine's stream, then records IcpReadyEvent again behind that work
+    LmProblem CeresProblem(const PendingFrame &f);
+    // recorded on the engine's stream after the state upload and the sampling of the pending frame (and CeresProblem)
     cudaEvent_t IcpReadyEvent() const { return ev_[1].get(); }
     // the grouped launch that ran the pending frame's ICP is enqueued, `launched` recorded behind it; `groups` problems
     void AdoptGroupedIcp(PendingFrame &f, cudaEvent_t launched, int groups);
@@ -341,8 +347,8 @@ struct BatchItem {
     cticp_summary *out = nullptr;
     std::exception_ptr error;      // out: what the item's single-frame call would have thrown
 };
-// One frame on each engine (all distinct, one device, none sharded), their eligible GN loops in one grouped launch
-// (cticp_odometry_register_batch has the contract). A failing item ends alone with its exception in `error`.
+// One frame on each engine (all distinct, one device, none sharded), the eligible ICP loops in one grouped launch per
+// kind, PendingFrame::joins (cticp_odometry_register_batch has the contract). A failing item ends alone with its exception in `error`.
 void RegisterBatch(std::vector<BatchItem> &items);
 
 // conversions shared with capi.cu

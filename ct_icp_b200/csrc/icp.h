@@ -110,6 +110,24 @@ struct GnProblem {
     IcpState *d_state;
 };
 
+// One registration of a grouped CERES / ROBUST launch (IcpSolver::EnqueueCeresGroups). Options checked by CheckCeresOptions;
+// the per-keypoint buffers and the uploaded strategy as IcpSolver::PrepareCeres leaves them.
+struct LmProblem {
+    const DeviceMap *map;
+    const cticp_icp_options *opt;
+    const cticp_strategy_options *strategy;
+    const float4 *keypoints;
+    const float4 *keypoints_lo;     // residual plane of the keypoints (nullptr: none; se3.cuh load_raw)
+    const int *d_num_keypoints;     // device keypoint count; nullptr: exactly n keypoints
+    size_t n;                       // the keypoint count, or with d_num_keypoints the estimate a solo launch sizes its grid
+                                    // from (EnqueueCeres's k_hint)
+    IcpState *d_state;
+    ResidualBlock *blocks;          // ncn residual blocks per keypoint
+    int *sel_idx;                   // ncn per keypoint
+    unsigned char *classes;         // solver ROBUST: one per keypoint, NEIGHBORHOOD_TYPE::NONE on entry
+    const DistanceStrategy *distance;   // CERES with the distance-based strategy: its parameters and the map's levels
+};
+
 class IcpSolver {
 public:
     explicit IcpSolver(cudaStream_t stream);
@@ -148,12 +166,24 @@ public:
     // the option checks of EnqueueCeres, without touching the device: UnsupportedError / std::invalid_argument
     void CheckCeresOptions(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy) const;
     // B independent CERES / ROBUST registrations against `map` with shared options and strategy, in ONE launch of the
-    // persistent LM kernel (k_lm_persistent over groups, separated by group barriers). Keypoints and states are laid out as
-    // for EnqueueGaussNewtonBatch; the CTA policy and its bit-identity contract are BatchGatherCtas' with the LM kernel's
-    // co-resident count. A group whose barrier times out ends with failed = 2 without holding up the others. Throws
-    // CapacityError when the device cannot hold two CTAs per problem; requires use_persistent().
+    // persistent LM kernel (EnqueueCeresGroups, every group on the same map, this solver's buffers). Keypoints and states
+    // are laid out as for EnqueueGaussNewtonBatch.
     void EnqueueCeresBatch(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
                            int batch, const size_t *h_n, const float4 *d_keypoints, IcpState *d_states);
+    // What EnqueueCeres does before its launch, for a registration that a grouped launch will run: the option checks, this
+    // solver's per-keypoint buffers sized for k_capacity keypoints, the strategy upload and ROBUST's class reset, all on
+    // this solver's stream. Returns the problem with this solver's buffers and residual plane (set_keypoints_lo).
+    LmProblem PrepareCeres(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
+                           const float4 *d_keypoints, const int *d_num_keypoints, size_t k_hint, size_t k_capacity,
+                           IcpState *d_state);
+    // B independent CERES / ROBUST registrations of one k_lm_persistent mode (CERES nearest neighbour, CERES
+    // distance-based, ROBUST), each with its own map, options, keypoints, state and buffers, in ONE launch of the grouped
+    // persistent LM kernel (groups separated by group barriers) on this solver's stream, with this solver's group area and
+    // table; one problem takes the solo launch. CTA policy and its bit-identity contract with the solo launch:
+    // BatchGatherCtas (icp_batch.cu) on the problems' n with the LM kernel's co-resident count. A group whose barrier
+    // times out ends with failed = 2 without holding up the others. Throws CapacityError when the device cannot hold two
+    // CTAs per problem; requires use_persistent(). The table is built on the host before this returns.
+    void EnqueueCeresGroups(const LmProblem *problems, int batch);
     bool use_persistent() const { return use_persistent_; }
 
     // single linearisation at the current state → A (12x12, after 1/n and regularisers), b, n_used (debug tap)
@@ -201,10 +231,8 @@ private:
     GnParams MakeParams(const DeviceMap &map, const cticp_icp_options &opt) const;
     int GnCoresident(bool peers);          // co-resident CTAs of k_gn_persistent<peers> on this device
     unsigned int ReserveLoopTags(int rows, int groups, int num_iters);   // k_gn_persistent's words and tags (icp_gn.cu)
-    // group table of a batched LM launch (first_cta | kp_base | count, BatchGatherCtas) built and uploaded to d_groups_;
-    // returns the grid (icp_batch.cu)
-    int UploadGroupTable(const size_t *h_n, int batch, int coresident);
-    int LmCoresident(int variant, void *kernel);   // co-resident CTAs of a k_lm_persistent instantiation (icp_lm.cu)
+    // co-resident CTAs of a k_lm_persistent instantiation with `smem` bytes of dynamic shared memory (icp_lm.cu)
+    int LmCoresident(int variant, void *kernel, size_t smem);
     bool UploadLmStrategy(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy);
 
     cudaStream_t stream_;
@@ -218,10 +246,10 @@ private:
     DeviceArray<unsigned long long> d_loop_rows_;   // k_gn_persistent: tagged partial rows of the gather CTAs (grow-only)
     DeviceArray<unsigned long long> d_loop_pose_;   // k_gn_persistent: tagged pose words, one block per group (grow-only)
     unsigned int loop_tag_ = 1;                     // next tag to hand out (never 0)
-    DeviceArray<int> d_groups_;                // batched LM launches: first_cta | kp_base | keypoint counts (grow-only)
-    std::vector<int> h_groups_;
     DeviceArray<unsigned char> d_gn_table_;    // grouped GN launches: GnGroup table | first_cta | counts (grow-only)
     std::vector<unsigned char> h_gn_table_;
+    DeviceArray<unsigned char> d_lm_table_;    // grouped LM launches: LmGroup table | first_cta | counts (grow-only)
+    std::vector<unsigned char> h_lm_table_;
     // solver CERES (icp_lm.cu)
     DeviceArray<LmState> d_lm_state_;
     DeviceArray<unsigned long long> d_lm_stats_;

@@ -1,8 +1,6 @@
 // icp_batch.cu — CTA policy of the persistent registration kernels (EnqueueGaussNewtonGroups, icp_gn.cu;
-// EnqueueCeresBatch, icp_lm.cu) and the group table of the batched LM launch. Host code only.
+// EnqueueCeresGroups, icp_lm.cu). Host code only.
 #include <algorithm>
-#include <cstdint>
-#include <string>
 #include <vector>
 
 #include "icp.h"
@@ -52,25 +50,6 @@ void BatchGatherCtas(const size_t *n, int batch, int coresident, int kp_per_cta,
         if (best < 0) break;
         gather[best] += 1;
     }
-}
-
-int IcpSolver::UploadGroupTable(const size_t *h_n, int batch, int coresident) {
-    // table: first_cta[0..B] | kp_base[0..B-1] | count[0..B-1]
-    h_groups_.assign(3 * (size_t) batch + 1, 0);
-    int *first_cta = h_groups_.data(), *kp_base = first_cta + batch + 1, *count = kp_base + batch;
-    std::vector<int> gather(batch);
-    BatchGatherCtas(h_n, batch, coresident, kp_per_cta_, gather.data());
-    long long base = 0;
-    for (int b = 0; b < batch; ++b) {
-        first_cta[b + 1] = first_cta[b] + 1 + gather[b];
-        kp_base[b] = (int) base;
-        count[b] = (int) h_n[b];
-        base += (long long) h_n[b];
-    }
-    if (base > (long long) INT32_MAX) throw std::invalid_argument("too many keypoints in one batch");
-    d_groups_.reserve(h_groups_.size(), stream_);
-    CT_CUDA_CHECK(cudaMemcpyAsync(d_groups_.data(), h_groups_.data(), sizeof(int) * h_groups_.size(), cudaMemcpyHostToDevice, stream_));
-    return first_cta[batch];
 }
 
 }  // namespace cticp

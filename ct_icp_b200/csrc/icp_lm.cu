@@ -136,7 +136,8 @@ __device__ __forceinline__ int lm_grab_tile(int *next, int W, int lane) {
 }
 
 // One warp's share of the residual assembly of solver CERES (ct_icp.cpp:561-604).
-template <bool kDB>
+// kCopy: the grouped k_lm_persistent's own copy (its G0 / P are in shared memory): the solo kernels' code stays as it is
+template <bool kDB, bool kCopy = false>
 __device__ __noinline__ void lm_gather_tiles(const GatherConfig &G0, const LmParams &P, const int *stencil,
                                                 const float4 *__restrict__ keypoints, int K, const IcpState *st,
                                                 ResidualBlock *__restrict__ blocks, unsigned long long *stats,
@@ -293,6 +294,7 @@ k_lm_gather(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoints, c
 // slam::NEIGHBORHOOD_TYPE per keypoint ACROSS the ICP iterations: the reference keeps its `neighborhoods` vector alive
 // (:1214) and ClassifyNeighborhood (neighborhood.h:268-282) leaves the previous class in place when neither threshold
 // is passed.
+template <bool kCopy = false>   // (as lm_gather_tiles)
 __device__ __noinline__ void rb_gather_tiles(const GatherConfig &G, const LmParams &P, const int *stencil,
                                                 const float4 *__restrict__ keypoints, int K, const IcpState *st,
                                                 ResidualBlock *__restrict__ blocks, unsigned char *__restrict__ classes,
@@ -536,7 +538,7 @@ k_lm_select(LmParams P, int mode, const int *__restrict__ d_num_keypoints, const
 // `half_index` / `halves_total`: this half-warp's index among all evaluating half-warps of the launch. s_u / s_acc: this
 // CTA's scratch, one row per half-warp (hw = local half-warp index). Writes the CTA's sum to `row_out` (kAcc doubles).
 // Called by ALL threads of the CTA.
-template <int kHalves>
+template <int kHalves, bool kCopy = false>   // (kCopy as lm_gather_tiles)
 __device__ __noinline__ void lm_eval_device(const LmParams &P, int which, const ResidualBlock *__restrict__ blocks,
                                                const int *__restrict__ sel_idx, const IcpState *st, const LmState *lm,
                                                double (*s_u)[16], double (*s_acc)[kAcc], int half_index, int halves_total,
@@ -1088,16 +1090,34 @@ __device__ __forceinline__ void lm_publish(LmState *dst, const LmState *src, int
     }
 }
 
-// Groups of a batched launch (EnqueueCeresBatch): group g owns the CTAs [first_cta[g], first_cta[g + 1]) of the grid — the
-// first is g's solver CTA, the others its workers — its keypoints [kp_base[g], kp_base[g] + count[g]) of the launch's
-// keypoint (and residual plane) array, the residual blocks / sel_idx / classes from kp_base[g] · ncn on, the states st[g]
-// and the LmState at kLmStateStride · g, its stats pair, the partial rows [first_cta[g] - g, first_cta[g + 1] - g - 1) and
-// its barrier words. `table` (device) = first_cta[0..B] | kp_base[0..B-1] | count[0..B-1] (the GN batch's table).
+// One registration of a grouped k_lm_persistent launch (LmGroups): everything a solo launch takes as kernel parameters.
+// Groups may search different maps with different options and buffers (the odometry's batch: one handle per group).
+struct LmGroup {
+    GatherConfig G;              // map level and search of the default radius
+    LmParams P;                  // options; P.kp_lo: the group's residual plane
+    const float4 *keypoints;
+    const int *num_keypoints;    // device count
+    IcpState *st;
+    ResidualBlock *blocks;       // the group's residual blocks, sel_idx and (ROBUST) classes
+    int *sel_idx;
+    unsigned char *classes;
+    const DistanceStrategy *D;   // mode 1
+};
+
+// The groups of one grouped k_lm_persistent launch (k_lm_persistent<mode, false, true>). Group g owns the CTAs
+// [first_cta[g], first_cta[g + 1]) of the grid — the first is g's solver CTA, the others its workers — the registration
+// table[g], and in the launch-wide area the LmState at kLmStateStride · g, its stats line, the partial rows
+// [first_cta[g] - g, first_cta[g + 1] - g - 1) and its barrier words. `table` (device) = LmGroup[B] | first_cta[0..B]
+// (IcpSolver::EnqueueCeresGroups).
 struct LmGroups {
-    const int *table;
+    const LmGroup *table;
     int num_groups;
     unsigned int *barrier;   // kLmBarrierWords per group: arrival counter at [0], abort word at [32]; zeroed before each launch
 };
+// dynamic shared memory of the grouped instantiations: the solo kernel's, then the CTA's entry of the table
+constexpr size_t kLmGroupedShared = sizeof(LmPShared) + sizeof(LmGroup);
+static_assert(kLmGroupedShared <= 227 * 1024, "k_lm_persistent<mode, false, true>: dynamic shared memory of one CTA");
+static_assert(sizeof(LmGroup) % sizeof(int) == 0, "the CTAs copy their entry word by word");
 constexpr int kLmBarrierWords = 64;                                        // two 128-byte lines per group
 constexpr size_t kLmStateStride = (sizeof(LmState) + 127) / 128 * 128;     // LmStates of the groups on separate lines
 constexpr int kLmStatsStride = 16;                                         // one 128-byte line of stats per group
@@ -1187,11 +1207,11 @@ __device__ __forceinline__ void lm_persistent_body(const GatherConfig &G0, const
             if (tid == 0) sh.next = 0;
             __syncthreads();
             if (kMode == 2)
-                rb_gather_tiles(G0, P, stencil, keypoints, K, st, blocks, classes, stats, sh.tile[w], wi, workers, kLmPWarps, &sh.next, lane);
+                rb_gather_tiles<kGrouped>(G0, P, stencil, keypoints, K, st, blocks, classes, stats, sh.tile[w], wi, workers, kLmPWarps, &sh.next, lane);
             else if (kMode == 1)
-                lm_gather_tiles<true>(G0, P, stencil, keypoints, K, st, blocks, stats, D, sh.tile[w], wi, workers, kLmPWarps, &sh.next, lane);
+                lm_gather_tiles<true, kGrouped>(G0, P, stencil, keypoints, K, st, blocks, stats, D, sh.tile[w], wi, workers, kLmPWarps, &sh.next, lane);
             else
-                lm_gather_tiles<false>(G0, P, stencil, keypoints, K, st, blocks, stats, D, sh.tile[w], wi, workers, kLmPWarps, &sh.next, lane);
+                lm_gather_tiles<false, kGrouped>(G0, P, stencil, keypoints, K, st, blocks, stats, D, sh.tile[w], wi, workers, kLmPWarps, &sh.next, lane);
         }
         if (!sync()) {
             live = false;
@@ -1229,7 +1249,7 @@ __device__ __forceinline__ void lm_persistent_body(const GatherConfig &G0, const
             const int phase = ev > 0 ? 1 : 0;
             if (!solver) {
                 const int hw = w * 2 + (lane >> 4);
-                lm_eval_device<kLmPWarps * 2>(P, phase, blocks, sel_idx, st, lm_g, sh.eval.u, sh.eval.acc,
+                lm_eval_device<kLmPWarps * 2, kGrouped>(P, phase, blocks, sel_idx, st, lm_g, sh.eval.u, sh.eval.acc,
                                               hw * workers + wi, workers * kLmPWarps * 2, partials + (size_t) wi * kAcc);
             }
             if (!sync()) {
@@ -1323,8 +1343,9 @@ __device__ __forceinline__ void lm_persistent_body(const GatherConfig &G0, const
     }
 }
 
-// kGrouped: one launch runs the groups of `groups` (EnqueueCeresBatch); otherwise the grid is one registration and
-// `groups` is not read.
+// kGrouped: one launch runs the groups of `groups` (EnqueueCeresGroups), each CTA with its group's entry copied to shared
+// memory behind LmPShared (kLmGroupedShared), and the parameters G0 … D are not read (lm_g, stats and partials are the
+// launch-wide areas); otherwise the grid is one registration and `groups` is not read.
 template <int kMode, bool kPeers, bool kGrouped = false>
 __global__ void __launch_bounds__(kLmPWarps * 32, 1)
 k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoints, const int *__restrict__ d_num_keypoints,
@@ -1333,20 +1354,21 @@ k_lm_persistent(GatherConfig G0, LmParams P, const float4 *__restrict__ keypoint
                 double *__restrict__ partials, PeerLinks links, LmGroups groups) {
     if constexpr (kGrouped) {
         static_assert(!kPeers, "a batched launch is not sharded");
-        const int *first_cta = groups.table;
-        const int B = groups.num_groups;
+        const int *first_cta = reinterpret_cast<const int *>(groups.table + groups.num_groups);
         int g = 0;
         while (first_cta[g + 1] <= (int) blockIdx.x) ++g;
-        const int kp_base = first_cta[B + 1 + g];
-        const size_t block_base = (size_t) P.ncn * kp_base;
-        LmParams Pg = P;
-        if (Pg.kp_lo) Pg.kp_lo += kp_base;
+        LmGroup &e = *reinterpret_cast<LmGroup *>(lm_smem_raw + sizeof(LmPShared));
+        {
+            const int *src = reinterpret_cast<const int *>(groups.table + g);
+            int *dst = reinterpret_cast<int *>(&e);
+            for (int i = threadIdx.x; i < (int) (sizeof(LmGroup) / sizeof(int)); i += blockDim.x) dst[i] = src[i];
+        }
+        __syncthreads();
         lm_persistent_body<kMode, false, true>(
-            G0, Pg, keypoints + kp_base, first_cta + 2 * B + 1 + g, st + g,
-            reinterpret_cast<LmState *>(reinterpret_cast<char *>(lm_g) + kLmStateStride * g), blocks + block_base,
-            sel_idx + block_base, classes + block_base, stats + (size_t) kLmStatsStride * g, D,
-            partials + (size_t) (first_cta[g] - g) * kAcc, links, (int) blockIdx.x - first_cta[g],
-            first_cta[g + 1] - first_cta[g], groups.barrier + (size_t) kLmBarrierWords * g);
+            e.G, e.P, e.keypoints, e.num_keypoints, e.st,
+            reinterpret_cast<LmState *>(reinterpret_cast<char *>(lm_g) + kLmStateStride * g), e.blocks, e.sel_idx, e.classes,
+            stats + (size_t) kLmStatsStride * g, e.D, partials + (size_t) (first_cta[g] - g) * kAcc, links,
+            (int) blockIdx.x - first_cta[g], first_cta[g + 1] - first_cta[g], groups.barrier + (size_t) kLmBarrierWords * g);
     } else {
         lm_persistent_body<kMode, kPeers, false>(G0, P, keypoints, d_num_keypoints, st, lm_g, blocks, sel_idx, classes, stats,
                                                  D, partials, links, (int) blockIdx.x, (int) gridDim.x, nullptr);
@@ -1386,12 +1408,12 @@ static void *LmPersistentKernel(int mode, bool peers, bool grouped) {
         default: return (void *) k_lm_persistent<2, true>;
     }
 }
-int IcpSolver::LmCoresident(int variant, void *kernel) {
+int IcpSolver::LmCoresident(int variant, void *kernel, size_t smem) {
     int &coresident = lm_coresident_[variant];
     if (coresident == 0) {
-        CT_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) sizeof(LmPShared)));
+        CT_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
         int per_sm = 0;
-        CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kLmPWarps * 32, sizeof(LmPShared)));
+        CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kLmPWarps * 32, smem));
         coresident = std::max(1, per_sm * num_sms_);
     }
     return coresident;
@@ -1520,7 +1542,7 @@ void IcpSolver::EnqueueCeres(const DeviceMap &map, const cticp_icp_options &opt,
         const int mode = robust ? 2 : (distance_based ? 1 : 0);
         const bool peers = sharded;
         void *kernel = LmPersistentKernel(mode, peers, false);
-        const int coresident = LmCoresident(mode * 2 + (peers ? 1 : 0), kernel);
+        const int coresident = LmCoresident(mode * 2 + (peers ? 1 : 0), kernel, sizeof(LmPShared));
         const size_t k_share = (k_hint + (size_t) P.shard_world - 1) / (size_t) P.shard_world + 16;
         int grid = (int) std::min<size_t>((size_t) coresident, 1 + std::max<size_t>(1, (k_share + kp_per_cta_ - 1) / kp_per_cta_));
         grid = std::max(grid, 2);
@@ -1599,19 +1621,86 @@ void IcpSolver::EnqueueCeresBatch(const DeviceMap &map, const cticp_icp_options 
     if (batch < 1) throw std::invalid_argument("batch must be at least 1");
     CheckCeresOptions(map, opt, strategy);
     const bool robust = opt.solver == CTICP_SOLVER_ROBUST;
-    const int mode = robust ? 2 : (strategy.type == CTICP_STRATEGY_DISTANCE_BASED ? 1 : 0);
-    // one problem: the solo launch (grid barriers, the table is not read), with its count taken from the table
+    const size_t ncn = robust ? 1 : (size_t) opt.num_closest_neighbors;
+    size_t total = 0;
+    for (int b = 0; b < batch; ++b) total += h_n[b];
+    if (total > (size_t) INT32_MAX) throw std::invalid_argument("too many keypoints in one batch");
+    // one set of buffers for the batch: problem b's blocks, sel_idx and classes from ncn · (its first keypoint) on
+    EnsureLmBuffers(std::max<size_t>(total, 1) * ncn);
+    const DistanceStrategy *distance = UploadLmStrategy(map, opt, strategy) ? d_lm_strategy_.data() : nullptr;
+    if (robust) CT_CUDA_CHECK(cudaMemsetAsync(d_lm_classes_.data(), 0, total, stream_));   // NEIGHBORHOOD_TYPE::NONE
+    std::vector<LmProblem> problems(batch);
+    size_t base = 0;
+    for (int b = 0; b < batch; ++b) {
+        problems[b] = LmProblem{&map, &opt, &strategy, d_keypoints + base, kp_lo_ ? kp_lo_ + base : nullptr, nullptr, h_n[b],
+                                d_states + b, d_lm_blocks_.data() + ncn * base, d_lm_sel_.data() + ncn * base,
+                                d_lm_classes_.data() + ncn * base, distance};
+        base += h_n[b];
+    }
+    EnqueueCeresGroups(problems.data(), batch);
+}
+
+LmProblem IcpSolver::PrepareCeres(const DeviceMap &map, const cticp_icp_options &opt, const cticp_strategy_options &strategy,
+                                  const float4 *d_keypoints, const int *d_num_keypoints, size_t k_hint, size_t k_capacity,
+                                  IcpState *d_state) {
+    CheckCeresOptions(map, opt, strategy);
+    const bool robust = opt.solver == CTICP_SOLVER_ROBUST;
+    const int ncn = robust ? 1 : opt.num_closest_neighbors;
+    EnsureLmBuffers(k_capacity * (size_t) ncn);
+    const bool distance_based = UploadLmStrategy(map, opt, strategy);
+    if (robust) CT_CUDA_CHECK(cudaMemsetAsync(d_lm_classes_.data(), 0, k_capacity, stream_));   // NEIGHBORHOOD_TYPE::NONE
+    return LmProblem{&map, &opt, &strategy, d_keypoints, kp_lo_, d_num_keypoints, k_hint, d_state, d_lm_blocks_.data(),
+                     d_lm_sel_.data(), d_lm_classes_.data(), distance_based ? d_lm_strategy_.data() : nullptr};
+}
+
+void IcpSolver::EnqueueCeresGroups(const LmProblem *problems, int batch) {
+    if (!use_persistent_) throw std::logic_error("batched CERES / ROBUST registration needs the persistent loop");
+    if (batch < 1) throw std::invalid_argument("batch must be at least 1");
+    // k_lm_persistent's mode (0 = CERES nearest neighbour, 1 = CERES distance-based, 2 = ROBUST): one per launch
+    const auto mode_of = [](const LmProblem &p) {
+        return p.opt->solver == CTICP_SOLVER_ROBUST ? 2 : (p.strategy->type == CTICP_STRATEGY_DISTANCE_BASED ? 1 : 0);
+    };
+    const int mode = mode_of(problems[0]);
+    for (int b = 1; b < batch; ++b)
+        if (mode_of(problems[b]) != mode) throw std::invalid_argument("a grouped LM launch runs problems of one mode");
+    // one problem: the solo launch (grid barriers, the table is not read but for its count)
     const bool grouped = batch > 1;
     void *kernel = LmPersistentKernel(mode, false, grouped);
-    const int coresident = LmCoresident(grouped ? 6 + mode : mode * 2, kernel);
+    const size_t smem = grouped ? kLmGroupedShared : sizeof(LmPShared);
+    const int coresident = LmCoresident(grouped ? 6 + mode : mode * 2, kernel, smem);
     if (2 * batch > coresident)
         throw CapacityError("batch of " + std::to_string(batch) + " registrations: the device holds " +
                             std::to_string(coresident) + " CTAs of the LM kernel, two per registration needed");
-    size_t total = 0;
-    for (int b = 0; b < batch; ++b) total += h_n[b];
-    LmParams P = MakeLmParams(map, opt, strategy, kp_lo_, 0, 1);
-    GatherConfig G = LmGatherConfig(map, P);
-    EnsureLmBuffers(std::max<size_t>(total, 1) * (size_t) P.ncn);
+    // table: LmGroup[B] | first_cta[0..B] | the counts of the problems without a device count
+    std::vector<size_t> n(batch);
+    for (int b = 0; b < batch; ++b) n[b] = problems[b].n;
+    std::vector<int> gather(batch);
+    BatchGatherCtas(n.data(), batch, coresident, kp_per_cta_, gather.data());
+    const size_t cta_off = sizeof(LmGroup) * (size_t) batch, count_off = cta_off + sizeof(int) * (size_t) (batch + 1);
+    const size_t bytes = count_off + sizeof(int) * (size_t) batch;
+    d_lm_table_.reserve(bytes, stream_);
+    h_lm_table_.assign(bytes, 0);
+    LmGroup *table = reinterpret_cast<LmGroup *>(h_lm_table_.data());
+    int *first_cta = reinterpret_cast<int *>(h_lm_table_.data() + cta_off);
+    int *count = reinterpret_cast<int *>(h_lm_table_.data() + count_off);
+    const int *d_count = reinterpret_cast<const int *>(d_lm_table_.data() + count_off);
+    for (int b = 0; b < batch; ++b) {
+        const LmProblem &p = problems[b];
+        if (p.n > (size_t) INT32_MAX) throw std::invalid_argument("too many keypoints in one problem");
+        LmGroup &e = table[b];
+        e.P = MakeLmParams(*p.map, *p.opt, *p.strategy, p.keypoints_lo, 0, 1);
+        e.G = LmGatherConfig(*p.map, e.P);
+        e.keypoints = p.keypoints;
+        count[b] = (int) p.n;
+        e.num_keypoints = p.d_num_keypoints ? p.d_num_keypoints : d_count + b;
+        e.st = p.d_state;
+        e.blocks = p.blocks;
+        e.sel_idx = p.sel_idx;
+        e.classes = p.classes;
+        e.D = p.distance;
+        first_cta[b + 1] = first_cta[b] + 1 + gather[b];
+    }
+    const int grid = first_cta[batch];
     // per group: its LmState (kLmStateStride), its stats line and its barrier words, each area after the B of the one before
     constexpr size_t kGroupBytes = kLmStateStride + sizeof(unsigned long long) * kLmStatsStride + sizeof(unsigned int) * kLmBarrierWords;
     d_lm_groups_.reserve(kGroupBytes * (size_t) batch, stream_);
@@ -1619,25 +1708,27 @@ void IcpSolver::EnqueueCeresBatch(const DeviceMap &map, const cticp_icp_options 
     auto *lm = reinterpret_cast<LmState *>(area);
     auto *stats = reinterpret_cast<unsigned long long *>(area + kLmStateStride * batch);
     auto *barrier = reinterpret_cast<unsigned int *>(area + (kLmStateStride + sizeof(unsigned long long) * kLmStatsStride) * batch);
-    UploadLmStrategy(map, opt, strategy);
-    auto *classes = d_lm_classes_.data();
-    if (robust) CT_CUDA_CHECK(cudaMemsetAsync(classes, 0, total, stream_));   // NEIGHBORHOOD_TYPE::NONE
-    const int grid = UploadGroupTable(h_n, batch, coresident);
     EnsurePartials(grid - batch);
+    CT_CUDA_CHECK(cudaMemcpyAsync(d_lm_table_.data(), h_lm_table_.data(), bytes, cudaMemcpyHostToDevice, stream_));
     CT_CUDA_CHECK(cudaMemsetAsync(barrier, 0, sizeof(unsigned int) * kLmBarrierWords * batch, stream_));
 
-    const float4 *kp = d_keypoints;
-    const int *nk = d_groups_.data() + 2 * batch + 1;   // count[0] (read by the solo launch only)
-    auto *blocks_buf = d_lm_blocks_.data();
-    int *sel = d_lm_sel_.data();
-    const DistanceStrategy *dstrat = d_lm_strategy_.data();
+    // the solo launch takes problem 0's entry as its parameters; the grouped one reads the table only
+    GatherConfig G = grouped ? GatherConfig{} : table[0].G;
+    LmParams P = grouped ? LmParams{} : table[0].P;
+    const float4 *kp = grouped ? nullptr : table[0].keypoints;
+    const int *nk = grouped ? nullptr : table[0].num_keypoints;
+    IcpState *st = grouped ? nullptr : table[0].st;
+    ResidualBlock *blocks_buf = grouped ? nullptr : table[0].blocks;
+    int *sel = grouped ? nullptr : table[0].sel_idx;
+    unsigned char *classes = grouped ? nullptr : table[0].classes;
+    const DistanceStrategy *dstrat = grouped ? nullptr : table[0].D;
     double *parts = d_partials_.data();
     PeerLinks links{};
-    LmGroups groups = grouped ? LmGroups{d_groups_.data(), batch, barrier} : LmGroups{};
-    void *args[] = {&G, &P, &kp, &nk, &d_states, &lm, &blocks_buf, &sel, &classes, &stats, &dstrat, &parts, &links, &groups};
+    LmGroups groups = grouped ? LmGroups{reinterpret_cast<const LmGroup *>(d_lm_table_.data()), batch, barrier} : LmGroups{};
+    void *args[] = {&G, &P, &kp, &nk, &st, &lm, &blocks_buf, &sel, &classes, &stats, &dstrat, &parts, &links, &groups};
     const bool timed = time_gather_ && ev_used_ < kMaxEvents;
     if (timed) cudaEventRecord(ev_begin_[ev_used_].get(), stream_);
-    CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kLmPWarps * 32), args, sizeof(LmPShared), stream_));
+    CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kLmPWarps * 32), args, smem, stream_));
     if (timed) cudaEventRecord(ev_end_[ev_used_++].get(), stream_);
     gather_launches_ += 1;
     launches_ += 1;

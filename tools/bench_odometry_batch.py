@@ -3,14 +3,16 @@ handle after the other) against one cticp_odometry_register_batch call per step 
 B in {1, 2, 4, 8, 16}.
 
 Workloads: the bench workload (BASELINE.json configs[1]: bench.py's GN options and KITTI-shape 64-beam scans, one seed
-per sequence) and a small-scan one (the same options on 16-beam ~10k-pt scans). Every sequence first registers
+per sequence) and a small-scan one (the same options on 16-beam ~10k-pt scans); bench.py's kitti64_ceres workload
+(BASELINE.json configs[2]: driving_config.yaml, solver CERES) on the same two scan kinds, and its options with solver
+ROBUST (robust_registration off) on the small scans. Every sequence first registers
 --preroll frames untimed (past init_num_frames), then --warmup frames, then --steps timed steps. A step is host-timed
 and ends in a device synchronise. The two modes have their own handles over the same scans and take turns step by step.
 
 Checks: each batched trajectory equals its sequential twin byte for byte when the batch's problems fit on the device
 with their solo grids; otherwise a second batched run over the first frames must reproduce the first run byte for byte.
-A separate run under torch.profiler gives the device time of the ICP launches per step (k_gn_persistent: B solo
-launches against one grouped launch). The card name and power limit come from a read-only nvidia-smi query in the same
+A separate run under torch.profiler gives the device time of the ICP launches per step (k_gn_persistent and
+k_lm_persistent: B solo launches against one grouped launch). The card name and power limit come from a read-only nvidia-smi query in the same
 run.
 
 usage: python tools/bench_odometry_batch.py [--steps 20] [--warmup 3] [--preroll 20] [--sizes 1,2,4,8,16] [--out DIR]
@@ -32,7 +34,11 @@ import bench  # noqa: E402
 import ct_icp_b200  # noqa: E402
 from ct_icp_b200 import synthetic as syn  # noqa: E402
 
-WORKLOADS = {"kitti64_gn": "HDL64E", "small16_gn": "SMALL16"}
+# name: (sensor, bench.py workload whose options the handles take, solver override)
+WORKLOADS = {"kitti64_gn": ("HDL64E", "kitti64_gn", None), "small16_gn": ("SMALL16", "kitti64_gn", None),
+             "kitti64_ceres": ("HDL64E", "kitti64_ceres", None), "small16_ceres": ("SMALL16", "kitti64_ceres", None),
+             "small16_robust": ("SMALL16", "kitti64_ceres", "ROBUST")}
+KERNELS = ("k_gn_persistent", "k_lm_persistent")
 
 
 def card():
@@ -42,6 +48,17 @@ def card():
         return out[0] if out else "unknown"
     except (OSError, subprocess.SubprocessError):
         return "unknown"
+
+
+def make_options(eng, workload):
+    _, bench_workload, solver = WORKLOADS[workload]
+    bench._WORKLOAD = bench_workload
+    o = bench.make_options(eng)
+    if solver:
+        from ct_icp_b200 import _abi as abi
+        o.ct_icp_options.solver = abi.SOLVER[solver]
+        o.robust_registration = 0
+    return o
 
 
 def make_sequence(n_frames, sensor, seed):
@@ -57,10 +74,10 @@ def trajectory_bytes(od, n=None):
 class Arm:
     """B handles over B sequences, their scans staged on each handle"""
 
-    def __init__(self, eng, seqs):
+    def __init__(self, eng, seqs, workload):
         self.eng = eng
         self.seqs = seqs
-        self.ods = [eng.odometry(bench.make_options(eng)) for _ in seqs]
+        self.ods = [eng.odometry(make_options(eng, workload)) for _ in seqs]
         self.slots = [[od.stage_frame(s["xyz"], s["t"]) for s in seq] for od, seq in zip(self.ods, seqs)]
 
     def step(self, k, batched):
@@ -76,10 +93,11 @@ class Arm:
             od.close()
 
 
-def gn_device_ms(eng, seqs, first, steps, batched, torch):
-    """mean device time of the k_gn_persistent launches per step, from a torch.profiler run of its own"""
+def icp_device_ms(eng, seqs, workload, first, steps, batched, torch):
+    """per ICP kernel (KERNELS): mean device time of its launches per step and launches per step, from a torch.profiler
+    run of its own"""
     from torch.profiler import ProfilerActivity, profile
-    arm = Arm(eng, seqs)
+    arm = Arm(eng, seqs, workload)
     for k in range(first):
         arm.step(k, batched)
     torch.cuda.synchronize()
@@ -87,9 +105,12 @@ def gn_device_ms(eng, seqs, first, steps, batched, torch):
         for k in range(first, first + steps):
             arm.step(k, batched)
         torch.cuda.synchronize()
-    us = [e.device_time_total for e in prof.events() if "k_gn_persistent" in e.name]
+    out = {}
+    for kernel in KERNELS:
+        us = [e.device_time_total for e in prof.events() if kernel in e.name]
+        out[kernel] = (sum(us) / 1000.0 / steps, len(us) / steps)
     arm.close()
-    return sum(us) / 1000.0 / steps, len(us) / steps
+    return out
 
 
 def main():
@@ -111,10 +132,10 @@ def main():
     print("card (name, power limit):", result["card"], flush=True)
     for wl in args.workloads.split(","):
         with multiprocessing.get_context("fork").Pool(min(max(sizes), os.cpu_count() or 1)) as pool:
-            all_seqs = pool.starmap(make_sequence, [(n_frames, WORKLOADS[wl], 1234 + b) for b in range(max(sizes))])
+            all_seqs = pool.starmap(make_sequence, [(n_frames, WORKLOADS[wl][0], 1234 + b) for b in range(max(sizes))])
         for B in sizes:
             seqs = all_seqs[:B]
-            arms = {"sequential": Arm(eng, seqs), "batch": Arm(eng, seqs)}
+            arms = {"sequential": Arm(eng, seqs, wl), "batch": Arm(eng, seqs, wl)}
             step_s = {m: [] for m in arms}
             for k in range(n_frames):
                 for m in (("sequential", "batch") if k % 2 == 0 else ("batch", "sequential")):
@@ -128,7 +149,7 @@ def main():
                             for a, b in zip(arms["sequential"].ods, arms["batch"].ods))
             check = "bit-identical to sequential"
             if not identical:   # the problems share the device's CTAs: the batch must reproduce itself
-                again = Arm(eng, seqs)
+                again = Arm(eng, seqs, wl)
                 for k in range(args.preroll):
                     again.step(k, True)
                 assert all(trajectory_bytes(a, args.preroll) == trajectory_bytes(b)
@@ -138,16 +159,19 @@ def main():
             groups = arms["batch"].ods[0].last_timing().icp_batch_groups
             for a in arms.values():
                 a.close()
-            seq_ms, seq_n = gn_device_ms(eng, seqs, first, min(args.steps, 10), False, torch)
-            bat_ms, bat_n = gn_device_ms(eng, seqs, first, min(args.steps, 10), True, torch)
+            dev = {m: icp_device_ms(eng, seqs, wl, first, min(args.steps, 10), m == "batch", torch)
+                   for m in ("sequential", "batch")}
             row = {"workload": wl, "B": B,
                    "sequential_scans_per_s": B / float(np.median(step_s["sequential"])),
                    "batch_scans_per_s": B / float(np.median(step_s["batch"])),
                    "sequential_step_ms_median": 1e3 * float(np.median(step_s["sequential"])),
                    "batch_step_ms_median": 1e3 * float(np.median(step_s["batch"])),
-                   "gn_device_ms_per_step_sequential": seq_ms, "gn_launches_per_step_sequential": seq_n,
-                   "gn_device_ms_per_step_batch": bat_ms, "gn_launches_per_step_batch": bat_n,
                    "icp_batch_groups": groups, "check": check}
+            for m in dev:
+                for kernel, (ms, n) in dev[m].items():
+                    short = kernel.split("_")[1]   # gn / lm
+                    row[f"{short}_device_ms_per_step_{m}"] = ms
+                    row[f"{short}_launches_per_step_{m}"] = n
             row["speedup"] = row["batch_scans_per_s"] / row["sequential_scans_per_s"]
             result["rows"].append(row)
             print(json.dumps(row), flush=True)
