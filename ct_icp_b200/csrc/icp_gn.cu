@@ -63,9 +63,10 @@ struct GnGroup {
 // dynamically — a warp whose keypoint has a sparse stencil takes the next one while a neighbour is still busy with a
 // dense one — and the registration stays bit-reproducible. Per-warp clock64 stamps of the static tiles of
 // two that came before showed a long tail of slow tiles, and every iteration waited for the slowest while half of the
-// warps had no tile at all. The exception (gn_pair_schedule): in k_gn_persistent, from the second iteration on, a range of
-// more keypoints than warps but at most two per warp gets one tile per warp from the last iteration's costs — the
-// heaviest keypoints alone, the others in pairs — instead of a few warps running a second whole chain after their first.
+// warps had no tile at all. The exception (gn_pair_schedule): in k_gn_persistent, a range of more keypoints than warps but
+// at most two per warp gets one tile per warp from the last iteration's costs (the first iteration: in keypoint order) —
+// the heaviest keypoints alone, the others in pairs — instead of a few warps running a second whole chain after their
+// first.
 struct GnPose {
     Q4 qb, qe;
     V3 tb, te;
@@ -121,7 +122,8 @@ __device__ __forceinline__ bool gn_pairs_apply(int span) {
 // The static schedule of a range of kGatherWarps < n <= 2 kGatherWarps keypoints from the costs of the last iteration
 // (R.cost[0..n), written by every keypoint's phase C): one tile per warp, S = 2 kGatherWarps - n single tiles and
 // n - kGatherWarps pairs. The S heaviest keypoints (most stencil points; ties: lower index first) get a warp each and the
-// remaining ones are paired heaviest with lightest, which makes the largest pair cost as small as it can be. A pair runs
+// remaining ones are paired heaviest with lightest, which makes the largest pair cost as small as it can be (the first
+// iteration has no costs: all zero, the order is the keypoint order). A pair runs
 // phases A and C once for both keypoints (lanes 0 and 1) instead of a second whole chain on the warp that grabbed it.
 // The schedule is a function of the costs alone; the rows go to R.u by keypoint as before, so the result does not depend
 // on it. One warp; writes R.pair.
@@ -147,13 +149,11 @@ __device__ __noinline__ void gn_pair_schedule(CtaRows &R, int n, int lane) {
 
 // The tiles of the chunk [lo, hi) of this CTA's range (hi - lo <= kRowCap); R.next must be 0 and visible (barrier) on entry.
 // `pair` (nullptr: tiles of W keypoints grabbed from R.next): this warp's one tile of the paired schedule (R.pair).
-__device__ __forceinline__ void gn_gather_tiles(const GatherLaunch &cfg, const int *stencil,
+__device__ __forceinline__ void gn_gather_tiles(const GatherConfig &G, const GnParams &P, const int *stencil,
                                                 const float4 *__restrict__ keypoints, int lo, int hi, int W,
                                                 const unsigned char *pair, const GnPose &pose, TileScratch &T,
                                                 CtaRows &R, int lane, GnWarpAcc &A, void *bulk = nullptr,
                                                 bool rigid = false) {
-    const GatherConfig &G = cfg.G;
-    const GnParams &P = cfg.P;
     if (hi <= lo) return;
     const int need = P.kmin > 5 ? P.kmin : 5;   // ct_icp.cpp:769 ; neighborhood.h:227
     const double inv_res = 1.0 / G.L.res;
@@ -318,7 +318,7 @@ struct GnShared {
         unsigned long long *pose;   // the group's tagged pose words
         int gather_ctas;
     } grp;
-    GnGroup group;    // grouped k_gn_persistent: this CTA's entry of the group table
+    GnGroup group;    // k_gn_persistent: this CTA's entry of the group table (solo: the kernel parameters)
     unsigned long long mbar[kGatherWarps];   // -DCTICP_SEL_BULK: one mbarrier per warp for the bulk copies
 };
 
@@ -374,15 +374,15 @@ __device__ __forceinline__ void gn_reduce_rows(GnShared &sh, const double *__res
 // the CTA's partial row (kAcc doubles): thread t < kAcc returns entry t. On entry sh.pose is valid and sh.rows.next == 0,
 // both visible to the CTA (the thread that fetched the pose set them before a barrier). `paired`: sh.rows.pair holds the
 // schedule of this range (gn_pair_schedule; only for gn_pairs_apply ranges, which are one chunk). All threads call.
-__device__ __forceinline__ double gn_cta_gather(const GatherLaunch &cfg, const int *stencil, const float4 *__restrict__ keypoints,
-                                                int c_lo, int c_hi, GnShared &sh, int lane, int w, GnWarpAcc &A, void *bulk,
-                                                bool rigid, bool paired = false) {
+__device__ __forceinline__ double gn_cta_gather(const GatherConfig &G, const GnParams &P, const int *stencil,
+                                                const float4 *__restrict__ keypoints, int c_lo, int c_hi, GnShared &sh,
+                                                int lane, int w, GnWarpAcc &A, void *bulk, bool rigid, bool paired = false) {
     const int W = gn_tile_width(c_hi - c_lo);
     const unsigned char *pair = paired ? sh.rows.pair[w] : nullptr;
     double carry = 0;
     for (int base = c_lo;; base += kRowCap) {
         const int top = (c_hi - base) > kRowCap ? base + kRowCap : c_hi;
-        gn_gather_tiles(cfg, stencil, keypoints, base, top, W, pair, sh.pose, sh.tile[w], sh.rows, lane, A, bulk, rigid);
+        gn_gather_tiles(G, P, stencil, keypoints, base, top, W, pair, sh.pose, sh.tile[w], sh.rows, lane, A, bulk, rigid);
         gn_cta_reduce_rows(sh.rows, top > base ? top - base : 0, carry);
         if (top >= c_hi) break;
         if (threadIdx.x == 0) sh.rows.next = 0;
@@ -447,7 +447,7 @@ k_gn_iterate(GatherLaunch cfg, const float4 *__restrict__ keypoints, const int *
             c_lo = lo + (int) ((long long) (hi - lo) * blockIdx.x / gridDim.x);
             c_hi = lo + (int) ((long long) (hi - lo) * (blockIdx.x + 1) / gridDim.x);
         }
-        const double s = gn_cta_gather(cfg, stencil, keypoints, c_lo, c_hi, sh, lane, w, A, bulk_ptr,
+        const double s = gn_cta_gather(cfg.G, cfg.P, stencil, keypoints, c_lo, c_hi, sh, lane, w, A, bulk_ptr,
                                        active && P.rigid_first && __ldcg(&st->iter) == 0);
         if (threadIdx.x < kAcc) __stcg(partials + (size_t) blockIdx.x * kAcc + threadIdx.x, s);
     }
@@ -600,7 +600,7 @@ __device__ __forceinline__ void gn_fetch_pose(GnShared &sh, unsigned int tag, lo
 // its own map, options, keypoints, iteration count, solver CTA, state, partial rows and pose words; everything above holds
 // per group. A group that converges or fails leaves the loop alone while the others go on, and one group's serial tail
 // overlaps the others' gathers. Each CTA copies its group's entry to shared memory and reads it from there; the solo
-// instantiation reads the same values from its kernel parameters and never the table. kPeers and the frame tail are solo.
+// instantiation copies its kernel parameters to the same place and never reads the table. kPeers and the frame tail are solo.
 //
 // kPeers (multi-GPU, keypoints sharded): between its reduction and its solve the solver CTA exchanges the accumulator
 // with the other ranks' solver CTAs through NVLink peer memory (peer_exchange.cuh) — the all-reduce of SURVEY §8e
@@ -631,11 +631,20 @@ k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints
         for (int i = threadIdx.x; i < (int) (sizeof(GnGroup) / sizeof(int)); i += blockDim.x) dst[i] = src[i];
         __syncthreads();
         st = sh.group.st;
+    } else {
+        // the solo launch keeps its parameters in the same place: read from shared memory where used, they hold no
+        // registers across the gather (read from the kernel parameters, some stayed live and `-Xptxas -v` showed 232 / 320 B
+        // of spill stores / loads instead of 124 / 176 B)
+        if (threadIdx.x == 0) sh.group = GnGroup{solo_cfg, solo_keypoints, d_num_keypoints, st, solo_iters};
+        __syncthreads();
     }
-    const GatherLaunch &cfg = kGrouped ? sh.group.cfg : solo_cfg;
-    const float4 *__restrict__ keypoints = kGrouped ? sh.group.keypoints : solo_keypoints;
+    const GatherLaunch &cfg = sh.group.cfg;
+    const float4 *__restrict__ keypoints = sh.group.keypoints;
     const GnParams &P = cfg.P;
-    const int num_iters = kGrouped ? sh.group.num_iters : solo_iters;
+    // except the gather's map level and radius, which its inner loops read: from the kernel parameters in the solo launch
+    // (with every field from shared memory, dense128_gn's wide tiles took 4 % longer)
+    const GatherConfig &gather_G = kGrouped ? sh.group.cfg.G : solo_cfg.G;
+    const int num_iters = sh.group.num_iters;
     const bool solver_cta = cta == 0;
     unsigned int peer_seq = 0;   // sequence number of the last exchange (solver CTA only)
     if (kPeers && solver_cta) peer_seq = *links.seq;
@@ -647,6 +656,7 @@ k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints
         sh.grp.pose = pose_words;
         sh.grp.gather_ctas = gather_ctas;
     }
+    for (int i = threadIdx.x; i < kRowCap; i += blockDim.x) sh.rows.cost[i] = 0u;   // iteration 0's paired schedule
     __syncthreads();
 
     if (solver_cta) {   // working copy of the state in shared memory: the serial tail never waits for global memory
@@ -681,7 +691,7 @@ k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints
     long long t_loop = 0, t_solve = 0;
     if (solver_cta && threadIdx.x == 0) t_loop = clock64();
     // this rank's keypoint range and the tile width: constant over the iterations (integer divisions)
-    const int K = kGrouped ? *sh.group.num_keypoints : *d_num_keypoints;
+    const int K = *sh.group.num_keypoints;
     int kp_lo = 0, kp_hi = K;
     if (P.shard_world > 1) {
         kp_lo = (int) ((long long) K * P.shard_rank / P.shard_world);
@@ -700,11 +710,11 @@ k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints
         } else {
             GnWarpAcc A;
             CT_STAMP(const long long t_it = clock64();)
-            // from the second iteration on, a range of more keypoints than warps but at most two per warp takes the paired
-            // schedule, built from the last iteration's costs by warp 1 while warp 0 waits for the pose (the first iteration,
-            // and every one with CTICP_DEBUG_FLAGS & 8, a debug switch for bit-identity tests: tiles of one keypoint grabbed
-            // from the counter)
-            const bool paired = it > 0 && !(P.debug_flags & (2 | 8)) && gn_pairs_apply(c_hi - c_lo);
+            // a range of more keypoints than warps but at most two per warp takes the paired schedule, built from the last
+            // iteration's costs by warp 1 while warp 0 waits for the pose; the first iteration has no costs yet (all zero:
+            // the schedule in keypoint order). With CTICP_DEBUG_FLAGS & 8, a debug switch for bit-identity tests, every
+            // iteration takes tiles of one keypoint grabbed from the counter.
+            const bool paired = !(P.debug_flags & (2 | 8)) && gn_pairs_apply(c_hi - c_lo);
             if (w == 1 && paired) gn_pair_schedule(sh.rows, c_hi - c_lo, lane);
             if (w == 0) {   // phases A / C read the pose from shared memory: 34 registers less to keep live
                 if (it == 0) {   // the state the host uploaded
@@ -725,7 +735,7 @@ k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints
             CT_STAMP(const long long t_g0 = clock64();)
             // (CTICP_DEBUG_FLAGS & 2, timing only: an empty range — the hand-off and the reduction without the gather work)
             const bool skip = (P.debug_flags & 2) != 0;
-            const double s = gn_cta_gather(cfg, stencil, keypoints, skip ? 0 : c_lo, skip ? 0 : c_hi, sh, lane, w, A, bulk_ptr,
+            const double s = gn_cta_gather(gather_G, P, stencil, keypoints, skip ? 0 : c_lo, skip ? 0 : c_hi, sh, lane, w, A, bulk_ptr,
                                            P.rigid_first && it == 0, paired);
             if (threadIdx.x < kAcc) tagged_store_double(sh.grp.rows + 2 * threadIdx.x, tag, s);
             CT_STAMP(const long long t_g = clock64();)
