@@ -189,7 +189,8 @@ class Binding:
     def register_batch(self, odometries, scans, frame_ids, initial_estimates=None, motion_models=None):
         """One frame on each Odometry of `odometries` in one call (cticp_odometry_register_batch): the eligible
         Gauss-Newton loops run in one grouped launch, the eligible CERES / ROBUST loops in one grouped launch per LM mode
-        (CERES nearest neighbour, CERES distance-based, ROBUST); every result is that of the single-frame call.
+        (CERES nearest neighbour, CERES distance-based, ROBUST); the attempts of robust_registration frames run in rounds
+        of such launches, apart from the plain frames; every result is that of the single-frame call.
         scans[i]: (xyz, timestamps) NumPy arrays (RegisterFrame's host path), (xyz, timestamps) torch CUDA tensors (read
         after the work queued on torch's current stream, as RegisterFrame), or an int staged slot (RegisterStaged).
         initial_estimates / motion_models: None or one entry (abi.Frame / abi.MotionPrior or None) per item.

@@ -350,6 +350,10 @@ k_map_update_fused(FusedUpdateArgs a) {
             double *o = a.frame_origins_mut + 3 * (size_t) a.frame_ordinal;
             o[0] = a.tb.x; o[1] = a.tb.y; o[2] = a.tb.z;
         }
+    } else {
+        // the slerp constants with the device's arithmetic, as k_frame_policy derives them for the speculative launch:
+        // the host-side tail (UpdateMap) gives the same world points, bit for bit
+        a.sc = slerp_consts(a.qb, a.qe);
     }
     const int n = *a.d_n;
     // phase 1: world points of the frame; eviction on every level; reset the per-level touched counters

@@ -27,12 +27,13 @@ struct NvtxRange {
 
 using hclock = std::chrono::steady_clock;
 
-// ---- the tail of a plain registration, decided on the device (frame_policy.h) ------------------------------------------
-// One warp. AssessRegistration (odometry.cpp:604-684, the branch without robust_registration) and UpdateMap's insertion
-// policy (:903-925) on the registration state the ICP kernel left in HBM; the verdict goes to device memory (read by the
-// speculative k_map_update_fused enqueued right behind) and to mapped pinned host memory, sequence number last.
+// ---- the tail of a registration attempt, decided on the device (frame_policy.h) ----------------------------------------
+// One warp. AssessRegistration (odometry.cpp:604-684) and UpdateMap's insertion policy (:855-925) on the registration
+// state the ICP kernel left in HBM: the plain branch, or one attempt of the robust ladder when rob.enabled. The verdict
+// goes to device memory (read by the speculative k_map_update_fused enqueued right behind) and to mapped pinned host
+// memory, sequence number last.
 __global__ void __launch_bounds__(32) k_frame_policy(const IcpState *__restrict__ st, const int *__restrict__ counts,
-                                                     FramePolicyIn in, FrameVerdict *dv, FrameVerdict *hv) {
+                                                     FramePolicyIn in, RobustPolicyIn rob, FrameVerdict *dv, FrameVerdict *hv) {
     __shared__ FrameVerdict v;
     const int lane = threadIdx.x;
     {
@@ -42,7 +43,10 @@ __global__ void __launch_bounds__(32) k_frame_policy(const IcpState *__restrict_
     }
     if (lane < 4) v.counts[lane] = __ldcg(counts + lane);
     __syncwarp();
-    if (lane == 0) frame_policy_decide(v, in);
+    if (lane == 0) {
+        if (rob.enabled) frame_policy_decide_robust(v, in, rob);
+        else frame_policy_decide(v, in);
+    }
     __syncwarp();
     frame_verdict_publish(v, dv, hv, lane);
 }
@@ -181,6 +185,14 @@ void Engine::SetSummaryPoints(int mask) {
     CT_CUDA_CHECK(cudaSetDevice(device_));
     summary_points_mask_ = mask & 7;
     if (summary_points_mask_) AllocEgress();
+}
+
+// The keypoint voxel size of a registration at robustness level `level`: RobustRegistrationAttempt's constructor, then
+// IncreaseRobustnessLevel (odometry.cpp:996-1018, 1028-1041), whose size does not depend on how many levels were added
+double Engine::LadderSampleSize(int k, int level) const {
+    if (level <= 0) return k < options_.init_num_frames ? options_.init_sample_voxel_size : options_.sample_voxel_size;
+    const double min_voxel_size = std::min(options_.init_voxel_size, options_.voxel_size);
+    return std::max(options_.sample_voxel_size / 1.5, double(min_voxel_size));
 }
 void Engine::AllocEgress() {
     if (!ev_egress_chunk_[kEgressChunks - 1].get()) {   // created last: a set that failed part way is created again
@@ -323,9 +335,10 @@ void Engine::IngestImpl(const ScanView &scan, const FrameInfo &info, int64_t sta
     // motion compensation CONSTANT_VELOCITY moves the raw points of the sub-sampled frame into the end pose's frame before
     // anything samples from it (DistortFrame, odometry.cpp:161-168,364-369)
     const bool distort = k > 1 && options_.motion_compensation == CTICP_MC_CONSTANT_VELOCITY;
-    if (fused_sampling_ && !distort && k > 0 && !options_.robust_registration && options_.sampling == CTICP_SAMPLING_GRID &&
+    if (fused_sampling_ && !distort && k > 0 && options_.sampling == CTICP_SAMPLING_GRID &&
         (at_startup || options_.max_num_keypoints <= 0)) {
-        const double kp_size = at_startup ? options_.init_sample_voxel_size : options_.sample_voxel_size;
+        // (a robust frame's first attempt samples at the size of the level it starts at)
+        const double kp_size = LadderSampleSize(k, options_.robust_registration ? next_robust_level_ : 0);
         pipe_->SampleFused(sample_size, kp_size, options_.shuffle_seed, ShuffleCounter(k, 0), ShuffleCounter(k, 1),
                            override_alpha, alpha_value);
         keypoints_sampled_ = true;
@@ -754,14 +767,8 @@ void Engine::FlushL2(size_t bytes) {
     CT_CUDA_CHECK(cudaMemsetAsync(d_flush_.data(), 0x5A, bytes, stream_.get()));
 }
 
-// TryRegister, odometry.cpp:525-601, in three parts: the work up to the ICP launch, the launch, the work after it
-void Engine::TryRegister(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
-                         const MotionModel *mm, int attempt_idx) {
-    NvtxRange range("cticp.icp");
-    TryRegisterBegin(info, options, rs, sample_voxel_size, mm, attempt_idx);
-    LaunchIcp(options);
-    TryRegisterEnd(info, options, rs);
-}
+// TryRegister, odometry.cpp:525-601, in three parts: the work up to the ICP launch (TryRegisterBegin), the launch
+// (LaunchIcp or a grouped launch), the work after it (TryRegisterEnd)
 
 // sampling, the registration state to the device, ev_[1]
 void Engine::TryRegisterBegin(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
@@ -839,7 +846,7 @@ void Engine::LaunchIcp(const cticp_icp_options &options) {
             verdict_by_icp_kernel_ =
                 icp_->EnqueueGaussNewton(*map_, options, pipe_->d_keypoints(), pipe_->d_count_keypoints(), KeypointHint(),
                                          options.num_iters_icp, d_state_.data(), shard_rank_, shard_world_, nccl_comm_,
-                                         (tail_armed_ && tail_in_kernel_) ? &tail : nullptr);
+                                         (tail_armed_ && tail_in_kernel_ && !tail_robust_.enabled) ? &tail : nullptr);
             break;
         case CTICP_SOLVER_CERES:
         case CTICP_SOLVER_ROBUST:
@@ -876,24 +883,31 @@ void Engine::AdoptGroupedIcp(PendingFrame &f, cudaEvent_t launched, int groups) 
     f.icp_launched = true;
 }
 
+// device tail (frame_policy.h): verdict + speculative map update behind the ICP launch, when armed
+void Engine::EnqueueTail() {
+    if (!tail_armed_) return;
+    CT_CUDA_CHECK(cudaSetDevice(device_));
+    tail_armed_ = false;
+    if (!verdict_by_icp_kernel_) {   // (k_gn_persistent's solver CTA writes the verdict itself)
+        k_frame_policy<<<1, 32, 0, stream_.get()>>>(d_state_.data(), pipe_->d_counts(), tail_in_, tail_robust_, d_verdict_.data(),
+                                                    h_verdict_dev_);
+        CT_CUDA_CHECK(cudaGetLastError());
+        tail_launches_ += 1;
+    }
+    {
+        NvtxRange range_map("cticp.map_update");
+        map_->UpdateFused(pipe_->d_frame(), pipe_->d_frame_lo(), pipe_->d_count_frame(), pipe_->n(), pipe_->d_frame_world_mut(),
+                          Q4{0, 0, 0, 1}, V3{0, 0, 0}, Q4{0, 0, 0, 1}, V3{0, 0, 0}, true, V3{0, 0, 0}, options_.max_distance,
+                          true, V3{0, 0, 0}, d_verdict_.data());
+    }
+    tail_launched_ = true;
+}
+
 // the verdict or the state back to the host, the registration summary
 void Engine::TryRegisterEnd(const FrameInfo &info, const cticp_icp_options &options, Summary &rs) {
-    if (tail_armed_) {
-        // device tail (frame_policy.h): verdict + speculative map update behind the ICP kernel; the host waits for the
-        // verdict's sequence number in mapped pinned memory, not for the stream
-        tail_armed_ = false;
-        if (!verdict_by_icp_kernel_) {   // (k_gn_persistent's solver CTA writes the verdict itself)
-            k_frame_policy<<<1, 32, 0, stream_.get()>>>(d_state_.data(), pipe_->d_counts(), tail_in_, d_verdict_.data(), h_verdict_dev_);
-            CT_CUDA_CHECK(cudaGetLastError());
-            tail_launches_ += 1;
-        }
-        {
-            NvtxRange range_map("cticp.map_update");
-            map_->UpdateFused(pipe_->d_frame(), pipe_->d_frame_lo(), pipe_->d_count_frame(), pipe_->n(), pipe_->d_frame_world_mut(),
-                              Q4{0, 0, 0, 1}, V3{0, 0, 0}, Q4{0, 0, 0, 1}, V3{0, 0, 0}, true, V3{0, 0, 0}, options_.max_distance,
-                              true, V3{0, 0, 0}, d_verdict_.data());
-        }
-        tail_launched_ = true;
+    EnqueueTail();
+    if (tail_launched_) {
+        // the host waits for the verdict's sequence number in mapped pinned memory, not for the stream
         WaitVerdict(tail_in_.seq);
         memcpy(h_state_.data(), &h_verdict_.data()->state, sizeof(IcpState));
         pipe_->SetHostCounts(h_verdict_.data()->counts);
@@ -985,8 +999,10 @@ void Engine::WaitVerdict(unsigned seq) {
 void Engine::AdoptDeviceMapUpdate(Summary &s) {
     const FrameVerdict &v = *h_verdict_.data();
     const bool inserted = v.action == kFrameInsert;
-    tracker_.cum_orientation += s.relative_orientation;
-    tracker_.cum_distance += s.relative_distance;
+    if (!options_.robust_registration) {   // (the robust branch of UpdateMap leaves the cumulated motion alone)
+        tracker_.cum_orientation += s.relative_orientation;
+        tracker_.cum_distance += s.relative_distance;
+    }
     s.points_added = v.add_points_policy != 0;
     map_->CommitSpeculativeInsert(inserted);
     frame_world_valid_ = true;
@@ -1000,79 +1016,147 @@ void Engine::AdoptDeviceMapUpdate(Summary &s) {
     map_->QueueCounterReadback();
 }
 
-// AssessRegistration, odometry.cpp:604-684
+// AssessRegistration, odometry.cpp:604-684, the branch without robust_registration (robust frames: robust_attempt_decide)
 bool Engine::AssessRegistration(Summary &s) const {
     if (s.relative_distance > options_.distance_error_threshold) return false;
     if (s.relative_orientation > options_.orientation_error_threshold ||
         s.ego_orientation > options_.orientation_error_threshold)
         return false;
-    bool success = s.success;
-    if (options_.robust_registration) {
-        if (s.robust_level == 0 && (s.relative_orientation > options_.robust_threshold_relative_orientation ||
-                                    s.ego_orientation > options_.robust_threshold_ego_orientation)) {
-            if (s.robust_level < options_.robust_num_attempts_when_rotation) {
-                s.error_message = "Large rotations require at a robust_level of at least 1 (got:" +
-                                  std::to_string(s.robust_level) + ").";
-                return false;
-            }
-        }
-        if (s.relative_distance > options_.robust_relative_trans_threshold) {
-            s.error_message = "The relative distance is too important";
-            return false;
-        }
-    }
-    return success;
+    return s.success;
 }
 
-// RobustRegistration + RobustRegistrationAttempt, odometry.cpp:780-852, 996-1050
-void Engine::RobustRegistration(const FrameInfo &info, Summary &rs, const MotionModel *mm) {
-    const int k = info.registered_fid;
-    const HostFrame initial_estimate = rs.frame;
-    cticp_icp_options reg = options_.ct_icp_options;
-    int robust_level = 0;
-    double sample_voxel_size = k < options_.init_num_frames ? options_.init_sample_voxel_size : options_.sample_voxel_size;
-    Summary attempt = rs;
-    attempt.number_of_attempts = 0;
-    auto increase = [&]() {   // IncreaseRobustnessLevel, :996-1018
-        const double min_voxel_size = std::min(options_.init_voxel_size, options_.voxel_size);
-        attempt.frame = initial_estimate;
-        reg.ls_max_num_iters += 30;
-        if (reg.max_num_residuals > 0) reg.max_num_residuals = reg.max_num_residuals * 2;
-        reg.num_iters_icp = std::min(reg.num_iters_icp + 20, 50);
-        reg.threshold_orientation_norm = std::max(reg.threshold_orientation_norm / 10, 1.e-5);
-        reg.threshold_translation_norm = std::max(reg.threshold_orientation_norm / 10, 1.e-4);
-        sample_voxel_size = std::max(options_.sample_voxel_size / 1.5, double(min_voxel_size));
-        reg.ls_sigma *= 1.2;
-        reg.max_dist_to_plane_ct_icp *= 1.5;
-        robust_level++;
-    };
-    while (robust_level < next_robust_level_) increase();
-    bool good_enough = false;
-    int attempt_idx = 0;
-    do {
-        TryRegister(info, reg, attempt, sample_voxel_size, mm, attempt_idx++);
-        if (k > 0) {
-            const auto &prev = trajectory_[k - 1];
-            const V3 d = attempt.frame.begin_pose.pose.t - prev.end_pose.pose.t;
-            attempt.distance_correction = norm(d);
-            attempt.relative_orientation = angular_distance_deg(prev.end_pose.pose.q, attempt.frame.end_pose.pose.q);
-            attempt.ego_orientation = EgoAngularDistance(attempt.frame);
-        }
-        attempt.relative_distance = norm(attempt.frame.end_pose.pose.t - attempt.frame.begin_pose.pose.t);
-        good_enough = AssessRegistration(attempt);
-        attempt.number_of_attempts++;
-        if (!good_enough) {
-            if (attempt.number_of_attempts < options_.robust_num_attempts)
-                increase();
-            else
-                good_enough = true;
-        }
-    } while (!good_enough);
-    rs = attempt;
-    if (rs.number_of_attempts > options_.robust_num_attempts)
-        robust_num_consecutive_failures_++;
-    else
-        robust_num_consecutive_failures_ = 0;
+// ---- the robust ladder: RobustRegistration + RobustRegistrationAttempt, odometry.cpp:780-852, 996-1050 -----------------
+// In steps a caller drives: BeginLadder (the attempt state at the starting level, then BeginAttempt), the ICP launch
+// (LaunchIcp, or a grouped launch in RegisterBatch), EndAttempt (the decision; a rejected attempt raises the level and
+// begins the next one, which again stops before its launch). The single-frame entries run them back to back
+// (CompleteFrame). Every attempt takes the device tail under the plain path's conditions: k_frame_policy decides it, the
+// speculative map update behind it does nothing for a rejected attempt (kFrameRetry).
+//
+// Stream hazards between attempt r and attempt r + 1 of one frame, all on this engine:
+//  - d_state_: attempt r + 1's state goes up on aux_stream_ while attempt r's no-op k_map_update_fused may still run on
+//    stream_. That kernel reads the verdict, not d_state_; d_state_'s readers (the ICP launch, k_frame_policy) completed
+//    before k_frame_policy published the verdict the host waited for.
+//  - d_verdict_: attempt r + 1's k_frame_policy overwrites it on stream_, behind attempt r's map update that reads it.
+//    The host copy is consumed before attempt r + 1 begins, and its sequence number rises, so a stale copy never passes
+//    WaitVerdict.
+//  - keypoint buffers: attempt r + 1's SampleKeypoints runs on stream_ behind attempt r's ICP, solo on stream_ or grouped
+//    (AdoptGroupedIcp made stream_ wait for the group), and behind k_frame_policy, which follows the ICP.
+void Engine::BeginLadder(PendingFrame &f) {
+    const int k = f.info.registered_fid;
+    f.ladder = true;
+    f.ladder_accepted = false;
+    f.ladder_initial = f.summary.frame;
+    f.icp_options = options_.ct_icp_options;
+    f.robust_level = 0;
+    f.sample_voxel_size = LadderSampleSize(k, 0);
+    f.summary.number_of_attempts = 0;
+    f.attempt = 0;
+    while (f.robust_level < next_robust_level_) IncreaseRobustness(f);   // SetRobustLevel
+    ladder_tail_ = device_tail_ && fused_map_update_ && !callback_ && options_.motion_compensation == CTICP_MC_CONTINUOUS &&
+                   pipe_->n() > 0;
+    if (ladder_tail_) ArmTail(angular_distance_deg(trajectory_[k - 1].end_pose.pose.q, trajectory_[k].end_pose.pose.q));
+    BeginAttempt(f);
+}
+
+// IncreaseRobustnessLevel, odometry.cpp:996-1018
+void Engine::IncreaseRobustness(PendingFrame &f) {
+    cticp_icp_options &reg = f.icp_options;
+    f.summary.frame = f.ladder_initial;
+    reg.ls_max_num_iters += 30;
+    if (reg.max_num_residuals > 0) reg.max_num_residuals = reg.max_num_residuals * 2;
+    reg.num_iters_icp = std::min(reg.num_iters_icp + 20, 50);
+    reg.threshold_orientation_norm = std::max(reg.threshold_orientation_norm / 10, 1.e-5);
+    reg.threshold_translation_norm = std::max(reg.threshold_orientation_norm / 10, 1.e-4);
+    f.robust_level++;
+    f.sample_voxel_size = LadderSampleSize(f.info.registered_fid, f.robust_level);
+    reg.ls_sigma *= 1.2;
+    reg.max_dist_to_plane_ct_icp *= 1.5;
+}
+
+// What the decision of attempt f.attempt needs from the host (RobustPolicyIn), for k_frame_policy and the host tail alike
+RobustPolicyIn Engine::LadderInputs(const PendingFrame &f) const {
+    const int k = f.info.registered_fid;
+    const HostPose &prev = trajectory_[k - 1].end_pose;
+    RobustPolicyIn r{};
+    r.prev_qe[0] = prev.pose.q.x; r.prev_qe[1] = prev.pose.q.y; r.prev_qe[2] = prev.pose.q.z; r.prev_qe[3] = prev.pose.q.w;
+    r.prev_te[0] = prev.pose.t.x; r.prev_te[1] = prev.pose.t.y; r.prev_te[2] = prev.pose.t.z;
+    r.threshold_relative_orientation = options_.robust_threshold_relative_orientation;
+    r.threshold_ego_orientation = options_.robust_threshold_ego_orientation;
+    r.relative_trans_threshold = options_.robust_relative_trans_threshold;
+    r.num_attempts_when_rotation = options_.robust_num_attempts_when_rotation;
+    r.minimal_level = options_.robust_minimal_level;
+    r.number_of_attempts = f.attempt + 1;
+    r.last_attempt = r.number_of_attempts >= options_.robust_num_attempts;
+    // :848-851, evaluated for the case that this attempt ends the ladder
+    r.consecutive_failures = r.number_of_attempts > options_.robust_num_attempts ? robust_num_consecutive_failures_ + 1 : 0;
+    r.enabled = 1;
+    return r;
+}
+
+// Step 1: the attempt's sampling and state upload (TryRegisterBegin), with the device tail armed when the frame takes it.
+// Stops before the ICP launch: f.icp_pending, f.joins.
+void Engine::BeginAttempt(PendingFrame &f) {
+    CT_CUDA_CHECK(cudaSetDevice(device_));
+    tail_robust_ = LadderInputs(f);
+    tail_armed_ = ladder_tail_;   // (tail_in_ was filled once for the frame by BeginLadder)
+    {
+        NvtxRange range("cticp.icp");
+        TryRegisterBegin(f.info, f.icp_options, f.summary, f.sample_voxel_size, ModelOf(f), f.attempt);
+    }
+    f.icp_pending = true;
+    f.icp_launched = false;
+    const int kind = JoinKind(f.icp_options);
+    f.joins = kind == kJoinsNone ? kJoinsNone : kind + kJoinsLadderGn;
+}
+
+// Step 3, after the attempt's ICP launch: the verdict (device tail) or the read-back, the decision; an accepted attempt
+// leaves f ready for FinishFrame, a rejected one raises the level and begins the next attempt (step 1).
+void Engine::EndAttempt(PendingFrame &f) {
+    CT_CUDA_CHECK(cudaSetDevice(device_));
+    Summary &a = f.summary;
+    const RobustPolicyIn r = tail_robust_;
+    TryRegisterEnd(f.info, f.icp_options, a);
+    FramePolicyIn in = tail_in_;
+    if (!tail_launched_) {   // host tail: the same decision, the map update is UpdateMap's
+        in.distance_error_threshold = options_.distance_error_threshold;
+        in.orientation_error_threshold = options_.orientation_error_threshold;
+        in.do_no_insert = options_.do_no_insert ? 1 : 0;
+        in.always_insert = options_.always_insert ? 1 : 0;
+        in.room_for = pipe_->h_counts()[1];
+    }
+    const Q4 qb = a.frame.begin_pose.pose.q, qe = a.frame.end_pose.pose.q;
+    const V3 tb = a.frame.begin_pose.pose.t, te = a.frame.end_pose.pose.t;
+    RobustDecision d = robust_attempt_decide(qb, tb, qe, te, h_state_.data()->failed, pipe_->h_counts()[1], in, r);
+    if (tail_launched_) {   // the device acted on ITS evaluation of the same formulas
+        const FrameVerdict &v = *h_verdict_.data();
+        d.accepted = v.action != kFrameRetry;
+        d.add_points_policy = v.add_points_policy;
+        d.next_robust_level = v.next_robust_level;
+        d.action = v.action;
+    }
+    a.distance_correction = d.distance_correction;
+    a.relative_orientation = d.relative_orientation;
+    a.ego_orientation = d.ego_orientation;
+    a.relative_distance = d.relative_distance;
+    if (d.reject_reason == kRejectRotation)
+        a.error_message = "Large rotations require at a robust_level of at least 1 (got:" + std::to_string(a.robust_level) + ").";
+    else if (d.reject_reason == kRejectTranslation)
+        a.error_message = "The relative distance is too important";
+    a.number_of_attempts++;
+    f.ladder_decision = d;
+    if (d.accepted) {
+        f.ladder_accepted = true;
+        f.icp_pending = false;
+        f.joins = kJoinsNone;
+        if (a.number_of_attempts > options_.robust_num_attempts)
+            robust_num_consecutive_failures_++;
+        else
+            robust_num_consecutive_failures_ = 0;
+        return;
+    }
+    IncreaseRobustness(f);
+    f.attempt++;
+    BeginAttempt(f);
 }
 
 // ComputeSummaryMetrics, odometry.cpp:978-988
@@ -1087,25 +1171,13 @@ void Engine::ComputeSummaryMetrics(Summary &s, int k) {
     }
 }
 
-// UpdateMap, odometry.cpp:855-953
-void Engine::UpdateMap(Summary &s, int registered_fid) {
+// UpdateMap, odometry.cpp:855-953. A robust frame brings the decision of its accepted attempt (robust_attempt_decide: the
+// robust branch :861-901 on the same pose pair, success flag and attempt count); the caller set next_robust_level_.
+void Engine::UpdateMap(Summary &s, int registered_fid, const RobustDecision *robust) {
     NvtxRange range("cticp.map_update");
     bool add_points = true;
-    if (options_.robust_registration) {
-        suspect_registration_error_ = s.number_of_attempts >= options_.robust_num_attempts;
-        if (s.ego_orientation > options_.robust_threshold_ego_orientation ||
-            s.relative_orientation > options_.robust_threshold_relative_orientation)
-            add_points = false;
-        if (suspect_registration_error_) add_points |= (robust_num_consecutive_failures_ > 5);
-        next_robust_level_ = add_points ? options_.robust_minimal_level : options_.robust_minimal_level + 1;
-        if (!s.success)
-            next_robust_level_ = options_.robust_minimal_level + 2;
-        else {
-            if (s.relative_orientation > options_.robust_threshold_relative_orientation ||
-                s.ego_orientation > options_.robust_threshold_ego_orientation)
-                next_robust_level_ = options_.robust_minimal_level + 1;
-            if (s.number_of_attempts > 1) next_robust_level_ = options_.robust_minimal_level + 1;
-        }
+    if (robust) {
+        add_points = robust->add_points_policy != 0;
     } else {
         tracker_.cum_orientation += s.relative_orientation;
         tracker_.cum_distance += s.relative_distance;
@@ -1180,10 +1252,19 @@ void Engine::BeginStaged(int64_t slot, uint32_t frame_id, cticp_summary *out, Pe
     PrepareFrame(none, frame_id, nullptr, slot, out, nullptr, f);
 }
 
-void Engine::CompleteFrame(PendingFrame &f) {
+void Engine::LaunchPending(PendingFrame &f) {
     if (f.icp_pending && !f.icp_launched) {
+        CT_CUDA_CHECK(cudaSetDevice(device_));
         LaunchIcp(f.icp_options);
         f.icp_launched = true;
+    }
+}
+
+void Engine::CompleteFrame(PendingFrame &f) {
+    for (;;) {
+        LaunchPending(f);
+        if (!f.ladder || f.ladder_accepted) break;
+        EndAttempt(f);   // the robust ladder: accepted, or the next attempt begun
     }
     FinishFrame(f);
 }
@@ -1192,8 +1273,51 @@ const Engine::MotionModel *Engine::ModelOf(const PendingFrame &f) const {
     return f.caller_model.present ? &f.caller_model : f.default_model ? &default_motion_model_ : nullptr;
 }
 
+// The plain-path inputs of the device tail (tail_in_), and room in the map tables for the frame. Does not set tail_armed_.
+void Engine::ArmTail(double relative_orientation) {
+    FramePolicyIn &in = tail_in_;
+    in = FramePolicyIn{};
+    in.distance_error_threshold = options_.distance_error_threshold;
+    in.orientation_error_threshold = options_.orientation_error_threshold;
+    in.relative_orientation = relative_orientation;
+    in.insertion_ego_rotation_threshold = options_.insertion_ego_rotation_threshold;
+    in.quit_on_error = options_.quit_on_error ? 1 : 0;
+    in.has_insertions = tracker_.total_insertions > 0;
+    in.skipped_enough = tracker_.skipped_frames > options_.insertion_threshold_frames_skipped;
+    in.do_no_insert = options_.do_no_insert ? 1 : 0;
+    in.always_insert = options_.always_insert ? 1 : 0;
+    // F is still on the device: room for the previous frame's count with head-room (a frame beyond it is
+    // deferred to the host-side UpdateMap). Before the ICP is enqueued — a grown table is a new table.
+    const size_t prev_f = (size_t) std::max(0, pipe_->h_counts()[1]);
+    size_t room = std::min(pipe_->n(), prev_f + prev_f / 2 + 4096);
+    if (const char *e = getenv("CTICP_TAIL_ROOM")) room = std::min(room, (size_t) std::max(0, atoi(e)));   // test hook: force the deferred path
+    map_->EnsureRoomFor(room);
+    in.room_for = (int) room;
+}
+
+// The grouped launch (RegisterBatch) a registration with these options can run in: exactly those the solo launch would
+// run through the persistent GN loop, or the solo launch of k_lm_persistent, with the armed device tail
+int Engine::JoinKind(const cticp_icp_options &o) {
+    if (!tail_armed_ || nccl_comm_ || shard_world_ > 1) return kJoinsNone;
+    const int solver = o.solver;
+    if (solver == CTICP_SOLVER_GN && icp_->batch_supported() && o.max_number_neighbors >= 1 && o.max_number_neighbors <= 32)
+        return kJoinsGn;
+    if ((solver == CTICP_SOLVER_CERES || solver == CTICP_SOLVER_ROBUST) && icp_->use_persistent()) {
+        // options the LM path rejects keep the single-frame path, which fails them alone
+        try {
+            icp_->CheckCeresOptions(*map_, o, options_.neighborhood_strategy);
+        } catch (const std::exception &) {
+            return kJoinsNone;
+        }
+        return solver == CTICP_SOLVER_ROBUST ? kJoinsRobust
+               : options_.neighborhood_strategy.type == CTICP_STRATEGY_DISTANCE_BASED ? kJoinsCeresDistance
+                                                                                        : kJoinsCeresNearest;
+    }
+    return kJoinsNone;
+}
+
 // Phase 1 of a frame: ingest, motion initialisation, arming the device tail, sampling, the state upload. A plain
-// registration stops before its ICP launch (f.icp_pending); a robust one runs its attempts here.
+// registration stops before its ICP launch (f.icp_pending); a robust one stops before the launch of its first attempt.
 void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate,
                           int64_t staged_slot, cticp_summary *out, const cticp_motion_prior *motion_model, PendingFrame &f) {
     const size_t n = scan.n;
@@ -1287,7 +1411,7 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
         const MotionModel *mm = ModelOf(f);
         f.ran_icp = true;
         if (options_.robust_registration) {
-            RobustRegistration(info, summary, mm);
+            BeginLadder(f);
         } else {
             cticp_icp_options &ct_icp_options = f.icp_options;
             ct_icp_options = options_.ct_icp_options;
@@ -1297,54 +1421,17 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
             // NB trajectory_[k] is still the INITIAL estimate here (odometry.cpp:429-431)
             const double relative_orientation =
                 angular_distance_deg(trajectory_[k - 1].end_pose.pose.q, trajectory_[k].end_pose.pose.q);
+            tail_robust_ = RobustPolicyIn{};
             if (device_tail_ && fused_map_update_ && !callback_ && options_.motion_compensation == CTICP_MC_CONTINUOUS &&
                 pipe_->n() > 0) {
-                // the tail of this registration is decided on the device (frame_policy.h)
-                FramePolicyIn &in = tail_in_;
-                in = FramePolicyIn{};
-                in.distance_error_threshold = options_.distance_error_threshold;
-                in.orientation_error_threshold = options_.orientation_error_threshold;
-                in.relative_orientation = relative_orientation;
-                in.insertion_ego_rotation_threshold = options_.insertion_ego_rotation_threshold;
-                in.quit_on_error = options_.quit_on_error ? 1 : 0;
-                in.has_insertions = tracker_.total_insertions > 0;
-                in.skipped_enough = tracker_.skipped_frames > options_.insertion_threshold_frames_skipped;
-                in.do_no_insert = options_.do_no_insert ? 1 : 0;
-                in.always_insert = options_.always_insert ? 1 : 0;
-                // F is still on the device: room for the previous frame's count with head-room (a frame beyond it is
-                // deferred to the host-side UpdateMap). Before the ICP is enqueued — a grown table is a new table.
-                const size_t prev_f = (size_t) std::max(0, pipe_->h_counts()[1]);
-                size_t room = std::min(pipe_->n(), prev_f + prev_f / 2 + 4096);
-                if (const char *e = getenv("CTICP_TAIL_ROOM")) room = std::min(room, (size_t) std::max(0, atoi(e)));   // test hook: force the deferred path
-                map_->EnsureRoomFor(room);
-                in.room_for = (int) room;
+                ArmTail(relative_orientation);   // the tail of this registration is decided on the device (frame_policy.h)
                 tail_armed_ = true;
             }
             f.relative_orientation = relative_orientation;
             NvtxRange range("cticp.icp");
             TryRegisterBegin(info, ct_icp_options, summary, sample_voxel_size, mm, 0);
             f.icp_pending = true;
-            // the frames whose ICP can run in a grouped launch (RegisterBatch): exactly those the solo launch would run
-            // through the persistent GN loop, or the solo launch of k_lm_persistent, with the armed device tail
-            if (tail_armed_ && !nccl_comm_ && shard_world_ <= 1) {
-                const int solver = ct_icp_options.solver;
-                if (solver == CTICP_SOLVER_GN && icp_->batch_supported() && ct_icp_options.max_number_neighbors >= 1 &&
-                    ct_icp_options.max_number_neighbors <= 32) {
-                    f.joins = kJoinsGn;
-                } else if ((solver == CTICP_SOLVER_CERES || solver == CTICP_SOLVER_ROBUST) && icp_->use_persistent()) {
-                    // options the LM path rejects keep the single-frame path, which fails them alone
-                    bool accepted = true;
-                    try {
-                        icp_->CheckCeresOptions(*map_, ct_icp_options, options_.neighborhood_strategy);
-                    } catch (const std::exception &) {
-                        accepted = false;
-                    }
-                    if (accepted)
-                        f.joins = solver == CTICP_SOLVER_ROBUST ? kJoinsRobust
-                                  : options_.neighborhood_strategy.type == CTICP_STRATEGY_DISTANCE_BASED ? kJoinsCeresDistance
-                                                                                                           : kJoinsCeresNearest;
-                }
-            }
+            f.joins = JoinKind(ct_icp_options);
         }
     } else {
         CT_CUDA_CHECK(cudaEventRecord(ev_[1].get(), stream_.get()));
@@ -1364,6 +1451,7 @@ void Engine::FinishFrame(PendingFrame &f) {
     bool &early_return = f.early_return;
     const bool ran_icp = f.ran_icp;
     cticp_summary *out = f.out;
+    const RobustDecision *robust = f.ladder ? &f.ladder_decision : nullptr;
     if (k > 0) {
         if (f.icp_pending) {
             TryRegisterEnd(info, f.icp_options, summary);
@@ -1397,10 +1485,14 @@ void Engine::FinishFrame(PendingFrame &f) {
             if (summary_points_mask_) EnqueueEgress(f, ran_icp);
         }
         ComputeSummaryMetrics(summary, k);
+        if (robust) {   // UpdateMap's robust branch (:861-901), as decided with the accepted attempt
+            suspect_registration_error_ = summary.number_of_attempts >= options_.robust_num_attempts;
+            next_robust_level_ = robust->next_robust_level;
+        }
         if (tail_launched_ && h_verdict_.data()->action != kFrameDeferred)
             AdoptDeviceMapUpdate(summary);   // evicted / inserted already, behind the ICP kernel
         else
-            UpdateMap(summary, k);
+            UpdateMap(summary, k, robust);
         if (fused_map_update_ && summary_points_mask_) EnqueueEgress(f, ran_icp);   // (the fused update wrote d_frame_world)
         if (callback_) {   // odometry.cpp:491
             const bool fw = frame_world_valid_, aw = last_all_world_valid_, kw = last_kp_world_valid_;

@@ -123,12 +123,17 @@ public:
     ~Engine();
 
     // A frame between the three phases every registration goes through: Begin* (ingest, motion initialisation, arming
-    // the device tail, sampling, the state upload; a robust registration runs its attempts here), the ICP launch (solo:
-    // LaunchIcp; or a grouped launch shared with other handles, RegisterBatch), FinishFrame (verdict, map update,
-    // summary). RegisterFrame / RegisterDevice / RegisterStaged run them back to back.
+    // the device tail, sampling, the state upload), the ICP launch (solo: LaunchIcp; or a grouped launch shared with
+    // other handles, RegisterBatch), FinishFrame (verdict, map update, summary). RegisterFrame / RegisterDevice /
+    // RegisterStaged run them back to back. A robust registration (robust_registration) repeats the first two per
+    // attempt: EndAttempt decides an attempt and, when it is rejected, begins the next one up to its launch.
     // The grouped ICP launches of RegisterBatch, one per kind of joining frame: solver GN (k_gn_persistent), and solver
-    // CERES with the nearest-neighbour strategy, CERES with the distance-based strategy and ROBUST (k_lm_persistent's modes).
-    enum { kJoinsNone = -1, kJoinsGn = 0, kJoinsCeresNearest, kJoinsCeresDistance, kJoinsRobust, kJoinKinds };
+    // CERES with the nearest-neighbour strategy, CERES with the distance-based strategy and ROBUST (k_lm_persistent's
+    // modes); the attempts of robust registrations in four kinds of their own, the same four solvers.
+    enum {
+        kJoinsNone = -1, kJoinsGn = 0, kJoinsCeresNearest, kJoinsCeresDistance, kJoinsRobust,
+        kJoinsLadderGn, kJoinsLadderCeresNearest, kJoinsLadderCeresDistance, kJoinsLadderRobust, kJoinKinds
+    };
     struct PendingFrame {
         size_t n = 0;
         cticp_summary *out = nullptr;
@@ -141,17 +146,32 @@ public:
         int launches0 = 0;
         cticp_icp_options icp_options{};
         bool ran_icp = false, early_return = false;
-        bool icp_pending = false;     // a plain registration waits for its ICP launch and its TryRegisterEnd
+        bool icp_pending = false;     // a registration (attempt) waits for its ICP launch and its TryRegisterEnd
         bool icp_launched = false;
         int joins = kJoinsNone;       // the grouped launch its ICP may run in (persistent loop, armed device tail)
+        // the robust ladder (RobustRegistrationAttempt): icp_options are the attempt's registration options, summary its
+        // summary
+        bool ladder = false, ladder_accepted = false;
+        int attempt = 0, robust_level = 0;
+        double sample_voxel_size = 0;
+        HostFrame ladder_initial;
+        RobustDecision ladder_decision{};   // of the last decided attempt
     };
     void BeginFrame(const ScanView &scan, uint32_t frame_id, const cticp_frame *initial_estimate, cticp_summary *out,
                     const cticp_motion_prior *motion_model, PendingFrame &f);
     void BeginDevice(ScanView scan, cudaStream_t producer, uint32_t frame_id, const cticp_frame *initial_estimate,
                      cticp_summary *out, const cticp_motion_prior *motion_model, PendingFrame &f);
     void BeginStaged(int64_t slot, uint32_t frame_id, cticp_summary *out, PendingFrame &f);
-    // the solo launch when still pending, then FinishFrame
+    // the solo launch when still pending (each remaining attempt of a robust ladder: launch, EndAttempt), then FinishFrame
     void CompleteFrame(PendingFrame &f);
+    // the solo ICP launch of the pending registration (attempt), unless a grouped launch ran it
+    void LaunchPending(PendingFrame &f);
+    // a robust registration after its attempt's ICP launch: the verdict and the decision. Accepted: f.ladder_accepted,
+    // ready for CompleteFrame. Rejected: the next attempt is begun and waits for its launch (f.icp_pending, f.joins).
+    void EndAttempt(PendingFrame &f);
+    // the device tail of the launched attempt (k_frame_policy + the speculative map update), when armed; EndAttempt and
+    // TryRegisterEnd enqueue it themselves if nobody did
+    void EnqueueTail();
     // a joining frame's registration in a grouped launch (valid until FinishFrame)
     GnProblem IcpProblem(const PendingFrame &f) const;
     // the same for a CERES / ROBUST frame: prepares this handle's LM buffers for it (IcpSolver::PrepareCeres) on the
@@ -237,17 +257,23 @@ private:
     std::vector<StagedScan> staged_;
     Event timer_ev_[2];
     DeviceArray<unsigned char> d_flush_;
-    void TryRegister(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
-                     const MotionModel *mm, int attempt_idx);
     void TryRegisterBegin(const FrameInfo &info, cticp_icp_options &options, Summary &rs, double sample_voxel_size,
                           const MotionModel *mm, int attempt_idx);
     void LaunchIcp(const cticp_icp_options &options);
     void TryRegisterEnd(const FrameInfo &info, const cticp_icp_options &options, Summary &rs);
     bool verdict_by_icp_kernel_ = false;   // the last ICP launch decided the frame's tail itself (CTICP_TAIL_IN_KERNEL)
     bool AssessRegistration(Summary &s) const;
-    void RobustRegistration(const FrameInfo &info, Summary &rs, const MotionModel *mm);
+    // the robust ladder (RobustRegistration) in steps: engine.cu
+    void BeginLadder(PendingFrame &f);
+    void BeginAttempt(PendingFrame &f);
+    void IncreaseRobustness(PendingFrame &f);
+    RobustPolicyIn LadderInputs(const PendingFrame &f) const;
+    double LadderSampleSize(int k, int level) const;
+    bool ladder_tail_ = false;   // the current robust frame's attempts take the device tail
+    void ArmTail(double relative_orientation);
+    int JoinKind(const cticp_icp_options &o);
     void ComputeSummaryMetrics(Summary &s, int k);
-    void UpdateMap(Summary &s, int registered_fid);
+    void UpdateMap(Summary &s, int registered_fid, const RobustDecision *robust);
     // The tail of a plain registration decided on the device (frame_policy.h): TryRegister enqueues k_frame_policy and a
     // speculative k_map_update_fused right behind the ICP kernel, then waits for the verdict in mapped pinned memory — no
     // copy-engine operation and no host round trip between the ICP loop and the map update.
@@ -258,6 +284,7 @@ private:
     bool tail_armed_ = false;      // the coming TryRegister enqueues the device tail (tail_in_ is filled)
     bool tail_launched_ = false;   // the last TryRegister did: h_verdict_ holds this frame's verdict
     FramePolicyIn tail_in_{};
+    RobustPolicyIn tail_robust_{};   // the robust ladder's inputs of the coming attempt (enabled = 0 on the plain path)
     DeviceArray<FrameVerdict> d_verdict_;
     PinnedArray<FrameVerdict> h_verdict_{cudaHostAllocMapped};
     FrameVerdict *h_verdict_dev_ = nullptr;   // its device address

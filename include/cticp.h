@@ -472,7 +472,8 @@ typedef struct cticp_device_timing {
     int32_t gather_launches;               /* launches of the neighbor-gather kernel */
     int32_t icp_batch_groups;              /* problems in the ICP launch of the last frame: 1 solo, B in a grouped launch of
                                               cticp_odometry_register_batch (the frames of its kind: GN, CERES nearest
-                                              neighbour, CERES distance-based or ROBUST), 0 without an ICP */
+                                              neighbour, CERES distance-based or ROBUST), 0 without an ICP. With
+                                              robust_registration: the launch that ran the frame's last attempt */
 } cticp_device_timing;
 int cticp_odometry_last_timing(cticp_odometry *h, cticp_device_timing *out);
 
@@ -489,11 +490,13 @@ int cticp_odometry_register_staged(cticp_odometry *h, int64_t slot, uint32_t fra
  *   CTICP_BATCH_HOST    xyz / t / n with strides in host memory (cticp_odometry_register_frame_ex)
  *   CTICP_BATCH_DEVICE  device_scan + producer stream (cticp_odometry_register_device)
  *   CTICP_BATCH_STAGED  staged_slot (cticp_odometry_register_staged; initial_estimate and motion_model must be NULL)
- * The frames whose single-frame call would run its ICP loop through a persistent kernel with the device tail (k > 0, no
- * robust_registration, motion compensation CONTINUOUS, no callback, not sharded, a non-empty scan; solver GN, or solver
- * CERES / ROBUST with options the LM loop accepts) join: the joining frames of each kind — GN, CERES with the
- * nearest-neighbour strategy, CERES with the distance-based strategy, ROBUST — run their loops in ONE grouped launch per
- * kind, each against its own handle's map and options. A kind with a single joining frame keeps its solo launch; every
+ * The frames whose single-frame call would run its ICP loop through a persistent kernel with the device tail (k > 0,
+ * motion compensation CONTINUOUS, no callback, not sharded, a non-empty scan; solver GN, or solver CERES / ROBUST with
+ * options the LM loop accepts) join: the joining frames of each kind — GN, CERES with the nearest-neighbour strategy,
+ * CERES with the distance-based strategy, ROBUST — run their loops in ONE grouped launch per kind, each against its own
+ * handle's map and options. Frames with robust_registration form four kinds of their own (the same four solvers) and run
+ * their attempts in rounds: round r launches attempt r of every such frame still running, one grouped launch per kind;
+ * a rejected attempt's next one joins round r + 1. A kind with a single joining frame keeps its solo launch; every
  * other frame takes its single-frame path inside the call. Each item's summary, trajectory entry, map and point vectors
  * are those of the single-frame call, byte for byte when the joining problems of a kind fit on the device together (each
  * gets its solo grid); otherwise they differ by the summation order only and are reproducible from run to run.

@@ -5,7 +5,8 @@ B in {1, 2, 4, 8, 16}.
 Workloads: the bench workload (BASELINE.json configs[1]: bench.py's GN options and KITTI-shape 64-beam scans, one seed
 per sequence) and a small-scan one (the same options on 16-beam ~10k-pt scans); bench.py's kitti64_ceres workload
 (BASELINE.json configs[2]: driving_config.yaml, solver CERES) on the same two scan kinds, and its options with solver
-ROBUST (robust_registration off) on the small scans. Every sequence first registers
+ROBUST (robust_registration off) on the small scans; and the kitti64_ceres options with robust_registration on (the
+attempt ladder of RobustRegistration, run in rounds of grouped launches) on both scan kinds. Every sequence first registers
 --preroll frames untimed (past init_num_frames), then --warmup frames, then --steps timed steps. A step is host-timed
 and ends in a device synchronise. The two modes have their own handles over the same scans and take turns step by step.
 
@@ -15,7 +16,12 @@ A separate run under torch.profiler gives the device time of the ICP launches pe
 k_lm_persistent: B solo launches against one grouped launch). The card name and power limit come from a read-only nvidia-smi query in the same
 run.
 
+--single-frame: instead, for each workload, one handle with the device tail against one with CTICP_DEVICE_TAIL=0 (the
+host-side tail), single-frame calls on the same staged scans, taking turns frame by frame; reports the median frame time
+of each and the attempts per frame.
+
 usage: python tools/bench_odometry_batch.py [--steps 20] [--warmup 3] [--preroll 20] [--sizes 1,2,4,8,16] [--out DIR]
+                                            [--workloads a,b] [--single-frame]
 """
 import argparse
 import json
@@ -34,10 +40,11 @@ import bench  # noqa: E402
 import ct_icp_b200  # noqa: E402
 from ct_icp_b200 import synthetic as syn  # noqa: E402
 
-# name: (sensor, bench.py workload whose options the handles take, solver override)
-WORKLOADS = {"kitti64_gn": ("HDL64E", "kitti64_gn", None), "small16_gn": ("SMALL16", "kitti64_gn", None),
-             "kitti64_ceres": ("HDL64E", "kitti64_ceres", None), "small16_ceres": ("SMALL16", "kitti64_ceres", None),
-             "small16_robust": ("SMALL16", "kitti64_ceres", "ROBUST")}
+# name: (sensor, bench.py workload whose options the handles take, solver override, robust_registration)
+WORKLOADS = {"kitti64_gn": ("HDL64E", "kitti64_gn", None, 0), "small16_gn": ("SMALL16", "kitti64_gn", None, 0),
+             "kitti64_ceres": ("HDL64E", "kitti64_ceres", None, 0), "small16_ceres": ("SMALL16", "kitti64_ceres", None, 0),
+             "small16_robust": ("SMALL16", "kitti64_ceres", "ROBUST", 0),
+             "kitti64_ladder": ("HDL64E", "kitti64_ceres", None, 1), "small16_ladder": ("SMALL16", "kitti64_ceres", None, 1)}
 KERNELS = ("k_gn_persistent", "k_lm_persistent")
 
 
@@ -51,13 +58,13 @@ def card():
 
 
 def make_options(eng, workload):
-    _, bench_workload, solver = WORKLOADS[workload]
+    _, bench_workload, solver, robust = WORKLOADS[workload]
     bench._WORKLOAD = bench_workload
     o = bench.make_options(eng)
     if solver:
         from ct_icp_b200 import _abi as abi
         o.ct_icp_options.solver = abi.SOLVER[solver]
-        o.robust_registration = 0
+    o.robust_registration = robust
     return o
 
 
@@ -113,6 +120,45 @@ def icp_device_ms(eng, seqs, workload, first, steps, batched, torch):
     return out
 
 
+def single_frame(eng, seqs, workload, args, torch):
+    """device tail against host tail (CTICP_DEVICE_TAIL, read when a handle is created), one handle each, frame by frame
+    in turns on the same staged scans"""
+    arms = {}
+    for mode, env in (("device_tail", "1"), ("host_tail", "0")):
+        old = os.environ.get("CTICP_DEVICE_TAIL")
+        os.environ["CTICP_DEVICE_TAIL"] = env
+        try:
+            arms[mode] = Arm(eng, seqs, workload)
+        finally:
+            if old is None:
+                os.environ.pop("CTICP_DEVICE_TAIL")
+            else:
+                os.environ["CTICP_DEVICE_TAIL"] = old
+    first = args.preroll + args.warmup
+    frame_s = {m: [] for m in arms}
+    attempts = {m: [] for m in arms}
+    od = {m: arms[m].ods[0] for m in arms}
+    for k in range(first + args.steps):
+        for m in (("device_tail", "host_tail") if k % 2 == 0 else ("host_tail", "device_tail")):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            sm = od[m].RegisterStaged(arms[m].slots[0][k], seqs[0][k]["frame_idx"])
+            torch.cuda.synchronize()
+            if k >= first:
+                frame_s[m].append(time.perf_counter() - t0)
+                attempts[m].append(sm.number_of_attempts)
+    same = trajectory_bytes(od["device_tail"]) == trajectory_bytes(od["host_tail"])
+    row = {"workload": workload, "mode": "single_frame", "trajectories_identical": same}
+    for m in arms:
+        row[f"{m}_frame_ms_median"] = 1e3 * float(np.median(frame_s[m]))
+        row[f"{m}_frame_ms_min"] = 1e3 * float(np.min(frame_s[m]))
+        row[f"{m}_attempts_per_frame"] = float(np.mean(attempts[m]))
+    row["host_over_device_tail"] = row["host_tail_frame_ms_median"] / row["device_tail_frame_ms_median"]
+    for a in arms.values():
+        a.close()
+    return row
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -121,6 +167,7 @@ def main():
     ap.add_argument("--sizes", default="1,2,4,8,16")
     ap.add_argument("--workloads", default=",".join(WORKLOADS))
     ap.add_argument("--out", default=None)
+    ap.add_argument("--single-frame", action="store_true")
     args = ap.parse_args()
     import torch
 
@@ -133,6 +180,11 @@ def main():
     for wl in args.workloads.split(","):
         with multiprocessing.get_context("fork").Pool(min(max(sizes), os.cpu_count() or 1)) as pool:
             all_seqs = pool.starmap(make_sequence, [(n_frames, WORKLOADS[wl][0], 1234 + b) for b in range(max(sizes))])
+        if args.single_frame:
+            row = single_frame(eng, all_seqs[:1], wl, args, torch)
+            result["rows"].append(row)
+            print(json.dumps(row), flush=True)
+            continue
         for B in sizes:
             seqs = all_seqs[:B]
             arms = {"sequential": Arm(eng, seqs, wl), "batch": Arm(eng, seqs, wl)}
