@@ -19,6 +19,28 @@
 
 namespace cticp {
 
+#ifdef CTICP_DEBUG_TIMERS
+void phase_stamps_reset(unsigned long long *stamps, cudaStream_t stream) {
+    if (!getenv("CTICP_DEBUG_TIMERS")) return;
+    unsigned long long init[kPhaseSlots] = {~0ull};
+    CT_CUDA_CHECK(cudaMemcpyAsync(stamps, init, sizeof(init), cudaMemcpyHostToDevice, stream));
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream));   // (init lives on this stack)
+}
+// one line per launch: the end of every phase in µs after the first CTA started (0: a phase the launch skipped)
+void phase_stamps_print(const unsigned long long *stamps, cudaStream_t stream, const char *kernel, const char *const *labels,
+                        int num_labels) {
+    if (!getenv("CTICP_DEBUG_TIMERS")) return;
+    unsigned long long h[kPhaseSlots];
+    CT_CUDA_CHECK(cudaMemcpyAsync(h, stamps, sizeof(h), cudaMemcpyDeviceToHost, stream));
+    CT_CUDA_CHECK(cudaStreamSynchronize(stream));
+    fprintf(stderr, "[cticp] phase ends %s (us):", kernel);
+    for (int i = 0; i < num_labels && i + 1 < kPhaseSlots; ++i)
+        fprintf(stderr, " %s=%.2f", labels[i], h[i + 1] > h[0] ? 1e-3 * (double) (h[i + 1] - h[0]) : 0.0);
+    fprintf(stderr, "\n");
+}
+__device__ unsigned long long g_update_stamps[kPhaseSlots];
+#endif
+
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void k_clear_level(MapLevel L) {
     const uint32_t cap = L.cap_mask + 1;
@@ -69,7 +91,14 @@ __device__ __forceinline__ void insert_claim_dev(const MapLevel &L, MapCounters 
         }
         const int old = atomicExch(&L.head[slot], i);
         next[i] = old;
-        if (old == kNil) touched[atomicAdd(&ctr->num_touched, 1u)] = (uint32_t) slot;
+        if (old == kNil) {
+            // one counter atomic per group of lanes that touched a voxel together, not one per voxel. The order of touched
+            // follows atomic arrival either way, and nothing in the map depends on it: voxels are committed independently.
+            const cooperative_groups::coalesced_group g = cooperative_groups::coalesced_threads();
+            unsigned first = 0;
+            if (g.thread_rank() == 0) first = atomicAdd(&ctr->num_touched, g.size());
+            touched[g.shfl(first, 0) + g.thread_rank()] = (uint32_t) slot;
+        }
     }
 }
 __global__ void k_insert_claim(MapLevel L, MapCounters *ctr, const double *__restrict__ world, const int *d_n,
@@ -330,47 +359,57 @@ struct FusedUpdateArgs {
 };
 // (4 CTAs per SM: the cooperative grid is sized from the occupancy, so the register budget is enforced here)
 __global__ void __launch_bounds__(kInsertWarps * 32, 4)
-k_map_update_fused(FusedUpdateArgs a) {
+k_map_update_fused(const FusedUpdateArgs a) {
     namespace cg = cooperative_groups;
     cg::grid_group grid = cg::this_grid();
     __shared__ CommitScratch sc;
+    PHASE_STAMP(phase_begin(g_update_stamps);)
+    // The speculative launch's pose pair, eviction centre and insert decision go to locals, never into `a`: a kernel
+    // parameter the kernel writes is first copied to local memory by every thread (~0.75 KB each, ~50 MB over the grid).
+    Q4 qb = a.qb, qe = a.qe;
+    V3 tb = a.tb, te = a.te, location = a.location;
+    SlerpConsts slerp;
+    int do_insert = a.do_insert;
     if (a.verdict) {
         const FrameVerdict &v = *a.verdict;
         const int action = v.action;
         if (action != kFrameEvict && action != kFrameInsert) return;   // uniform over the grid (before any barrier)
-        a.qb = Q4{v.state.qb[0], v.state.qb[1], v.state.qb[2], v.state.qb[3]};
-        a.qe = Q4{v.state.qe[0], v.state.qe[1], v.state.qe[2], v.state.qe[3]};
-        a.tb = V3{v.state.tb[0], v.state.tb[1], v.state.tb[2]};
-        a.te = V3{v.state.te[0], v.state.te[1], v.state.te[2]};
-        a.sc = v.sc;
-        a.location = a.te;   // trajectory_.back().end_pose.tr (odometry.cpp:942)
-        a.do_insert = action == kFrameInsert;
+        qb = Q4{v.state.qb[0], v.state.qb[1], v.state.qb[2], v.state.qb[3]};
+        qe = Q4{v.state.qe[0], v.state.qe[1], v.state.qe[2], v.state.qe[3]};
+        tb = V3{v.state.tb[0], v.state.tb[1], v.state.tb[2]};
+        te = V3{v.state.te[0], v.state.te[1], v.state.te[2]};
+        slerp = v.sc;
+        location = te;   // trajectory_.back().end_pose.tr (odometry.cpp:942)
+        do_insert = action == kFrameInsert;
         // frame_poses.front().tr of this insert (odometry.cpp:949); read by insert_commit_dev behind the grid barriers
-        if (a.do_insert && a.frame_origins_mut && blockIdx.x == 0 && threadIdx.x == 0) {
+        if (do_insert && a.frame_origins_mut && blockIdx.x == 0 && threadIdx.x == 0) {
             double *o = a.frame_origins_mut + 3 * (size_t) a.frame_ordinal;
-            o[0] = a.tb.x; o[1] = a.tb.y; o[2] = a.tb.z;
+            o[0] = tb.x; o[1] = tb.y; o[2] = tb.z;
         }
     } else {
         // the slerp constants with the device's arithmetic, as k_frame_policy derives them for the speculative launch:
         // the host-side tail (UpdateMap) gives the same world points, bit for bit
-        a.sc = slerp_consts(a.qb, a.qe);
+        slerp = slerp_consts(qb, qe);
     }
     const int n = *a.d_n;
     // phase 1: world points of the frame; eviction on every level; reset the per-level touched counters
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const RawPoint p = load_raw(a.frame, a.frame_lo, i);
-        const V3 w = ct_transform_c(a.qb, a.tb, a.qe, a.te, p.alpha, V3{p.x, p.y, p.z}, a.sc);
+        const V3 w = ct_transform_c(qb, tb, qe, te, p.alpha, V3{p.x, p.y, p.z}, slerp);
         a.world[3 * i] = w.x; a.world[3 * i + 1] = w.y; a.world[3 * i + 2] = w.z;
     }
     if (a.do_remove)
-        for (int l = 0; l < a.num_levels; ++l) remove_far_dev(a.levels[l], a.counters + l, a.location, a.max_distance);
+        for (int l = 0; l < a.num_levels; ++l) remove_far_dev(a.levels[l], a.counters + l, location, a.max_distance);
     if (blockIdx.x == 0 && threadIdx.x < a.num_levels) a.counters[threadIdx.x].num_touched = 0;
-    if (!a.do_insert) return;   // uniform
+    PHASE_STAMP(phase_end(g_update_stamps, 1);)
+    if (!do_insert) return;   // uniform
     for (int l = 0; l < a.num_levels; ++l) {
         grid.sync();
         insert_claim_dev(a.levels[l], a.counters + l, a.world, n, a.next, a.touched);
+        PHASE_STAMP(if (l < 4) phase_end(g_update_stamps, 2 + 2 * l);)
         grid.sync();
         insert_commit_dev(a.levels[l], a.counters + l, a.world, a.next, a.touched, a.frame_origins, a.frame_ordinal, sc);
+        PHASE_STAMP(if (l < 4) phase_end(g_update_stamps, 3 + 2 * l);)
     }
 }
 
@@ -563,7 +602,16 @@ void DeviceMap::UpdateFused(const float4 *d_frame, const float4 *d_frame_lo, con
     a.verdict = d_verdict;
     a.frame_origins_mut = with_normals_ ? d_frame_origins_.data() : nullptr;
     void *args[] = {&a};
+#ifdef CTICP_DEBUG_TIMERS
+    unsigned long long *stamps = nullptr;
+    CT_CUDA_CHECK(cudaGetSymbolAddress((void **) &stamps, g_update_stamps));
+    phase_stamps_reset(stamps, stream_);
+#endif
     CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_map_update_fused, dim3(fused_grid_), dim3(kInsertWarps * 32), args, 0, stream_));
+#ifdef CTICP_DEBUG_TIMERS
+    static const char *const labels[] = {"world_evict", "claim0", "commit0", "claim1", "commit1", "claim2", "commit2", "claim3", "commit3"};
+    phase_stamps_print(stamps, stream_, "k_map_update_fused", labels, 1 + 2 * std::min(a.num_levels, 4));   // (first 4 levels)
+#endif
     launches_ += 1;
     dirty_ = true;
 }

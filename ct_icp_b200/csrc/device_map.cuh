@@ -96,6 +96,30 @@ __device__ __forceinline__ int map_find(const MapLevel &L, unsigned long long ke
     }
     return -1;
 }
+
+// -DCTICP_DEBUG_TIMERS builds: phase stamps of the fused sampler and the fused map update. Slot 0 takes the earliest start of
+// a CTA, every other slot the latest end of one phase over the CTAs, all in %globaltimer ns (comparable across SMs, unlike
+// clock64; a few reads per CTA and launch cost nothing, unlike the per-iteration reads icp.h warns about). The host prints
+// them per launch when the environment has CTICP_DEBUG_TIMERS. Default builds compile none of this.
+#ifdef CTICP_DEBUG_TIMERS
+constexpr int kPhaseSlots = 16;
+__device__ __forceinline__ unsigned long long phase_clock() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ void phase_begin(unsigned long long *stamps) {
+    if (threadIdx.x == 0) atomicMin(stamps, phase_clock());
+}
+// every thread of the CTA
+__device__ __forceinline__ void phase_end(unsigned long long *stamps, int slot) {
+    __syncthreads();
+    if (threadIdx.x == 0) atomicMax(stamps + slot, phase_clock());
+}
+#define PHASE_STAMP(...) __VA_ARGS__
+#else
+#define PHASE_STAMP(...)
+#endif
 #endif
 
 }  // namespace cticp

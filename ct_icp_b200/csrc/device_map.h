@@ -17,6 +17,14 @@ struct CapacityError : std::runtime_error {
 
 struct FrameVerdict;   // frame_policy.h
 
+#ifdef CTICP_DEBUG_TIMERS
+// host side of the phase stamps (device_map.cuh); `stamps` is a kernel's stamp array (cudaGetSymbolAddress). Both do
+// nothing unless the environment has CTICP_DEBUG_TIMERS; print waits for the stream.
+void phase_stamps_reset(unsigned long long *stamps, cudaStream_t stream);
+void phase_stamps_print(const unsigned long long *stamps, cudaStream_t stream, const char *kernel, const char *const *labels,
+                        int num_labels);
+#endif
+
 class DeviceMap {
 public:
     // with_normals: maintain the per-voxel normals that RadiusSearchInPlace's sensor_location filter reads (map.h:482-490)

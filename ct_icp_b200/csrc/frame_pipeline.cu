@@ -26,6 +26,7 @@ constexpr int kTileShift = 10, kTile = 1 << kTileShift, kTileThreads = kTile / 4
 // d_desc_: the fused sampler's look-back descriptors (selection 1 | selection 2 | the capacity of grid 2 its last launch
 // used), then the standalone selection's descriptors and tile ticket
 constexpr size_t kFusedDescWords = 2 * kMaxTiles + 1, kDescWords = kFusedDescWords + kMaxTiles + 1;
+PHASE_STAMP(__device__ unsigned long long g_sample_stamps[kPhaseSlots];)   // k_sample_fused (device_map.cuh)
 
 // voxel key of sub_sample_frame: static_cast<short>(raw / size) per axis (ct_icp.cpp:70-72)
 __device__ __forceinline__ unsigned long long short_voxel_key(const RawPoint &p, double voxel_size) {
@@ -184,22 +185,35 @@ k_grid_emit(const float4 *__restrict__ pts, const float4 *__restrict__ lo, const
 // A tile only waits on tiles with smaller indices, which are processed by CTAs that are already running: the cooperative
 // launch has every CTA resident and each CTA takes its tiles in ascending order; the standalone kernel hands tiles out
 // in launch order from an atomic ticket.
+// The walk is one warp reading a window of 32 predecessors per L2 round trip (lane j: tile end - 32 + j). The tiles of a
+// launch start together, and a walk of one descriptor per trip took ~sqrt(2t) dependent trips for tile t (16 for the last
+// of the 128 tiles of a 130k-point scan); a window takes at most ceil(t / 32) (3 there). The counts are integers, so every
+// prefix is the one the one-descriptor walk finds. All 32 lanes of one warp; every lane returns the prefix.
 __device__ __forceinline__ uint32_t tile_lookback(unsigned long long *desc, int tile, uint32_t count) {
+    const int lane = threadIdx.x & 31;
     if (tile == 0) {
-        atomicExch(&desc[0], (2ull << 32) | count);
+        if (lane == 0) atomicExch(&desc[0], (2ull << 32) | count);
         return 0u;
     }
-    atomicExch(&desc[tile], (1ull << 32) | count);
+    if (lane == 0) atomicExch(&desc[tile], (1ull << 32) | count);
     uint32_t before = 0;
-    for (int t = tile - 1;;) {
-        const unsigned long long d = *reinterpret_cast<volatile unsigned long long *>(&desc[t]);
-        const uint32_t status = (uint32_t) (d >> 32);
-        if (status == 0u) continue;
-        before += (uint32_t) d;
-        if (status == 2u) break;
-        --t;
+    for (int end = tile;; end -= 32) {
+        const int t = end - 32 + lane;
+        unsigned long long d = 2ull << 32;   // before tile 0: an inclusive prefix of 0 (never the highest: tile 0 is status 2)
+        if (t >= 0) {
+            do d = *reinterpret_cast<volatile unsigned long long *>(&desc[t]);
+            while ((uint32_t) (d >> 32) == 0u);
+        }
+        const uint32_t value = (uint32_t) d;
+        const unsigned inclusive = __ballot_sync(0xffffffffu, (uint32_t) (d >> 32) == 2u);
+        if (inclusive) {   // the highest inclusive prefix in the window plus the counts of the tiles after it
+            const int hi = 31 - __clz(inclusive);
+            before += __reduce_add_sync(0xffffffffu, lane >= hi ? value : 0u);
+            break;
+        }
+        before += __reduce_add_sync(0xffffffffu, value);
     }
-    atomicExch(&desc[tile], (2ull << 32) | (before + count));
+    if (lane == 0) atomicExch(&desc[tile], (2ull << 32) | (before + count));
     return before;
 }
 // the winner at `i` goes to `dst` (alpha override: frames 0 and 1, odometry.cpp:355-359)
@@ -217,11 +231,13 @@ __device__ __forceinline__ void emit_point(const float4 *in, const float4 *in_lo
 }
 // one tile, all kTileThreads threads of the CTA. win != nullptr: the winners' point indices are compacted into win (a
 // second permutation scatters them once their total is known); otherwise the winners themselves are written, compacted.
-// The last tile writes the total to *d_total.
+// The last tile writes the total to *d_total. stamp_slot: -DCTICP_DEBUG_TIMERS builds stamp the start and the end of the
+// look-back in g_sample_stamps[stamp_slot] and [stamp_slot + 1] (-1: no stamps)
 __device__ __forceinline__ void select_tile_dev(int tile, int n, const uint32_t *src, const int *slot_at,
                                                 const unsigned long long *vals, unsigned long long *desc, int *d_total,
                                                 uint32_t *win, const float4 *in, const float4 *in_lo, const uint32_t *in_src,
-                                                float4 *out, float4 *out_lo, uint32_t *out_src, EmitScratch &sc) {
+                                                float4 *out, float4 *out_lo, uint32_t *out_src, EmitScratch &sc,
+                                                int stamp_slot) {
     uint32_t (&s_warp)[kTileThreads / 32] = sc.warp;
     const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
     const int p0 = (tile << kTileShift) + tid * 4;
@@ -246,16 +262,22 @@ __device__ __forceinline__ void select_tile_dev(int tile, int n, const uint32_t 
     __syncthreads();   // s_warp / s_before reuse across tiles
     if (lane == 31) s_warp[w] = incl;
     __syncthreads();
-    if (tid == 0) {
+    if (w == 0) {
         uint32_t run = 0;
-        for (int i = 0; i < kTileThreads / 32; ++i) {
-            const uint32_t c = s_warp[i];
-            s_warp[i] = run;
-            run += c;
-        }
+        if (lane == 0)
+            for (int i = 0; i < kTileThreads / 32; ++i) {
+                const uint32_t c = s_warp[i];
+                s_warp[i] = run;
+                run += c;
+            }
+        run = __shfl_sync(0xffffffffu, run, 0);
+        PHASE_STAMP(if (stamp_slot >= 0 && lane == 0) atomicMax(g_sample_stamps + stamp_slot, phase_clock());)
         const uint32_t before = tile_lookback(desc, tile, run);
-        sc.before = before;
-        if (tile == ((n + kTile - 1) >> kTileShift) - 1) *d_total = (int) (before + run);
+        PHASE_STAMP(if (stamp_slot >= 0 && lane == 0) atomicMax(g_sample_stamps + stamp_slot + 1, phase_clock());)
+        if (lane == 0) {
+            sc.before = before;
+            if (tile == ((n + kTile - 1) >> kTileShift) - 1) *d_total = (int) (before + run);
+        }
     }
     __syncthreads();
     uint32_t excl = sc.before + s_warp[w] + (incl - tsum);
@@ -284,7 +306,7 @@ k_grid_select(const int *__restrict__ d_n, const uint32_t *__restrict__ src, con
         if (tile == 0 && threadIdx.x == 0) *d_total = 0;
         return;
     }
-    select_tile_dev(tile, n, src, slot_at, vals, desc, d_total, win, in, in_lo, in_src, out, out_lo, out_src, sc);
+    select_tile_dev(tile, n, src, slot_at, vals, desc, d_total, win, in, in_lo, in_src, out, out_lo, out_src, sc, -1);
 }
 // the second shuffle: winner k (in first-permutation order) goes to perm2(k)
 __global__ void k_grid_scatter(const int *__restrict__ d_total, const uint32_t *__restrict__ win, const float4 *__restrict__ in,
@@ -335,6 +357,7 @@ k_sample_fused(FusedSampleArgs a) {
     const size_t gtid = (size_t) blockIdx.x * blockDim.x + threadIdx.x, gsize = (size_t) gridDim.x * blockDim.x;
     const int n = a.n, tiles1 = (n + kTile - 1) >> kTileShift;
     unsigned long long *desc1 = a.desc, *desc2 = a.desc + kMaxTiles, *cap2_used = a.desc + 2 * kMaxTiles;
+    PHASE_STAMP(phase_begin(g_sample_stamps);)
     if (blockIdx.x == 0 && threadIdx.x == 0) a.counts[0] = n;
     if (!a.pre_cleared) {
         for (size_t i = gtid; i < 2 * (size_t) a.cap1; i += gsize) a.grid[i] = kGridEmpty;
@@ -345,12 +368,14 @@ k_sample_fused(FusedSampleArgs a) {
     const size_t prev2 = 2 * (size_t) *cap2_used;   // written in phase 3 of the previous launch
     for (size_t i = gtid; i < prev2; i += gsize) a.grid2[i] = kGridEmpty;
     for (size_t i = gtid; i < (size_t) tiles1; i += gsize) desc2[i] = 0ull;   // F <= N: selection 2 has at most tiles1 tiles
+    PHASE_STAMP(phase_end(g_sample_stamps, 1);)
     grid.sync();
     // phase 2
     for (int tile = blockIdx.x; tile < tiles1; tile += gridDim.x)
         select_tile_dev(tile, n, a.src, a.slot_at, a.grid + a.cap1, desc1, a.counts + 1, a.win, nullptr, nullptr, nullptr,
-                        nullptr, nullptr, nullptr, sc);
+                        nullptr, nullptr, nullptr, sc, 2);
     if (tiles1 == 0 && blockIdx.x == 0 && threadIdx.x == 0) a.counts[1] = 0;
+    PHASE_STAMP(phase_end(g_sample_stamps, 4);)
     grid.sync();
     // phase 3
     const uint32_t F = (uint32_t) *reinterpret_cast<volatile int *>(a.counts + 1);
@@ -368,16 +393,19 @@ k_sample_fused(FusedSampleArgs a) {
             a.slot_at[j] = (int) grid_bid(key, ((unsigned long long) j << 32) | j, a.grid2, a.grid2 + cap2, cap2 - 1);
         }
     }
+    PHASE_STAMP(phase_end(g_sample_stamps, 5);)
     grid.sync();
     // phase 4
     const int tiles2 = (int) ((F + kTile - 1) >> kTileShift);
     for (int tile = blockIdx.x; tile < tiles2; tile += gridDim.x)
         select_tile_dev(tile, (int) F, nullptr, a.slot_at, a.grid2 + cap2, desc2, a.counts + 2, nullptr, a.frame, frame_lo,
-                        a.frame_src, a.keypoints, kp_lo, a.kp_src, sc);
+                        a.frame_src, a.keypoints, kp_lo, a.kp_src, sc, 6);
     if (tiles2 == 0 && blockIdx.x == 0 && threadIdx.x == 0) a.counts[2] = 0;
+    PHASE_STAMP(phase_end(g_sample_stamps, 8);)
     for (size_t i = gtid; i < (size_t) tiles1; i += gsize) desc1[i] = 0ull;
     if (a.clear_after)
         for (size_t i = gtid; i < 2 * (size_t) a.cap1; i += gsize) a.grid[i] = kGridEmpty;
+    PHASE_STAMP(phase_end(g_sample_stamps, 9);)
 }
 // ---- adaptive (distance-banded) grid sampling: AdaptiveSamplePointsInGrid, include/ct_icp/algorithm/sampling.h:55-110
 struct AdaptiveBands {
@@ -854,7 +882,18 @@ void FramePipeline::SampleFused(double voxel_size, double sample_voxel_size, uin
     a.frame = d_frame_.data(); a.keypoints = d_keypoints_.data();
     a.frame_src = d_frame_src_.data(); a.kp_src = d_kp_src_.data();
     void *args[] = {&a};
+#ifdef CTICP_DEBUG_TIMERS
+    unsigned long long *stamps = nullptr;
+    CT_CUDA_CHECK(cudaGetSymbolAddress((void **) &stamps, g_sample_stamps));
+    phase_stamps_reset(stamps, stream_);
+#endif
     CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_sample_fused, dim3(fused_grid_), dim3(kTileThreads), args, 0, stream_));
+#ifdef CTICP_DEBUG_TIMERS
+    // sel*_count: the last tile ready to look back; sel*_lookback: the last tile with its prefix; sel*_write: the phase's end
+    static const char *const labels[] = {"claim1", "sel1_count", "sel1_lookback", "sel1_write", "scatter_claim2",
+                                         "sel2_count", "sel2_lookback", "sel2_write", "clear"};
+    phase_stamps_print(stamps, stream_, "k_sample_fused", labels, 9);
+#endif
     launches_ += 1;
 }
 
