@@ -38,6 +38,17 @@ def _as_f64_rows(a, cols):
     return a
 
 
+_SNAPSHOT_HEADER_BYTES = 72   # snapshot_format.h kHeaderBytes
+
+
+def _snapshot_bytes(binding, fn, handle):
+    n = binding.check(binding.fn(fn)(handle, None, 0))
+    buf = C.create_string_buffer(n)
+    m = binding.check(binding.fn(fn)(handle, buf, n))
+    assert m == n, (m, n)
+    return buf.raw
+
+
 class Binding:
     def __init__(self, lib, prefix):
         self.lib = lib
@@ -120,6 +131,11 @@ class Binding:
             "odometry_reset_options": (C.c_int, [vp, P(abi.OdometryOptions)]),
             "odometry_enable_sharding": (C.c_int, [vp, vp, C.c_int, C.c_int]),
             "odometry_sharding_mode": (C.c_int, [vp]),
+            "odometry_save": (i64, [vp, vp, sz]),
+            "odometry_load": (C.c_int, [vp, sz, P(abi.OdometryOptions), C.c_int, P(vp)]),
+            "odometry_clone": (C.c_int, [vp, C.c_int, P(vp)]),
+            "map_save": (i64, [vp, vp, sz]),
+            "map_load": (C.c_int, [vp, sz, C.c_int, P(vp)]),
             # oracle only (KAT taps)
             "odometry_last_counters": (None, [vp, P(u64), P(u64)]),
             "neighborhood_describe": (C.c_int, [vp, sz, vp, P(dbl), P(dbl), P(dbl), vp]),
@@ -184,6 +200,28 @@ class Binding:
 
     def voxel_map(self, options, device=0):
         return VoxelMap(self, options=options, device=device)
+
+    # ---- snapshots -----------------------------------------------------------------------------------------
+    def load_odometry(self, blob, options=None, device=0):
+        """A new Odometry on `device` from the bytes of Odometry.save() (cticp_odometry_load). options None: the saved
+        options, and every later frame registers exactly as on the saved handle; otherwise options may differ from the
+        saved ones only outside map_options (e.g. do_no_insert = 1 to localise against the saved map)."""
+        blob = bytes(blob)
+        h = C.c_void_p()
+        self.check(self.fn("odometry_load")(blob, len(blob), C.byref(options) if options is not None else None, device,
+                                            C.byref(h)))
+        if options is None:   # the options section follows the fixed header (snapshot_format.h)
+            options = abi.OdometryOptions.from_buffer_copy(blob, _SNAPSHOT_HEADER_BYTES)
+        return Odometry._adopt(self, h, options, device)
+
+    def load_voxel_map(self, blob, device=0):
+        """A new standalone VoxelMap on `device` from the bytes of VoxelMap.save() (cticp_map_load)."""
+        blob = bytes(blob)
+        m = VoxelMap.__new__(VoxelMap)
+        m.b, m._owner, m._borrowed, m._free_wrapper = self, None, False, False
+        m.h = C.c_void_p()
+        self.check(self.fn("map_load")(blob, len(blob), device, C.byref(m.h)))
+        return m
 
     # ---- many handles, one frame each ------------------------------------------------------------------------
     def register_batch(self, odometries, scans, frame_ids, initial_estimates=None, motion_models=None):
@@ -340,6 +378,11 @@ class VoxelMap:
     def clear(self):
         self.b.check(self.b.fn("map_clear")(self.h))
 
+    def save(self):
+        """The map's snapshot (cticp_map_save): every table slot, point and normal, loadable bit for bit with
+        Binding.load_voxel_map. For an odometry's map it is the map section of the odometry's snapshot."""
+        return _snapshot_bytes(self.b, "map_save", self.h)
+
     # CT_ICP_Registration::Register(map, keypoints, frame, motion_model), ct_icp.cpp:1026-1037
     def icp_register(self, icp_options, keypoints, frame, previous_frame=None, motion_options=None,
                      strategy=None):
@@ -420,6 +463,24 @@ class Odometry:
         self.device = device
         self.h = C.c_void_p()
         binding.check(binding.fn("odometry_create")(C.byref(self.options), device, C.byref(self.h)))
+
+    @classmethod
+    def _adopt(cls, binding, handle, options, device):
+        od = cls.__new__(cls)
+        od.b, od.options, od.device, od.h = binding, options.copy(), device, handle
+        return od
+
+    def save(self):
+        """The handle's snapshot (cticp_odometry_save): voxel map, trajectory, motion model and counters as bytes;
+        Binding.load_odometry resumes from it bit for bit."""
+        return _snapshot_bytes(self.b, "odometry_save", self.h)
+
+    def clone(self, device=None):
+        """A new Odometry holding the same state, on `device` (None: this handle's), copied device to device."""
+        device = self.device if device is None else device
+        h = C.c_void_p()
+        self.b.check(self.b.fn("odometry_clone")(self.h, device, C.byref(h)))
+        return Odometry._adopt(self.b, h, self.options, device)
 
     def close(self):
         if self.h:

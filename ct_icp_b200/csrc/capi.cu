@@ -455,6 +455,44 @@ int cticp_odometry_reset(cticp_odometry *h) {
     });
 }
 cticp_map *cticp_odometry_map(cticp_odometry *h) { return h ? &h->map_view : nullptr; }
+
+/* ---- snapshots (snapshot.cu, snapshot_format.h) ----------------------------------------------------------------------- */
+static cticp_odometry *WrapEngine(std::unique_ptr<Engine> engine) {
+    auto h = std::make_unique<cticp_odometry>();
+    h->engine = std::move(engine);
+    h->map_view.map = &h->engine->Map();
+    h->map_view.icp = &h->engine->Solver();
+    h->map_view.stream = h->engine->Stream();
+    h->map_view.device = h->engine->Device();
+    h->map_view.owned = false;
+    return h.release();
+}
+int64_t cticp_odometry_save(cticp_odometry *h, void *dst, size_t cap_bytes) {
+    int64_t n = 0;
+    const int rc = Guard([&] {
+        if (!h) throw std::invalid_argument("null handle");
+        n = h->engine->Save(dst, cap_bytes);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : n;
+}
+int cticp_odometry_load(const void *src, size_t n_bytes, const cticp_odometry_options *options, int device,
+                        cticp_odometry **out) {
+    return Guard([&] {
+        if (!src || !out) throw std::invalid_argument("null argument");
+        RequireDevice(device);
+        *out = WrapEngine(Engine::Load(src, n_bytes, options, device));
+        return (int) CTICP_OK;
+    });
+}
+int cticp_odometry_clone(cticp_odometry *h, int device, cticp_odometry **out) {
+    return Guard([&] {
+        if (!h || !out) throw std::invalid_argument("null argument");
+        RequireDevice(device);
+        *out = WrapEngine(h->engine->Clone(device));
+        return (int) CTICP_OK;
+    });
+}
 int cticp_odometry_last_timing(cticp_odometry *h, cticp_device_timing *out) {
     return Guard([&] {
         *out = h->engine->LastTiming();
@@ -698,6 +736,38 @@ int cticp_map_radius_search(cticp_map *m, const double *queries_xyz, const doubl
         CT_CUDA_CHECK(cudaMemcpyAsync(out_points, d_out.data(), sizeof(double) * 3 * n * max_num_neighbors, cudaMemcpyDeviceToHost, m->stream));
         CT_CUDA_CHECK(cudaMemcpyAsync(out_counts, d_cnt.data(), sizeof(int) * n, cudaMemcpyDeviceToHost, m->stream));
         CT_CUDA_CHECK(cudaStreamSynchronize(m->stream));
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_map_save(cticp_map *m, void *dst, size_t cap_bytes) {
+    int64_t n = 0;
+    const int rc = Guard([&] {
+        if (!m) throw std::invalid_argument("null handle");
+        CT_CUDA_CHECK(cudaSetDevice(m->device));
+        CT_CUDA_CHECK(cudaStreamSynchronize(m->stream));   // (an odometry's map: its frames' work is on this stream)
+        n = SaveMap(*m->map, dst, cap_bytes);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : n;
+}
+int cticp_map_load(const void *src, size_t n_bytes, int device, cticp_map **out) {
+    return Guard([&] {
+        if (!src || !out) throw std::invalid_argument("null argument");
+        snap::Parsed p;
+        ValidateMapSnapshot(src, n_bytes, &p);
+        RequireDevice(device);
+        auto m = std::make_unique<cticp_map>();
+        m->device = device;
+        m->owned = true;
+        m->owned_stream = cticp::Stream(cudaStreamNonBlocking);
+        m->stream = m->owned_stream.get();
+        // (the normals the snapshot keeps: an odometry's map keeps them only for the distance-based strategy)
+        m->owned_map = std::make_unique<DeviceMap>(p.map.options, m->stream, p.map.has_normals != 0);
+        m->map = m->owned_map.get();
+        m->owned_icp = std::make_unique<IcpSolver>(m->stream);
+        m->icp = m->owned_icp.get();
+        m->map->LoadSection(p);
+        *out = m.release();
         return (int) CTICP_OK;
     });
 }

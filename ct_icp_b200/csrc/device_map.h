@@ -8,6 +8,7 @@
 #include "../../include/cticp.h"
 #include "cuda_owner.h"
 #include "device_map.cuh"
+#include "snapshot_format.h"
 
 namespace cticp {
 
@@ -75,6 +76,16 @@ public:
     int launches() const { return launches_; }
     int rebuilds() const { return rebuilds_; }
 
+    // snapshots (snapshot.cu, snapshot_format.h). SnapshotMeta: capacities, device counters and frame count of every level
+    // (synchronises the stream; the host copy of the counters is left alone)
+    snap::MapMeta SnapshotMeta() const;
+    // the map section: its header, then the packed levels with one D2H copy, and the frame origins (synchronous)
+    void SaveSection(uint8_t *section, uint8_t *origins, const snap::MapMeta &meta);
+    // a map section that passed snap::Validate: one H2D copy of the packed levels, then Unpack
+    void LoadSection(const snap::Parsed &p);
+    // pack on this map's stream, copy device to device (peer copy when the devices differ), unpack into dst on its stream
+    void CloneInto(DeviceMap &dst, int src_device, int dst_device);
+
 private:
     // the tables a MapLevel points into
     struct LevelStorage {
@@ -85,6 +96,11 @@ private:
     };
     LevelStorage AllocLevel(MapLevel &L, uint32_t cap, const cticp_resolution_param &rp);
     void RebuildLevel(size_t i, uint64_t new_cap);
+    // every level's non-empty slots, point runs and normals into d_out (the map section's payload), in slot order
+    void Pack(unsigned char *d_out, const snap::MapMeta &meta);
+    // the payload back: every level cleared at the snapshot's capacity, each record scattered to its slot and its run to
+    // slot · B; the counters and the frame origins (host or device memory) restored
+    void Unpack(const unsigned char *d_payload, const snap::MapMeta &meta, const double *origins);
     void EnsureScratch(size_t n_upper);
     void EnsureFrameOrigin();
 

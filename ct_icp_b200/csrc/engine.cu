@@ -1288,7 +1288,7 @@ void Engine::ArmTail(double relative_orientation) {
     in.always_insert = options_.always_insert ? 1 : 0;
     // F is still on the device: room for the previous frame's count with head-room (a frame beyond it is
     // deferred to the host-side UpdateMap). Before the ICP is enqueued — a grown table is a new table.
-    const size_t prev_f = (size_t) std::max(0, pipe_->h_counts()[1]);
+    const size_t prev_f = (size_t) PrevFramePoints();
     size_t room = std::min(pipe_->n(), prev_f + prev_f / 2 + 4096);
     if (const char *e = getenv("CTICP_TAIL_ROOM")) room = std::min(room, (size_t) std::max(0, atoi(e)));   // test hook: force the deferred path
     map_->EnsureRoomFor(room);
@@ -1340,6 +1340,7 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
         egress_pending_ = false;
     }
     scan_in_staging_ = staged_slot < 0 && !scan.on_device;
+    frame_events_recorded_ = true;   // ev_[0] is recorded below on every path
 
     // compute_frame_info, odometry.cpp:186-196
     FrameInfo &info = f.info;
@@ -1443,6 +1444,7 @@ void Engine::PrepareFrame(const ScanView &scan, uint32_t frame_id, const cticp_f
 // Phase 3 of a frame, after its ICP launch: the verdict, the assessment, the map update, the summary.
 void Engine::FinishFrame(PendingFrame &f) {
     CT_CUDA_CHECK(cudaSetDevice(device_));
+    restored_prev_frame_points_ = -1;   // (ArmTail of this frame has read it; from now on h_counts()[1] holds the frame's F)
     const size_t n = f.n;
     const auto t_start = f.t_start;
     const FrameInfo &info = f.info;
@@ -1544,7 +1546,9 @@ void Engine::FillSummary(const Summary &s, cticp_summary *out) const {
 
 cticp_device_timing Engine::LastTiming() {
     cudaSetDevice(device_);
-    if (registered_frames_ == 0) {   // nothing recorded yet: querying the events would leave a sticky CUDA error
+    // nothing recorded yet (a fresh handle, or one loaded or cloned from a snapshot before its first frame): querying the
+    // events would leave a sticky CUDA error
+    if (registered_frames_ == 0 || !frame_events_recorded_) {
         cudaStreamSynchronize(stream_.get());
         return timing_;
     }

@@ -215,12 +215,21 @@ public:
     int Device() const { return device_; }
     cticp_device_timing LastTiming();   // synchronises on the last frame's final event
     void SetTimeGather(bool on) { icp_->set_time_gather(on); }
+    // snapshots (snapshot.cu): Save returns the snapshot's size and, with dst, writes it (cap_bytes below the size is
+    // refused); Load builds a handle on `device` from a snapshot (options nullptr: the saved ones); Clone builds one holding
+    // the same state on `device`, copied device to device. All three wait for the work queued on the streams.
+    int64_t Save(void *dst, size_t cap_bytes);
+    static std::unique_ptr<Engine> Load(const void *src, size_t n_bytes, const cticp_odometry_options *options, int device);
+    std::unique_ptr<Engine> Clone(int device);
     void EnableSharding(const void *unique_id, int rank, int world);
     void DestroySharding();
     int ShardingMode() const { return shard_world_ <= 1 ? 0 : (icp_ && icp_->peers_ready() ? 2 : 1); }
 
 private:
     void InitializeMotion(const FrameInfo &info, const cticp_frame *initial_estimate);
+    void DrainStreams();
+    snap::HostState SnapshotHostState() const;
+    void RestoreHostState(const snap::HostState &s, std::vector<HostFrame> trajectory);
     void ResolvePoints(int which, const float4 **out_pts, const float4 **out_lo, const double **out_world, size_t *out_count);
     void CheckSink(const cticp_cloud_sink &sink) const;
     // The owning members below are released in reverse declaration order once the destructor has synchronised stream_:
@@ -304,6 +313,14 @@ private:
         return last_num_keypoints_ ? std::min(pipe_->n(), last_num_keypoints_ + last_num_keypoints_ / 4 + 64) : pipe_->n();
     }
     size_t last_num_keypoints_ = 0;
+    // the previous frame's sub-sampled point count F, which sizes the device tail's head-room (ArmTail): h_counts()[1],
+    // or, on a handle loaded or cloned from a snapshot until its first frame finishes, the saved handle's value (the
+    // pipeline's counts stay those of a fresh handle, so get_points answers as on one)
+    int PrevFramePoints() const {
+        return restored_prev_frame_points_ >= 0 ? restored_prev_frame_points_ : std::max(0, pipe_->h_counts()[1]);
+    }
+    int restored_prev_frame_points_ = -1;
+    bool frame_events_recorded_ = false;   // ev_[0..3] hold a frame's events (LastTiming may query them)
     bool keypoints_in_summary_ = false;   // the last TryRegister's ICP succeeded: RegistrationSummary::keypoints is filled
     static uint64_t ShuffleCounter(int registered_fid, int purpose) {
         return (uint64_t(uint32_t(registered_fid)) << 8) | uint64_t(purpose & 0xff);
@@ -377,6 +394,10 @@ struct BatchItem {
 // One frame on each engine (all distinct, one device, none sharded), the eligible ICP loops in one grouped launch per
 // kind, PendingFrame::joins (cticp_odometry_register_batch has the contract). A failing item ends alone with its exception in `error`.
 void RegisterBatch(std::vector<BatchItem> &items);
+
+// standalone maps (snapshot.cu): the size of the map snapshot and, with dst, the snapshot; a map snapshot's validation
+int64_t SaveMap(DeviceMap &map, void *dst, size_t cap_bytes);
+void ValidateMapSnapshot(const void *src, size_t n_bytes, snap::Parsed *p);
 
 // conversions shared with capi.cu
 HostPose PoseFromC(const cticp_pose &c);

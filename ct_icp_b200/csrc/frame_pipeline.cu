@@ -10,6 +10,7 @@
 // and the second shuffle is one scatter through a second permutation — no sort anywhere.
 #include "frame_pipeline.h"
 #include "scan_pack.cuh"
+#include "tile_lookback.cuh"
 
 #include <cooperative_groups.h>
 #include <cstdlib>
@@ -184,38 +185,7 @@ k_grid_emit(const float4 *__restrict__ pts, const float4 *__restrict__ lo, const
 // inclusive prefix. desc[t] = status << 32 | value, one 64-bit word, so a reader never sees a status without its value.
 // A tile only waits on tiles with smaller indices, which are processed by CTAs that are already running: the cooperative
 // launch has every CTA resident and each CTA takes its tiles in ascending order; the standalone kernel hands tiles out
-// in launch order from an atomic ticket.
-// The walk is one warp reading a window of 32 predecessors per L2 round trip (lane j: tile end - 32 + j). The tiles of a
-// launch start together, and a walk of one descriptor per trip took ~sqrt(2t) dependent trips for tile t (16 for the last
-// of the 128 tiles of a 130k-point scan); a window takes at most ceil(t / 32) (3 there). The counts are integers, so every
-// prefix is the one the one-descriptor walk finds. All 32 lanes of one warp; every lane returns the prefix.
-__device__ __forceinline__ uint32_t tile_lookback(unsigned long long *desc, int tile, uint32_t count) {
-    const int lane = threadIdx.x & 31;
-    if (tile == 0) {
-        if (lane == 0) atomicExch(&desc[0], (2ull << 32) | count);
-        return 0u;
-    }
-    if (lane == 0) atomicExch(&desc[tile], (1ull << 32) | count);
-    uint32_t before = 0;
-    for (int end = tile;; end -= 32) {
-        const int t = end - 32 + lane;
-        unsigned long long d = 2ull << 32;   // before tile 0: an inclusive prefix of 0 (never the highest: tile 0 is status 2)
-        if (t >= 0) {
-            do d = *reinterpret_cast<volatile unsigned long long *>(&desc[t]);
-            while ((uint32_t) (d >> 32) == 0u);
-        }
-        const uint32_t value = (uint32_t) d;
-        const unsigned inclusive = __ballot_sync(0xffffffffu, (uint32_t) (d >> 32) == 2u);
-        if (inclusive) {   // the highest inclusive prefix in the window plus the counts of the tiles after it
-            const int hi = 31 - __clz(inclusive);
-            before += __reduce_add_sync(0xffffffffu, lane >= hi ? value : 0u);
-            break;
-        }
-        before += __reduce_add_sync(0xffffffffu, value);
-    }
-    if (lane == 0) atomicExch(&desc[tile], (2ull << 32) | (before + count));
-    return before;
-}
+// in launch order from an atomic ticket. The walk itself is tile_lookback (tile_lookback.cuh).
 // the winner at `i` goes to `dst` (alpha override: frames 0 and 1, odometry.cpp:355-359)
 __device__ __forceinline__ void emit_point(const float4 *in, const float4 *in_lo, const uint32_t *in_src, uint32_t i, uint32_t dst,
                                            int override_alpha, float alpha_value, float4 *out, float4 *out_lo, uint32_t *out_src) {

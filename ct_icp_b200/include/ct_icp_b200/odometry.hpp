@@ -319,7 +319,36 @@ public:
     const OdometryOptions &Options() const { return options_; }
     cticp_odometry *handle() const { return h_; }
 
+    // Snapshots (cticp_odometry_save / _load / _clone): the whole state of the handle as bytes. A handle loaded with the
+    // saved options (options == nullptr) registers every later frame exactly as this one would have.
+    std::vector<unsigned char> Save() const {
+        const int64_t n = cticp_odometry_save(h_, nullptr, 0);
+        if (n < 0) cticp_check((int) n);
+        std::vector<unsigned char> out((size_t) n);
+        const int64_t m = cticp_odometry_save(h_, out.data(), out.size());
+        if (m < 0) cticp_check((int) m);
+        return out;
+    }
+    static std::unique_ptr<Odometry> Load(const std::vector<unsigned char> &snapshot, const OdometryOptions *options = nullptr,
+                                          int device = 0) {
+        cticp_odometry *h = nullptr;
+        cticp_check(cticp_odometry_load(snapshot.data(), snapshot.size(), options, device, &h));
+        OdometryOptions o;
+        if (options) o = *options;
+        else std::memcpy(&o, snapshot.data() + kSnapshotHeaderBytes, sizeof(o));   // the options section follows the header
+        return std::unique_ptr<Odometry>(new Odometry(h, o));
+    }
+    std::unique_ptr<Odometry> Clone(int device) const {
+        cticp_odometry *h = nullptr;
+        cticp_check(cticp_odometry_clone(h_, device, &h));
+        return std::unique_ptr<Odometry>(new Odometry(h, options_));
+    }
+
 private:
+    static constexpr size_t kSnapshotHeaderBytes = 72;   // ct_icp_b200/csrc/snapshot_format.h kHeaderBytes
+    Odometry(cticp_odometry *h, const OdometryOptions &options) : h_(h), options_(options) {
+        cticp_odometry_set_summary_points(h_, 7);
+    }
     int SummaryMask() const {
         return (copy_back.corrected_points ? 1 : 0) | (copy_back.all_corrected_points ? 2 : 0) | (copy_back.keypoints ? 4 : 0);
     }

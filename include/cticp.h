@@ -446,6 +446,22 @@ int cticp_odometry_reset_options(cticp_odometry *h, const cticp_odometry_options
 /* ct_icp::Odometry::GetMapPointer(), src/ct_icp/odometry.cpp:991-993 (borrowed; owned by the odometry) */
 cticp_map *cticp_odometry_map(cticp_odometry *h);
 
+/* Snapshots (new): the whole state of a handle — voxel map, trajectory, motion model, robust and insertion counters — as
+ * bytes, so that a sequence can be resumed, a map reused and a handle forked. A handle loaded from a snapshot with the
+ * saved options registers every later frame exactly as the handle it was saved from (on GPUs with the same SM count).
+ * save: dst == NULL returns the size; otherwise writes the snapshot (cap_bytes below the size is refused and nothing is
+ * written). Returns the size in bytes or a negative status. Orders itself after all work queued on the handle.
+ * Sharded handles: CTICP_ERR_UNSUPPORTED. */
+int64_t cticp_odometry_save(cticp_odometry *h, void *dst, size_t cap_bytes);
+/* a new handle on `device` from a snapshot; options == NULL: the saved options. Other options may differ from the saved
+ * ones only outside map_options and may not need voxel normals the snapshot does not keep (e.g. do_no_insert = 1 to
+ * localise against a saved map). A malformed snapshot is CTICP_ERR_INVALID_ARGUMENT, before the device is touched. */
+int cticp_odometry_load(const void *src, size_t n_bytes, const cticp_odometry_options *options, int device,
+                        cticp_odometry **out);
+/* a new handle holding the same state, on `device` (this GPU or another), copied device to device: a direct peer copy
+ * when the two GPUs can reach each other, else one the driver stages through host memory */
+int cticp_odometry_clone(cticp_odometry *h, int device, cticp_odometry **out);
+
 /* multi-GPU (new; SURVEY §8e): keypoints sharded rank/world, one exchange (sum over ranks) of JTJ/JTr per GN
  * iteration / LM evaluation. unique_id is the 128-byte ncclUniqueId produced by cticp_nccl_unique_id on rank 0 and
  * broadcast by the caller; NCCL bootstraps NVLink peer mailboxes (CUDA IPC) through which the ICP kernels exchange
@@ -568,6 +584,10 @@ int cticp_map_radius_search(cticp_map *m, const double *queries_xyz, const doubl
                             int32_t *out_counts);
 /* ClearMap(), include/ct_icp/map.h:296 */
 int cticp_map_clear(cticp_map *m);
+/* Snapshots of a map (new): a standalone map or the borrowed map of an odometry (the bytes are the map section of the
+ * odometry's snapshot); sizing and refusals as cticp_odometry_save / _load. A loaded map is a new standalone map. */
+int64_t cticp_map_save(cticp_map *m, void *dst, size_t cap_bytes);
+int cticp_map_load(const void *src, size_t n_bytes, int device, cticp_map **out);
 
 /* ---- Registration (L3 boundary) ------------------------------------------------------------------------- */
 
