@@ -240,6 +240,13 @@ def wpoint_dtype():
                      ("_pad0", "<u4")])
 
 
+# numpy dtype of cticp_pose (72 bytes): the output of ContinuousTrajectory.interpolate
+def pose_dtype():
+    import numpy as np
+    return np.dtype([("quat", "<f8", 4), ("tr", "<f8", 3), ("ref_timestamp", "<f8"), ("dest_timestamp", "<f8"),
+                     ("ref_frame_id", "<u4"), ("dest_frame_id", "<u4")])
+
+
 def frame_to_arrays(frame):
     """cticp_frame → (begin_quat, begin_tr, end_quat, end_tr) as python lists."""
     return (list(frame.begin_pose.quat), list(frame.begin_pose.tr), list(frame.end_pose.quat),

@@ -136,6 +136,12 @@ class Binding:
             "odometry_clone": (C.c_int, [vp, C.c_int, P(vp)]),
             "map_save": (i64, [vp, vp, sz]),
             "map_load": (C.c_int, [vp, sz, C.c_int, P(vp)]),
+            "trajectory_create": (C.c_int, [vp, sz, C.c_int, P(vp)]),
+            "trajectory_destroy": (None, [vp]),
+            "trajectory_poses": (i64, [vp, vp, sz]),
+            "trajectory_interpolate": (C.c_int, [vp, vp, vp, sz, vp]),
+            "trajectory_transform": (i64, [vp, P(abi.CloudView), vp, vp, sz, P(abi.CloudSink)]),
+            "trajectory_transform_device": (i64, [vp, P(abi.DeviceScan), vp, vp, sz, P(abi.CloudSink), vp]),
             # oracle only (KAT taps)
             "odometry_last_counters": (None, [vp, P(u64), P(u64)]),
             "neighborhood_describe": (C.c_int, [vp, sz, vp, P(dbl), P(dbl), P(dbl), vp]),
@@ -222,6 +228,11 @@ class Binding:
         m.h = C.c_void_p()
         self.check(self.fn("map_load")(blob, len(blob), device, C.byref(m.h)))
         return m
+
+    def continuous_trajectory(self, poses_or_frames, device=0):
+        """slam::LinearContinuousTrajectory::Create (cticp_trajectory_create) of abi.Pose items, or of abi.Frame items
+        (each contributes its begin and end pose, e.g. Odometry.Trajectory())."""
+        return ContinuousTrajectory(self, poses_or_frames, device)
 
     # ---- many handles, one frame each ------------------------------------------------------------------------
     def register_batch(self, odometries, scans, frame_ids, initial_estimates=None, motion_models=None):
@@ -725,3 +736,140 @@ class Odometry:
     def sharding_mode(self):
         """0 = single GPU, 1 = NCCL all-reduce per exchange, 2 = in-kernel exchange over NVLink peer mailboxes."""
         return self.b.fn("odometry_sharding_mode")(self.h)
+
+
+class ContinuousTrajectory:
+    """slam::LinearContinuousTrajectory (include/SlamCore/trajectory.h:28-130) behind the C ABI: the sorted poses, the
+    pose at any timestamp, and RawPointsToWorldPoints (src/SlamCore/pointcloud.cxx:313-326) of host or device points."""
+
+    def __init__(self, binding, poses_or_frames, device=0):
+        self.b = binding
+        self.device = device
+        poses = []
+        for item in poses_or_frames:
+            if isinstance(item, abi.Frame):
+                poses += [item.begin_pose, item.end_pose]
+            elif isinstance(item, abi.Pose):
+                poses.append(item)
+            else:
+                raise TypeError("expected abi.Pose or abi.Frame items, got %r" % type(item))
+        arr = (abi.Pose * max(len(poses), 1))()
+        for i, p in enumerate(poses):
+            C.memmove(C.addressof(arr[i]), C.addressof(p), C.sizeof(abi.Pose))
+        self.h = C.c_void_p()
+        binding.check(binding.fn("trajectory_create")(arr, len(poses), device, C.byref(self.h)))
+
+    def close(self):
+        if self.h:
+            self.b.fn("trajectory_destroy")(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def poses(self):
+        """Poses(): sorted by (dest_frame_id, dest_timestamp), as a structured array of abi.pose_dtype()"""
+        n = self.b.check(self.b.fn("trajectory_poses")(self.h, None, 0))
+        out = np.zeros(n, dtype=abi.pose_dtype())
+        self.b.check(self.b.fn("trajectory_poses")(self.h, out.ctypes.data, n))
+        return out
+
+    def interpolate(self, timestamps, frame_ids=None):
+        """InterpolatePose(t) of every timestamp, or InterpolatePoseWithFrameId(t, frame_id) when frame_ids is given
+        (one per timestamp); a structured array of abi.pose_dtype()."""
+        ts = np.ascontiguousarray(timestamps, dtype=np.float64).reshape(-1)
+        fid = None
+        if frame_ids is not None:
+            fid = np.ascontiguousarray(frame_ids, dtype=np.uint32).reshape(-1)
+            if len(fid) != len(ts):
+                raise ValueError("frame_ids must have one entry per timestamp")
+        out = np.zeros(len(ts), dtype=abi.pose_dtype())
+        self.b.check(self.b.fn("trajectory_interpolate")(self.h, ts.ctypes.data, fid.ctypes.data if fid is not None else None,
+                                                         len(ts), out.ctypes.data))
+        return out
+
+    @staticmethod
+    def _segments(segments, n):
+        """segments: None, or (ends, frame_ids): segment s holds points [ends[s-1], ends[s]) of frame frame_ids[s]"""
+        if segments is None:
+            return None, None, 0
+        ends, fids = segments
+        ends = np.ascontiguousarray(ends, dtype=np.uint64).reshape(-1)
+        fids = np.ascontiguousarray(fids, dtype=np.uint32).reshape(-1)
+        if len(ends) != len(fids):
+            raise ValueError("segment ends and frame ids must have the same length")
+        return ends, fids, len(ends)
+
+    def transform_records(self, records, sink, segments=None):
+        """cticp_trajectory_transform of a 1-D structured host array (fields x, y, z contiguous of one float type and t)
+        into `sink`, a 1-D structured host array with x, y, z and optionally t; returns the number of points."""
+        view = Odometry._cloud_view(records)
+        f = sink.dtype.fields
+        has_t = "t" in f
+        cs = abi.CloudSink(sink.ctypes.data, len(sink), sink.dtype.itemsize, f["x"][1], abi.DTYPE[f["x"][0].name],
+                           f["t"][1] if has_t else 0, abi.DTYPE[f["t"][0].name] if has_t else 0, 1)
+        ends, fids, ns = self._segments(segments, len(records))
+        return self.b.check(self.b.fn("trajectory_transform")(
+            self.h, C.byref(view), ends.ctypes.data if ns else None, fids.ctypes.data if ns else None, ns, C.byref(cs)))
+
+    def transform_device(self, scan, sink, segments=None, stream=0):
+        """cticp_trajectory_transform_device of an abi.DeviceScan into an abi.CloudSink in device memory"""
+        ends, fids, ns = self._segments(segments, scan.num_points)
+        return self.b.check(self.b.fn("trajectory_transform_device")(
+            self.h, C.byref(scan), ends.ctypes.data if ns else None, fids.ctypes.data if ns else None, ns, C.byref(sink),
+            C.c_void_p(stream or None)))
+
+    def transform(self, xyz, t, segments=None, dtype=np.float64, with_timestamps=False):
+        """World coordinates of raw points xyz (N, 3) with timestamps t (N,): TransformPoint(raw, t) of every point, or
+        TransformPoint(raw, t, frame_id) with segments = (ends, frame_ids) for N scans concatenated.
+        NumPy arrays: the host path, returns an (N, 3) array of `dtype` ((N, 4) with the timestamps).
+        torch CUDA tensors on the trajectory's device (xyz (N, >=3) float32 / float64 with unit column stride, t 1-D of any
+        supported dtype): the device path, read after and written before the work of torch's current stream; returns a
+        CUDA tensor."""
+        if _is_cuda_tensor(xyz) or _is_cuda_tensor(t):
+            return self._transform_tensors(xyz, t, segments, dtype, with_timestamps)
+        xyz = np.asarray(xyz)
+        t = np.asarray(t).reshape(-1)
+        if xyz.ndim != 2 or xyz.shape[1] < 3 or xyz.dtype not in (np.float32, np.float64):
+            raise ValueError("xyz must be an (N, >=3) float32 / float64 array")
+        if len(xyz) != len(t):
+            raise ValueError("xyz and t must have the same length")
+        rec = np.zeros(len(xyz), dtype=np.dtype([("x", xyz.dtype), ("y", xyz.dtype), ("z", xyz.dtype), ("t", t.dtype)]))
+        rec["x"], rec["y"], rec["z"], rec["t"] = xyz[:, 0], xyz[:, 1], xyz[:, 2], t
+        dtype = np.dtype(dtype)
+        fields = [("x", dtype), ("y", dtype), ("z", dtype)] + ([("t", dtype)] if with_timestamps else [])
+        out = np.zeros(len(xyz), dtype=np.dtype(fields))
+        self.transform_records(rec, out, segments)
+        return out.view(dtype).reshape(len(xyz), len(fields))
+
+    def _transform_tensors(self, xyz, t, segments, dtype, with_timestamps):
+        import torch
+        if not (_is_cuda_tensor(xyz) and _is_cuda_tensor(t)):
+            raise ValueError("xyz and t must both be CUDA tensors (or both host arrays)")
+        if xyz.device.index != self.device or t.device.index != self.device:
+            raise ValueError("xyz and t must be on cuda:%d, the trajectory's device" % self.device)
+        if xyz.dim() != 2 or xyz.shape[1] < 3 or xyz.stride(1) != 1 or xyz.dtype not in (torch.float32, torch.float64):
+            raise ValueError("xyz must be an (N, >=3) float32 / float64 tensor with unit column stride")
+        codes = _torch_dtype_codes(torch)
+        if t.dim() != 1 or t.dtype not in codes:
+            raise ValueError("t must be a 1-D tensor of a supported dtype")
+        if xyz.shape[0] != t.shape[0]:
+            raise ValueError("xyz and t must have the same length")
+        tdtype = {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64}.get(np.dtype(dtype), dtype)
+        if tdtype not in (torch.float32, torch.float64):
+            raise ValueError("dtype must be float32 or float64")
+        n = xyz.shape[0]
+        scan = abi.DeviceScan(xyz.data_ptr(), xyz.stride(0) * xyz.element_size(), t.data_ptr(),
+                              t.stride(0) * t.element_size(), n, codes[xyz.dtype], codes[t.dtype])
+        cols = 4 if with_timestamps else 3
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        out = torch.empty((n, cols), dtype=tdtype, device=torch.device("cuda", self.device))
+        code = abi.DTYPE["float32" if tdtype == torch.float32 else "float64"]
+        size = out.element_size()
+        sink = abi.CloudSink(out.data_ptr() if n else None, n, cols * size, 0, code, 3 * size,
+                             code if with_timestamps else 0, 1)
+        self.transform_device(scan, sink, segments, stream)
+        return out

@@ -8,6 +8,7 @@
 
 #include "../../include/cticp.h"
 #include "engine.h"
+#include "trajectory.h"
 
 using namespace cticp;
 
@@ -68,6 +69,9 @@ struct cticp_map {
 struct cticp_odometry {
     std::unique_ptr<Engine> engine;
     cticp_map map_view;
+};
+struct cticp_trajectory {
+    std::unique_ptr<ContinuousTrajectory> impl;
 };
 
 extern "C" {
@@ -614,6 +618,56 @@ int cticp_odometry_enable_sharding(cticp_odometry *h, const void *unique_id_128_
     });
 }
 int cticp_odometry_sharding_mode(cticp_odometry *h) { return h->engine->ShardingMode(); }
+
+/* ---- continuous trajectories (trajectory.cu) ------------------------------------------------------------------------ */
+int cticp_trajectory_create(const cticp_pose *poses, size_t n, int device, cticp_trajectory **out) {
+    return Guard([&] {
+        if (!poses || !out) throw std::invalid_argument("null argument");
+        RequireDevice(device);
+        auto t = std::make_unique<cticp_trajectory>();
+        t->impl = std::make_unique<ContinuousTrajectory>(poses, n, device);
+        *out = t.release();
+        return (int) CTICP_OK;
+    });
+}
+void cticp_trajectory_destroy(cticp_trajectory *t) { delete t; }
+int64_t cticp_trajectory_poses(cticp_trajectory *t, cticp_pose *dst, size_t cap) {
+    if (!t) return Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+    const auto &p = t->impl->Poses();
+    const size_t m = std::min(cap, p.size());
+    for (size_t i = 0; i < m && dst; ++i) dst[i] = p[i];
+    return (int64_t) p.size();
+}
+int cticp_trajectory_interpolate(cticp_trajectory *t, const double *timestamps, const uint32_t *frame_ids, size_t m,
+                                 cticp_pose *out) {
+    return Guard([&] {
+        if (!t) throw std::invalid_argument("null handle");
+        t->impl->Interpolate(timestamps, frame_ids, m, out);
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_trajectory_transform(cticp_trajectory *t, const cticp_cloud_view *cloud, const uint64_t *segment_ends,
+                                   const uint32_t *segment_frame_ids, size_t num_segments, const cticp_cloud_sink *sink) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!t || !cloud || !sink) throw std::invalid_argument("null argument");
+        count = t->impl->Transform(*cloud, segment_ends, segment_frame_ids, num_segments, *sink);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int64_t cticp_trajectory_transform_device(cticp_trajectory *t, const cticp_device_scan *scan, const uint64_t *segment_ends,
+                                          const uint32_t *segment_frame_ids, size_t num_segments,
+                                          const cticp_cloud_sink *sink, void *stream) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!t || !scan || !sink) throw std::invalid_argument("null argument");
+        count = t->impl->TransformDevice(*scan, segment_ends, segment_frame_ids, num_segments, *sink,
+                                         static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
 
 /* ---- Map ----------------------------------------------------------------------------------------------------- */
 int cticp_map_create(const cticp_map_options *options, int device, cticp_map **out) {

@@ -1,5 +1,6 @@
 // engine.cu — host orchestration of the H100-native odometry (see engine.h).
 #include "engine.h"
+#include "device_checks.h"
 #include "scan_pack.cuh"
 
 #include <algorithm>
@@ -13,7 +14,6 @@
 #include <emmintrin.h>
 #include <xmmintrin.h>
 
-#include <cudaTypedefs.h>   // PFN_cuMemGetAddressRange (types only: the driver is reached through cudart)
 #include <nvtx3/nvToolsExt.h>   // header-only: ranges are no-ops unless a profiler injects the NVTX library
 
 namespace cticp {
@@ -1574,43 +1574,7 @@ cticp_device_timing Engine::LastTiming() {
 }
 
 // ---- a scan in device memory / point vectors into device memory ------------------------------------------------------
-namespace {
-// [p, p + bytes) must be device (or managed) memory of `device`, inside one allocation: a short buffer is an error here,
-// not a fault in a kernel. The library links cudart statically: the driver's cuMemGetAddressRange comes through the
-// runtime's entry-point query.
-void RequireDeviceRange(const void *p, uint64_t bytes, int device, const char *what) {
-    cudaPointerAttributes a{};
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-        cudaGetLastError();
-        throw std::invalid_argument(std::string(what) + ": not a CUDA pointer");
-    }
-    if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != device)
-        throw std::invalid_argument(std::string(what) + ": not device memory of the handle's device");
-    static PFN_cuMemGetAddressRange get_range = [] {
-        void *fn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-            q != cudaDriverEntryPointSuccess)
-            fn = nullptr;
-        return reinterpret_cast<PFN_cuMemGetAddressRange>(fn);
-    }();
-    if (!get_range) throw CudaError("cuMemGetAddressRange is not available");
-    CUdeviceptr base = 0;
-    size_t size = 0;
-    if (get_range(&base, &size, (CUdeviceptr) reinterpret_cast<uintptr_t>(p)) != CUDA_SUCCESS)
-        throw std::invalid_argument(std::string(what) + ": not inside a device allocation");
-    const uint64_t off = (uint64_t) reinterpret_cast<uintptr_t>(p) - (uint64_t) base;
-    if (bytes > size || off > size - bytes)
-        throw std::invalid_argument(std::string(what) + ": the described buffer extends past the end of its allocation");
-}
-// bytes spanned by n records of `width` bytes every `stride` bytes
-uint64_t SpanBytes(uint64_t n, uint64_t stride, uint64_t width, const char *what) {
-    uint64_t span = 0;
-    if (__builtin_mul_overflow(n - 1, stride, &span) || __builtin_add_overflow(span, width, &span))
-        throw std::invalid_argument(std::string(what) + ": the described buffer overflows the address space");
-    return span;
-}
-}  // namespace
+// (RequireDeviceRange, SpanBytes, CheckSink: device_checks.cu)
 
 void Engine::RegisterDevice(ScanView scan, cudaStream_t producer, uint32_t frame_id, const cticp_frame *initial_estimate,
                             cticp_summary *out, const cticp_motion_prior *motion_model) {
@@ -1633,17 +1597,6 @@ void Engine::BeginDevice(ScanView scan, cudaStream_t producer, uint32_t frame_id
     scan.on_device = true;
     scan.producer = producer;
     PrepareFrame(scan, frame_id, initial_estimate, -1, out, motion_model, f);
-}
-
-void Engine::CheckSink(const cticp_cloud_sink &sink) const {
-    const size_t xs = sink.xyz_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8;
-    if (sink.xyz_dtype != CTICP_DTYPE_FLOAT32 && sink.xyz_dtype != CTICP_DTYPE_FLOAT64)
-        throw std::invalid_argument("sink: x/y/z must be FLOAT32 or FLOAT64");
-    if (sink.t_dtype != 0 && sink.t_dtype != CTICP_DTYPE_FLOAT32 && sink.t_dtype != CTICP_DTYPE_FLOAT64)
-        throw std::invalid_argument("sink: timestamp must be FLOAT32 or FLOAT64");
-    if ((size_t) sink.xyz_offset + 3 * xs > sink.point_step ||
-        (sink.t_dtype && (size_t) sink.t_offset + (sink.t_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8) > sink.point_step))
-        throw std::invalid_argument("sink: a field lies outside the record (point_step)");
 }
 
 int64_t Engine::WritePointsDevice(int which, const cticp_cloud_sink &sink, cudaStream_t consumer) {

@@ -231,7 +231,6 @@ private:
     snap::HostState SnapshotHostState() const;
     void RestoreHostState(const snap::HostState &s, std::vector<HostFrame> trajectory);
     void ResolvePoints(int which, const float4 **out_pts, const float4 **out_lo, const double **out_world, size_t *out_count);
-    void CheckSink(const cticp_cloud_sink &sink) const;
     // The owning members below are released in reverse declaration order once the destructor has synchronised stream_:
     // stream_ comes first so that it is destroyed after everything that was enqueued on it, the egress stream after its
     // events and buffers.

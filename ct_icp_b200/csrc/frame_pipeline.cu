@@ -9,6 +9,7 @@
 //   output order  = ascending perm(i) of the winners                   [flag array in permuted index space + scan]
 // and the second shuffle is one scatter through a second permutation — no sort anywhere.
 #include "frame_pipeline.h"
+#include "record_io.cuh"
 #include "scan_pack.cuh"
 #include "tile_lookback.cuh"
 
@@ -506,35 +507,7 @@ struct ScanPartial {
     double mn, mx;
     int lo, pad;
 };
-// x, y, z of one record: byte-assembled (any address), natural scalar loads, or one 16-byte load (float32, 16-aligned)
-enum { kLoadBytes = 0, kLoadNatural = 1, kLoadVec4 = 2 };
-template <typename XT, int LOAD>
-__device__ __forceinline__ void load_xyz(const unsigned char *p, XT &x, XT &y, XT &z) {
-    if constexpr (LOAD == kLoadVec4) {
-        const float4 v = __ldg(reinterpret_cast<const float4 *>(p));
-        x = v.x; y = v.y; z = v.z;
-    } else if constexpr (LOAD == kLoadNatural) {
-        const XT *q = reinterpret_cast<const XT *>(p);
-        x = __ldg(q); y = __ldg(q + 1); z = __ldg(q + 2);
-    } else {
-        x = scan_pack::load_unaligned<XT>(p);
-        y = scan_pack::load_unaligned<XT>(p + sizeof(XT));
-        z = scan_pack::load_unaligned<XT>(p + 2 * sizeof(XT));
-    }
-}
-__device__ __forceinline__ double load_timestamp(const unsigned char *p, int dtype, bool aligned) {
-    if (!aligned) return scan_pack::decode_timestamp(p, dtype);
-    switch (dtype) {
-        case CTICP_DTYPE_INT8: return (double) *reinterpret_cast<const int8_t *>(p);
-        case CTICP_DTYPE_UINT8: return (double) *p;
-        case CTICP_DTYPE_INT16: return (double) __ldg(reinterpret_cast<const short *>(p));
-        case CTICP_DTYPE_UINT16: return (double) __ldg(reinterpret_cast<const unsigned short *>(p));
-        case CTICP_DTYPE_INT32: return (double) __ldg(reinterpret_cast<const int *>(p));
-        case CTICP_DTYPE_UINT32: return (double) __ldg(reinterpret_cast<const unsigned *>(p));
-        case CTICP_DTYPE_FLOAT32: return (double) __ldg(reinterpret_cast<const float *>(p));
-        default: return __ldg(reinterpret_cast<const double *>(p));
-    }
-}
+// (load_xyz, load_timestamp and store_field: record_io.cuh)
 // timestamp min / max (NaN skipped, as by the host's comparisons) and, for float64 x, y, z, whether some coordinate is not
 // float32-representable. Per-CTA partials; the last CTA combines them in CTA order and publishes the result to device
 // memory (read by k_scan_pack) and to mapped pinned memory, sequence number last (read by the host).
@@ -615,10 +588,6 @@ __global__ void __launch_bounds__(kScanThreads) k_scan_pack(const unsigned char 
     }
 }
 // one of the summary's vectors into the caller's record layout: the fields of cticp_odometry_write_points, nothing else
-template <typename T> __device__ __forceinline__ void store_field(unsigned char *p, T v, bool aligned) {
-    if (aligned) *reinterpret_cast<T *>(p) = v;
-    else scan_pack::store_unaligned<T>(p, v);
-}
 __global__ void __launch_bounds__(kScanThreads) k_write_points(const float4 *__restrict__ pts, const float4 *__restrict__ lo,
                                                                const double *__restrict__ world, int m,
                                                                unsigned char *__restrict__ data, uint32_t step,

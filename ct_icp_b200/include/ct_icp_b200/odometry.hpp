@@ -17,6 +17,7 @@
 #include <cmath>
 #include <cstdint>
 #include <cstring>
+#include <limits>
 #include <map>
 #include <memory>
 #include <stdexcept>
@@ -466,3 +467,126 @@ private:
 };
 
 }  // namespace ct_icp
+
+namespace slam {
+
+// slam::LinearContinuousTrajectory (include/SlamCore/trajectory.h:28-130) over cticp_trajectory_*: the sorted poses live on
+// a device, which evaluates every lookup, interpolation and point transform (semantics: include/cticp.h). Move-only.
+class LinearContinuousTrajectory {
+public:
+    // Create(poses, check_consistency = true) on CUDA device `device`; throws ct_icp::CticpFailure where the reference's
+    // CheckConsistency would fail (CTICP_ERR_INVALID_ARGUMENT)
+    static LinearContinuousTrajectory Create(std::vector<Pose> &&poses, int device = 0) {
+        std::vector<cticp_pose> c;
+        c.reserve(poses.size());
+        for (const Pose &p : poses) c.push_back(ct_icp::detail::pose_to_c(p));
+        LinearContinuousTrajectory t;
+        ct_icp::cticp_check(cticp_trajectory_create(c.data(), c.size(), device, &t.h_));
+        const int64_t n = cticp_trajectory_poses(t.h_, nullptr, 0);
+        c.resize((size_t) n);
+        cticp_trajectory_poses(t.h_, c.data(), c.size());
+        // Create (trajectory.cxx:170-177): the maximum starts at numeric_limits<double>::min(), as the reference's does
+        t.min_ts_ = std::numeric_limits<double>::max();
+        t.max_ts_ = std::numeric_limits<double>::min();
+        for (const cticp_pose &p : c) {
+            t.poses_.push_back(ct_icp::detail::pose_from_c(p));
+            if (p.dest_timestamp < t.min_ts_) t.min_ts_ = p.dest_timestamp;
+            if (p.dest_timestamp > t.max_ts_) t.max_ts_ = p.dest_timestamp;
+        }
+        return t;
+    }
+    LinearContinuousTrajectory(LinearContinuousTrajectory &&o) noexcept
+        : h_(std::exchange(o.h_, nullptr)), poses_(std::move(o.poses_)), min_ts_(o.min_ts_), max_ts_(o.max_ts_) {}
+    LinearContinuousTrajectory &operator=(LinearContinuousTrajectory &&o) noexcept {
+        if (this != &o) {
+            if (h_) cticp_trajectory_destroy(h_);
+            h_ = std::exchange(o.h_, nullptr);
+            poses_ = std::move(o.poses_);
+            min_ts_ = o.min_ts_;
+            max_ts_ = o.max_ts_;
+        }
+        return *this;
+    }
+    LinearContinuousTrajectory(const LinearContinuousTrajectory &) = delete;
+    LinearContinuousTrajectory &operator=(const LinearContinuousTrajectory &) = delete;
+    ~LinearContinuousTrajectory() {
+        if (h_) cticp_trajectory_destroy(h_);
+    }
+
+    const std::vector<Pose> &Poses() const { return poses_; }
+    double MinTimestamp() const { return min_ts_; }
+    double MaxTimestamp() const { return max_ts_; }
+
+    // clip_on_bounds: only true is built (the value every point transform of the reference uses)
+    Pose InterpolatePose(double timestamp, bool clip_on_bounds = true) const {
+        RequireClip(clip_on_bounds);
+        cticp_pose out;
+        ct_icp::cticp_check(cticp_trajectory_interpolate(h_, &timestamp, nullptr, 1, &out));
+        return ct_icp::detail::pose_from_c(out);
+    }
+    Pose InterpolatePoseWithFrameId(double timestamp, int frame_id, bool clip_on_bounds = true) const {
+        RequireClip(clip_on_bounds);
+        const uint32_t fid = (uint32_t) frame_id;
+        cticp_pose out;
+        ct_icp::cticp_check(cticp_trajectory_interpolate(h_, &timestamp, &fid, 1, &out));
+        return ct_icp::detail::pose_from_c(out);
+    }
+    // TransformPoint (trajectory.cxx:143-155): quat.normalized() * raw + tr of the interpolated pose
+    Vec3d TransformPoint(const Vec3d &relative_point, double timestamp) const {
+        return Transform(relative_point, timestamp, nullptr);
+    }
+    Vec3d TransformPoint(const Vec3d &relative_point, double timestamp, int frame_id) const {
+        const uint32_t fid = (uint32_t) frame_id;
+        return Transform(relative_point, timestamp, &fid);
+    }
+
+    cticp_trajectory *Handle() const { return h_; }
+
+private:
+    LinearContinuousTrajectory() = default;
+    static void RequireClip(bool clip_on_bounds) {
+        if (!clip_on_bounds) throw ct_icp::CticpFailure(CTICP_ERR_UNSUPPORTED, "clip_on_bounds = false is not built");
+    }
+    Vec3d Transform(const Vec3d &p, double t, const uint32_t *fid) const {
+        struct {
+            double xyz[3], t;
+        } rec{{p[0], p[1], p[2]}, t};
+        Vec3d w;
+        const cticp_cloud_view view{&rec, 1, sizeof(rec), 0, CTICP_DTYPE_FLOAT64, 24, CTICP_DTYPE_FLOAT64, 0};
+        const cticp_cloud_sink sink{w.v, 1, sizeof(w.v), 0, CTICP_DTYPE_FLOAT64, 0, 0, 1};
+        const uint64_t end = 1;
+        const int64_t rc = cticp_trajectory_transform(h_, &view, fid ? &end : nullptr, fid, fid ? 1 : 0, &sink);
+        if (rc < 0) ct_icp::cticp_check((int) rc);
+        return w;
+    }
+
+    cticp_trajectory *h_ = nullptr;
+    std::vector<Pose> poses_;
+    double min_ts_ = 0, max_ts_ = 0;
+};
+
+// PointCloud::RawPointsToWorldPoints(const LinearContinuousTrajectory&) (src/SlamCore/pointcloud.cxx:313-326) on the
+// reference's point vector: world_point of every point from its raw point and timestamp, in one device launch. Each run of
+// points with the same index_frame is looked up with that frame id (InterpolatePoseWithFrameId), so N scans concatenated
+// take each scan's own poses even where two frames share a timestamp.
+inline void RawPointsToWorldPoints(std::vector<WPoint3D> &points, const LinearContinuousTrajectory &trajectory) {
+    if (points.empty()) return;
+    std::vector<uint64_t> ends;
+    std::vector<uint32_t> fids;
+    for (size_t i = 0; i < points.size(); ++i) {
+        if (i > 0 && points[i].index_frame != points[i - 1].index_frame) {
+            ends.push_back(i);
+            fids.push_back(points[i - 1].index_frame);
+        }
+    }
+    ends.push_back(points.size());
+    fids.push_back(points.back().index_frame);
+    // the records are read and written in place: raw xyz at 0, timestamp at 24, world xyz at 32 (cticp_wpoint)
+    const cticp_cloud_view view{points.data(), points.size(), sizeof(WPoint3D), 0, CTICP_DTYPE_FLOAT64, 24,
+                                CTICP_DTYPE_FLOAT64, 0};
+    const cticp_cloud_sink sink{points.data(), points.size(), sizeof(WPoint3D), 32, CTICP_DTYPE_FLOAT64, 0, 0, 1};
+    const int64_t rc = cticp_trajectory_transform(trajectory.Handle(), &view, ends.data(), fids.data(), ends.size(), &sink);
+    if (rc < 0) ct_icp::cticp_check((int) rc);
+}
+
+}  // namespace slam

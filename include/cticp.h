@@ -553,6 +553,54 @@ int cticp_odometry_set_gather_timing(cticp_odometry *h, int on);
 /* writes `bytes` of device memory (> L2 size flushes the L2) on the handle's stream */
 int cticp_odometry_flush_l2(cticp_odometry *h, size_t bytes);
 
+/* ---- Continuous trajectories (slam::LinearContinuousTrajectory, include/SlamCore/trajectory.h:28-130) -----------------
+ * A sorted list of poses on one device, the pose at any timestamp, and RawPointsToWorldPoints
+ * (src/SlamCore/pointcloud.cxx:313-326) over point records in host or device memory. Build one from
+ * cticp_odometry_trajectory: the begin and end pose of every frame. Semantics are the reference's
+ * (src/SlamCore/trajectory.cxx), including its quirks:
+ *   - Create sorts by (dest_frame_id, dest_timestamp), keeping poses with equal keys in their input order; MaxTimestamp
+ *     starts at DBL_MIN (the smallest positive double), as the reference's does.
+ *   - lookups clip on bounds: a timestamp with MinTimestamp >= t && t >= MaxTimestamp (sic, trajectory.cxx:58) takes the
+ *     first pose when t <= MinTimestamp, else the last; past the last pose, the last pose; a NaN timestamp, pose 0.
+ *   - equal lookup indices return that pose unchanged; otherwise alpha is GetAlphaTimestamp (below the pair → 0, above the
+ *     pair → 0, equal timestamps → 1) and the pose is slerp (not renormalised) + lerp; dest_timestamp is the lerp of the
+ *     two timestamps, dest_frame_id and ref_* come from the lower pose. A point is quat.normalized() * raw + tr of it.
+ *   - by frame id: lower_bound on (dest_frame_id, dest_timestamp) and the pose before it; a frame id between the frames
+ *     present takes the pair around where it would sort.
+ * All arithmetic is fp64, and coordinates and timestamps are read in fp64: no fp32 packing and no alpha rounding (unlike
+ * the point vectors of a registration). The device slerp agrees with libm's to the last bit or two. */
+typedef struct cticp_trajectory cticp_trajectory;   /* opaque: one device, its own stream */
+/* LinearContinuousTrajectory::Create(poses, check_consistency = true). CTICP_ERR_INVALID_ARGUMENT: no poses, a pose whose
+ * ref_frame_id differs from the first (sorted) pose's, a timestamp that decreases where dest_frame_id changes, a NaN
+ * dest_timestamp. Sorts and uploads the poses and computes the slerp constants of every adjacent pair on the device. */
+int cticp_trajectory_create(const cticp_pose *poses, size_t n, int device, cticp_trajectory **out);
+void cticp_trajectory_destroy(cticp_trajectory *t);
+/* Poses(): the sorted poses; copies min(cap, count), returns the count */
+int64_t cticp_trajectory_poses(cticp_trajectory *t, cticp_pose *dst, size_t cap);
+/* InterpolatePose(timestamps[i], true) (frame_ids == NULL) or InterpolatePoseWithFrameId(timestamps[i], frame_ids[i],
+ * true) of m host timestamps into out[m]. A frame id above every pose's whose query the bounds check does not clip is
+ * CTICP_ERR_INVALID_ARGUMENT (the reference's CHECK), and nothing is written. */
+int cticp_trajectory_interpolate(cticp_trajectory *t, const double *timestamps, const uint32_t *frame_ids, size_t m,
+                                 cticp_pose *out);
+/* RawPointsToWorldPoints of the records of `cloud` (host memory; the dtypes, strides and unaligned records that
+ * cticp_odometry_register_cloud accepts) into `sink` (host memory, world = 1 required): x, y, z in the world frame as
+ * FLOAT32 or FLOAT64 and, when sink->t_dtype != 0, the input timestamp. Writes min(capacity_points, num_points) records
+ * and returns num_points. Segments (optional, num_segments = 0 for none): segment s holds points
+ * [segment_ends[s-1], segment_ends[s]) of frame segment_frame_ids[s] (segment_ends[-1] = 0) and its points are looked up
+ * with that frame id; without segments the lookup is by timestamp. The records and the sink are copied to the device as
+ * they are, so the sink's bytes outside its fields are kept; the bytes written are those of cticp_trajectory_transform_device.
+ * CTICP_ERR_INVALID_ARGUMENT, before anything is written: null pointers, unknown dtypes, fields outside point_step,
+ * sink->world == 0, segment ends that decrease or whose last one is not num_points, a frame id above every pose's. */
+int64_t cticp_trajectory_transform(cticp_trajectory *t, const cticp_cloud_view *cloud, const uint64_t *segment_ends,
+                                   const uint32_t *segment_frame_ids, size_t num_segments, const cticp_cloud_sink *sink);
+/* The same on a scan and a sink in device memory of the trajectory's device: enqueued after the work already queued on
+ * `stream` (a cudaStream_t; NULL = the legacy default stream), which is made to wait for the result; no host
+ * synchronisation. In addition to the checks above: pointers that are not device memory of the trajectory's device, or
+ * a described buffer that extends past its allocation (CTICP_ERR_INVALID_ARGUMENT), checked before anything is enqueued. */
+int64_t cticp_trajectory_transform_device(cticp_trajectory *t, const cticp_device_scan *scan, const uint64_t *segment_ends,
+                                          const uint32_t *segment_frame_ids, size_t num_segments,
+                                          const cticp_cloud_sink *sink, void *stream);
+
 /* ---- Map (L2 boundary; used directly by the parity tests) ---------------------------------------------- */
 
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */
