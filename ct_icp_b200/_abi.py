@@ -221,6 +221,26 @@ class DeviceTiming(_Struct):
     ]
 
 
+class KittiErrors(_Struct):   # cticp_kitti_errors: kitti::seq_errors without tab_errors and the runner-filled fields
+    _fields_ = [("mean_rpe", C.c_double), ("mean_ape", C.c_double), ("max_ape", C.c_double),
+                ("mean_local_err", C.c_double), ("max_local_err", C.c_double), ("index_max_local_err", C.c_int64)]
+
+
+class TrajSegment(_Struct):   # cticp_traj_segment: slam::segment_t of a counted segment and its loc error
+    _fields_ = [("segment_length", C.c_double), ("start_idx", C.c_int64), ("end_idx", C.c_int64),
+                ("loc_error", C.c_double), ("quat", C.c_double * 4), ("tr", C.c_double * 3)]
+
+
+class TrajMetrics(_Struct):   # cticp_traj_metrics: slam::metrics_t without the vectors
+    _fields_ = [("total_distance", C.c_double), ("mean_ate", C.c_double), ("max_ate", C.c_double),
+                ("max_ate_idx", C.c_int64), ("segment_mean_ate", C.c_double), ("segment_mean_ate_ratio", C.c_double),
+                ("num_segments", C.c_int64), ("quat", C.c_double * 4), ("tr", C.c_double * 3)]
+
+
+KITTI_LENGTHS = {"driving": (100., 200., 300., 400., 500., 600., 700., 800.),   # eval.h kitti_segment_lengths
+                 "indoor": (10., 20., 30., 40., 50., 60., 70., 80.)}            # eval.h indoor_segment_lengths
+
+
 # cticp_batch_frame kinds
 BATCH_HOST, BATCH_DEVICE, BATCH_STAGED = 0, 1, 2
 
@@ -245,6 +265,13 @@ def pose_dtype():
     import numpy as np
     return np.dtype([("quat", "<f8", 4), ("tr", "<f8", 3), ("ref_timestamp", "<f8"), ("dest_timestamp", "<f8"),
                      ("ref_frame_id", "<u4"), ("dest_frame_id", "<u4")])
+
+
+# numpy dtype of cticp_traj_segment (88 bytes): the segments of Binding.trajectory_metrics
+def traj_segment_dtype():
+    import numpy as np
+    return np.dtype([("segment_length", "<f8"), ("start_idx", "<i8"), ("end_idx", "<i8"), ("loc_error", "<f8"),
+                     ("quat", "<f8", 4), ("tr", "<f8", 3)])
 
 
 def frame_to_arrays(frame):

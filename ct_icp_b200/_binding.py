@@ -38,6 +38,51 @@ def _as_f64_rows(a, cols):
     return a
 
 
+def _pose_array(poses):
+    """a contiguous array of abi.pose_dtype() from abi.Pose items or such an array"""
+    if isinstance(poses, np.ndarray):
+        if poses.dtype != abi.pose_dtype():
+            raise TypeError("expected an array of abi.pose_dtype()")
+        return np.ascontiguousarray(poses.reshape(-1))
+    out = np.zeros(len(poses), dtype=abi.pose_dtype())
+    for i, p in enumerate(poses):
+        if not isinstance(p, abi.Pose):
+            raise TypeError("expected abi.Pose items, got %r" % type(p))
+        C.memmove(out.ctypes.data + i * out.itemsize, C.addressof(p), C.sizeof(abi.Pose))
+    return out
+
+
+def _estimates_array(estimates, n):
+    """(B × n poses, B, single): one estimate (a pose list or array) or a list of them; each must have n poses"""
+    single = isinstance(estimates, np.ndarray) or (len(estimates) > 0 and isinstance(estimates[0], abi.Pose))
+    ests = [_pose_array(estimates)] if single else [_pose_array(e) for e in estimates]
+    if not ests:
+        raise CticpError(abi.ERR_INVALID_ARGUMENT, "no estimates")
+    for e in ests:
+        if len(e) != n:
+            raise CticpError(abi.ERR_INVALID_ARGUMENT, "an estimate has %d poses, the ground truth %d" % (len(e), n))
+    return np.concatenate(ests), len(ests), single
+
+
+def _lengths(lengths):
+    if isinstance(lengths, str):
+        lengths = abi.KITTI_LENGTHS[lengths]
+    return np.ascontiguousarray(lengths, dtype=np.float64).reshape(-1)
+
+
+def _kitti_dict(e, tab):
+    d = {name: getattr(e, name) for name, _ in abi.KittiErrors._fields_}
+    d["tab_errors"] = np.array(tab)
+    return d
+
+
+def _metrics_dict(m, segs):
+    d = {name: getattr(m, name) for name, _ in abi.TrajMetrics._fields_ if name not in ("quat", "tr")}
+    d["quat"], d["tr"] = np.array(m.quat[:]), np.array(m.tr[:])
+    d["segments"] = np.array(segs)
+    return d
+
+
 _SNAPSHOT_HEADER_BYTES = 72   # snapshot_format.h kHeaderBytes
 
 
@@ -142,6 +187,10 @@ class Binding:
             "trajectory_interpolate": (C.c_int, [vp, vp, vp, sz, vp]),
             "trajectory_transform": (i64, [vp, P(abi.CloudView), vp, vp, sz, P(abi.CloudSink)]),
             "trajectory_transform_device": (i64, [vp, P(abi.DeviceScan), vp, vp, sz, P(abi.CloudSink), vp]),
+            "kitti_evaluate": (i64, [C.c_int, vp, sz, vp, sz, vp, sz, vp, vp, sz]),
+            "trajectory_kitti_evaluate": (i64, [vp, vp, sz, vp, sz, vp, vp, sz]),
+            "trajectory_metrics": (i64, [C.c_int, vp, sz, vp, sz, dbl, vp, vp, sz]),
+            "trajectory_distances": (C.c_int, [C.c_int, vp, sz, C.c_int, vp]),
             # oracle only (KAT taps)
             "odometry_last_counters": (None, [vp, P(u64), P(u64)]),
             "neighborhood_describe": (C.c_int, [vp, sz, vp, P(dbl), P(dbl), P(dbl), vp]),
@@ -233,6 +282,46 @@ class Binding:
         """slam::LinearContinuousTrajectory::Create (cticp_trajectory_create) of abi.Pose items, or of abi.Frame items
         (each contributes its begin and end pose, e.g. Odometry.Trajectory())."""
         return ContinuousTrajectory(self, poses_or_frames, device)
+
+    # ---- scoring against ground truth ----------------------------------------------------------------------
+    def kitti_evaluate(self, gt, estimates, lengths="driving", device=0):
+        """kitti::EvaluatePoses (cticp_kitti_evaluate) of one estimate or of a list of estimates against the ground truth
+        `gt`. Poses: lists of abi.Pose or arrays of abi.pose_dtype(). lengths: "driving", "indoor" or a sequence.
+        Returns a dict (a list of dicts for a list of estimates): the seq_errors fields and tab_errors, a (count, 2)
+        array of (t_err / len, r_err / len)."""
+        g = _pose_array(gt)
+        est, B, single = _estimates_array(estimates, len(g))
+        lens = _lengths(lengths)
+        cap = -(-len(g) // 10) * len(lens)   # every (first frame, length) pair kept
+        out = (abi.KittiErrors * B)()
+        tab = np.zeros((B, max(cap, 1), 2))
+        count = self.check(self.fn("kitti_evaluate")(device, g.ctypes.data, len(g), est.ctypes.data, B, lens.ctypes.data,
+                                                     len(lens), out, tab.ctypes.data, cap))
+        res = [_kitti_dict(out[b], tab[b, :count]) for b in range(B)]
+        return res[0] if single else res
+
+    def trajectory_metrics(self, gt, estimates, segment_length=10.0, device=0):
+        """ComputeTrajectoryMetrics (cticp_trajectory_metrics) of one estimate or of a list of estimates against the
+        ground truth `gt`. Returns a dict (a list of dicts for a list of estimates): the metrics_t scalars, the global
+        rigid transform (quat, tr) and `segments`, an array of abi.traj_segment_dtype() holding the counted segments."""
+        g = _pose_array(gt)
+        est, B, single = _estimates_array(estimates, len(g))
+        cap = max((len(g) - 1) // 5, 1)   # a counted segment spans at least 5 steps
+        out = (abi.TrajMetrics * B)()
+        segs = np.zeros((B, cap), dtype=abi.traj_segment_dtype())
+        count = self.check(self.fn("trajectory_metrics")(device, g.ctypes.data, len(g), est.ctypes.data, B,
+                                                         float(segment_length), out, segs.ctypes.data, cap))
+        res = [_metrics_dict(out[b], segs[b, :count]) for b in range(B)]
+        return res[0] if single else res
+
+    def trajectory_distances(self, gt, kind="kitti", device=0):
+        """The distances along the ground truth that kitti_evaluate ("kitti") or trajectory_metrics ("metrics") selects
+        pairs and segments with (cticp_trajectory_distances)."""
+        g = _pose_array(gt)
+        out = np.zeros(len(g))
+        self.check(self.fn("trajectory_distances")(device, g.ctypes.data, len(g), {"kitti": 0, "metrics": 1}[kind],
+                                                   out.ctypes.data))
+        return out
 
     # ---- many handles, one frame each ------------------------------------------------------------------------
     def register_batch(self, odometries, scans, frame_ids, initial_estimates=None, motion_models=None):
@@ -790,6 +879,19 @@ class ContinuousTrajectory:
         self.b.check(self.b.fn("trajectory_interpolate")(self.h, ts.ctypes.data, fid.ctypes.data if fid is not None else None,
                                                          len(ts), out.ctypes.data))
         return out
+
+    def kitti_evaluate(self, gt, lengths="driving"):
+        """kitti::EvaluatePoses(gt, trajectory) (cticp_trajectory_kitti_evaluate): the estimate is the pose of this
+        trajectory at every ground-truth dest_timestamp, interpolated on the trajectory's device. A dict as
+        Binding.kitti_evaluate returns."""
+        g = _pose_array(gt)
+        lens = _lengths(lengths)
+        cap = -(-len(g) // 10) * len(lens)
+        out = abi.KittiErrors()
+        tab = np.zeros((max(cap, 1), 2))
+        count = self.b.check(self.b.fn("trajectory_kitti_evaluate")(self.h, g.ctypes.data, len(g), lens.ctypes.data,
+                                                                    len(lens), C.byref(out), tab.ctypes.data, cap))
+        return _kitti_dict(out, tab[:count])
 
     @staticmethod
     def _segments(segments, n):

@@ -9,6 +9,7 @@
 #include "../../include/cticp.h"
 #include "engine.h"
 #include "trajectory.h"
+#include "trajectory_eval.h"
 
 using namespace cticp;
 
@@ -96,6 +97,9 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_adaptive_options") return sizeof(cticp_adaptive_options);
     if (s == "cticp_device_scan") return sizeof(cticp_device_scan);
     if (s == "cticp_batch_frame") return sizeof(cticp_batch_frame);
+    if (s == "cticp_kitti_errors") return sizeof(cticp_kitti_errors);
+    if (s == "cticp_traj_segment") return sizeof(cticp_traj_segment);
+    if (s == "cticp_traj_metrics") return sizeof(cticp_traj_metrics);
     return 0;
 }
 
@@ -667,6 +671,51 @@ int64_t cticp_trajectory_transform_device(cticp_trajectory *t, const cticp_devic
         return (int) CTICP_OK;
     });
     return rc < 0 ? rc : count;
+}
+
+/* ---- Scoring against ground truth ------------------------------------------------------------------------------ */
+int64_t cticp_kitti_evaluate(int device, const cticp_pose *gt, size_t n, const cticp_pose *est, size_t num_estimates,
+                             const double *lengths, size_t num_lengths, cticp_kitti_errors *out, double *tab_errors,
+                             size_t cap) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        CheckKittiArgs(gt, n, est, num_estimates, lengths, num_lengths, out);
+        RequireDevice(device);
+        count = KittiEvaluate(gt, n, est, num_estimates, lengths, num_lengths, out, tab_errors, cap);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int64_t cticp_trajectory_kitti_evaluate(cticp_trajectory *t, const cticp_pose *gt, size_t n, const double *lengths,
+                                        size_t num_lengths, cticp_kitti_errors *out, double *tab_errors, size_t cap) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!t) throw std::invalid_argument("null handle");
+        CheckKittiTrajectoryArgs(gt, n, lengths, num_lengths, out);
+        count = KittiEvaluateTrajectory(*t->impl, gt, n, lengths, num_lengths, out, tab_errors, cap);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int64_t cticp_trajectory_metrics(int device, const cticp_pose *gt, size_t n, const cticp_pose *est,
+                                 size_t num_estimates, double segment_length, cticp_traj_metrics *out,
+                                 cticp_traj_segment *segments, size_t cap) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        CheckMetricsArgs(gt, n, est, num_estimates, segment_length, out);
+        RequireDevice(device);
+        count = TrajectoryMetrics(gt, n, est, num_estimates, segment_length, out, segments, cap);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int cticp_trajectory_distances(int device, const cticp_pose *gt, size_t n, int kind, double *out) {
+    return Guard([&] {
+        CheckDistancesArgs(gt, n, kind, out);
+        RequireDevice(device);
+        TrajectoryDistances(gt, n, kind, out);
+        return (int) CTICP_OK;
+    });
 }
 
 /* ---- Map ----------------------------------------------------------------------------------------------------- */

@@ -280,6 +280,15 @@ void ContinuousTrajectory::Interpolate(const double *timestamps, const uint32_t 
     CT_CUDA_CHECK(cudaStreamSynchronize(s));
 }
 
+void ContinuousTrajectory::InterpolateDevice(const double *d_timestamps, size_t m, cticp_pose *d_out) {
+    if (m == 0) return;
+    CT_CUDA_CHECK(cudaSetDevice(device_));
+    const Lookup L{d_ts_.data(), (uint32_t) poses_.size(), min_ts_, max_ts_};
+    k_interpolate<<<Blocks(m), kTrajThreads, 0, stream_.get()>>>(d_poses_.data(), d_sc_.data(), L, d_timestamps, nullptr,
+                                                                 m, d_out);
+    CT_CUDA_CHECK(cudaGetLastError());
+}
+
 std::vector<TrajSegment> ContinuousTrajectory::ResolveSegments(const uint64_t *segment_ends,
                                                                const uint32_t *segment_frame_ids, size_t num_segments,
                                                                uint64_t num_points) const {

@@ -35,6 +35,9 @@ public:
 
     // InterpolatePose (frame_ids == nullptr) / InterpolatePoseWithFrameId of m host timestamps; synchronous
     void Interpolate(const double *timestamps, const uint32_t *frame_ids, size_t m, cticp_pose *out);
+    // InterpolatePose of m timestamps in device memory into device memory, enqueued on Stream(); no synchronisation
+    void InterpolateDevice(const double *d_timestamps, size_t m, cticp_pose *d_out);
+    cudaStream_t Stream() const { return stream_.get(); }
     // RawPointsToWorldPoints of host records into a host sink (synchronous) / of device records into a device sink (ordered
     // after and before `stream`, no host synchronisation). Return the number of points; write min(capacity, count).
     int64_t Transform(const cticp_cloud_view &cloud, const uint64_t *segment_ends, const uint32_t *segment_frame_ids,

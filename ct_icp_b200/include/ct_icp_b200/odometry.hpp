@@ -20,6 +20,7 @@
 #include <limits>
 #include <map>
 #include <memory>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -587,6 +588,151 @@ inline void RawPointsToWorldPoints(std::vector<WPoint3D> &points, const LinearCo
     const cticp_cloud_sink sink{points.data(), points.size(), sizeof(WPoint3D), 32, CTICP_DTYPE_FLOAT64, 0, 0, 1};
     const int64_t rc = cticp_trajectory_transform(trajectory.Handle(), &view, ends.data(), fids.data(), ends.size(), &sink);
     if (rc < 0) ct_icp::cticp_check((int) rc);
+}
+
+// ---- Scoring against ground truth (include/SlamCore/eval.h) over cticp_kitti_evaluate / cticp_trajectory_metrics -------
+// Semantics, quirks and refusals: include/cticp.h. The runner-filled fields keep the reference's defaults.
+namespace kitti {
+
+struct errors {
+    double t_err;
+    double r_err;
+    errors() = default;
+    errors(double t_err, double r_err) : t_err(t_err), r_err(r_err) {}
+};
+
+struct seq_errors {
+    std::vector<errors> tab_errors;
+    bool success = false;
+    bool finished = false;
+    double mean_rpe;
+    double mean_ape;
+    double max_ape;
+    double mean_local_err;
+    double max_local_err;
+    double average_elapsed_ms = -1.0;
+    int index_max_local_err;
+    double mean_num_attempts;
+};
+
+const auto kitti_segment_lengths = std::vector<double>{100., 200., 300., 400., 500., 600., 700., 800.};
+const auto indoor_segment_lengths = std::vector<double>{10., 20., 30., 40., 50., 60., 70., 80.};
+
+namespace detail {
+inline std::vector<cticp_pose> poses_to_c(const std::vector<Pose> &poses) {
+    std::vector<cticp_pose> c;
+    c.reserve(poses.size());
+    for (const Pose &p : poses) c.push_back(ct_icp::detail::pose_to_c(p));
+    return c;
+}
+// (first frame, length) pairs of ComputeMeanRPE with step size 10: an upper bound of the kept ones
+inline size_t max_pairs(size_t n, size_t num_lengths) { return ((n + 9) / 10) * num_lengths; }
+inline seq_errors to_seq_errors(const cticp_kitti_errors &e, const std::vector<double> &tab, int64_t count) {
+    seq_errors s;
+    s.mean_rpe = e.mean_rpe;
+    s.mean_ape = e.mean_ape;
+    s.max_ape = e.max_ape;
+    s.mean_local_err = e.mean_local_err;
+    s.max_local_err = e.max_local_err;
+    s.index_max_local_err = (int) e.index_max_local_err;
+    for (int64_t k = 0; k < count; ++k) s.tab_errors.emplace_back(tab[2 * k], tab[2 * k + 1]);
+    return s;
+}
+}  // namespace detail
+
+// EvaluatePoses(poses_gt, poses_estimated, lengths) (eval.cxx:136-178) on CUDA device `device`
+inline seq_errors EvaluatePoses(const std::vector<Pose> &poses_gt, const std::vector<Pose> &poses_estimated,
+                                const std::vector<double> &lengths, int device = 0) {
+    if (poses_estimated.size() != poses_gt.size())
+        throw ct_icp::CticpFailure(CTICP_ERR_INVALID_ARGUMENT, "[ERROR] Couldn't evaluate (all) poses");
+    const std::vector<cticp_pose> gt = detail::poses_to_c(poses_gt), est = detail::poses_to_c(poses_estimated);
+    const size_t cap = detail::max_pairs(gt.size(), lengths.size());
+    std::vector<double> tab(2 * std::max<size_t>(cap, 1));
+    cticp_kitti_errors e;
+    const int64_t count = cticp_kitti_evaluate(device, gt.data(), gt.size(), est.data(), 1, lengths.data(), lengths.size(),
+                                               &e, tab.data(), cap);
+    if (count < 0) ct_icp::cticp_check((int) count);
+    return detail::to_seq_errors(e, tab, count);
+}
+inline seq_errors EvaluatePoses(const std::vector<Pose> &poses_gt, const std::vector<Pose> &poses_estimated,
+                                bool driving = true, int device = 0) {
+    return EvaluatePoses(poses_gt, poses_estimated, driving ? kitti_segment_lengths : indoor_segment_lengths, device);
+}
+// EvaluatePoses(poses_gt, trajectory) (eval.cxx:103-111): the estimate is trajectory.InterpolatePose(gt_i.dest_timestamp,
+// true), interpolated on the trajectory's device
+inline seq_errors EvaluatePoses(const std::vector<Pose> &poses_gt, const LinearContinuousTrajectory &trajectory,
+                                const std::vector<double> &lengths) {
+    const std::vector<cticp_pose> gt = detail::poses_to_c(poses_gt);
+    const size_t cap = detail::max_pairs(gt.size(), lengths.size());
+    std::vector<double> tab(2 * std::max<size_t>(cap, 1));
+    cticp_kitti_errors e;
+    const int64_t count = cticp_trajectory_kitti_evaluate(trajectory.Handle(), gt.data(), gt.size(), lengths.data(),
+                                                          lengths.size(), &e, tab.data(), cap);
+    if (count < 0) ct_icp::cticp_check((int) count);
+    return detail::to_seq_errors(e, tab, count);
+}
+inline seq_errors EvaluatePoses(const std::vector<Pose> &poses_gt, const LinearContinuousTrajectory &trajectory,
+                                bool driving = true) {
+    return EvaluatePoses(poses_gt, trajectory, driving ? kitti_segment_lengths : indoor_segment_lengths);
+}
+
+}  // namespace kitti
+
+struct segment_t {   // slam::segment_t; rigid_transform is set on every counted segment
+    double segment_length = 0.;
+    size_t start_idx = -1, end_idx = -1;
+    std::optional<SE3> rigid_transform;
+};
+
+struct metrics_t {   // slam::metrics_t; segment_mean_ate_ratio starts at 0 (the reference leaves it uninitialised)
+    std::vector<segment_t> trajectory_segments;
+    std::vector<double> loc_errors, distances;
+    double segment_mean_ate_ratio = 0., segment_mean_ate = 0.;
+    double total_distance = 0.;
+    double mean_ate = 0.;
+    double max_ate = 0.;
+    size_t max_ate_idx = -1;
+    std::optional<SE3> rigid_transform;
+};
+
+// ComputeTrajectoryMetrics (eval.cxx:184-291) on CUDA device `device`
+inline metrics_t ComputeTrajectoryMetrics(const std::vector<Pose> &gt_trajectory, const std::vector<Pose> &trajectory,
+                                          double segment_length = 10., int device = 0) {
+    if (trajectory.size() != gt_trajectory.size())
+        throw ct_icp::CticpFailure(CTICP_ERR_INVALID_ARGUMENT, "the estimate and the ground truth differ in size");
+    const std::vector<cticp_pose> gt = kitti::detail::poses_to_c(gt_trajectory), est = kitti::detail::poses_to_c(trajectory);
+    const size_t cap = gt.size() > 1 ? std::max<size_t>((gt.size() - 1) / 5, 1) : 1;   // a counted segment spans >= 5 steps
+    std::vector<cticp_traj_segment> segs(cap);
+    cticp_traj_metrics m;
+    const int64_t count = cticp_trajectory_metrics(device, gt.data(), gt.size(), est.data(), 1, segment_length, &m,
+                                                   segs.data(), cap);
+    if (count < 0) ct_icp::cticp_check((int) count);
+    auto se3 = [](const double q[4], const double t[3]) {
+        SE3 s;
+        for (int k = 0; k < 4; ++k) s.quat.c[k] = q[k];
+        for (int k = 0; k < 3; ++k) s.tr[k] = t[k];
+        return s;
+    };
+    metrics_t r;
+    r.distances.resize(gt.size());
+    ct_icp::cticp_check(cticp_trajectory_distances(device, gt.data(), gt.size(), 1, r.distances.data()));
+    r.total_distance = m.total_distance;
+    r.mean_ate = m.mean_ate;
+    r.max_ate = m.max_ate;
+    r.max_ate_idx = (size_t) m.max_ate_idx;
+    r.segment_mean_ate = m.segment_mean_ate;
+    r.segment_mean_ate_ratio = m.segment_mean_ate_ratio;
+    r.rigid_transform = se3(m.quat, m.tr);
+    for (int64_t k = 0; k < count; ++k) {
+        segment_t s;
+        s.segment_length = segs[k].segment_length;
+        s.start_idx = (size_t) segs[k].start_idx;
+        s.end_idx = (size_t) segs[k].end_idx;
+        s.rigid_transform = se3(segs[k].quat, segs[k].tr);
+        r.trajectory_segments.push_back(s);
+        r.loc_errors.push_back(segs[k].loc_error);
+    }
+    return r;
 }
 
 }  // namespace slam

@@ -601,6 +601,73 @@ int64_t cticp_trajectory_transform_device(cticp_trajectory *t, const cticp_devic
                                           const uint32_t *segment_frame_ids, size_t num_segments,
                                           const cticp_cloud_sink *sink, void *stream);
 
+/* ---- Scoring a trajectory against ground truth (include/SlamCore/eval.h, src/SlamCore/eval.cxx) -----------------------
+ * kitti::EvaluatePoses and ComputeTrajectoryMetrics on the device, B estimates against one ground truth per call. Each
+ * function takes the device first and is synchronous on return. Estimates are num_estimates × n poses, estimate b at
+ * est[b * n]. Semantics are the reference's, quirks included:
+ *   - KITTI: poses become matrices with quat.normalized(); dist[i] = dist[i-1] + |t[i-1] - t[i]| over the ground truth;
+ *     first frames 0, 10, 20, ... < n, and for each one every length in order; the pair ends at the first i >= first with
+ *     dist[i] > dist[first] + len (strict: a distance exactly equal does not end it) and is skipped when there is none.
+ *     E = (est_f^-1 est_l)^-1 (gt_f^-1 gt_l); t_err = |E.t|, r_err = acos(clamp(0.5 (trace(R_E) - 1), -1, 1)), stored as
+ *     (t_err / len, r_err / len), first-frame-major; mean_rpe = 100 sum(t_err / len) / count (NaN for no pair).
+ *     ape_i = |(est_i^-1 gt_i).t|; local_i = | |gt_i.t - gt_{i-1}.t| - |est_i.t - est_{i-1}.t| | for i >= 1, its mean
+ *     over n - 1 (NaN for n = 1); maxima start at 0 and update on a strict <, index_max_local_err starts at 0.
+ *   - metrics: dist[i+1] = dist[i] + |(gt_i.pose.Inverse() * gt_{i+1}.pose).tr| (TSE3 arithmetic); the global
+ *     OrthogonalProcrustes (src/SlamCore/geometry.cxx:7-46) of the ground-truth translations onto the estimate's; ate_i =
+ *     |quat.normalized() gt_i.t + tr - est_i.t|, max_ate_idx -1 until a value exceeds the running max (from 0, strict >).
+ *     Segments form a greedy chain: [start, idx] closes at the first idx with dist[idx] - dist[start] > segment_length,
+ *     then start = idx; the trailing part is dropped. A segment of <= 5 poses is skipped (not counted, no fit) but still
+ *     advances the chain. Each counted segment gets its own fit and loc_error = the largest |(T_s * gt_i.pose).tr -
+ *     est_i.t| over it; segment_mean_ate = sum(loc) / count, segment_mean_ate_ratio = sum(loc / segment_length) / count
+ *     (NaN for no counted segment; the reference leaves the ratio's accumulator uninitialised, here it starts at 0).
+ *   - a rank-deficient cross-covariance (straight or stationary segments) gives finite metrics; a zero one gives the
+ *     identity rotation, as Eigen's JacobiSVD does.
+ * The pair selection and the segment chain are exact: both distance arrays are summed in index order with the
+ * reference's operation order and no FMA contraction. The other sums are fixed-order block reductions: bit-reproducible
+ * from run to run and for each estimate whatever the batch holds, within ~1e-15 relative of a sequential sum.
+ * CTICP_ERR_INVALID_ARGUMENT, before anything is written: null pointers (tab_errors / segments may be NULL), n = 0,
+ * num_estimates = 0, n <= 5 for the metrics, an empty length list, a length or segment_length that is not finite and
+ * > 0, a quaternion that is not finite or is zero, a translation that is not finite, a ground-truth dest_timestamp that
+ * is not finite. (Refusing non-finite poses is a deviation: the reference scores them into NaN or undefined behaviour.) */
+typedef struct cticp_kitti_errors {   /* kitti::seq_errors without tab_errors and the runner-filled fields */
+    double mean_rpe, mean_ape, max_ape, mean_local_err, max_local_err;
+    int64_t index_max_local_err;
+} cticp_kitti_errors;
+typedef struct cticp_traj_segment {   /* slam::segment_t of a counted segment, with its own loc error */
+    double segment_length;
+    int64_t start_idx, end_idx;       /* inclusive */
+    double loc_error;
+    double quat[4], tr[3];            /* rigid_transform: estimate ≈ T * ground truth */
+} cticp_traj_segment;
+typedef struct cticp_traj_metrics {   /* slam::metrics_t without the vectors */
+    double total_distance, mean_ate, max_ate;
+    int64_t max_ate_idx;
+    double segment_mean_ate, segment_mean_ate_ratio;
+    int64_t num_segments;
+    double quat[4], tr[3];            /* the global rigid_transform */
+} cticp_traj_metrics;
+/* kitti::EvaluatePoses(gt, est_b, lengths) (eval.cxx:136-178, step size 10) of every estimate. out: num_estimates
+ * records. tab_errors (nullable): num_estimates × cap × 2 doubles, estimate b's (t_err / len, r_err / len) pairs at
+ * tab_errors[2 * b * cap], min(cap, count) of them. Returns the pair count, which depends on the ground truth only. */
+int64_t cticp_kitti_evaluate(int device, const cticp_pose *gt, size_t n, const cticp_pose *est, size_t num_estimates,
+                             const double *lengths, size_t num_lengths, cticp_kitti_errors *out, double *tab_errors,
+                             size_t cap);
+/* kitti::EvaluatePoses(gt, LinearContinuousTrajectory, ...) (eval.cxx:103-111): the estimate is InterpolatePose(
+ * gt_i.dest_timestamp, true) of the trajectory, evaluated on the trajectory's device and stream without a host round
+ * trip; the same as cticp_kitti_evaluate fed with cticp_trajectory_interpolate's output, bit for bit. */
+int64_t cticp_trajectory_kitti_evaluate(cticp_trajectory *t, const cticp_pose *gt, size_t n, const double *lengths,
+                                        size_t num_lengths, cticp_kitti_errors *out, double *tab_errors, size_t cap);
+/* ComputeTrajectoryMetrics(gt, est_b, segment_length) (eval.cxx:184-291) of every estimate. out: num_estimates records.
+ * segments (nullable): num_estimates × cap records, estimate b's counted segments at segments[b * cap], min(cap, count)
+ * of them. Returns the number of counted segments, which depends on the ground truth only. */
+int64_t cticp_trajectory_metrics(int device, const cticp_pose *gt, size_t n, const cticp_pose *est,
+                                 size_t num_estimates, double segment_length, cticp_traj_metrics *out,
+                                 cticp_traj_segment *segments, size_t cap);
+/* The distances along the ground truth the two functions above select pairs and segments with (metrics_t::distances and
+ * the KITTI trajectory_distances): kind 0 = KITTI (matrix translations), kind 1 = ComputeTrajectoryMetrics (TSE3
+ * relative poses). out: n doubles. Refusals as above (n >= 1 for both kinds). */
+int cticp_trajectory_distances(int device, const cticp_pose *gt, size_t n, int kind, double *out);
+
 /* ---- Map (L2 boundary; used directly by the parity tests) ---------------------------------------------- */
 
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */
