@@ -237,6 +237,15 @@ class TrajMetrics(_Struct):   # cticp_traj_metrics: slam::metrics_t without the 
                 ("num_segments", C.c_int64), ("quat", C.c_double * 4), ("tr", C.c_double * 3)]
 
 
+class GridSamplingOptions(_Struct):   # cticp_grid_sampling_options: slam::GridSamplingOptions
+    _fields_ = [("grid_size", C.c_double), ("num_points_per_voxel", C.c_int32), ("_pad0", C.c_int32),
+                ("max_num_points", C.c_int64)]
+
+
+class WorldCloudStats(_Struct):   # cticp_world_cloud_stats: what one add of a world cloud did
+    _fields_ = [("submitted", C.c_uint64), ("kept", C.c_uint64), ("rejected", C.c_uint64), ("new_voxels", C.c_uint64)]
+
+
 KITTI_LENGTHS = {"driving": (100., 200., 300., 400., 500., 600., 700., 800.),   # eval.h kitti_segment_lengths
                  "indoor": (10., 20., 30., 40., 50., 60., 70., 80.)}            # eval.h indoor_segment_lengths
 

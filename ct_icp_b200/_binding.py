@@ -191,6 +191,18 @@ class Binding:
             "trajectory_kitti_evaluate": (i64, [vp, vp, sz, vp, sz, vp, vp, sz]),
             "trajectory_metrics": (i64, [C.c_int, vp, sz, vp, sz, dbl, vp, vp, sz]),
             "trajectory_distances": (C.c_int, [C.c_int, vp, sz, C.c_int, vp]),
+            "default_grid_sampling_options": (None, [P(abi.GridSamplingOptions)]),
+            "sample_points_in_grid": (i64, [C.c_int, P(abi.GridSamplingOptions), vp, sz, sz, vp, sz]),
+            "world_cloud_create": (C.c_int, [P(abi.GridSamplingOptions), u64, u64, C.c_int, P(vp)]),
+            "world_cloud_destroy": (None, [vp]),
+            "world_cloud_add": (C.c_int, [vp, vp, P(abi.CloudView), vp, vp, sz, P(abi.WorldCloudStats)]),
+            "world_cloud_add_device": (C.c_int, [vp, vp, P(abi.DeviceScan), vp, vp, sz, P(abi.WorldCloudStats), vp]),
+            "world_cloud_add_odometry": (C.c_int, [vp, vp, P(abi.WorldCloudStats)]),
+            "world_cloud_num_points": (i64, [vp]),
+            "world_cloud_num_voxels": (i64, [vp]),
+            "world_cloud_export": (i64, [vp, P(abi.CloudSink), vp]),
+            "world_cloud_export_device": (i64, [vp, P(abi.CloudSink), vp, vp]),
+            "world_cloud_clear": (C.c_int, [vp]),
             # oracle only (KAT taps)
             "odometry_last_counters": (None, [vp, P(u64), P(u64)]),
             "neighborhood_describe": (C.c_int, [vp, sz, vp, P(dbl), P(dbl), P(dbl), vp]),
@@ -396,6 +408,28 @@ class Binding:
         n = self.check(self.fn("adaptive_sample_indices")(device, C.byref(options), xyz.ctypes.data, 24, len(xyz),
                                                            out.ctypes.data, len(out)))
         return out[:n].copy()
+
+    def grid_sampling_options(self, grid_size=1.0, num_points_per_voxel=1, max_num_points=-1):
+        o = abi.GridSamplingOptions()
+        self.fn("default_grid_sampling_options")(C.byref(o))
+        o.grid_size, o.num_points_per_voxel, o.max_num_points = float(grid_size), int(num_points_per_voxel), int(max_num_points)
+        return o
+
+    def sample_points_in_grid(self, xyz, grid_size, num_points_per_voxel=1, max_num_points=-1, device=0):
+        """slam::SamplePointsInGrid (cticp_sample_points_in_grid) of (n, 3) points: the indices kept (uint64), voxel by
+        voxel in order of first appearance, each voxel's points in input order."""
+        xyz = _as_f64_rows(xyz, 3)
+        o = self.grid_sampling_options(grid_size, num_points_per_voxel, max_num_points)
+        out = np.empty(max(len(xyz), 1), dtype=np.uint64)
+        n = self.check(self.fn("sample_points_in_grid")(device, C.byref(o), xyz.ctypes.data, 24, len(xyz), out.ctypes.data,
+                                                        len(out)))
+        return out[:n].copy()
+
+    def world_cloud(self, grid_size=1.0, num_points_per_voxel=1, max_num_points=-1, capacity_voxels=0,
+                    capacity_points=0, device=0):
+        """A WorldCloud (cticp_world_cloud_create): SamplePointsInGrid grown add by add on `device`."""
+        return WorldCloud(self, self.grid_sampling_options(grid_size, num_points_per_voxel, max_num_points),
+                          capacity_voxels, capacity_points, device)
 
     def permutation(self, seed, counter, n):
         out = np.empty(n, dtype=np.uint32)
@@ -975,3 +1009,159 @@ class ContinuousTrajectory:
                              code if with_timestamps else 0, 1)
         self.transform_device(scan, sink, segments, stream)
         return out
+
+
+class WorldCloud:
+    """slam::SamplePointsInGrid grown call by call on the device (cticp_world_cloud_*): after any sequence of adds, export
+    returns SamplePointsInGrid over every point submitted, in call order, with each point's source index (its position in
+    that concatenation) and timestamp."""
+
+    def __init__(self, binding, options, capacity_voxels=0, capacity_points=0, device=0):
+        self.b = binding
+        self.device = device
+        self.options = options.copy()
+        self.h = C.c_void_p()
+        binding.check(binding.fn("world_cloud_create")(C.byref(self.options), int(capacity_voxels), int(capacity_points),
+                                                       device, C.byref(self.h)))
+
+    def close(self):
+        if self.h:
+            self.b.fn("world_cloud_destroy")(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _traj(trajectory):
+        return trajectory.h if trajectory is not None else None
+
+    def add_records(self, records, trajectory=None, segments=None, t_field="t"):
+        """cticp_world_cloud_add of a 1-D structured host array (x, y, z contiguous of one float type, and a timestamp
+        field, which may be absent without a trajectory). Returns abi.WorldCloudStats."""
+        assert records.ndim == 1 and records.flags.c_contiguous and records.dtype.fields is not None
+        f = records.dtype.fields
+        xdt, xoff = f["x"][0], f["x"][1]
+        assert f["y"] == (xdt, xoff + xdt.itemsize) and f["z"] == (xdt, xoff + 2 * xdt.itemsize), "x, y, z must be contiguous"
+        has_t = t_field in f
+        view = abi.CloudView(records.ctypes.data if len(records) else None, len(records), records.dtype.itemsize, xoff,
+                             abi.DTYPE[xdt.name], f[t_field][1] if has_t else 0, abi.DTYPE[f[t_field][0].name] if has_t else 0,
+                             0)
+        ends, fids, ns = ContinuousTrajectory._segments(segments, len(records))
+        st = abi.WorldCloudStats()
+        self.b.check(self.b.fn("world_cloud_add")(self.h, self._traj(trajectory), C.byref(view),
+                                                  ends.ctypes.data if ns else None, fids.ctypes.data if ns else None, ns,
+                                                  C.byref(st)))
+        return st
+
+    def add_device(self, scan, trajectory=None, segments=None, stream=0):
+        """cticp_world_cloud_add_device of an abi.DeviceScan; stream: the producer's cudaStream_t"""
+        ends, fids, ns = ContinuousTrajectory._segments(segments, scan.num_points)
+        st = abi.WorldCloudStats()
+        self.b.check(self.b.fn("world_cloud_add_device")(self.h, self._traj(trajectory), C.byref(scan),
+                                                         ends.ctypes.data if ns else None,
+                                                         fids.ctypes.data if ns else None, ns, C.byref(st),
+                                                         C.c_void_p(stream or None)))
+        return st
+
+    def add(self, xyz, t=None, trajectory=None, segments=None):
+        """Adds points: world coordinates without a trajectory, else raw coordinates placed by
+        trajectory.transform(xyz, t, segments). NumPy arrays: the host path; torch CUDA tensors on the cloud's device
+        (xyz (N, >=3) float32 / float64 with unit column stride, t 1-D of any supported dtype or None): read in place
+        after the work of torch's current stream. Returns abi.WorldCloudStats."""
+        if _is_cuda_tensor(xyz) or _is_cuda_tensor(t):
+            return self._add_tensors(xyz, t, trajectory, segments)
+        xyz = np.asarray(xyz)
+        if xyz.ndim != 2 or xyz.shape[1] < 3 or xyz.dtype not in (np.float32, np.float64):
+            raise ValueError("xyz must be an (N, >=3) float32 / float64 array")
+        fields = [("x", xyz.dtype), ("y", xyz.dtype), ("z", xyz.dtype)]
+        if t is not None:
+            t = np.asarray(t).reshape(-1)
+            if len(t) != len(xyz):
+                raise ValueError("xyz and t must have the same length")
+            fields.append(("t", t.dtype))
+        rec = np.zeros(len(xyz), dtype=np.dtype(fields))
+        rec["x"], rec["y"], rec["z"] = xyz[:, 0], xyz[:, 1], xyz[:, 2]
+        if t is not None:
+            rec["t"] = t
+        return self.add_records(rec, trajectory, segments)
+
+    def _add_tensors(self, xyz, t, trajectory, segments):
+        import torch
+        if not _is_cuda_tensor(xyz) or (t is not None and not _is_cuda_tensor(t)):
+            raise ValueError("xyz and t must both be CUDA tensors (or both host arrays)")
+        if xyz.device.index != self.device or (t is not None and t.device.index != self.device):
+            raise ValueError("xyz and t must be on cuda:%d, the cloud's device" % self.device)
+        if xyz.dim() != 2 or xyz.shape[1] < 3 or xyz.stride(1) != 1 or xyz.dtype not in (torch.float32, torch.float64):
+            raise ValueError("xyz must be an (N, >=3) float32 / float64 tensor with unit column stride")
+        codes = _torch_dtype_codes(torch)
+        if t is not None and (t.dim() != 1 or t.dtype not in codes or t.shape[0] != xyz.shape[0]):
+            raise ValueError("t must be a 1-D tensor of a supported dtype, one entry per point")
+        scan = abi.DeviceScan(xyz.data_ptr() if xyz.shape[0] else None, xyz.stride(0) * xyz.element_size(),
+                              t.data_ptr() if t is not None and t.shape[0] else None,
+                              t.stride(0) * t.element_size() if t is not None else 0, xyz.shape[0], codes[xyz.dtype],
+                              codes[t.dtype] if t is not None else 0)
+        return self.add_device(scan, trajectory, segments, torch.cuda.current_stream(self.device).cuda_stream)
+
+    def add_odometry(self, odometry):
+        """The odometry's last CTICP_POINTS_ALL_CORRECTED world points and timestamps, device to device"""
+        st = abi.WorldCloudStats()
+        self.b.check(self.b.fn("world_cloud_add_odometry")(self.h, odometry.h, C.byref(st)))
+        return st
+
+    def num_points(self):
+        """what export returns (max_num_points applied)"""
+        return self.b.check(self.b.fn("world_cloud_num_points")(self.h))
+
+    def num_voxels(self):
+        return self.b.check(self.b.fn("world_cloud_num_voxels")(self.h))
+
+    def clear(self):
+        self.b.check(self.b.fn("world_cloud_clear")(self.h))
+
+    def export_sink(self, sink, src_index=None):
+        """cticp_world_cloud_export into an abi.CloudSink in host memory; src_index: None or a uint64 array"""
+        return self.b.check(self.b.fn("world_cloud_export")(self.h, C.byref(sink),
+                                                            src_index.ctypes.data if src_index is not None else None))
+
+    def export_device_sink(self, sink, src_index_ptr=None, stream=0):
+        """cticp_world_cloud_export_device into an abi.CloudSink in device memory"""
+        return self.b.check(self.b.fn("world_cloud_export_device")(self.h, C.byref(sink), src_index_ptr or None,
+                                                                   C.c_void_p(stream or None)))
+
+    def export(self, dtype=np.float64, with_timestamps=False, with_source_index=False, device=False):
+        """The cloud as an (n, 3) array of `dtype` ((n, 4) with the timestamps); with_source_index: (points, source
+        indices uint64). device=True: torch CUDA tensors on the cloud's device, written in order with torch's current
+        stream (dtype torch.float32 / torch.float64 or the NumPy equivalents)."""
+        n = self.num_points()
+        cols = 4 if with_timestamps else 3
+        if device:
+            import torch
+            tdtype = {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64}.get(
+                np.dtype(dtype) if not isinstance(dtype, torch.dtype) else None, dtype)
+            if tdtype not in (torch.float32, torch.float64):
+                raise ValueError("dtype must be float32 or float64")
+            dev = torch.device("cuda", self.device)
+            out = torch.empty((n, cols), dtype=tdtype, device=dev)
+            src = torch.empty(n, dtype=torch.int64, device=dev) if with_source_index else None
+            if n:
+                code = abi.DTYPE["float32" if tdtype == torch.float32 else "float64"]
+                size = out.element_size()
+                sink = abi.CloudSink(out.data_ptr(), n, cols * size, 0, code, 3 * size, code if with_timestamps else 0, 1)
+                self.export_device_sink(sink, src.data_ptr() if src is not None else None,
+                                        torch.cuda.current_stream(self.device).cuda_stream)
+            return (out, src) if with_source_index else out
+        dtype = np.dtype(dtype)
+        if dtype not in (np.dtype(np.float32), np.dtype(np.float64)):
+            raise ValueError("dtype must be float32 or float64")
+        out = np.zeros((n, cols), dtype=dtype)
+        src = np.zeros(n, dtype=np.uint64) if with_source_index else None
+        if n:
+            code = abi.DTYPE[dtype.name]
+            sink = abi.CloudSink(out.ctypes.data, n, cols * dtype.itemsize, 0, code, 3 * dtype.itemsize,
+                                 code if with_timestamps else 0, 1)
+            self.export_sink(sink, src)
+        return (out, src) if with_source_index else out

@@ -10,6 +10,7 @@
 #include "engine.h"
 #include "trajectory.h"
 #include "trajectory_eval.h"
+#include "world_cloud.h"
 
 using namespace cticp;
 
@@ -74,6 +75,9 @@ struct cticp_odometry {
 struct cticp_trajectory {
     std::unique_ptr<ContinuousTrajectory> impl;
 };
+struct cticp_world_cloud {
+    std::unique_ptr<WorldCloud> impl;
+};
 
 extern "C" {
 
@@ -85,6 +89,8 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_icp_options") return sizeof(cticp_icp_options);
     if (s == "cticp_resolution_param") return sizeof(cticp_resolution_param);
     if (s == "cticp_map_options") return sizeof(cticp_map_options);
+    if (s == "cticp_grid_sampling_options") return sizeof(cticp_grid_sampling_options);
+    if (s == "cticp_world_cloud_stats") return sizeof(cticp_world_cloud_stats);
     if (s == "cticp_strategy_options") return sizeof(cticp_strategy_options);
     if (s == "cticp_motion_model_options") return sizeof(cticp_motion_model_options);
     if (s == "cticp_odometry_options") return sizeof(cticp_odometry_options);
@@ -671,6 +677,112 @@ int64_t cticp_trajectory_transform_device(cticp_trajectory *t, const cticp_devic
         return (int) CTICP_OK;
     });
     return rc < 0 ? rc : count;
+}
+
+/* ---- world clouds (world_cloud.cu) ------------------------------------------------------------------------------ */
+void cticp_default_grid_sampling_options(cticp_grid_sampling_options *out) {
+    if (!out) return;
+    *out = cticp_grid_sampling_options{};
+    out->grid_size = 1.0;               // GridSamplingOptions, grid_sampling.h:12-16
+    out->num_points_per_voxel = 1;
+    out->max_num_points = -1;
+}
+int64_t cticp_sample_points_in_grid(int device, const cticp_grid_sampling_options *options, const double *xyz,
+                                    size_t stride_bytes, size_t n, uint64_t *out_indices, size_t cap) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!options || (n && !xyz)) throw std::invalid_argument("null argument");
+        WorldCloud::CheckOptions(*options);
+        if (stride_bytes < 24 || stride_bytes > 0xFFFFFFFFull) throw std::invalid_argument("stride_bytes outside [24, 2^32)");
+        RequireDevice(device);
+        WorldCloud wc(*options, std::max<size_t>(n, 1), std::max<size_t>(n, 1), device);
+        cticp_cloud_view v{};
+        v.data = xyz;
+        v.num_points = n;
+        v.point_step = (uint32_t) stride_bytes;
+        v.xyz_dtype = CTICP_DTYPE_FLOAT64;
+        wc.Add(nullptr, v, nullptr, nullptr, 0, nullptr);
+        cticp_cloud_sink sink{};
+        sink.capacity_points = out_indices ? cap : 0;
+        sink.world = 1;
+        count = wc.Export(sink, out_indices);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int cticp_world_cloud_create(const cticp_grid_sampling_options *options, uint64_t capacity_voxels,
+                             uint64_t capacity_points, int device, cticp_world_cloud **out) {
+    return Guard([&] {
+        if (!options || !out) throw std::invalid_argument("null argument");
+        WorldCloud::CheckOptions(*options);
+        RequireDevice(device);
+        auto wc = std::make_unique<cticp_world_cloud>();
+        wc->impl = std::make_unique<WorldCloud>(*options, capacity_voxels, capacity_points, device);
+        *out = wc.release();
+        return (int) CTICP_OK;
+    });
+}
+void cticp_world_cloud_destroy(cticp_world_cloud *wc) { delete wc; }
+int cticp_world_cloud_add(cticp_world_cloud *wc, cticp_trajectory *trajectory, const cticp_cloud_view *cloud,
+                          const uint64_t *segment_ends, const uint32_t *segment_frame_ids, size_t num_segments,
+                          cticp_world_cloud_stats *stats_out) {
+    return Guard([&] {
+        if (!wc || !cloud) throw std::invalid_argument("null argument");
+        wc->impl->Add(trajectory ? trajectory->impl.get() : nullptr, *cloud, segment_ends, segment_frame_ids,
+                      num_segments, stats_out);
+        return (int) CTICP_OK;
+    });
+}
+int cticp_world_cloud_add_device(cticp_world_cloud *wc, cticp_trajectory *trajectory, const cticp_device_scan *scan,
+                                 const uint64_t *segment_ends, const uint32_t *segment_frame_ids, size_t num_segments,
+                                 cticp_world_cloud_stats *stats_out, void *stream) {
+    return Guard([&] {
+        if (!wc || !scan) throw std::invalid_argument("null argument");
+        wc->impl->AddDevice(trajectory ? trajectory->impl.get() : nullptr, *scan, segment_ends, segment_frame_ids,
+                            num_segments, stats_out, static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+}
+int cticp_world_cloud_add_odometry(cticp_world_cloud *wc, cticp_odometry *odometry, cticp_world_cloud_stats *stats_out) {
+    return Guard([&] {
+        if (!wc || !odometry) throw std::invalid_argument("null argument");
+        wc->impl->AddOdometry(*odometry->engine, stats_out);
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_world_cloud_num_points(cticp_world_cloud *wc) {
+    if (!wc) return Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+    return (int64_t) wc->impl->NumPoints();
+}
+int64_t cticp_world_cloud_num_voxels(cticp_world_cloud *wc) {
+    if (!wc) return Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+    return (int64_t) wc->impl->NumVoxels();
+}
+int64_t cticp_world_cloud_export(cticp_world_cloud *wc, const cticp_cloud_sink *sink, uint64_t *src_index) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!wc || !sink) throw std::invalid_argument("null argument");
+        count = wc->impl->Export(*sink, src_index);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int64_t cticp_world_cloud_export_device(cticp_world_cloud *wc, const cticp_cloud_sink *sink, uint64_t *src_index,
+                                        void *stream) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!wc || !sink) throw std::invalid_argument("null argument");
+        count = wc->impl->ExportDevice(*sink, src_index, static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int cticp_world_cloud_clear(cticp_world_cloud *wc) {
+    return Guard([&] {
+        if (!wc) throw std::invalid_argument("null handle");
+        wc->impl->Clear();
+        return (int) CTICP_OK;
+    });
 }
 
 /* ---- Scoring against ground truth ------------------------------------------------------------------------------ */

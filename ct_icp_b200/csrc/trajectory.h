@@ -38,6 +38,11 @@ public:
     // InterpolatePose of m timestamps in device memory into device memory, enqueued on Stream(); no synchronisation
     void InterpolateDevice(const double *d_timestamps, size_t m, cticp_pose *d_out);
     cudaStream_t Stream() const { return stream_.get(); }
+    // the refusals a transform of num_points points makes of its segment arguments, before anything is enqueued
+    void CheckSegments(const uint64_t *segment_ends, const uint32_t *segment_frame_ids, size_t num_segments,
+                       uint64_t num_points) const {
+        (void) ResolveSegments(segment_ends, segment_frame_ids, num_segments, num_points);
+    }
     // RawPointsToWorldPoints of host records into a host sink (synchronous) / of device records into a device sink (ordered
     // after and before `stream`, no host synchronisation). Return the number of points; write min(capacity, count).
     int64_t Transform(const cticp_cloud_view &cloud, const uint64_t *segment_ends, const uint32_t *segment_frame_ids,

@@ -13,6 +13,7 @@
 // (`pose.quat`, `pose.tr`, `dest_timestamp`, `RawPoint()`, `WorldPoint()`, `Timestamp()`): this header has no
 // dependency besides cticp.h. INTEGRATION.md shows the variant that keeps the reference's own headers.
 #pragma once
+#include <algorithm>
 #include <array>
 #include <cmath>
 #include <cstdint>
@@ -734,5 +735,123 @@ inline metrics_t ComputeTrajectoryMetrics(const std::vector<Pose> &gt_trajectory
     }
     return r;
 }
+
+// ---- A dense map of a whole run (include/SlamCore/algorithm/grid_sampling.h) over cticp_sample_points_in_grid /
+// cticp_world_cloud_*. Semantics, quirks, the two deviations and the refusals: include/cticp.h.
+struct GridSamplingOptions {
+    double grid_size = 1.0;
+    int num_points_per_voxel = 1;
+    int max_num_points = -1;
+};
+
+namespace detail {
+inline cticp_grid_sampling_options grid_options_to_c(const GridSamplingOptions &o) {
+    cticp_grid_sampling_options c{};
+    cticp_default_grid_sampling_options(&c);
+    c.grid_size = o.grid_size;
+    c.num_points_per_voxel = o.num_points_per_voxel;
+    c.max_num_points = o.max_num_points;
+    return c;
+}
+}  // namespace detail
+
+// SamplePointsInGrid(begin, end, options) over points in host memory, on CUDA device `device`: the indices kept, voxel by
+// voxel in order of first appearance (the reference walks an unordered_map), each voxel's points in input order
+inline std::vector<size_t> SamplePointsInGrid(const std::vector<Vec3d> &points, const GridSamplingOptions &options,
+                                              int device = 0) {
+    const cticp_grid_sampling_options o = detail::grid_options_to_c(options);
+    std::vector<uint64_t> idx(std::max<size_t>(points.size(), 1));
+    const int64_t n = cticp_sample_points_in_grid(device, &o, points.empty() ? nullptr : points[0].v, sizeof(Vec3d),
+                                                  points.size(), idx.data(), idx.size());
+    if (n < 0) ct_icp::cticp_check((int) n);
+    return std::vector<size_t>(idx.begin(), idx.begin() + n);
+}
+
+// SamplePointsInGrid grown call by call on one device: Points() / SourceIndices() always equal SamplePointsInGrid over
+// every point added so far, in call order (world points: the trajectory's RawPointsToWorldPoints of raw ones)
+class WorldCloud {
+public:
+    // capacity 0: the default rule of cticp_world_cloud_create
+    explicit WorldCloud(const GridSamplingOptions &options, uint64_t capacity_voxels = 0, uint64_t capacity_points = 0,
+                        int device = 0) {
+        const cticp_grid_sampling_options o = detail::grid_options_to_c(options);
+        ct_icp::cticp_check(cticp_world_cloud_create(&o, capacity_voxels, capacity_points, device, &h_));
+    }
+    WorldCloud(WorldCloud &&o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+    WorldCloud &operator=(WorldCloud &&o) noexcept {
+        if (this != &o) {
+            if (h_) cticp_world_cloud_destroy(h_);
+            h_ = std::exchange(o.h_, nullptr);
+        }
+        return *this;
+    }
+    WorldCloud(const WorldCloud &) = delete;
+    WorldCloud &operator=(const WorldCloud &) = delete;
+    ~WorldCloud() {
+        if (h_) cticp_world_cloud_destroy(h_);
+    }
+
+    // world points with their timestamps
+    cticp_world_cloud_stats AddWorldPoints(const std::vector<Vec3d> &xyz, const std::vector<double> &timestamps) {
+        if (xyz.size() != timestamps.size())
+            throw ct_icp::CticpFailure(CTICP_ERR_INVALID_ARGUMENT, "xyz and timestamps must have the same length");
+        std::vector<WPoint3D> rec(xyz.size());
+        for (size_t i = 0; i < xyz.size(); ++i) {
+            rec[i].raw_point.point = xyz[i];
+            rec[i].raw_point.timestamp = timestamps[i];
+        }
+        return AddRecords(rec, nullptr, false);
+    }
+    // raw points (raw_point, timestamp) placed by the trajectory; each run of equal index_frame is looked up with that
+    // frame id, as RawPointsToWorldPoints does
+    cticp_world_cloud_stats AddRawPoints(const std::vector<WPoint3D> &points, const LinearContinuousTrajectory &trajectory) {
+        return AddRecords(points, trajectory.Handle(), true);
+    }
+    cticp_world_cloud_stats AddOdometry(cticp_odometry *odometry) {
+        cticp_world_cloud_stats st{};
+        ct_icp::cticp_check(cticp_world_cloud_add_odometry(h_, odometry, &st));
+        return st;
+    }
+    size_t NumPoints() const { return (size_t) cticp_world_cloud_num_points(h_); }
+    size_t NumVoxels() const { return (size_t) cticp_world_cloud_num_voxels(h_); }
+    // the cloud as world points with their timestamps (raw_point = world_point) and their source indices
+    std::vector<WPoint3D> Points(std::vector<size_t> *source_indices = nullptr) const {
+        const size_t n = NumPoints();
+        std::vector<WPoint3D> out(n);
+        std::vector<uint64_t> src(std::max<size_t>(n, 1));
+        const cticp_cloud_sink sink{out.empty() ? nullptr : out.data(), n, sizeof(WPoint3D), 32, CTICP_DTYPE_FLOAT64,
+                                    24, CTICP_DTYPE_FLOAT64, 1};
+        const int64_t rc = cticp_world_cloud_export(h_, &sink, src.data());
+        if (rc < 0) ct_icp::cticp_check((int) rc);
+        for (auto &p : out) p.raw_point.point = p.world_point;
+        if (source_indices) source_indices->assign(src.begin(), src.begin() + n);
+        return out;
+    }
+    void Clear() { ct_icp::cticp_check(cticp_world_cloud_clear(h_)); }
+    cticp_world_cloud *Handle() const { return h_; }
+
+private:
+    cticp_world_cloud_stats AddRecords(const std::vector<WPoint3D> &points, cticp_trajectory *traj, bool by_frame) {
+        std::vector<uint64_t> ends;
+        std::vector<uint32_t> fids;
+        if (by_frame && !points.empty()) {
+            for (size_t i = 1; i < points.size(); ++i)
+                if (points[i].index_frame != points[i - 1].index_frame) {
+                    ends.push_back(i);
+                    fids.push_back(points[i - 1].index_frame);
+                }
+            ends.push_back(points.size());
+            fids.push_back(points.back().index_frame);
+        }
+        const cticp_cloud_view view{points.empty() ? nullptr : points.data(), points.size(), sizeof(WPoint3D), 0,
+                                    CTICP_DTYPE_FLOAT64, 24, CTICP_DTYPE_FLOAT64, 0};
+        cticp_world_cloud_stats st{};
+        ct_icp::cticp_check(cticp_world_cloud_add(h_, traj, &view, ends.empty() ? nullptr : ends.data(),
+                                                  fids.empty() ? nullptr : fids.data(), ends.size(), &st));
+        return st;
+    }
+
+    cticp_world_cloud *h_ = nullptr;
+};
 
 }  // namespace slam

@@ -668,6 +668,76 @@ int64_t cticp_trajectory_metrics(int device, const cticp_pose *gt, size_t n, con
  * relative poses). out: n doubles. Refusals as above (n >= 1 for both kinds). */
 int cticp_trajectory_distances(int device, const cticp_pose *gt, size_t n, int kind, double *out);
 
+/* ---- A dense map of a whole run (slam::SamplePointsInGrid, include/SlamCore/algorithm/grid_sampling.h:12-79) -----------
+ * SamplePointsInGrid keeps, per voxel int(p / grid_size) (truncation toward zero, slam::Voxel::Coordinates, so voxel 0
+ * spans (-grid_size, grid_size)), the first point that falls into it and then each later one while the voxel holds fewer
+ * than num_points_per_voxel points (so 0 and 1 both keep one). The output lists voxel by voxel, in order of first
+ * appearance, each voxel's points in input order; max_num_points >= 0 stops it at max_num_points + 1 points (the
+ * reference tests size() > max before each push), < 0 means no limit.
+ * Two deviations, where the reference has undefined behaviour: a point with a non-finite coordinate or a voxel coordinate
+ * outside [-2^20, 2^20) is rejected (not inserted, but counted and numbered), and num_points_per_voxel outside [0, 64]
+ * is CTICP_ERR_UNSUPPORTED (a voxel holds at most 64 slots; the reference's negative value means no limit). */
+typedef struct cticp_grid_sampling_options {
+    double grid_size;               /* 1.0 */
+    int32_t num_points_per_voxel;   /* 1 */
+    int32_t _pad0;
+    int64_t max_num_points;         /* -1 */
+} cticp_grid_sampling_options;
+void cticp_default_grid_sampling_options(cticp_grid_sampling_options *out);
+/* SamplePointsInGrid of n fp64 xyz triples (host memory, stride in bytes) on `device`: the indices kept, min(cap, count)
+ * of them into out_indices (nullable); returns the count. CTICP_ERR_INVALID_ARGUMENT for a grid_size that is not finite
+ * and > 0 or null pointers; CTICP_ERR_UNSUPPORTED as above. */
+int64_t cticp_sample_points_in_grid(int device, const cticp_grid_sampling_options *options, const double *xyz,
+                                    size_t stride_bytes, size_t n, uint64_t *out_indices, size_t cap);
+
+/* A world cloud: SamplePointsInGrid grown call by call on one device. After any sequence of adds, an export equals
+ * SamplePointsInGrid over the concatenation of every point submitted, in call order, bit for bit: the same points in the
+ * same order with the same fp64 values, and each point's source index (its position in that concatenation, rejected
+ * points included). Splitting the points into calls, empty ones included, does not change the export; max_num_points
+ * applies at export only. Each point is stored in fp64 with its timestamp (0.0 when the input has none).
+ * With a trajectory, a point is the world point cticp_trajectory_transform(_device) writes for it (by timestamp, or by
+ * frame id with segments), with that function's refusals; without (NULL), the records are world coordinates and may have
+ * no timestamp (t_dtype 0). Adds are synchronous on return. Every refusal happens before the cloud changes: null
+ * pointers, unknown dtypes, fields outside point_step, device pointers that are not memory of the cloud's device or
+ * buffers that end past their allocation, a trajectory or odometry on another device (CTICP_ERR_INVALID_ARGUMENT), more
+ * than 2^30 points in one call (CTICP_ERR_INVALID_ARGUMENT), and an add after which the cloud would hold more voxels or
+ * points than its capacity (CTICP_ERR_CAPACITY: the cloud stays exactly as it was). */
+typedef struct cticp_world_cloud cticp_world_cloud;   /* opaque: one device, its own stream */
+typedef struct cticp_world_cloud_stats {
+    uint64_t submitted;    /* points of the call */
+    uint64_t kept;         /* stored by the call */
+    uint64_t rejected;     /* non-finite, or outside the voxel coordinate range */
+    uint64_t new_voxels;
+} cticp_world_cloud_stats;
+/* capacity_voxels 0: clamp(2^22 (0.2 / grid_size)^2, 2^16, 2^26) voxels (16.7M at 0.1 m, 4.2M at 0.2 m);
+ * capacity_points 0: capacity_voxels × max(1, num_points_per_voxel). At most 2^30 voxels and 2^32 - 1 points. The
+ * device holds ~(44 + 4 max(1, num_points_per_voxel)) bytes per voxel and 40 bytes per point of capacity. */
+int cticp_world_cloud_create(const cticp_grid_sampling_options *options, uint64_t capacity_voxels,
+                             uint64_t capacity_points, int device, cticp_world_cloud **out);
+void cticp_world_cloud_destroy(cticp_world_cloud *wc);
+/* host records (the layouts cticp_trajectory_transform reads; t_dtype 0 = no timestamp, without a trajectory only) */
+int cticp_world_cloud_add(cticp_world_cloud *wc, cticp_trajectory *trajectory, const cticp_cloud_view *cloud,
+                          const uint64_t *segment_ends, const uint32_t *segment_frame_ids, size_t num_segments,
+                          cticp_world_cloud_stats *stats_out);
+/* device records (scan->t may be NULL with t_dtype 0, without a trajectory only), read after the work queued on `stream`
+ * (a cudaStream_t; NULL = the legacy default stream) */
+int cticp_world_cloud_add_device(cticp_world_cloud *wc, cticp_trajectory *trajectory, const cticp_device_scan *scan,
+                                 const uint64_t *segment_ends, const uint32_t *segment_frame_ids, size_t num_segments,
+                                 cticp_world_cloud_stats *stats_out, void *stream);
+/* the handle's last CTICP_POINTS_ALL_CORRECTED world points and timestamps, exactly those
+ * cticp_odometry_write_points_device writes, device to device */
+int cticp_world_cloud_add_odometry(cticp_world_cloud *wc, cticp_odometry *odometry, cticp_world_cloud_stats *stats_out);
+int64_t cticp_world_cloud_num_points(cticp_world_cloud *wc);   /* what an export returns (after max_num_points) */
+int64_t cticp_world_cloud_num_voxels(cticp_world_cloud *wc);
+/* min(capacity_points, num_points) points into a host sink (world = 1 required; sink->data may be NULL to take the
+ * source indices only) and, when src_index != NULL, as many source indices; returns num_points */
+int64_t cticp_world_cloud_export(cticp_world_cloud *wc, const cticp_cloud_sink *sink, uint64_t *src_index);
+/* the same into device memory of the cloud's device, ordered after the work queued on `stream` and before what it queues
+ * next, without a host synchronisation */
+int64_t cticp_world_cloud_export_device(cticp_world_cloud *wc, const cticp_cloud_sink *sink, uint64_t *src_index,
+                                        void *stream);
+int cticp_world_cloud_clear(cticp_world_cloud *wc);
+
 /* ---- Map (L2 boundary; used directly by the parity tests) ---------------------------------------------- */
 
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */
