@@ -246,6 +246,26 @@ class WorldCloudStats(_Struct):   # cticp_world_cloud_stats: what one add of a w
     _fields_ = [("submitted", C.c_uint64), ("kept", C.c_uint64), ("rejected", C.c_uint64), ("new_voxels", C.c_uint64)]
 
 
+class NeighborhoodDescription(_Struct):   # cticp_neighborhood_description: slam::NeighborhoodDescription<double>
+    _fields_ = [("planarity", C.c_double), ("linearity", C.c_double), ("a2D", C.c_double), ("cov_det", C.c_double),
+                ("line", C.c_double * 3), ("normal", C.c_double * 3), ("barycenter", C.c_double * 3),
+                ("covariance", C.c_double * 6), ("is_valid", C.c_int32), ("type", C.c_int32)]
+
+
+def neighborhood_description_dtype():
+    """NumPy view of cticp_neighborhood_description (160 bytes)"""
+    import numpy as np
+    return np.dtype([("planarity", "f8"), ("linearity", "f8"), ("a2D", "f8"), ("cov_det", "f8"), ("line", "f8", 3),
+                     ("normal", "f8", 3), ("barycenter", "f8", 3), ("covariance", "f8", 6), ("is_valid", "i4"),
+                     ("type", "i4")])
+
+
+# slam::NEIGHBORHOOD_PROPERTIES and slam::NEIGHBORHOOD_TYPE (neighborhood.h), the reference's values
+NB = {"NO_VALUES": 0, "LINE": 1, "NORMAL": 2, "PLANARITY": 4, "LINEARITY": 8, "COV_DET": 16, "KDTREE": 32, "A2D": 64,
+      "ALL": 127, "ALL_BUT_KDTREE": 95}
+NB_TYPE = {"NONE": 0, "LINEAR": 1, "PLANAR": 2, "VOLUMIC": 3}
+
+
 KITTI_LENGTHS = {"driving": (100., 200., 300., 400., 500., 600., 700., 800.),   # eval.h kitti_segment_lengths
                  "indoor": (10., 20., 30., 40., 50., 60., 70., 80.)}            # eval.h indoor_segment_lengths
 

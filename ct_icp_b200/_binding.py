@@ -223,6 +223,22 @@ class Binding:
             "symmetric_svd3": (None, [vp, vp, vp]),
             "ldlt_solve12": (None, [vp, vp, vp]),
         }
+        if self.prefix == "cticp_":
+            # the engine's cticp_neighborhood_describe is the index's; the oracle's orc_neighborhood_describe (above) is
+            # the KAT tap of the GN gather
+            sigs["neighborhood_describe"] = (C.c_int, [vp, vp, sz, C.c_int, dbl, C.c_int, dbl, dbl, vp])
+        sigs.update({
+            "neighborhood_describe_sets": (C.c_int, [C.c_int, vp, sz, sz, vp, sz, C.c_int, dbl, dbl, vp]),
+            "neighborhood_create": (C.c_int, [vp, sz, sz, C.c_int, P(vp)]),
+            "neighborhood_create_device": (C.c_int, [P(abi.DeviceScan), vp, C.c_int, P(vp)]),
+            "neighborhood_create_world_cloud": (C.c_int, [vp, P(vp)]),
+            "neighborhood_destroy": (None, [vp]),
+            "neighborhood_num_points": (i64, [vp]),
+            "neighborhood_num_rejected": (i64, [vp]),
+            "neighborhood_search": (C.c_int, [vp, vp, sz, C.c_int, dbl, vp, vp, vp]),
+            "neighborhood_search_device": (C.c_int, [vp, vp, sz, C.c_int, dbl, vp, vp, vp, vp]),
+            "neighborhood_describe_device": (C.c_int, [vp, vp, sz, C.c_int, dbl, C.c_int, dbl, dbl, vp, vp]),
+        })
         for name, (res, args) in sigs.items():
             if self.has(name):
                 f = self.fn(name)
@@ -430,6 +446,26 @@ class Binding:
         """A WorldCloud (cticp_world_cloud_create): SamplePointsInGrid grown add by add on `device`."""
         return WorldCloud(self, self.grid_sampling_options(grid_size, num_points_per_voxel, max_num_points),
                           capacity_voxels, capacity_points, device)
+
+    def neighborhood(self, points, device=0):
+        """A Neighborhood (cticp_neighborhood_create / _create_device): the k-nearest index of slam::TNeighborhood over
+        (n, 3) points, a NumPy array (fp64) or a torch CUDA tensor (float32 / float64, unit column stride) on `device`,
+        read after the work of torch's current stream. Index i is row i."""
+        return Neighborhood(self, points, device)
+
+    def describe_point_sets(self, points, segment_ends=None, values=abi.NB["ALL"], linearity_threshold=0.8,
+                            planarity_threshold=0.8, device=0):
+        """TNeighborhood(points).ComputeNeighborhood(values) + ClassifyNeighborhood(linearity, planarity) of each set
+        (cticp_neighborhood_describe_sets): set s is rows [segment_ends[s - 1], segment_ends[s]); None: one set of every
+        row. Returns an array of abi.neighborhood_description_dtype()."""
+        xyz = _as_f64_rows(points, 3)
+        ends = np.ascontiguousarray([len(xyz)] if segment_ends is None else segment_ends, dtype=np.uint64).reshape(-1)
+        out = np.zeros(len(ends), dtype=abi.neighborhood_description_dtype())
+        self.check(self.fn("neighborhood_describe_sets")(device, xyz.ctypes.data if len(xyz) else None, 24, len(xyz),
+                                                         ends.ctypes.data if len(ends) else None, len(ends), int(values),
+                                                         float(linearity_threshold), float(planarity_threshold),
+                                                         out.ctypes.data if len(out) else None))
+        return out
 
     def permutation(self, seed, counter, n):
         out = np.empty(n, dtype=np.uint32)
@@ -1119,6 +1155,12 @@ class WorldCloud:
     def num_voxels(self):
         return self.b.check(self.b.fn("world_cloud_num_voxels")(self.h))
 
+    def neighborhood(self):
+        """A Neighborhood over the points export() returns, in that order (cticp_neighborhood_create_world_cloud)"""
+        h = C.c_void_p()
+        self.b.check(self.b.fn("neighborhood_create_world_cloud")(self.h, C.byref(h)))
+        return Neighborhood(self.b, device=self.device, handle=h.value)
+
     def clear(self):
         self.b.check(self.b.fn("world_cloud_clear")(self.h))
 
@@ -1165,3 +1207,112 @@ class WorldCloud:
                                  code if with_timestamps else 0, 1)
             self.export_sink(sink, src)
         return (out, src) if with_source_index else out
+
+
+class Neighborhood:
+    """slam::TNeighborhood's k-nearest index and descriptions over one point set on one device (cticp_neighborhood_*).
+    search / describe take queries as an (m, 3) NumPy array (the host path) or a torch CUDA tensor on the index's device
+    (fp64, contiguous; the outputs are CUDA tensors written in order with torch's current stream); None: the indexed
+    points themselves, in index order (host outputs)."""
+
+    def __init__(self, binding, points=None, device=0, handle=None):
+        self.b = binding
+        self.device = device
+        self.h = C.c_void_p(handle) if handle is not None else C.c_void_p()
+        if handle is not None:
+            return
+        if _is_cuda_tensor(points):
+            import torch
+            if points.device.index != device:
+                raise ValueError("points must be on cuda:%d" % device)
+            if points.dim() != 2 or points.shape[1] < 3 or points.stride(1) != 1 or \
+                    points.dtype not in (torch.float32, torch.float64):
+                raise ValueError("points must be an (N, >=3) float32 / float64 tensor with unit column stride")
+            scan = abi.DeviceScan(points.data_ptr() if points.shape[0] else None, points.stride(0) * points.element_size(),
+                                  None, 0, points.shape[0], abi.DTYPE["float32" if points.dtype == torch.float32 else
+                                                                     "float64"], 0)
+            binding.check(binding.fn("neighborhood_create_device")(C.byref(scan),
+                                                                   C.c_void_p(torch.cuda.current_stream(device).cuda_stream),
+                                                                   device, C.byref(self.h)))
+        else:
+            xyz = _as_f64_rows(points, 3)
+            binding.check(binding.fn("neighborhood_create")(xyz.ctypes.data if len(xyz) else None, 24, len(xyz), device,
+                                                            C.byref(self.h)))
+
+    def close(self):
+        if self.h:
+            self.b.fn("neighborhood_destroy")(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def num_points(self):
+        return self.b.check(self.b.fn("neighborhood_num_points")(self.h))
+
+    def num_rejected(self):
+        return self.b.check(self.b.fn("neighborhood_num_rejected")(self.h))
+
+    def _queries(self, queries):
+        if queries is None:
+            return None, self.num_points()
+        q = _as_f64_rows(queries, 3)
+        return q, len(q)
+
+    def search(self, queries=None, k=1, max_radius=np.finfo(np.float64).max):
+        """NearestNeighborSearchResult(k, max_radius) + SearchNearestNeighbors for every query: (indices (m, k) uint64,
+        d2 (m, k) float64, counts (m,) int32); row q ascending by d2 (ties: lower index first), ~0 / +inf past its count."""
+        if _is_cuda_tensor(queries):
+            return self._search_device(queries, k, max_radius)
+        q, m = self._queries(queries)
+        idx = np.zeros((m, max(k, 0)), dtype=np.uint64)
+        d2 = np.zeros((m, max(k, 0)), dtype=np.float64)
+        cnt = np.zeros(m, dtype=np.int32)
+        self.b.check(self.b.fn("neighborhood_search")(self.h, q.ctypes.data if q is not None and m else None, m, int(k),
+                                                      float(max_radius), idx.ctypes.data, d2.ctypes.data,
+                                                      cnt.ctypes.data))
+        return idx, d2, cnt
+
+    def describe(self, queries=None, k=20, max_radius=np.finfo(np.float64).max, values=abi.NB["ALL"],
+                 linearity_threshold=0.8, planarity_threshold=0.8):
+        """ComputeNeighborhood(values) + ClassifyNeighborhood(linearity, planarity) of each query's k nearest: an array
+        of abi.neighborhood_description_dtype() (a torch uint8 tensor of 160-byte records for CUDA queries)."""
+        if _is_cuda_tensor(queries):
+            return self._describe_device(queries, k, max_radius, values, linearity_threshold, planarity_threshold)
+        q, m = self._queries(queries)
+        out = np.zeros(m, dtype=abi.neighborhood_description_dtype())
+        self.b.check(self.b.fn("neighborhood_describe")(self.h, q.ctypes.data if q is not None and m else None, m, int(k),
+                                                        float(max_radius), int(values), float(linearity_threshold),
+                                                        float(planarity_threshold), out.ctypes.data if m else None))
+        return out
+
+    def _device_queries(self, queries):
+        import torch
+        if queries.device.index != self.device or queries.dtype != torch.float64 or queries.dim() != 2 or \
+                queries.shape[1] != 3 or not queries.is_contiguous():
+            raise ValueError("queries must be a contiguous (m, 3) float64 tensor on cuda:%d" % self.device)
+        return torch, queries.shape[0], torch.cuda.current_stream(self.device).cuda_stream
+
+    def _search_device(self, queries, k, max_radius):
+        torch, m, stream = self._device_queries(queries)
+        dev = queries.device
+        idx = torch.empty((m, max(k, 0)), dtype=torch.int64, device=dev)
+        d2 = torch.empty((m, max(k, 0)), dtype=torch.float64, device=dev)
+        cnt = torch.empty(m, dtype=torch.int32, device=dev)
+        if m:
+            self.b.check(self.b.fn("neighborhood_search_device")(self.h, queries.data_ptr(), m, int(k), float(max_radius),
+                                                                 idx.data_ptr(), d2.data_ptr(), cnt.data_ptr(),
+                                                                 C.c_void_p(stream)))
+        return idx, d2, cnt
+
+    def _describe_device(self, queries, k, max_radius, values, lin_t, plan_t):
+        torch, m, stream = self._device_queries(queries)
+        out = torch.empty((m, abi.neighborhood_description_dtype().itemsize), dtype=torch.uint8, device=queries.device)
+        if m:
+            self.b.check(self.b.fn("neighborhood_describe_device")(self.h, queries.data_ptr(), m, int(k),
+                                                                   float(max_radius), int(values), float(lin_t),
+                                                                   float(plan_t), out.data_ptr(), C.c_void_p(stream)))
+        return out

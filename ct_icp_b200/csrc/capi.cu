@@ -8,6 +8,7 @@
 
 #include "../../include/cticp.h"
 #include "engine.h"
+#include "neighborhood.h"
 #include "trajectory.h"
 #include "trajectory_eval.h"
 #include "world_cloud.h"
@@ -78,6 +79,9 @@ struct cticp_trajectory {
 struct cticp_world_cloud {
     std::unique_ptr<WorldCloud> impl;
 };
+struct cticp_neighborhood {
+    std::unique_ptr<NeighborhoodIndex> impl;
+};
 
 extern "C" {
 
@@ -91,6 +95,7 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_map_options") return sizeof(cticp_map_options);
     if (s == "cticp_grid_sampling_options") return sizeof(cticp_grid_sampling_options);
     if (s == "cticp_world_cloud_stats") return sizeof(cticp_world_cloud_stats);
+    if (s == "cticp_neighborhood_description") return sizeof(cticp_neighborhood_description);
     if (s == "cticp_strategy_options") return sizeof(cticp_strategy_options);
     if (s == "cticp_motion_model_options") return sizeof(cticp_motion_model_options);
     if (s == "cticp_odometry_options") return sizeof(cticp_odometry_options);
@@ -781,6 +786,97 @@ int cticp_world_cloud_clear(cticp_world_cloud *wc) {
     return Guard([&] {
         if (!wc) throw std::invalid_argument("null handle");
         wc->impl->Clear();
+        return (int) CTICP_OK;
+    });
+}
+
+/* ---- neighbourhoods of a point cloud (neighborhood.cu) ---------------------------------------------------------- */
+int cticp_neighborhood_describe_sets(int device, const double *xyz, size_t stride_bytes, size_t n,
+                                     const uint64_t *segment_ends, size_t num_sets, int values,
+                                     double linearity_threshold, double planarity_threshold,
+                                     cticp_neighborhood_description *out) {
+    return Guard([&] {
+        if ((n && !xyz) || (num_sets && (!segment_ends || !out))) throw std::invalid_argument("null argument");
+        RequireDevice(device);
+        DescribePointSets(device, xyz, stride_bytes, n, segment_ends, num_sets, values, linearity_threshold,
+                          planarity_threshold, out);
+        return (int) CTICP_OK;
+    });
+}
+int cticp_neighborhood_create(const double *xyz, size_t stride_bytes, size_t n, int device, cticp_neighborhood **out) {
+    return Guard([&] {
+        if (!out || (n && !xyz)) throw std::invalid_argument("null argument");
+        RequireDevice(device);
+        auto nb = std::make_unique<cticp_neighborhood>();
+        nb->impl = std::make_unique<NeighborhoodIndex>(device);
+        nb->impl->BuildHost(xyz, stride_bytes, n);
+        *out = nb.release();
+        return (int) CTICP_OK;
+    });
+}
+int cticp_neighborhood_create_device(const cticp_device_scan *scan, void *stream, int device, cticp_neighborhood **out) {
+    return Guard([&] {
+        if (!out || !scan) throw std::invalid_argument("null argument");
+        RequireDevice(device);
+        auto nb = std::make_unique<cticp_neighborhood>();
+        nb->impl = std::make_unique<NeighborhoodIndex>(device);
+        nb->impl->BuildDevice(*scan, static_cast<cudaStream_t>(stream));
+        *out = nb.release();
+        return (int) CTICP_OK;
+    });
+}
+int cticp_neighborhood_create_world_cloud(cticp_world_cloud *wc, cticp_neighborhood **out) {
+    return Guard([&] {
+        if (!out || !wc) throw std::invalid_argument("null argument");
+        RequireDevice(wc->impl->Device());
+        auto nb = std::make_unique<cticp_neighborhood>();
+        nb->impl = std::make_unique<NeighborhoodIndex>(wc->impl->Device());
+        nb->impl->BuildWorldCloud(*wc->impl);
+        *out = nb.release();
+        return (int) CTICP_OK;
+    });
+}
+void cticp_neighborhood_destroy(cticp_neighborhood *nb) { delete nb; }
+int64_t cticp_neighborhood_num_points(cticp_neighborhood *nb) {
+    if (!nb) return Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+    return (int64_t) nb->impl->NumPoints();
+}
+int64_t cticp_neighborhood_num_rejected(cticp_neighborhood *nb) {
+    if (!nb) return Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+    return (int64_t) nb->impl->NumRejected();
+}
+int cticp_neighborhood_search(cticp_neighborhood *nb, const double *queries, size_t m, int k, double max_radius,
+                              uint64_t *indices, double *d2, int32_t *counts) {
+    return Guard([&] {
+        if (!nb) throw std::invalid_argument("null handle");
+        nb->impl->Search(queries, m, k, max_radius, indices, d2, counts);
+        return (int) CTICP_OK;
+    });
+}
+int cticp_neighborhood_search_device(cticp_neighborhood *nb, const double *queries, size_t m, int k, double max_radius,
+                                     uint64_t *indices, double *d2, int32_t *counts, void *stream) {
+    return Guard([&] {
+        if (!nb) throw std::invalid_argument("null handle");
+        nb->impl->SearchDevice(queries, m, k, max_radius, indices, d2, counts, static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+}
+int cticp_neighborhood_describe(cticp_neighborhood *nb, const double *queries, size_t m, int k, double max_radius,
+                                int values, double linearity_threshold, double planarity_threshold,
+                                cticp_neighborhood_description *out) {
+    return Guard([&] {
+        if (!nb) throw std::invalid_argument("null handle");
+        nb->impl->Describe(queries, m, k, max_radius, values, linearity_threshold, planarity_threshold, out);
+        return (int) CTICP_OK;
+    });
+}
+int cticp_neighborhood_describe_device(cticp_neighborhood *nb, const double *queries, size_t m, int k,
+                                       double max_radius, int values, double linearity_threshold,
+                                       double planarity_threshold, cticp_neighborhood_description *out, void *stream) {
+    return Guard([&] {
+        if (!nb) throw std::invalid_argument("null handle");
+        nb->impl->DescribeDevice(queries, m, k, max_radius, values, linearity_threshold, planarity_threshold, out,
+                                 static_cast<cudaStream_t>(stream));
         return (int) CTICP_OK;
     });
 }

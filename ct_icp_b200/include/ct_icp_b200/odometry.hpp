@@ -44,6 +44,7 @@ struct Vec3d {   // stand-in for Eigen::Vector3d
     double z() const { return v[2]; }
     double norm() const { return std::sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]); }
     Vec3d operator-(const Vec3d &o) const { return {{v[0] - o.v[0], v[1] - o.v[1], v[2] - o.v[2]}}; }
+    double dot(const Vec3d &o) const { return v[0] * o.v[0] + v[1] * o.v[1] + v[2] * o.v[2]; }
 };
 struct Quatd {   // stand-in for Eigen::Quaterniond (coefficients x, y, z, w)
     double c[4] = {0, 0, 0, 1};
@@ -853,5 +854,225 @@ private:
 
     cticp_world_cloud *h_ = nullptr;
 };
+
+// ---- Neighbourhoods of a point cloud (include/SlamCore/experimental/neighborhood.h) over cticp_neighborhood_*.
+// Semantics, quirks, the deviations and the refusals: include/cticp.h. Source-compatible with the reference's uses with
+// Vec3d in place of Eigen::Vector3d: TNeighborhood(points) (ComputeNeighborhood(ALL)), ComputeNeighborhood(values),
+// SearchNearestNeighbors(query, result.ResultSet()), ClassifyNeighborhood(linearity, planarity), description.*.
+enum NEIGHBORHOOD_PROPERTIES {
+    NO_VALUES = CTICP_NB_NO_VALUES,
+    LINE = CTICP_NB_LINE,
+    NORMAL = CTICP_NB_NORMAL,
+    PLANARITY = CTICP_NB_PLANARITY,
+    LINEARITY = CTICP_NB_LINEARITY,
+    COV_DET = CTICP_NB_COV_DET,
+    KDTREE = CTICP_NB_KDTREE,
+    A2D = CTICP_NB_A2D,
+    ALL = CTICP_NB_ALL,
+    ALL_BUT_KDTREE = CTICP_NB_ALL_BUT_KDTREE
+};
+enum NEIGHBORHOOD_TYPE { NONE = CTICP_NB_TYPE_NONE, LINEAR, PLANAR, VOLUMIC };
+
+// nanoflann::KNNRadiusResultSet of the reference: k slots and a bound on d2; filled by SearchNearestNeighbors
+class KNNRadiusResultSet {
+public:
+    explicit KNNRadiusResultSet(size_t capacity = 1, double radius = std::numeric_limits<double>::max())
+        : max_radius_(radius), capacity_(capacity) {}
+    void init(size_t *indices, double *dists) {
+        indices_ = indices;
+        dists_ = dists;
+        count_ = 0;
+        if (capacity_) dists_[capacity_ - 1] = std::numeric_limits<double>::max();
+    }
+    size_t size() const { return count_; }
+    bool full() const { return count_ == capacity_; }
+    double worstDist() const { return std::min(dists_[capacity_ - 1], max_radius_); }
+    size_t capacity() const { return capacity_; }
+    double max_radius() const { return max_radius_; }
+    // the k nearest as the device found them (ascending by d2, ties by index)
+    void assign(const uint64_t *indices, const double *dists, size_t count) {
+        for (size_t i = 0; i < count; ++i) {
+            indices_[i] = (size_t) indices[i];
+            dists_[i] = dists[i];
+        }
+        count_ = count;
+    }
+
+private:
+    double max_radius_;
+    size_t capacity_, count_ = 0;
+    size_t *indices_ = nullptr;
+    double *dists_ = nullptr;
+};
+typedef KNNRadiusResultSet result_set_t;
+
+class NearestNeighborSearchResult {
+public:
+    // num_neighbors < 1 is the reference's CHECK (CTICP_ERR_INVALID_ARGUMENT); above 32 a search is CTICP_ERR_UNSUPPORTED
+    explicit NearestNeighborSearchResult(int num_neighbors = 1,
+                                         double max_radius = std::numeric_limits<double>::max()) {
+        if (num_neighbors <= 0)
+            throw ct_icp::CticpFailure(CTICP_ERR_INVALID_ARGUMENT, "The knn search only works for at least 1 neighbor");
+        indices_.resize((size_t) num_neighbors);
+        distances_.resize((size_t) num_neighbors);
+        result_set_ = KNNRadiusResultSet((size_t) num_neighbors, max_radius);
+        result_set_.init(indices_.data(), distances_.data());
+    }
+    NearestNeighborSearchResult(const NearestNeighborSearchResult &) = delete;   // the result set points into *this
+    NearestNeighborSearchResult &operator=(const NearestNeighborSearchResult &) = delete;
+    KNNRadiusResultSet &ResultSet() { return result_set_; }
+    int NumValidNeighbors() const { return (int) result_set_.size(); }
+    std::vector<size_t> Indices() const { return {indices_.begin(), indices_.begin() + NumValidNeighbors()}; }
+    std::vector<double> Distances() const { return {distances_.begin(), distances_.begin() + NumValidNeighbors()}; }
+    const std::vector<size_t> &AllIndices() const { return indices_; }
+    const std::vector<double> &AllDistances() const { return distances_; }
+
+private:
+    std::vector<size_t> indices_;
+    std::vector<double> distances_;
+    KNNRadiusResultSet result_set_;
+};
+
+template <typename T>
+struct NeighborhoodDescription {
+    T planarity = T(-1.0);
+    T linearity = T(-1.0);
+    T a2D = T(-1);
+    T cov_det = T(-1.0);
+    Vec3d line, normal, barycenter;
+    std::array<std::array<T, 3>, 3> covariance{};
+};
+
+struct IdentityConversion {
+    const Vec3d &operator()(const Vec3d &p) const { return p; }
+};
+struct WorldPointConversion {
+    const Vec3d &operator()(const WPoint3D &p) const { return p.WorldPoint(); }
+};
+
+namespace detail {
+inline NeighborhoodDescription<double> description_from_c(const cticp_neighborhood_description &c) {
+    NeighborhoodDescription<double> d;
+    d.planarity = c.planarity;
+    d.linearity = c.linearity;
+    d.a2D = c.a2D;
+    d.cov_det = c.cov_det;
+    for (int a = 0; a < 3; ++a) {
+        d.line[a] = c.line[a];
+        d.normal[a] = c.normal[a];
+        d.barycenter[a] = c.barycenter[a];
+    }
+    const int ij[6][2] = {{0, 0}, {0, 1}, {0, 2}, {1, 1}, {1, 2}, {2, 2}};
+    for (int t = 0; t < 6; ++t) d.covariance[ij[t][0]][ij[t][1]] = d.covariance[ij[t][1]][ij[t][0]] = c.covariance[t];
+    return d;
+}
+}  // namespace detail
+
+// TNeighborhood<SourcePoint, Conversion>: a copy of the points, their description, and a k-nearest index on CUDA
+// device `device` (built by ComputeNeighborhood(values & KDTREE), or by the first search: every index is searchable)
+template <typename SourcePointT = Vec3d, typename Conversion = IdentityConversion>
+struct TNeighborhood {
+    typedef std::vector<SourcePointT> vector_points_t;
+    static int MinNeighborhoodSize() { return 5; }
+
+    TNeighborhood() = default;
+    explicit TNeighborhood(const std::vector<SourcePointT> &pts, int device_ = 0) : points(pts), device(device_) {
+        ComputeNeighborhood();
+    }
+
+    // the description of the points (fewer than 5: is_valid = false, nothing else changes)
+    void ComputeNeighborhood(int values = int(ALL)) {
+        if (points.size() < (size_t) MinNeighborhoodSize()) {
+            is_valid = false;
+            return;
+        }
+        const std::vector<double> xyz = Packed();
+        const uint64_t end = points.size();
+        cticp_neighborhood_description c{};
+        ct_icp::cticp_check(cticp_neighborhood_describe_sets(device, xyz.data(), 24, points.size(), &end, 1, values,
+                                                             0.8, 0.8, &c));
+        description = detail::description_from_c(c);
+        computed_values = values;
+        if (values & KDTREE) BuildIndex();
+        is_valid = true;
+    }
+
+    // the k nearest of `query` within the result set's bound; true when k were found (nanoflann's result.full())
+    bool SearchNearestNeighbors(const Vec3d &query, result_set_t &result_set) {
+        const int k = (int) result_set.capacity();
+        std::vector<uint64_t> idx((size_t) k);
+        std::vector<double> d2((size_t) k);
+        int32_t count = 0;
+        ct_icp::cticp_check(cticp_neighborhood_search(Index(), query.v, 1, k, result_set.max_radius(), idx.data(),
+                                                      d2.data(), &count));
+        result_set.assign(idx.data(), d2.data(), (size_t) count);
+        return result_set.full();
+    }
+
+    // ClassifyNeighborhood(linearity_thresh, planarity_thresh): the definition's parameter order. As in the reference,
+    // a neighbourhood with both ratios computed that passes neither leaves `neighborhood` as it was.
+    void ClassifyNeighborhood(double linearity_thresh = 0.8, double planarity_thresh = 0.8) {
+        if ((computed_values & PLANARITY) && (computed_values & LINEARITY)) {
+            if (description.planarity > planarity_thresh) neighborhood = PLANAR;
+            else if (description.linearity > linearity_thresh) neighborhood = LINEAR;
+        } else if ((computed_values & COV_DET) && points.size() > 5) {
+            neighborhood = VOLUMIC;
+        } else {
+            neighborhood = NONE;
+        }
+    }
+
+    // batched: the k nearest of every query (row q of indices / d2: k slots, ~0 / +inf past counts[q])
+    void SearchNearestNeighbors(const std::vector<Vec3d> &queries, int k, double max_radius,
+                                std::vector<uint64_t> &indices, std::vector<double> &d2, std::vector<int32_t> &counts) {
+        indices.assign(queries.size() * (size_t) std::max(k, 0), 0);
+        d2.assign(indices.size(), 0.0);
+        counts.assign(queries.size(), 0);
+        ct_icp::cticp_check(cticp_neighborhood_search(Index(), queries.empty() ? nullptr : queries[0].v, queries.size(),
+                                                      k, max_radius, indices.data(), d2.data(), counts.data()));
+    }
+    // batched: ComputeNeighborhood(values) + ClassifyNeighborhood of every query's k nearest (queries empty: every
+    // point, in order), with is_valid and the class in each record
+    std::vector<cticp_neighborhood_description> DescribeNeighborhoods(
+        const std::vector<Vec3d> &queries, int k, double max_radius = std::numeric_limits<double>::max(),
+        int values = int(ALL), double linearity_thresh = 0.8, double planarity_thresh = 0.8) {
+        const size_t m = queries.empty() ? points.size() : queries.size();
+        std::vector<cticp_neighborhood_description> out(m);
+        ct_icp::cticp_check(cticp_neighborhood_describe(Index(), queries.empty() ? nullptr : queries[0].v, m, k,
+                                                        max_radius, values, linearity_thresh, planarity_thresh,
+                                                        out.data()));
+        return out;
+    }
+
+    NeighborhoodDescription<double> description;
+    vector_points_t points;
+    int computed_values = NO_VALUES;
+    NEIGHBORHOOD_TYPE neighborhood = NONE;
+    bool is_valid = false;
+    int device = 0;
+    std::shared_ptr<cticp_neighborhood> index_;
+
+private:
+    std::vector<double> Packed() const {
+        Conversion conversion;
+        std::vector<double> xyz(3 * std::max<size_t>(points.size(), 1));
+        for (size_t i = 0; i < points.size(); ++i)
+            for (int a = 0; a < 3; ++a) xyz[3 * i + a] = conversion(points[i])[a];
+        return xyz;
+    }
+    void BuildIndex() {
+        const std::vector<double> xyz = Packed();
+        cticp_neighborhood *h = nullptr;
+        ct_icp::cticp_check(cticp_neighborhood_create(xyz.data(), 24, points.size(), device, &h));
+        index_.reset(h, cticp_neighborhood_destroy);
+    }
+    cticp_neighborhood *Index() {
+        if (!index_) BuildIndex();
+        return index_.get();
+    }
+};
+
+typedef TNeighborhood<Vec3d> Neighborhood;
+typedef TNeighborhood<WPoint3D, WorldPointConversion> WorldPointNeighborhood;
 
 }  // namespace slam

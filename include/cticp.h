@@ -738,6 +738,90 @@ int64_t cticp_world_cloud_export_device(cticp_world_cloud *wc, const cticp_cloud
                                         void *stream);
 int cticp_world_cloud_clear(cticp_world_cloud *wc);
 
+/* ---- Neighbourhoods of a point cloud (slam::TNeighborhood, include/SlamCore/experimental/neighborhood.h) -----------------
+ * Search: NearestNeighborSearchResult(k, max_radius) + SearchNearestNeighbors. The distance is squared,
+ * d2 = ((dx dx + dy dy) + dz dz) with d = query - point, in fp64 without FMA contraction (the bits a host loop gives), and
+ * max_radius bounds d2, not the distance: a point is kept only when d2 < max_radius, strictly (nanoflann's leaf test
+ * dist < worstDist()). max_radius DBL_MAX (the default) is an unbounded k-nearest search; max_radius <= 0 finds nothing; a
+ * NaN max_radius is CTICP_ERR_INVALID_ARGUMENT. The neighbours come ascending by d2, with their count; the reference's bool
+ * is count == k. k < 1 is CTICP_ERR_INVALID_ARGUMENT (the reference's CHECK), k > 32 CTICP_ERR_UNSUPPORTED.
+ * One deviation: among equal d2, the lower point index comes first (and wins the k-th place); the reference's order there
+ * follows its kd-tree traversal.
+ * Description: ComputeNeighborhood(values) + ComputeNeighborhoodInfo + ClassifyNeighborhood of a query's k nearest (the
+ * query itself included when it is an indexed point) or of a point set. Fewer than 5 points: is_valid 0, every field at its
+ * default (scalars -1, vectors 0, type NONE). Otherwise barycenter and covariance are always set, and of the rest only the
+ * fields `values` asks for (CTICP_NB_*; the others keep their defaults). line = V.col(0), normal = V.col(2) of the SVD of
+ * the covariance, signs unspecified; the singular values are taken as abs before linearity, planarity and a2D; cov_det is
+ * Eigen's 3x3 cofactor expansion. A set of coincident points gives NaN (0 / 0) in linearity, planarity and a2D.
+ * ClassifyNeighborhood(linearity_threshold, planarity_threshold) (the definition's parameter order; 0.8, 0.8): with both
+ * PLANARITY and LINEARITY computed, PLANAR when planarity > its threshold, else LINEAR when linearity > its threshold,
+ * else NONE; otherwise VOLUMIC when COV_DET is computed and the neighbourhood has more than 5 points; otherwise NONE.
+ * One deviation: the covariance is accumulated centred on the query (on the first point of a point set) instead of the
+ * reference's uncentred sum p p^T / n - mu mu^T, which cancels catastrophically at map coordinates of hundreds of metres;
+ * the two differ by no more than the reference's own cancellation error.
+ * Deviations that replace the reference's aborts: an index of fewer than 5 points is searchable; a point with a
+ * non-finite coordinate is rejected when the index is built (it keeps its index, is counted, and is never returned); a
+ * query with a non-finite coordinate has 0 neighbours. */
+enum {
+    CTICP_NB_NO_VALUES = 0,
+    CTICP_NB_LINE = 1 << 0,
+    CTICP_NB_NORMAL = 1 << 1,
+    CTICP_NB_PLANARITY = 1 << 2,
+    CTICP_NB_LINEARITY = 1 << 3,
+    CTICP_NB_COV_DET = 1 << 4,
+    CTICP_NB_KDTREE = 1 << 5,        /* accepted and ignored: every index is searchable */
+    CTICP_NB_A2D = 1 << 6,
+    CTICP_NB_ALL = 0x7F,
+    CTICP_NB_ALL_BUT_KDTREE = 0x5F
+};
+enum { CTICP_NB_TYPE_NONE = 0, CTICP_NB_TYPE_LINEAR = 1, CTICP_NB_TYPE_PLANAR = 2, CTICP_NB_TYPE_VOLUMIC = 3 };
+typedef struct cticp_neighborhood_description {   /* slam::NeighborhoodDescription<double> + is_valid + the class */
+    double planarity, linearity, a2D, cov_det;   /* -1 when not computed */
+    double line[3], normal[3];                   /* 0 when not computed */
+    double barycenter[3];
+    double covariance[6];                        /* xx xy xz yy yz zz */
+    int32_t is_valid;                            /* at least 5 points */
+    int32_t type;                                /* CTICP_NB_TYPE_* */
+} cticp_neighborhood_description;
+/* The description of num_sets point sets (ComputeNeighborhood(values) then ClassifyNeighborhood) on `device`: set s is the
+ * points [segment_ends[s - 1], segment_ends[s]) (from 0) of n fp64 xyz triples in host memory, stride_bytes apart;
+ * segment_ends must be non-decreasing and end at n. Refusals (CTICP_ERR_INVALID_ARGUMENT) before anything is written. */
+int cticp_neighborhood_describe_sets(int device, const double *xyz, size_t stride_bytes, size_t n,
+                                     const uint64_t *segment_ends, size_t num_sets, int values,
+                                     double linearity_threshold, double planarity_threshold,
+                                     cticp_neighborhood_description *out);
+/* An index over one point set on one device (at most 2^31 - 1 points). The points are stored in fp64 in the cells of a
+ * uniform grid whose size follows from the data (INTEGRATION.md, "Neighbourhoods and normals of a point cloud"); an
+ * index is immutable: rebuild it when its points change. Creation is synchronous. */
+typedef struct cticp_neighborhood cticp_neighborhood;   /* opaque: one device, its own stream */
+int cticp_neighborhood_create(const double *xyz, size_t stride_bytes, size_t n, int device, cticp_neighborhood **out);
+/* a device scan's xyz (float32 or float64; t is ignored), read after the work queued on `stream` */
+int cticp_neighborhood_create_device(const cticp_device_scan *scan, void *stream, int device, cticp_neighborhood **out);
+/* the points cticp_world_cloud_export returns, in that order (index i = export position i), device to device */
+int cticp_neighborhood_create_world_cloud(cticp_world_cloud *wc, cticp_neighborhood **out);
+void cticp_neighborhood_destroy(cticp_neighborhood *nb);
+int64_t cticp_neighborhood_num_points(cticp_neighborhood *nb);     /* indexed, the rejected ones included */
+int64_t cticp_neighborhood_num_rejected(cticp_neighborhood *nb);   /* non-finite points */
+/* m queries, fp64 xyz triples (NULL: the indexed points themselves, in index order; m must then be num_points). Writes
+ * indices[m k] and d2[m k] (row q: the neighbours of query q ascending by d2, then ~0 and +inf past its count) and
+ * counts[m]. Host buffers; synchronous. Refusals before anything is written: null outputs, k, max_radius as above. */
+int cticp_neighborhood_search(cticp_neighborhood *nb, const double *queries, size_t m, int k, double max_radius,
+                              uint64_t *indices, double *d2, int32_t *counts);
+/* the same with the queries and outputs in device memory of the index's device, ordered after the work queued on
+ * `stream` and before what it queues next, without a host synchronisation. Buffers that are not memory of that device,
+ * end past their allocation, or are not aligned to their scalar (8 bytes; 4 for counts; 8 for descriptions) are
+ * CTICP_ERR_INVALID_ARGUMENT. */
+int cticp_neighborhood_search_device(cticp_neighborhood *nb, const double *queries, size_t m, int k, double max_radius,
+                                     uint64_t *indices, double *d2, int32_t *counts, void *stream);
+/* the description of each query's k nearest (within max_radius); with queries = NULL on a world-cloud index, the
+ * normals of the whole map, aligned with its export */
+int cticp_neighborhood_describe(cticp_neighborhood *nb, const double *queries, size_t m, int k, double max_radius,
+                                int values, double linearity_threshold, double planarity_threshold,
+                                cticp_neighborhood_description *out);
+int cticp_neighborhood_describe_device(cticp_neighborhood *nb, const double *queries, size_t m, int k,
+                                       double max_radius, int values, double linearity_threshold,
+                                       double planarity_threshold, cticp_neighborhood_description *out, void *stream);
+
 /* ---- Map (L2 boundary; used directly by the parity tests) ---------------------------------------------- */
 
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */
