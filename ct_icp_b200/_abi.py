@@ -136,6 +136,19 @@ class DeviceScan(_Struct):   # cticp_device_scan: a scan in device memory (cticp
                 ("num_points", C.c_uint64), ("xyz_dtype", C.c_int32), ("t_dtype", C.c_int32)]
 
 
+class SyntheticFrame(_Struct):   # cticp_synthetic_frame: one SyntheticSensorAcquisition::GenerateFrame call
+    _fields_ = [("begin_ts", C.c_double), ("end_ts", C.c_double), ("frame_id", C.c_uint32), ("_pad0", C.c_uint32)]
+
+
+def synthetic_frame_dtype():
+    import numpy as np
+    return np.dtype({"names": ["begin_ts", "end_ts", "frame_id"], "formats": [np.float64, np.float64, np.uint32],
+                     "offsets": [0, 8, 16], "itemsize": C.sizeof(SyntheticFrame)})
+
+
+SYN = {"TRIANGLE": 0, "LINE": 1, "SPHERE": 2, "BALL": 3}   # CTICP_SYN_*: primitive kinds, in generation order
+
+
 class OdometryOptions(_Struct):
     _fields_ = [
         ("ct_icp_options", IcpOptions), ("map_options", MapOptions),

@@ -5,6 +5,7 @@ prefix "cticp_"; the test-suite binds the CPU oracle (prefix "orc_") through the
 driven by identical calls. Nothing in this module computes anything: it marshals numpy arrays and PODs.
 """
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -84,6 +85,51 @@ def _metrics_dict(m, segs):
 
 
 _SNAPSHOT_HEADER_BYTES = 72   # snapshot_format.h kHeaderBytes
+
+
+def _pose_of_spec(p):
+    """slam::ReadPosesFromYAML of one pose: the quaternion (x, y, z, w) normalised as Eigen does, dest_frame_id also
+    setting dest_timestamp, dest_timestamp overriding it"""
+    q = [float(v) for v in p.get("quaternion", (0.0, 0.0, 0.0, 1.0))]
+    if "quaternion" in p:
+        nrm = math.sqrt(((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3])
+        q = [v / nrm for v in q]
+    pose = abi.Pose.make(q, [float(v) for v in p.get("translation", (0.0, 0.0, 0.0))])
+    if "dest_frame_id" in p:
+        pose.dest_frame_id = int(p["dest_frame_id"])
+        pose.dest_timestamp = float(pose.dest_frame_id)
+    if "dest_timestamp" in p:
+        pose.dest_timestamp = float(p["dest_timestamp"])
+    return pose
+
+
+def _qrot(q, v):   # Eigen _transformVector: uv = 2 (q.vec x v); v + w uv + q.vec x uv
+    x, y, z, w = q
+    uv = (y * v[2] - z * v[1], z * v[0] - x * v[2], x * v[1] - y * v[0])
+    uv = (uv[0] + uv[0], uv[1] + uv[1], uv[2] + uv[2])
+    c = (y * uv[2] - z * uv[1], z * uv[0] - x * uv[2], x * uv[1] - y * uv[0])
+    return [v[i] + w * uv[i] + c[i] for i in range(3)]
+
+
+def _qnormalized(q):
+    nrm = math.sqrt(((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3])
+    return [v / nrm for v in q]
+
+
+def _se3_inverse(q, t):   # slam::TSE3::Inverse: quat.inverse(), tr = -(quat.inverse() * tr)
+    q = [float(v) for v in q]
+    n2 = ((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3]
+    qi = [-q[0] / n2, -q[1] / n2, -q[2] / n2, q[3] / n2]
+    return qi, [-v for v in _qrot(qi, [float(v) for v in t])]
+
+
+def _se3_mul(a, b):   # slam::TSE3::operator*: normalised product, quat.normalized() * rhs.tr + tr
+    (ax, ay, az, aw), at = a
+    (bx, by, bz, bw), bt = [float(v) for v in b[0]], [float(v) for v in b[1]]
+    q = [aw * bx + ax * bw + ay * bz - az * by, aw * by + ay * bw + az * bx - ax * bz,
+         aw * bz + az * bw + ax * by - ay * bx, aw * bw - ax * bx - ay * by - az * bz]
+    r = _qrot(_qnormalized(a[0]), bt)
+    return _qnormalized(q), [r[i] + at[i] for i in range(3)]
 
 
 def _snapshot_bytes(binding, fn, handle):
@@ -238,6 +284,15 @@ class Binding:
             "neighborhood_search": (C.c_int, [vp, vp, sz, C.c_int, dbl, vp, vp, vp]),
             "neighborhood_search_device": (C.c_int, [vp, vp, sz, C.c_int, dbl, vp, vp, vp, vp]),
             "neighborhood_describe_device": (C.c_int, [vp, vp, sz, C.c_int, dbl, C.c_int, dbl, dbl, vp, vp]),
+            "synthetic_scene_create": (C.c_int, [vp, sz, vp, sz, vp, sz, vp, sz, C.c_int, P(vp)]),
+            "synthetic_scene_destroy": (None, [vp]),
+            "synthetic_scene_num_primitives": (i64, [vp]),
+            "synthetic_scene_distance": (C.c_int, [vp, vp, sz, vp]),
+            "synthetic_generate_points": (i64, [vp, sz, vp, dbl, u64, vp, sz, vp]),
+            "synthetic_generate_frames": (i64, [vp, vp, vp, sz, sz, dbl, u64, P(abi.CloudSink), vp, vp]),
+            "synthetic_generate_frames_device": (C.c_int, [vp, vp, vp, sz, sz, dbl, u64, P(abi.CloudSink), vp, vp, vp]),
+            "synthetic_generate_poses": (i64, [vp, dbl, vp, sz]),
+            "apply_uniform_noise": (C.c_int, [vp, sz, dbl, dbl, u64]),
         })
         for name, (res, args) in sigs.items():
             if self.has(name):
@@ -465,6 +520,52 @@ class Binding:
                                                          ends.ctypes.data if len(ends) else None, len(ends), int(values),
                                                          float(linearity_threshold), float(planarity_threshold),
                                                          out.ctypes.data if len(out) else None))
+        return out
+
+    def synthetic_scene(self, triangles=(), lines=(), spheres=(), balls=(), device=0):
+        """slam::Scene on `device`: triangles (n, 3, 3), lines (n, 2, 3), spheres and balls (n, 4) as (centre, radius);
+        primitive i runs over triangles, lines, spheres, balls in that order."""
+        return SyntheticScene(self, triangles, lines, spheres, balls, device)
+
+    def apply_uniform_noise(self, poses, scale_rot_deg, scale_trans_m, seed=0):
+        """slam::ApplyUniformNoise of every pose (a copy, as an array of abi.pose_dtype()); pose i draws under key
+        (seed, noise, i)"""
+        out = _pose_array(poses).copy()
+        self.check(self.fn("apply_uniform_noise")(out.ctypes.data, len(out), float(scale_rot_deg), float(scale_trans_m),
+                                                  int(seed)))
+        return out
+
+    def synthetic_sequence(self, spec, seed=0, num_frames=None, device=False, device_index=0):
+        """ct_icp::SyntheticSequence of `spec`, the dict the reference's YAML parses to (acquisition: {poses, triangles,
+        lines, balls, spheres}, sample_frequency 10, max_lidar_distance 100, num_points_per_primitives 300). Returns a dict:
+        ground_truth (init^-1 pose_k with dest_frame_id k, abi.pose_dtype()), frames (synthetic_frame_dtype(): frame k
+        spans [pose_k.ts, pose_k+1.ts]), and the raw points of the first num_frames frames (all by default) as xyz (N, 3)
+        float64, t (N,), frame_ends (m,) and src_index (N, 2): NumPy arrays, or torch CUDA tensors on device_index with
+        device=True (generated into device memory, without a host copy of the points)."""
+        acq = spec["acquisition"]
+        freq = float(spec.get("sample_frequency", 10.0))
+        d = float(spec.get("max_lidar_distance", 100.0))
+        n = int(spec.get("num_points_per_primitives", 300))
+        poses = [_pose_of_spec(p) for p in acq["poses"]]
+        def rounds(key):   # {center, radius} items → (centre, radius) rows
+            return [list(r["center"]) + [r["radius"]] for r in (acq.get(key) or ())]
+        scene = self.synthetic_scene(acq.get("triangles") or (), acq.get("lines") or (), rounds("spheres"),
+                                     rounds("balls"), device=device_index)
+        traj = self.continuous_trajectory(poses, device=device_index)
+        sampled = traj.generate_poses(freq)
+        init_inv = _se3_inverse(sampled[0]["quat"], sampled[0]["tr"])
+        gt = sampled.copy()
+        for k in range(len(gt)):
+            gt[k]["quat"], gt[k]["tr"] = _se3_mul(init_inv, (sampled[k]["quat"], sampled[k]["tr"]))
+            gt[k]["dest_frame_id"] = k
+        frames = np.zeros(max(len(sampled) - 1, 0), dtype=abi.synthetic_frame_dtype())
+        frames["begin_ts"] = sampled["dest_timestamp"][:-1]
+        frames["end_ts"] = sampled["dest_timestamp"][1:]
+        frames["frame_id"] = np.arange(len(frames))
+        if num_frames is not None:
+            frames = frames[:num_frames]
+        out = scene.generate_frames(traj, frames, n, d, seed=seed, with_source_index=True, device=device)
+        out.update(ground_truth=gt, frames=frames, scene=scene, trajectory=traj)
         return out
 
     def permutation(self, seed, counter, n):
@@ -950,6 +1051,14 @@ class ContinuousTrajectory:
                                                          len(ts), out.ctypes.data))
         return out
 
+    def generate_poses(self, frequency):
+        """SyntheticSensorAcquisition::GeneratePoses(frequency): InterpolatePose at MinTimestamp + k / frequency (summed
+        in fp64) up to MaxTimestamp, as an array of abi.pose_dtype()"""
+        n = self.b.check(self.b.fn("synthetic_generate_poses")(self.h, float(frequency), None, 0))
+        out = np.zeros(n, dtype=abi.pose_dtype())
+        self.b.check(self.b.fn("synthetic_generate_poses")(self.h, float(frequency), out.ctypes.data, n))
+        return out
+
     def kitti_evaluate(self, gt, lengths="driving"):
         """kitti::EvaluatePoses(gt, trajectory) (cticp_trajectory_kitti_evaluate): the estimate is the pose of this
         trajectory at every ground-truth dest_timestamp, interpolated on the trajectory's device. A dict as
@@ -1315,4 +1424,126 @@ class Neighborhood:
             self.b.check(self.b.fn("neighborhood_describe_device")(self.h, queries.data_ptr(), m, int(k),
                                                                    float(max_radius), int(values), float(lin_t),
                                                                    float(plan_t), out.data_ptr(), C.c_void_p(stream)))
+        return out
+
+
+class SyntheticScene:
+    """slam::Scene with SyntheticSensorAcquisition::GenerateFrame behind the C ABI (include/cticp.h, "Synthetic scenes
+    and sequences"): the distance of points to every primitive and the generation of points and frames."""
+
+    def __init__(self, binding, triangles=(), lines=(), spheres=(), balls=(), device=0):
+        self.b = binding
+        self.device = device
+        self._arrays = [np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(-1, w))
+                        for a, w in ((triangles, 9), (lines, 6), (spheres, 4), (balls, 4))]
+        args = []
+        for a in self._arrays:
+            args += [a.ctypes.data if len(a) else None, len(a)]
+        self.h = C.c_void_p()
+        binding.check(binding.fn("synthetic_scene_create")(*args, device, C.byref(self.h)))
+
+    def close(self):
+        if self.h:
+            self.b.fn("synthetic_scene_destroy")(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def num_primitives(self):
+        return self.b.check(self.b.fn("synthetic_scene_num_primitives")(self.h))
+
+    def distance(self, points):
+        """Distance of each point (m, 3) to every primitive: an (m, num_primitives) array"""
+        q = _as_f64_rows(np.asarray(points, dtype=np.float64).reshape(-1, 3), 3)
+        out = np.zeros((len(q), self.num_primitives()))
+        self.b.check(self.b.fn("synthetic_scene_distance")(self.h, q.ctypes.data, len(q), out.ctypes.data))
+        return out
+
+    def generate_points(self, num_points_per_primitive, location=None, distance=0.0, seed=0):
+        """GeneratePoints (location None) or GeneratePointsCloseToLocation: (xyz (N, 3), src_index (N, 2) uint32)"""
+        f = self.b.fn("synthetic_generate_points")
+        loc = None if location is None else np.ascontiguousarray(location, dtype=np.float64).reshape(3)
+        lp = None if loc is None else loc.ctypes.data
+        n = self.b.check(f(self.h, num_points_per_primitive, lp, float(distance), int(seed), None, 0, None))
+        xyz = np.zeros((n, 3))
+        src = np.zeros((n, 2), dtype=np.uint32)
+        self.b.check(f(self.h, num_points_per_primitive, lp, float(distance), int(seed), xyz.ctypes.data, n,
+                       src.ctypes.data))
+        return xyz, src
+
+    @staticmethod
+    def _frames(frames):
+        if isinstance(frames, np.ndarray) and frames.dtype == abi.synthetic_frame_dtype():
+            return np.ascontiguousarray(frames)
+        out = np.zeros(len(frames), dtype=abi.synthetic_frame_dtype())
+        for k, (b, e, fid) in enumerate(frames):
+            out[k] = (b, e, fid)
+        return out
+
+    def generate_frames_sink(self, trajectory, frames, num_points_per_primitive, distance, seed, sink, src_index=None,
+                             frame_ends=None):
+        """cticp_synthetic_generate_frames into an abi.CloudSink in host memory; src_index (N, 2) uint32 and frame_ends
+        (m,) uint64 host arrays. Returns the count."""
+        fr = self._frames(frames)
+        ends = frame_ends if frame_ends is not None else np.zeros(len(fr), dtype=np.uint64)
+        return self.b.check(self.b.fn("synthetic_generate_frames")(
+            self.h, trajectory.h, fr.ctypes.data, len(fr), num_points_per_primitive, float(distance), int(seed),
+            C.byref(sink), None if src_index is None else src_index.ctypes.data, ends.ctypes.data))
+
+    def generate_frames_device(self, trajectory, frames, num_points_per_primitive, distance, seed, sink, src_index_ptr,
+                               frame_ends_ptr, stream=0):
+        """cticp_synthetic_generate_frames_device: an abi.CloudSink, src_index and frame_ends in device memory (pointers),
+        ordered after and before `stream`"""
+        fr = self._frames(frames)
+        return self.b.check(self.b.fn("synthetic_generate_frames_device")(
+            self.h, trajectory.h, fr.ctypes.data, len(fr), num_points_per_primitive, float(distance), int(seed),
+            C.byref(sink), C.c_void_p(src_index_ptr or None), C.c_void_p(frame_ends_ptr or None),
+            C.c_void_p(stream or None)))
+
+    def generate_frames(self, trajectory, frames, num_points_per_primitive, distance, seed=0, world=False,
+                        with_source_index=False, device=False):
+        """GenerateFrame of every frame ((begin_ts, end_ts, frame_id) triples or a synthetic_frame_dtype() array): a dict
+        with xyz (N, 3) float64 (raw, or world with world=True), t (N,), frame_ends (m,) uint64 and, when asked,
+        src_index (N, 2) uint32. NumPy arrays, or torch CUDA tensors with device=True (generated on the device on torch's
+        current stream: one pass counts the points, a second writes them)."""
+        fr = self._frames(frames)
+        if device:
+            return self._generate_frames_tensors(trajectory, fr, num_points_per_primitive, distance, seed, world,
+                                                 with_source_index)
+        ends = np.zeros(len(fr), dtype=np.uint64)
+        count = self.generate_frames_sink(trajectory, fr, num_points_per_primitive, distance, seed,
+                                          abi.CloudSink(None, 0, 32, 0, abi.DTYPE["float64"], 24, abi.DTYPE["float64"],
+                                                        int(world)), None, ends)
+        rec = np.zeros((count, 4))
+        src = np.zeros((count, 2), dtype=np.uint32)
+        sink = abi.CloudSink(rec.ctypes.data if count else None, count, 32, 0, abi.DTYPE["float64"], 24,
+                             abi.DTYPE["float64"], int(world))
+        self.generate_frames_sink(trajectory, fr, num_points_per_primitive, distance, seed, sink,
+                                  src if with_source_index else None, ends)
+        out = {"xyz": rec[:, :3], "t": rec[:, 3], "frame_ends": ends}
+        if with_source_index:
+            out["src_index"] = src
+        return out
+
+    def _generate_frames_tensors(self, trajectory, fr, n, distance, seed, world, with_source_index):
+        import torch
+        dev = torch.device("cuda", self.device)
+        stream = torch.cuda.current_stream(self.device).cuda_stream
+        ends = torch.zeros(len(fr), dtype=torch.int64, device=dev)
+        empty = abi.CloudSink(None, 0, 32, 0, abi.DTYPE["float64"], 24, abi.DTYPE["float64"], int(world))
+        self.generate_frames_device(trajectory, fr, n, distance, seed, empty, None, ends.data_ptr(), stream)
+        count = int(ends[-1].item()) if len(fr) else 0
+        rec = torch.empty((count, 4), dtype=torch.float64, device=dev)
+        src = torch.empty((count, 2), dtype=torch.int32, device=dev) if with_source_index else None
+        sink = abi.CloudSink(rec.data_ptr() if count else None, count, 32, 0, abi.DTYPE["float64"], 24,
+                             abi.DTYPE["float64"], int(world))
+        self.generate_frames_device(trajectory, fr, n, distance, seed, sink,
+                                    src.data_ptr() if src is not None and count else None, ends.data_ptr(), stream)
+        out = {"xyz": rec[:, :3], "t": rec[:, 3], "frame_ends": ends}
+        if with_source_index:
+            out["src_index"] = src
         return out

@@ -9,6 +9,7 @@
 #include "../../include/cticp.h"
 #include "engine.h"
 #include "neighborhood.h"
+#include "synthetic.h"
 #include "trajectory.h"
 #include "trajectory_eval.h"
 #include "world_cloud.h"
@@ -82,6 +83,9 @@ struct cticp_world_cloud {
 struct cticp_neighborhood {
     std::unique_ptr<NeighborhoodIndex> impl;
 };
+struct cticp_synthetic_scene {
+    std::unique_ptr<SyntheticScene> impl;
+};
 
 extern "C" {
 
@@ -96,6 +100,7 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_grid_sampling_options") return sizeof(cticp_grid_sampling_options);
     if (s == "cticp_world_cloud_stats") return sizeof(cticp_world_cloud_stats);
     if (s == "cticp_neighborhood_description") return sizeof(cticp_neighborhood_description);
+    if (s == "cticp_synthetic_frame") return sizeof(cticp_synthetic_frame);
     if (s == "cticp_strategy_options") return sizeof(cticp_strategy_options);
     if (s == "cticp_motion_model_options") return sizeof(cticp_motion_model_options);
     if (s == "cticp_odometry_options") return sizeof(cticp_odometry_options);
@@ -786,6 +791,83 @@ int cticp_world_cloud_clear(cticp_world_cloud *wc) {
     return Guard([&] {
         if (!wc) throw std::invalid_argument("null handle");
         wc->impl->Clear();
+        return (int) CTICP_OK;
+    });
+}
+
+/* ---- synthetic scenes and sequences (synthetic.cu) -------------------------------------------------------------- */
+int cticp_synthetic_scene_create(const double *triangles, size_t num_triangles, const double *lines, size_t num_lines,
+                                 const double *spheres, size_t num_spheres, const double *balls, size_t num_balls,
+                                 int device, cticp_synthetic_scene **out) {
+    return Guard([&] {
+        if (!out) throw std::invalid_argument("null argument");
+        RequireDevice(device);
+        auto sc = std::make_unique<cticp_synthetic_scene>();
+        sc->impl = std::make_unique<SyntheticScene>(triangles, num_triangles, lines, num_lines, spheres, num_spheres, balls,
+                                                    num_balls, device);
+        *out = sc.release();
+        return (int) CTICP_OK;
+    });
+}
+void cticp_synthetic_scene_destroy(cticp_synthetic_scene *s) { delete s; }
+int64_t cticp_synthetic_scene_num_primitives(cticp_synthetic_scene *s) {
+    if (!s) return Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+    return (int64_t) s->impl->NumPrimitives();
+}
+int cticp_synthetic_scene_distance(cticp_synthetic_scene *s, const double *points, size_t m, double *out) {
+    return Guard([&] {
+        if (!s || (m && (!points || !out))) throw std::invalid_argument("null argument");
+        s->impl->Distance(points, m, out);
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_synthetic_generate_points(cticp_synthetic_scene *s, size_t num_points_per_primitive, const double *location,
+                                        double distance, uint64_t seed, double *xyz, size_t cap, uint32_t *src_index) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!s) throw std::invalid_argument("null handle");
+        count = s->impl->GeneratePoints(num_points_per_primitive, location, distance, seed, xyz, cap, src_index);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int64_t cticp_synthetic_generate_frames(cticp_synthetic_scene *s, cticp_trajectory *t, const cticp_synthetic_frame *frames,
+                                        size_t m, size_t num_points_per_primitive, double distance, uint64_t seed,
+                                        const cticp_cloud_sink *sink, uint32_t *src_index, uint64_t *frame_ends) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!s || !t || !sink) throw std::invalid_argument("null argument");
+        count = s->impl->GenerateFrames(*t->impl, frames, m, num_points_per_primitive, distance, seed, *sink, src_index,
+                                        frame_ends);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int cticp_synthetic_generate_frames_device(cticp_synthetic_scene *s, cticp_trajectory *t,
+                                           const cticp_synthetic_frame *frames, size_t m,
+                                           size_t num_points_per_primitive, double distance, uint64_t seed,
+                                           const cticp_cloud_sink *sink, uint32_t *src_index, uint64_t *frame_ends,
+                                           void *stream) {
+    return Guard([&] {
+        if (!s || !t || !sink) throw std::invalid_argument("null argument");
+        s->impl->GenerateFramesDevice(*t->impl, frames, m, num_points_per_primitive, distance, seed, *sink, src_index,
+                                      frame_ends, static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_synthetic_generate_poses(cticp_trajectory *t, double frequency, cticp_pose *out, size_t cap) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!t) throw std::invalid_argument("null handle");
+        count = GeneratePoses(*t->impl, frequency, out, cap);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int cticp_apply_uniform_noise(cticp_pose *poses, size_t n, double scale_rot_deg, double scale_trans_m, uint64_t seed) {
+    return Guard([&] {
+        if (n && !poses) throw std::invalid_argument("null argument");
+        ApplyUniformNoise(poses, n, scale_rot_deg, scale_trans_m, seed);
         return (int) CTICP_OK;
     });
 }

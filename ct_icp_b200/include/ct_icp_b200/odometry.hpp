@@ -1076,3 +1076,286 @@ typedef TNeighborhood<Vec3d> Neighborhood;
 typedef TNeighborhood<WPoint3D, WorldPointConversion> WorldPointNeighborhood;
 
 }  // namespace slam
+
+namespace slam {
+
+// ---- Synthetic scenes and sequences (include/SlamCore/experimental/synthetic.h) over cticp_synthetic_* ----------------
+// The reference's primitives, Scene, SyntheticSensorAcquisition and ApplyUniformNoise, with its method names. Every
+// Distance and every generation runs on a device (semantics and quirks: include/cticp.h). Where the reference draws from
+// the process-global rand(), these draw under the seed member / argument (the draw contract of include/cticp.h), so a
+// call is reproducible: the same seed gives the same points. RandomPoint and the YAML readers / writers are not provided.
+class Scene;
+namespace detail {
+// one device scene over the given primitives (created per call: the primitives are plain members the caller may edit)
+inline std::shared_ptr<cticp_synthetic_scene> synthetic_scene(const Scene &scene, int device);
+}  // namespace detail
+
+class Triangle {
+public:
+    typedef std::array<Vec3d, 3> PointsArray;
+    Triangle() = default;
+    Triangle(const PointsArray &array) : points_(array) {}
+    PointsArray &Points() { return points_; }
+    const PointsArray &Points() const { return points_; }
+    Vec3d Normal() const {   // (p0 - p2) x (p1 - p2), normalized
+        const Vec3d u = points_[0] - points_[2], v = points_[1] - points_[2];
+        Vec3d n{{u[1] * v[2] - u[2] * v[1], u[2] * v[0] - u[0] * v[2], u[0] * v[1] - u[1] * v[0]}};
+        const double z = n[0] * n[0] + n[1] * n[1] + n[2] * n[2];
+        if (z > 0)
+            for (double &c : n.v) c /= std::sqrt(z);
+        return n;
+    }
+    Vec3d Barycenter() const {
+        Vec3d b;
+        for (int k = 0; k < 3; ++k) b[k] = (points_[0][k] + points_[1][k] + points_[2][k]) / 3.0;
+        return b;
+    }
+    double Distance(const Vec3d &point, int device = 0) const;
+    double ComputeDistance(const Vec3d &point) const { return Distance(point); }
+
+private:
+    PointsArray points_;
+};
+
+class Line {
+public:
+    typedef std::array<Vec3d, 2> PointsArray;
+    Line() = default;
+    Line(const PointsArray &array) : points_(array) {}
+    PointsArray &Points() { return points_; }
+    const PointsArray &Points() const { return points_; }
+    Vec3d Barycenter() const {
+        Vec3d b;
+        for (int k = 0; k < 3; ++k) b[k] = (points_[0][k] + points_[1][k]) / 2.0;
+        return b;
+    }
+    Vec3d Direction() const {   // (p0 - p1).normalized()
+        Vec3d d = points_[0] - points_[1];
+        const double z = d[0] * d[0] + d[1] * d[1] + d[2] * d[2];
+        if (z > 0)
+            for (double &c : d.v) c /= std::sqrt(z);
+        return d;
+    }
+    double Distance(const Vec3d &point, int device = 0) const;
+    double ComputeDistance(const Vec3d &point) const { return Distance(point); }
+
+private:
+    PointsArray points_;
+};
+
+// Ball and Sphere: a centre and a radius (1 and the origin by default, as the reference's)
+template <int KIND>
+class RoundPrimitive {
+public:
+    RoundPrimitive() = default;
+    RoundPrimitive(const Vec3d &center, double radius) : radius_(radius), center_(center) {}
+    double &Radius() { return radius_; }
+    double Radius() const { return radius_; }
+    Vec3d &Center() { return center_; }
+    const Vec3d &Center() const { return center_; }
+    double Distance(const Vec3d &point, int device = 0) const;
+    double ComputeDistance(const Vec3d &point) const { return Distance(point); }
+
+private:
+    double radius_ = 1.0;
+    Vec3d center_;
+};
+typedef RoundPrimitive<CTICP_SYN_BALL> Ball;
+typedef RoundPrimitive<CTICP_SYN_SPHERE> Sphere;
+
+class Scene {
+public:
+    size_t NumPrimitives() const { return triangles_.size() + lines_.size() + spheres_.size() + balls_.size(); }
+    std::vector<Triangle> &Triangles() { return triangles_; }
+    const std::vector<Triangle> &Triangles() const { return triangles_; }
+    std::vector<Line> &Lines() { return lines_; }
+    const std::vector<Line> &Lines() const { return lines_; }
+    std::vector<Sphere> &Spheres() { return spheres_; }
+    const std::vector<Sphere> &Spheres() const { return spheres_; }
+    std::vector<Ball> &Balls() { return balls_; }
+    const std::vector<Ball> &Balls() const { return balls_; }
+
+    std::vector<Vec3d> GeneratePoints(size_t num_points_per_primitive) const {
+        return Points(num_points_per_primitive, nullptr, 0.0);
+    }
+    std::vector<Vec3d> GeneratePointsCloseToLocation(size_t num_points_per_primitive, const Vec3d &location,
+                                                     double distance) const {
+        return Points(num_points_per_primitive, &location, distance);
+    }
+    // GenerateSensorPoints between two poses: begin_pose.dest_frame_id keys the draws and is every point's index_frame.
+    // The two poses are looked up as a two-pose trajectory, so they must share ref_frame_id and end_pose.dest_timestamp
+    // must not lie below begin_pose.dest_timestamp.
+    std::vector<WPoint3D> GenerateSensorPoints(size_t num_points_per_primitive, const Pose &begin_pose,
+                                               const Pose &end_pose, double distance_to_sensor) const;
+    // Distance of every point to every primitive (row q: primitives in generation order), in one launch
+    std::vector<double> Distances(const std::vector<Vec3d> &points) const {
+        std::vector<double> out(points.size() * NumPrimitives());
+        if (out.empty()) return out;
+        ct_icp::cticp_check(cticp_synthetic_scene_distance(detail::synthetic_scene(*this, device).get(), points[0].v,
+                                                           points.size(), out.data()));
+        return out;
+    }
+
+    uint64_t seed = 0;   // the draws of every generation of this scene
+    int device = 0;
+
+private:
+    std::vector<Vec3d> Points(size_t n, const Vec3d *location, double distance) const {
+        auto h = detail::synthetic_scene(*this, device);
+        const double *loc = location ? location->v : nullptr;
+        const int64_t count = cticp_synthetic_generate_points(h.get(), n, loc, distance, seed, nullptr, 0, nullptr);
+        if (count < 0) ct_icp::cticp_check((int) count);
+        std::vector<Vec3d> out((size_t) count);
+        if (count) {
+            const int64_t rc = cticp_synthetic_generate_points(h.get(), n, loc, distance, seed, out[0].v, out.size(),
+                                                               nullptr);
+            if (rc < 0) ct_icp::cticp_check((int) rc);
+        }
+        return out;
+    }
+
+    std::vector<Line> lines_;
+    std::vector<Triangle> triangles_;
+    std::vector<Ball> balls_;
+    std::vector<Sphere> spheres_;
+};
+
+namespace detail {
+inline std::shared_ptr<cticp_synthetic_scene> synthetic_scene(const Scene &scene, int device) {
+    std::vector<double> tri, lin, sph, bal;
+    for (const Triangle &t : scene.Triangles())
+        for (const Vec3d &p : t.Points()) tri.insert(tri.end(), p.v, p.v + 3);
+    for (const Line &l : scene.Lines())
+        for (const Vec3d &p : l.Points()) lin.insert(lin.end(), p.v, p.v + 3);
+    for (const Sphere &s : scene.Spheres()) {
+        sph.insert(sph.end(), s.Center().v, s.Center().v + 3);
+        sph.push_back(s.Radius());
+    }
+    for (const Ball &b : scene.Balls()) {
+        bal.insert(bal.end(), b.Center().v, b.Center().v + 3);
+        bal.push_back(b.Radius());
+    }
+    cticp_synthetic_scene *h = nullptr;
+    ct_icp::cticp_check(cticp_synthetic_scene_create(tri.data(), scene.Triangles().size(), lin.data(),
+                                                     scene.Lines().size(), sph.data(), scene.Spheres().size(),
+                                                     bal.data(), scene.Balls().size(), device, &h));
+    return std::shared_ptr<cticp_synthetic_scene>(h, cticp_synthetic_scene_destroy);
+}
+template <typename Fill>
+inline double one_primitive_distance(const Vec3d &point, int device, Fill fill) {
+    Scene s;
+    s.device = device;
+    fill(s);
+    double d = 0;
+    ct_icp::cticp_check(cticp_synthetic_scene_distance(synthetic_scene(s, device).get(), point.v, 1, &d));
+    return d;
+}
+// GenerateFrame of `frames` into the reference's point records: raw xyz and timestamp, then world xyz (the second pass
+// keeps the first's bytes), index_frame = the frame's id
+inline std::vector<WPoint3D> generate_frames(cticp_synthetic_scene *scene, cticp_trajectory *traj,
+                                             const std::vector<cticp_synthetic_frame> &frames, size_t n, double d,
+                                             uint64_t seed) {
+    std::vector<uint64_t> ends(frames.size());
+    cticp_cloud_sink raw{nullptr, 0, sizeof(WPoint3D), 0, CTICP_DTYPE_FLOAT64, 24, CTICP_DTYPE_FLOAT64, 0};
+    int64_t count = cticp_synthetic_generate_frames(scene, traj, frames.data(), frames.size(), n, d, seed, &raw, nullptr,
+                                                    ends.data());
+    if (count < 0) ct_icp::cticp_check((int) count);
+    std::vector<WPoint3D> points((size_t) count);
+    if (count == 0) return points;
+    raw.data = points.data();
+    raw.capacity_points = points.size();
+    cticp_cloud_sink world{points.data(), points.size(), sizeof(WPoint3D), 32, CTICP_DTYPE_FLOAT64, 0, 0, 1};
+    for (const cticp_cloud_sink *sink : {&raw, &world}) {
+        count = cticp_synthetic_generate_frames(scene, traj, frames.data(), frames.size(), n, d, seed, sink, nullptr,
+                                                ends.data());
+        if (count < 0) ct_icp::cticp_check((int) count);
+    }
+    size_t i = 0;
+    for (size_t k = 0; k < frames.size(); ++k)
+        for (; i < ends[k]; ++i) points[i].index_frame = frames[k].frame_id;
+    return points;
+}
+}  // namespace detail
+
+inline double Triangle::Distance(const Vec3d &point, int device) const {
+    return detail::one_primitive_distance(point, device, [&](Scene &s) { s.Triangles().push_back(*this); });
+}
+inline double Line::Distance(const Vec3d &point, int device) const {
+    return detail::one_primitive_distance(point, device, [&](Scene &s) { s.Lines().push_back(*this); });
+}
+template <int KIND>
+inline double RoundPrimitive<KIND>::Distance(const Vec3d &point, int device) const {
+    return detail::one_primitive_distance(point, device, [&](Scene &s) {
+        if (KIND == CTICP_SYN_BALL) s.Balls().emplace_back(center_, radius_);
+        else s.Spheres().emplace_back(center_, radius_);
+    });
+}
+
+inline std::vector<WPoint3D> Scene::GenerateSensorPoints(size_t num_points_per_primitive, const Pose &begin_pose,
+                                                         const Pose &end_pose, double distance_to_sensor) const {
+    std::vector<Pose> two{begin_pose, end_pose};
+    two[0].dest_frame_id = 0;   // Create sorts by (dest_frame_id, dest_timestamp): keep begin first
+    two[1].dest_frame_id = 1;
+    const LinearContinuousTrajectory traj = LinearContinuousTrajectory::Create(std::move(two), device);
+    const std::vector<cticp_synthetic_frame> frames{
+        {begin_pose.dest_timestamp, end_pose.dest_timestamp, begin_pose.dest_frame_id, 0}};
+    return detail::generate_frames(detail::synthetic_scene(*this, device).get(), traj.Handle(), frames,
+                                   num_points_per_primitive, distance_to_sensor, seed);
+}
+
+class SyntheticSensorAcquisition {
+public:
+    SyntheticSensorAcquisition(std::shared_ptr<Scene> scene, LinearContinuousTrajectory &&trajectory)
+        : scene_(std::move(scene)), base_trajectory_(std::move(trajectory)) {}
+
+    std::shared_ptr<Scene> &GetScene() { return scene_; }
+    const std::shared_ptr<Scene> &GetScene() const { return scene_; }
+    LinearContinuousTrajectory &GetTrajectory() { return base_trajectory_; }
+    const LinearContinuousTrajectory &GetTrajectory() const { return base_trajectory_; }
+
+    // GenerateFrame: begin / end = InterpolatePose(min_timestamp / max_timestamp) of the trajectory
+    std::vector<WPoint3D> GenerateFrame(size_t num_points_per_primitive, double min_timestamp, double max_timestamp,
+                                        frame_id_t frame_id, double distance_to_sensor) const {
+        return GenerateFrames(num_points_per_primitive, {{min_timestamp, max_timestamp, frame_id, 0}}, distance_to_sensor);
+    }
+    // many GenerateFrame calls in one launch, frame after frame
+    std::vector<WPoint3D> GenerateFrames(size_t num_points_per_primitive,
+                                         const std::vector<cticp_synthetic_frame> &frames,
+                                         double distance_to_sensor) const {
+        if (!scene_) throw ct_icp::CticpFailure(CTICP_ERR_INVALID_ARGUMENT, "The scene is not defined");
+        return detail::generate_frames(detail::synthetic_scene(*scene_, scene_->device).get(),
+                                       base_trajectory_.Handle(), frames, num_points_per_primitive,
+                                       distance_to_sensor, scene_->seed);
+    }
+    std::vector<Pose> GeneratePoses(double frequency = 10) const {
+        const int64_t n = cticp_synthetic_generate_poses(base_trajectory_.Handle(), frequency, nullptr, 0);
+        if (n < 0) ct_icp::cticp_check((int) n);
+        std::vector<cticp_pose> c((size_t) n);
+        const int64_t rc = cticp_synthetic_generate_poses(base_trajectory_.Handle(), frequency, c.data(), c.size());
+        if (rc < 0) ct_icp::cticp_check((int) rc);
+        std::vector<Pose> out;
+        for (const cticp_pose &p : c) out.push_back(ct_icp::detail::pose_from_c(p));
+        return out;
+    }
+
+private:
+    std::shared_ptr<Scene> scene_;
+    LinearContinuousTrajectory base_trajectory_;
+};
+
+// ApplyUniformNoise: SE3(AngleAxis_x AngleAxis_y AngleAxis_z, t) * pose; pose i of the vector draws under key
+// (seed, noise, i), a single SE3 under (seed, noise, 0). Host arithmetic; no device needed.
+inline void ApplyUniformNoise(std::vector<Pose> &poses, double scale_rot_deg, double scale_trans_m, uint64_t seed = 0) {
+    std::vector<cticp_pose> c;
+    for (const Pose &p : poses) c.push_back(ct_icp::detail::pose_to_c(p));
+    ct_icp::cticp_check(cticp_apply_uniform_noise(c.data(), c.size(), scale_rot_deg, scale_trans_m, seed));
+    for (size_t i = 0; i < poses.size(); ++i) poses[i].pose = ct_icp::detail::pose_from_c(c[i]).pose;
+}
+inline SE3 ApplyUniformNoise(const SE3 &pose, double scale_rot_deg, double scale_trans_m, uint64_t seed = 0) {
+    std::vector<Pose> one(1);
+    one[0].pose = pose;
+    ApplyUniformNoise(one, scale_rot_deg, scale_trans_m, seed);
+    return one[0].pose;
+}
+
+}  // namespace slam

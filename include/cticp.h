@@ -822,6 +822,81 @@ int cticp_neighborhood_describe_device(cticp_neighborhood *nb, const double *que
                                        double max_radius, int values, double linearity_threshold,
                                        double planarity_threshold, cticp_neighborhood_description *out, void *stream);
 
+/* ---- Synthetic scenes and sequences (include/SlamCore/experimental/synthetic.h, src/SlamCore/experimental/synthetic.cxx)
+ * slam::Scene and slam::SyntheticSensorAcquisition on the device. A scene holds triangles, lines, spheres and balls;
+ * primitive index i runs over them in that order, the order every generation emits them in. Semantics are the
+ * reference's, quirks included:
+ *   - RandomPoint, with draws r uniform on [-1, 1]: triangle weights (r_i + 1)^1.5 over their sum, then sum w_i p_i; line
+ *     weights |r_0|, |r_1| over their sum; sphere c + R normalized(r_0..2); ball c + R |r_3| normalized(r_0..2).
+ *   - Distance: triangle min(|ptp| + (inside ? 0 : corner/barycentre distance of the plane projection), corner/barycentre
+ *     distance of the point), where ptp = (x - p2).Normal(), inside = every coefficient of Eigen's ColPivHouseholderQR
+ *     solve of [p0 p1 p2] c = projection lies in [0, 1] (rank-deficient A included: the free coefficients are 0); line:
+ *     the projection p0 + sqrt(((x - p0).d)^2) d with d = normalized(p0 - p1), the distance to it plus, outside [p0, p1],
+ *     the corner/barycentre distance of the projection, then the min with that of the point; ball max(0, |x - c| - R);
+ *     sphere ||x - c| - R|.
+ *   - GenerateFrame(n, begin_ts, end_ts, frame_id, d): begin / end = InterpolatePose of the trajectory (clipped on
+ *     bounds); a primitive is used when Distance(begin.tr) < d || Distance(end.tr) < d; each of its n points draws its
+ *     world point, then alpha = u / RAND_MAX, t = begin.ts (1 - alpha) + alpha end.ts, raw = InterpolatePoseAlpha(begin,
+ *     end, alpha).pose.Inverse() * world, and is kept when |raw| < d.
+ *   - GeneratePointsCloseToLocation keeps a primitive when Distance(location) <= distance (GeneratePoints: every one).
+ * Random numbers: every draw is an integer u in [0, 2^31 - 1] from splitmix64 keyed by (seed, frame id, primitive index,
+ * point index, draw index), mapped as Eigen 3.3 maps rand(): -1 + (2 u) / RAND_MAX, and u / RAND_MAX for alpha
+ * (RAND_MAX = 2^31 - 1). A frame's points are the same bytes whether it is generated alone or in a batch. The exact
+ * key is in DESIGN.md; the reference's process-global rand() stream is not reproduced. */
+enum { CTICP_SYN_TRIANGLE = 0, CTICP_SYN_LINE = 1, CTICP_SYN_SPHERE = 2, CTICP_SYN_BALL = 3 };
+typedef struct cticp_synthetic_scene cticp_synthetic_scene;   /* opaque: one device, its own stream */
+typedef struct cticp_synthetic_frame {   /* one GenerateFrame call */
+    double begin_ts, end_ts;
+    uint32_t frame_id;
+    uint32_t _pad0;
+} cticp_synthetic_frame;
+/* triangles: 9 doubles each (p0, p1, p2), lines: 6 (p0, p1), spheres and balls: 4 (centre, radius); any array may be NULL
+ * when its count is 0. CTICP_ERR_INVALID_ARGUMENT: a non-finite value, a negative radius. The triangles are factored
+ * here, once. */
+int cticp_synthetic_scene_create(const double *triangles, size_t num_triangles, const double *lines, size_t num_lines,
+                                 const double *spheres, size_t num_spheres, const double *balls, size_t num_balls,
+                                 int device, cticp_synthetic_scene **out);
+void cticp_synthetic_scene_destroy(cticp_synthetic_scene *s);
+int64_t cticp_synthetic_scene_num_primitives(cticp_synthetic_scene *s);
+/* Distance of m fp64 xyz triples (host) to every primitive: out[q * num_primitives + i]; synchronous */
+int cticp_synthetic_scene_distance(cticp_synthetic_scene *s, const double *points, size_t m, double *out);
+/* GeneratePoints(n) (location NULL) or GeneratePointsCloseToLocation(n, location, distance): world points as fp64 xyz
+ * triples and, when src_index != NULL, (primitive, point) uint32 pairs, min(cap, count) of each. Returns the count. */
+int64_t cticp_synthetic_generate_points(cticp_synthetic_scene *s, size_t num_points_per_primitive, const double *location,
+                                        double distance, uint64_t seed, double *xyz, size_t cap, uint32_t *src_index);
+/* GenerateFrame of m frames, frame k's points after frame k-1's. sink->world selects world (1) or raw (0) coordinates,
+ * sink->t_dtype the timestamp; src_index (nullable): (primitive, point) uint32 pairs; frame_ends[m]: frame k's points
+ * end at frame_ends[k] (the segment convention of cticp_trajectory_transform). Writes min(capacity_points, count)
+ * records and as many pairs; frame_ends hold the full count. Host memory, synchronous; returns the count. The sink's bytes
+ * outside its fields are kept. */
+int64_t cticp_synthetic_generate_frames(cticp_synthetic_scene *s, cticp_trajectory *t, const cticp_synthetic_frame *frames,
+                                        size_t m, size_t num_points_per_primitive, double distance, uint64_t seed,
+                                        const cticp_cloud_sink *sink, uint32_t *src_index, uint64_t *frame_ends);
+/* The same bytes into device memory of the scene's device (sink, src_index and frame_ends; frames stay on the host),
+ * enqueued after the work queued on `stream` (NULL = the legacy default stream), which is made to wait for the result;
+ * no host synchronisation, so the count is frame_ends[m - 1] on the device and the call returns CTICP_OK. A frame's slice
+ * [frame_ends[k-1], frame_ends[k]) of a world = 0 sink is a cticp_device_scan of that frame for
+ * cticp_odometry_register_device.
+ * Refusals of both, before anything is written or enqueued: null pointers; a distance that is not finite and > 0;
+ * num_points_per_primitive < 2 (the reference's CHECK); a frame with begin_ts > end_ts or a non-finite timestamp; unknown
+ * sink dtypes or fields outside point_step; a trajectory on another device (CTICP_ERR_INVALID_ARGUMENT); device pointers
+ * that are not memory of the scene's device, end past their allocation or are not aligned (src_index 4, frame_ends 8)
+ * (CTICP_ERR_INVALID_ARGUMENT); m × num_primitives × num_points_per_primitive above 2^32 - 1 (CTICP_ERR_CAPACITY). */
+int cticp_synthetic_generate_frames_device(cticp_synthetic_scene *s, cticp_trajectory *t,
+                                           const cticp_synthetic_frame *frames, size_t m,
+                                           size_t num_points_per_primitive, double distance, uint64_t seed,
+                                           const cticp_cloud_sink *sink, uint32_t *src_index, uint64_t *frame_ends,
+                                           void *stream);
+/* SyntheticSensorAcquisition::GeneratePoses(frequency): InterpolatePose of the trajectory at MinTimestamp, then
+ * t += 1 / frequency accumulated in fp64 while t <= MaxTimestamp. Writes min(cap, count) poses, returns the count.
+ * CTICP_ERR_INVALID_ARGUMENT: a frequency that is not finite and > 0, MaxTimestamp - MinTimestamp <= 1 / frequency (the
+ * reference's CHECK). */
+int64_t cticp_synthetic_generate_poses(cticp_trajectory *t, double frequency, cticp_pose *out, size_t cap);
+/* slam::ApplyUniformNoise of each pose, in place on the host: SE3(AngleAxis_x AngleAxis_y AngleAxis_z, tr) * pose, with
+ * angles r_0..2 scale_rot_deg pi / 180 and tr r_3..5 scale_trans_m (the rotation draws first), pose i drawing under key
+ * (seed, noise, i). */
+int cticp_apply_uniform_noise(cticp_pose *poses, size_t n, double scale_rot_deg, double scale_trans_m, uint64_t seed);
+
 /* ---- Map (L2 boundary; used directly by the parity tests) ---------------------------------------------- */
 
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */
