@@ -146,6 +146,22 @@ def synthetic_frame_dtype():
                      "offsets": [0, 8, 16], "itemsize": C.sizeof(SyntheticFrame)})
 
 
+class LidarSensor(_Struct):   # cticp_lidar_sensor: a spinning LiDAR (ring elevations in host memory)
+    _fields_ = [("elevations_deg", C.c_void_p), ("n_rings", C.c_uint32), ("n_azimuth", C.c_uint32),
+                ("period", C.c_double), ("min_range", C.c_double), ("max_range", C.c_double),
+                ("noise_sigma", C.c_double)]
+
+
+class LidarFrame(_Struct):   # cticp_lidar_frame: one sweep
+    _fields_ = [("t0", C.c_double), ("frame_id", C.c_uint32), ("_pad0", C.c_uint32)]
+
+
+def lidar_frame_dtype():
+    import numpy as np
+    return np.dtype({"names": ["t0", "frame_id"], "formats": [np.float64, np.uint32], "offsets": [0, 8],
+                     "itemsize": C.sizeof(LidarFrame)})
+
+
 SYN = {"TRIANGLE": 0, "LINE": 1, "SPHERE": 2, "BALL": 3}   # CTICP_SYN_*: primitive kinds, in generation order
 
 

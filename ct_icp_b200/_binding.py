@@ -293,6 +293,13 @@ class Binding:
             "synthetic_generate_frames_device": (C.c_int, [vp, vp, vp, sz, sz, dbl, u64, P(abi.CloudSink), vp, vp, vp]),
             "synthetic_generate_poses": (i64, [vp, dbl, vp, sz]),
             "apply_uniform_noise": (C.c_int, [vp, sz, dbl, dbl, u64]),
+            "lidar_scene_create": (C.c_int, [vp, sz, vp, sz, C.c_int, C.c_int, P(vp)]),
+            "lidar_scene_destroy": (None, [vp]),
+            "lidar_scene_raycast": (C.c_int, [vp, vp, vp, sz, dbl, u64, vp]),
+            "lidar_scene_raycast_device": (C.c_int, [vp, vp, vp, sz, dbl, u64, vp, vp]),
+            "lidar_generate_sweeps": (i64, [vp, vp, P(abi.LidarSensor), vp, sz, u64, P(abi.CloudSink), vp, vp]),
+            "lidar_generate_sweeps_device": (C.c_int, [vp, vp, P(abi.LidarSensor), vp, sz, u64, P(abi.CloudSink), vp, vp,
+                                                        vp]),
         })
         for name, (res, args) in sigs.items():
             if self.has(name):
@@ -526,6 +533,11 @@ class Binding:
         """slam::Scene on `device`: triangles (n, 3, 3), lines (n, 2, 3), spheres and balls (n, 4) as (centre, radius);
         primitive i runs over triangles, lines, spheres, balls in that order."""
         return SyntheticScene(self, triangles, lines, spheres, balls, device)
+
+    def lidar_scene(self, boxes=(), cylinders=(), ground=True, device=0):
+        """A ray-cast scene on `device`: boxes (n, 7) x0 y0 z0 x1 y1 z1 mean_free_path, cylinders (n, 4) cx cy r h and
+        the ground plane z = 0 (synthetic.UrbanScene's .boxes and .cyl load as they are)."""
+        return LidarScene(self, boxes, cylinders, ground, device)
 
     def apply_uniform_noise(self, poses, scale_rot_deg, scale_trans_m, seed=0):
         """slam::ApplyUniformNoise of every pose (a copy, as an array of abi.pose_dtype()); pose i draws under key
@@ -1547,3 +1559,154 @@ class SyntheticScene:
         if with_source_index:
             out["src_index"] = src
         return out
+
+
+def _lidar_sensor(sensor):
+    """(abi.LidarSensor, the elevation array it points to) of a synthetic.SensorModel or an abi.LidarSensor-like object
+    (n_rings, n_azimuth, period, min_range, max_range, elevations in degrees top to bottom, noise_sigma)"""
+    table = getattr(sensor, "elev_table_deg", None)
+    if table is None and hasattr(sensor, "elev_max_deg"):
+        table = np.linspace(sensor.elev_max_deg, sensor.elev_min_deg, sensor.n_rings)   # synthetic.generate_scan's rings
+    elif table is None:
+        table = sensor.elevations_deg
+    elev = np.ascontiguousarray(table, dtype=np.float64).reshape(-1)
+    if len(elev) != int(sensor.n_rings):
+        raise ValueError("the elevation table has %d rings, n_rings is %d" % (len(elev), sensor.n_rings))
+    s = abi.LidarSensor(elev.ctypes.data, int(sensor.n_rings), int(sensor.n_azimuth), float(sensor.period),
+                        float(sensor.min_range), float(sensor.max_range), float(getattr(sensor, "noise_sigma", 0.0)))
+    return s, elev
+
+
+class LidarScene:
+    """A spinning-LiDAR ray-cast scene behind the C ABI (include/cticp.h, "Spinning-LiDAR sweeps"): the ranges of given
+    rays, and sweeps of a sensor along a ContinuousTrajectory into host arrays or torch CUDA tensors."""
+
+    def __init__(self, binding, boxes=(), cylinders=(), ground=True, device=0):
+        self.b = binding
+        self.device = device
+        self.boxes = np.ascontiguousarray(np.asarray(boxes, dtype=np.float64).reshape(-1, 7))
+        self.cylinders = np.ascontiguousarray(np.asarray(cylinders, dtype=np.float64).reshape(-1, 4))
+        self.h = C.c_void_p()
+        binding.check(binding.fn("lidar_scene_create")(
+            self.boxes.ctypes.data if len(self.boxes) else None, len(self.boxes),
+            self.cylinders.ctypes.data if len(self.cylinders) else None, len(self.cylinders), int(bool(ground)),
+            device, C.byref(self.h)))
+
+    def close(self):
+        if self.h:
+            self.b.fn("lidar_scene_destroy")(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def raycast(self, o, d, max_range, seed=0):
+        """The range of each ray (origins o and unit directions d, (n, 3)), +inf where nothing is hit: a float64 array,
+        or a CUDA tensor for contiguous float64 CUDA tensors on the scene's device (ordered on torch's current stream)."""
+        if _is_cuda_tensor(o) or _is_cuda_tensor(d):
+            import torch
+            for a in (o, d):
+                if not _is_cuda_tensor(a) or a.device.index != self.device or a.dtype != torch.float64 or \
+                        a.dim() != 2 or a.shape[1] != 3 or not a.is_contiguous():
+                    raise ValueError("o and d must be contiguous (n, 3) float64 tensors on cuda:%d" % self.device)
+            if o.shape[0] != d.shape[0]:
+                raise ValueError("o and d must have the same length")
+            out = torch.empty(o.shape[0], dtype=torch.float64, device=o.device)
+            if o.shape[0]:
+                stream = torch.cuda.current_stream(self.device).cuda_stream
+                self.b.check(self.b.fn("lidar_scene_raycast_device")(self.h, o.data_ptr(), d.data_ptr(), o.shape[0],
+                                                                     float(max_range), int(seed) & (2 ** 64 - 1),
+                                                                     out.data_ptr(), C.c_void_p(stream)))
+            return out
+        o = _as_f64_rows(o, 3)
+        d = _as_f64_rows(d, 3)
+        if len(o) != len(d):
+            raise ValueError("o and d must have the same length")
+        out = np.empty(len(o))
+        if len(o):
+            self.b.check(self.b.fn("lidar_scene_raycast")(self.h, o.ctypes.data, d.ctypes.data, len(o), float(max_range),
+                                                          int(seed) & (2 ** 64 - 1), out.ctypes.data))
+        return out
+
+    @staticmethod
+    def _frames(frames):
+        """an abi.lidar_frame_dtype() array of (t0, frame_id) pairs or such an array"""
+        if isinstance(frames, np.ndarray) and frames.dtype == abi.lidar_frame_dtype():
+            return np.ascontiguousarray(frames)
+        out = np.zeros(len(frames), dtype=abi.lidar_frame_dtype())
+        for k, (t0, fid) in enumerate(frames):
+            out[k] = (t0, fid)
+        return out
+
+    def sweeps_sink(self, trajectory, sensor, frames, seed, sink, ray_index=None, frame_ends=None):
+        """cticp_lidar_generate_sweeps into an abi.CloudSink in host memory; ray_index (N,) uint32 and frame_ends (m,)
+        uint64 host arrays. Returns the count."""
+        s, elev = _lidar_sensor(sensor)
+        fr = self._frames(frames)
+        ends = frame_ends if frame_ends is not None else np.zeros(len(fr), dtype=np.uint64)
+        n = self.b.check(self.b.fn("lidar_generate_sweeps")(
+            self.h, trajectory.h, C.byref(s), fr.ctypes.data if len(fr) else None, len(fr), int(seed) & (2 ** 64 - 1),
+            C.byref(sink), None if ray_index is None else ray_index.ctypes.data, ends.ctypes.data if len(fr) else None))
+        del elev
+        return n
+
+    def sweeps_device(self, trajectory, sensor, frames, seed, sink, ray_index_ptr, frame_ends_ptr, stream=0):
+        """cticp_lidar_generate_sweeps_device: an abi.CloudSink, ray_index and frame_ends in device memory (pointers),
+        ordered after and before `stream`"""
+        s, elev = _lidar_sensor(sensor)
+        fr = self._frames(frames)
+        rc = self.b.check(self.b.fn("lidar_generate_sweeps_device")(
+            self.h, trajectory.h, C.byref(s), fr.ctypes.data if len(fr) else None, len(fr), int(seed) & (2 ** 64 - 1),
+            C.byref(sink), C.c_void_p(ray_index_ptr or None), C.c_void_p(frame_ends_ptr or None),
+            C.c_void_p(stream or None)))
+        del elev
+        return rc
+
+    def sweeps(self, trajectory, sensor, frames, seed=0, dtype=np.float64, world=False, device=True):
+        """Sweeps of `sensor` (a synthetic.SensorModel, with noise_sigma 0 unless it has one) along `trajectory` for each
+        frame ((t0, frame_id) pairs or an abi.lidar_frame_dtype() array): a dict with xyz (N, 3) of `dtype` (raw, or world
+        with world=True), t (N,) float64, ray_index (N,) and frame_ends (m,). torch CUDA tensors generated on torch's
+        current stream with device=True (one pass counts the points, a second writes them); NumPy arrays otherwise."""
+        fr = self._frames(frames)
+        dt = np.dtype(dtype)
+        if dt not in (np.dtype(np.float32), np.dtype(np.float64)):
+            raise ValueError("dtype must be float32 or float64")
+        code = abi.DTYPE["float32" if dt == np.float32 else "float64"]
+        size = dt.itemsize
+        step = 3 * size + 8 + (4 if size == 4 else 0)   # x y z, pad to 8, t
+        toff = step - 8
+        if device:
+            import torch
+            dev = torch.device("cuda", self.device)
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            ends = torch.zeros(len(fr), dtype=torch.int64, device=dev)
+            if len(fr) == 0:
+                return {"xyz": torch.empty((0, 3), dtype=getattr(torch, dt.name), device=dev),
+                        "t": torch.empty(0, dtype=torch.float64, device=dev),
+                        "ray_index": torch.empty(0, dtype=torch.int32, device=dev), "frame_ends": ends}
+            empty = abi.CloudSink(None, 0, step, 0, code, toff, abi.DTYPE["float64"], int(world))
+            self.sweeps_device(trajectory, sensor, fr, seed, empty, None, ends.data_ptr(), stream)
+            count = int(ends[-1].item())
+            rec = torch.empty((count, step), dtype=torch.uint8, device=dev)
+            idx = torch.empty(count, dtype=torch.int32, device=dev)
+            sink = abi.CloudSink(rec.data_ptr() if count else None, count, step, 0, code, toff, abi.DTYPE["float64"],
+                                 int(world))
+            self.sweeps_device(trajectory, sensor, fr, seed, sink, idx.data_ptr() if count else None, ends.data_ptr(),
+                               stream)
+            xyz = rec[:, :3 * size].view(getattr(torch, dt.name))
+            t = rec[:, toff:].view(torch.float64).reshape(-1)
+            return {"xyz": xyz, "t": t, "ray_index": idx, "frame_ends": ends}
+        ends = np.zeros(len(fr), dtype=np.uint64)
+        empty = abi.CloudSink(None, 0, step, 0, code, toff, abi.DTYPE["float64"], int(world))
+        count = self.sweeps_sink(trajectory, sensor, fr, seed, empty, None, ends)
+        rec = np.zeros(count, dtype=np.dtype({"names": ["xyz", "t"], "formats": [(dt, 3), np.float64],
+                                              "offsets": [0, toff], "itemsize": step}))
+        idx = np.zeros(count, dtype=np.uint32)
+        sink = abi.CloudSink(rec.ctypes.data if count else None, count, step, 0, code, toff, abi.DTYPE["float64"],
+                             int(world))
+        self.sweeps_sink(trajectory, sensor, fr, seed, sink, idx, ends)
+        return {"xyz": np.ascontiguousarray(rec["xyz"]), "t": np.ascontiguousarray(rec["t"]), "ray_index": idx,
+                "frame_ends": ends}

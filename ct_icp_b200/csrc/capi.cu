@@ -8,6 +8,7 @@
 
 #include "../../include/cticp.h"
 #include "engine.h"
+#include "lidar_sim.h"
 #include "neighborhood.h"
 #include "synthetic.h"
 #include "trajectory.h"
@@ -86,6 +87,9 @@ struct cticp_neighborhood {
 struct cticp_synthetic_scene {
     std::unique_ptr<SyntheticScene> impl;
 };
+struct cticp_lidar_scene {
+    std::unique_ptr<LidarScene> impl;
+};
 
 extern "C" {
 
@@ -101,6 +105,8 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_world_cloud_stats") return sizeof(cticp_world_cloud_stats);
     if (s == "cticp_neighborhood_description") return sizeof(cticp_neighborhood_description);
     if (s == "cticp_synthetic_frame") return sizeof(cticp_synthetic_frame);
+    if (s == "cticp_lidar_sensor") return sizeof(cticp_lidar_sensor);
+    if (s == "cticp_lidar_frame") return sizeof(cticp_lidar_frame);
     if (s == "cticp_strategy_options") return sizeof(cticp_strategy_options);
     if (s == "cticp_motion_model_options") return sizeof(cticp_motion_model_options);
     if (s == "cticp_odometry_options") return sizeof(cticp_odometry_options);
@@ -868,6 +874,58 @@ int cticp_apply_uniform_noise(cticp_pose *poses, size_t n, double scale_rot_deg,
     return Guard([&] {
         if (n && !poses) throw std::invalid_argument("null argument");
         ApplyUniformNoise(poses, n, scale_rot_deg, scale_trans_m, seed);
+        return (int) CTICP_OK;
+    });
+}
+
+/* ---- spinning-LiDAR sweeps (lidar_sim.cu) ---------------------------------------------------------------------- */
+int cticp_lidar_scene_create(const double *boxes, size_t num_boxes, const double *cylinders, size_t num_cylinders,
+                             int ground, int device, cticp_lidar_scene **out) {
+    return Guard([&] {
+        if (!out) throw std::invalid_argument("null argument");
+        RequireDevice(device);
+        auto sc = std::make_unique<cticp_lidar_scene>();
+        sc->impl = std::make_unique<LidarScene>(boxes, num_boxes, cylinders, num_cylinders, ground != 0, device);
+        *out = sc.release();
+        return (int) CTICP_OK;
+    });
+}
+void cticp_lidar_scene_destroy(cticp_lidar_scene *s) { delete s; }
+int cticp_lidar_scene_raycast(cticp_lidar_scene *s, const double *origins, const double *directions, size_t n,
+                              double max_range, uint64_t seed, double *out) {
+    return Guard([&] {
+        if (!s) throw std::invalid_argument("null handle");
+        s->impl->Raycast(origins, directions, n, max_range, seed, out);
+        return (int) CTICP_OK;
+    });
+}
+int cticp_lidar_scene_raycast_device(cticp_lidar_scene *s, const double *origins, const double *directions, size_t n,
+                                     double max_range, uint64_t seed, double *out, void *stream) {
+    return Guard([&] {
+        if (!s) throw std::invalid_argument("null handle");
+        s->impl->RaycastDevice(origins, directions, n, max_range, seed, out, static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_lidar_generate_sweeps(cticp_lidar_scene *s, cticp_trajectory *t, const cticp_lidar_sensor *sensor,
+                                    const cticp_lidar_frame *frames, size_t m, uint64_t seed,
+                                    const cticp_cloud_sink *sink, uint32_t *ray_index, uint64_t *frame_ends) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!s || !t || !sensor || !sink) throw std::invalid_argument("null argument");
+        count = s->impl->GenerateSweeps(*t->impl, *sensor, frames, m, seed, *sink, ray_index, frame_ends);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int cticp_lidar_generate_sweeps_device(cticp_lidar_scene *s, cticp_trajectory *t, const cticp_lidar_sensor *sensor,
+                                       const cticp_lidar_frame *frames, size_t m, uint64_t seed,
+                                       const cticp_cloud_sink *sink, uint32_t *ray_index, uint64_t *frame_ends,
+                                       void *stream) {
+    return Guard([&] {
+        if (!s || !t || !sensor || !sink) throw std::invalid_argument("null argument");
+        s->impl->GenerateSweepsDevice(*t->impl, *sensor, frames, m, seed, *sink, ray_index, frame_ends,
+                                      static_cast<cudaStream_t>(stream));
         return (int) CTICP_OK;
     });
 }

@@ -189,28 +189,6 @@ __global__ void __launch_bounds__(kThreads) k_select(const SynPrim *__restrict__
     }
 }
 
-struct SinkArgs {
-    unsigned char *data;
-    uint64_t cap;
-    uint32_t step, xoff, toff;
-    int xdt, tdt, x_aligned, t_aligned, world;
-};
-
-__device__ __forceinline__ void store_record(const SinkArgs &s, uint64_t pos, const V3 &p, double t) {
-    unsigned char *rec = s.data + pos * s.step;
-    if (s.xdt == CTICP_DTYPE_FLOAT32) {
-        store_field<float>(rec + s.xoff, scan_pack::hi_of(p.x), s.x_aligned);
-        store_field<float>(rec + s.xoff + 4, scan_pack::hi_of(p.y), s.x_aligned);
-        store_field<float>(rec + s.xoff + 8, scan_pack::hi_of(p.z), s.x_aligned);
-    } else {
-        store_field<double>(rec + s.xoff, p.x, s.x_aligned);
-        store_field<double>(rec + s.xoff + 8, p.y, s.x_aligned);
-        store_field<double>(rec + s.xoff + 16, p.z, s.x_aligned);
-    }
-    if (s.tdt == CTICP_DTYPE_FLOAT32) store_field<float>(rec + s.toff, scan_pack::hi_of(t), s.t_aligned);
-    else if (s.tdt == CTICP_DTYPE_FLOAT64) store_field<double>(rec + s.toff, t, s.t_aligned);
-}
-
 struct GenArgs {
     const SynPrim *prims;
     uint32_t np;
@@ -226,7 +204,7 @@ struct GenArgs {
 };
 
 // One tile = (frame f, primitive p, points [c kTile, (c + 1) kTile)); thread j holds points c kTile + kPerThread j + k.
-__global__ void __launch_bounds__(kThreads, 2) k_generate(GenArgs g, SinkArgs sink) {
+__global__ void __launch_bounds__(kThreads, 2) k_generate(GenArgs g, GenSink sink) {
     __shared__ unsigned long long s_tile;
     __shared__ uint32_t s_warp[kThreads / 32];
     __shared__ uint32_t s_base;
@@ -309,7 +287,7 @@ __global__ void __launch_bounds__(kThreads, 2) k_generate(GenArgs g, SinkArgs si
             if (!((keep >> k) & 1u)) continue;
             const uint64_t out = base + before + pos++;
             if (out < sink.cap) {
-                if (sink.data) store_record(sink, out, pts[k], ts[k]);
+                if (sink.data) store_gen_record(sink, out, pts[k], ts[k]);
                 if (g.src) {
                     g.src[2 * out] = p;
                     g.src[2 * out + 1] = (uint32_t) (c * kTile + (uint64_t) threadIdx.x * kPerThread + k);
@@ -333,24 +311,6 @@ void CheckFinite(const double *v, uint64_t n, const char *what) {
 
 void CheckDistance(double d) {
     if (!std::isfinite(d) || !(d > 0.0)) throw std::invalid_argument("distance must be finite and > 0");
-}
-
-SinkArgs MakeSink(unsigned char *data, const cticp_cloud_sink &sink, uint64_t cap) {
-    SinkArgs sa{};
-    sa.data = data;
-    sa.cap = cap;
-    sa.step = sink.point_step;
-    sa.xoff = sink.xyz_offset;
-    sa.toff = sink.t_offset;
-    sa.xdt = sink.xyz_dtype;
-    sa.tdt = sink.t_dtype;
-    sa.world = sink.world ? 1 : 0;
-    if (data) {
-        const size_t osz = sink.xyz_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8, otsz = sink.t_dtype == CTICP_DTYPE_FLOAT32 ? 4 : 8;
-        sa.x_aligned = ((reinterpret_cast<uintptr_t>(data) + sink.xyz_offset) % osz == 0 && sink.point_step % osz == 0);
-        sa.t_aligned = ((reinterpret_cast<uintptr_t>(data) + sink.t_offset) % otsz == 0 && sink.point_step % otsz == 0);
-    }
-    return sa;
 }
 
 }  // namespace
@@ -560,7 +520,7 @@ void SyntheticScene::Launch(int mode, const Plan &plan, double distance, const d
     g.ends = frame_ends;
     // as many CTAs as are resident at once (tiles are handed out by the ticket, so any grid size is correct)
     const int blocks = (int) std::min<uint64_t>(plan.tiles, (uint64_t) sms_ * generate_ctas_per_sm_);
-    k_generate<<<blocks, kThreads, 0, s>>>(g, MakeSink(sink_data, sink, sink_cap));
+    k_generate<<<blocks, kThreads, 0, s>>>(g, MakeGenSink(sink_data, sink, sink_cap));
     CT_CUDA_CHECK(cudaGetLastError());
 }
 

@@ -1358,4 +1358,80 @@ inline SE3 ApplyUniformNoise(const SE3 &pose, double scale_rot_deg, double scale
     return one[0].pose;
 }
 
+// ---- Spinning-LiDAR sweeps over cticp_lidar_* -------------------------------------------------------------------------
+// A ray-cast scene of a ground plane, axis-aligned boxes (solid or porous) and vertical cylinders, owned on one device,
+// with the ranges of given rays and sweeps of a spinning sensor along a trajectory (semantics: include/cticp.h).
+struct LidarSensor {
+    std::vector<double> elevations_deg;   // one per ring, top to bottom
+    uint32_t n_azimuth = 2083;
+    double period = 0.1, min_range = 3.0, max_range = 100.0, noise_sigma = 0.0;
+};
+
+class LidarScene {
+public:
+    // boxes: x0 y0 z0 x1 y1 z1 mean_free_path (0 = solid); cylinders: cx cy r h
+    LidarScene(const std::vector<std::array<double, 7>> &boxes, const std::vector<std::array<double, 4>> &cylinders,
+               bool ground = true, int device = 0) {
+        ct_icp::cticp_check(cticp_lidar_scene_create(boxes.empty() ? nullptr : boxes[0].data(), boxes.size(),
+                                                     cylinders.empty() ? nullptr : cylinders[0].data(), cylinders.size(),
+                                                     ground ? 1 : 0, device, &h_));
+    }
+    ~LidarScene() {
+        if (h_) cticp_lidar_scene_destroy(h_);
+    }
+    LidarScene(LidarScene &&o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+    LidarScene &operator=(LidarScene &&o) noexcept {
+        std::swap(h_, o.h_);
+        return *this;
+    }
+    LidarScene(const LidarScene &) = delete;
+    LidarScene &operator=(const LidarScene &) = delete;
+    cticp_lidar_scene *Handle() const { return h_; }
+
+    // the range of each ray (origin, unit direction; ray i keys the porous draws), +inf where nothing is hit
+    std::vector<double> Raycast(const std::vector<Vec3d> &origins, const std::vector<Vec3d> &directions, double max_range,
+                                uint64_t seed) const {
+        if (origins.size() != directions.size())
+            throw ct_icp::CticpFailure(CTICP_ERR_INVALID_ARGUMENT, "origins and directions differ in length");
+        std::vector<double> out(origins.size());
+        if (!out.empty())
+            ct_icp::cticp_check(cticp_lidar_scene_raycast(h_, origins[0].v, directions[0].v, out.size(), max_range, seed,
+                                                          out.data()));
+        return out;
+    }
+    // the sweeps of `frames` into the reference's point records: raw xyz and timestamp, world xyz, index_frame = the
+    // frame's id; frame_ends (nullable) gets each frame's end
+    std::vector<WPoint3D> GenerateSweeps(const LinearContinuousTrajectory &trajectory, const LidarSensor &sensor,
+                                         const std::vector<cticp_lidar_frame> &frames, uint64_t seed,
+                                         std::vector<uint64_t> *frame_ends = nullptr) const {
+        const cticp_lidar_sensor cs{sensor.elevations_deg.data(), (uint32_t) sensor.elevations_deg.size(),
+                                    sensor.n_azimuth, sensor.period, sensor.min_range, sensor.max_range,
+                                    sensor.noise_sigma};
+        std::vector<uint64_t> ends(frames.size());
+        cticp_cloud_sink raw{nullptr, 0, sizeof(WPoint3D), 0, CTICP_DTYPE_FLOAT64, 24, CTICP_DTYPE_FLOAT64, 0};
+        int64_t count = cticp_lidar_generate_sweeps(h_, trajectory.Handle(), &cs, frames.data(), frames.size(), seed, &raw,
+                                                    nullptr, ends.data());
+        if (count < 0) ct_icp::cticp_check((int) count);
+        std::vector<WPoint3D> points((size_t) count);
+        if (count) {
+            raw.data = points.data();
+            raw.capacity_points = points.size();
+            cticp_cloud_sink world{points.data(), points.size(), sizeof(WPoint3D), 32, CTICP_DTYPE_FLOAT64, 0, 0, 1};
+            for (const cticp_cloud_sink *sink : {&raw, &world}) {
+                count = cticp_lidar_generate_sweeps(h_, trajectory.Handle(), &cs, frames.data(), frames.size(), seed,
+                                                    sink, nullptr, ends.data());
+                if (count < 0) ct_icp::cticp_check((int) count);
+            }
+            size_t i = 0;
+            for (size_t k = 0; k < frames.size(); ++k)
+                for (; i < ends[k]; ++i) points[i].index_frame = frames[k].frame_id;
+        }
+        if (frame_ends) *frame_ends = ends;
+        return points;
+    }
+
+private:
+    cticp_lidar_scene *h_ = nullptr;
+};
+
 }  // namespace slam

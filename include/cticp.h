@@ -897,6 +897,78 @@ int64_t cticp_synthetic_generate_poses(cticp_trajectory *t, double frequency, ct
  * (seed, noise, i). */
 int cticp_apply_uniform_noise(cticp_pose *poses, size_t n, double scale_rot_deg, double scale_trans_m, uint64_t seed);
 
+/* ---- Spinning-LiDAR sweeps (a ray-cast scene of a ground plane, axis-aligned boxes and vertical cylinders) --------------
+ * A scene holds an optional ground plane z = 0, boxes (x0 y0 z0 x1 y1 z1 mean_free_path; 0 = solid, > 0 = porous) and
+ * vertical cylinders (cx cy r h, from z = 0 to h). The range of a ray (origin o, unit direction d, index i in its call,
+ * max_range R, 64-bit seed) is the minimum over this candidate set, +INFINITY when it is empty, all in fp64 without FMA:
+ *   - ground: -o.z / d.z when d.z < 0 and that is > 0;
+ *   - box b (its index in the array as given), unless x1 < o.x - R or x0 > o.x + R: the slab test with the reciprocals
+ *     1 / d, fmin / fmax per axis; none when !(tmax >= tmin) or tmin <= 0. A solid box gives tmin; a porous one gives
+ *     t = tmin - mfp log(u), u = ((h >> 11) + 0.5) 2^-53, h = splitmix64(seed ^ splitmix64(i 1315423911 + b)) (mod 2^64),
+ *     dropped when t > tmax;
+ *   - cylinder, unless |cx - o.x| > R: a = dx dx + dy dy, b = 2 (px dx + py dy), c = px px + py py - r r with
+ *     p = o - (cx, cy); none when a < 1e-12 or disc = b b - 4 a c <= 0; t = (-b - sqrt(disc)) / (2 a), none when t <= 0 or
+ *     z = o.z + t d.z lies outside [0, h].
+ * R prunes by x only and does not clip the range: a box inside the x-window may be hit beyond R. The device's log may
+ * differ from the host C library's in the last bit, so a porous return may differ by a few ulp; every other range is the
+ * host's bit for bit. A ray with a non-finite component gets NaN.
+ * Sweeps: rays i = ring n_azimuth + j of a frame (t0, frame_id) point along (cos el cos az, cos el sin az, sin el) in the
+ * sensor frame, el = elevations_deg[ring] pi / 180, az = (-2 pi j) / n_azimuth (clockwise), with cos and sin from the host
+ * C library; the column's timestamp is t0 + ((j + 0.5) / n_azimuth) period and its pose is the trajectory's
+ * InterpolatePose there (cticp_trajectory_interpolate's bits). The ray starts at the pose's translation with the direction
+ * quat.normalized() * d_sensor and is cast with seed * 1000003 + frame_id (mod 2^64) and its index i. When
+ * noise_sigma > 0 the range gets noise_sigma z, z a Box-Muller normal of two splitmix64 draws keyed by (seed, frame_id, i)
+ * (DESIGN.md §5.10 has the key). The ray is kept when the range r is finite and min_range < r < max_range: raw xyz is
+ * d_sensor r, world xyz origin + d_world r, the timestamp the column's. Points come in (frame, i) order. */
+typedef struct cticp_lidar_scene cticp_lidar_scene;   /* opaque: one device, its own stream */
+typedef struct cticp_lidar_sensor {
+    const double *elevations_deg;   /* n_rings ring elevations, top to bottom (host memory) */
+    uint32_t n_rings, n_azimuth;
+    double period;                  /* seconds per revolution */
+    double min_range, max_range;    /* the keep bounds (exclusive); max_range is also the cast's R */
+    double noise_sigma;             /* >= 0, metres */
+} cticp_lidar_sensor;
+typedef struct cticp_lidar_frame {   /* one sweep */
+    double t0;
+    uint32_t frame_id;
+    uint32_t _pad0;
+} cticp_lidar_frame;
+/* boxes: num_boxes × 7 doubles, cylinders: num_cylinders × 4 (either NULL when its count is 0); ground != 0 adds the
+ * plane. CTICP_ERR_INVALID_ARGUMENT: a non-finite value, x0 > x1 (or y, z), r < 0, a negative free path. The primitives
+ * are binned into a uniform xy grid on the device here, once. */
+int cticp_lidar_scene_create(const double *boxes, size_t num_boxes, const double *cylinders, size_t num_cylinders,
+                             int ground, int device, cticp_lidar_scene **out);
+void cticp_lidar_scene_destroy(cticp_lidar_scene *s);
+/* The ranges of n rays (fp64 xyz triples, ray i = index i) into out[n]. Host memory, synchronous. CTICP_ERR_INVALID_ARGUMENT:
+ * null pointers, a NaN or non-positive max_range, a non-finite origin or direction component. */
+int cticp_lidar_scene_raycast(cticp_lidar_scene *s, const double *origins, const double *directions, size_t n,
+                              double max_range, uint64_t seed, double *out);
+/* The same on device memory of the scene's device (8-byte aligned, inside their allocations), enqueued after the work
+ * queued on `stream` (NULL = the legacy default stream), which is made to wait for the result; no host synchronisation. */
+int cticp_lidar_scene_raycast_device(cticp_lidar_scene *s, const double *origins, const double *directions, size_t n,
+                                     double max_range, uint64_t seed, double *out, void *stream);
+/* m sweeps, frame k's points after frame k-1's. sink->world selects world (1) or raw (0) coordinates, sink->t_dtype the
+ * timestamp; ray_index (nullable): each point's ray i; frame_ends[m]: frame k's points end at frame_ends[k]. Writes
+ * min(capacity_points, count) records and as many ray indices; frame_ends hold the full count. Host memory, synchronous;
+ * returns the count. The sink's bytes outside its fields are kept. A frame is the same bytes alone or in a batch. */
+int64_t cticp_lidar_generate_sweeps(cticp_lidar_scene *s, cticp_trajectory *t, const cticp_lidar_sensor *sensor,
+                                    const cticp_lidar_frame *frames, size_t m, uint64_t seed,
+                                    const cticp_cloud_sink *sink, uint32_t *ray_index, uint64_t *frame_ends);
+/* The same bytes into device memory of the scene's device (sink, ray_index and frame_ends; sensor and frames stay on the
+ * host), enqueued after the work queued on `stream`, which is made to wait for the result; no host synchronisation, so
+ * the count is frame_ends[m - 1] on the device and the call returns CTICP_OK. A frame's slice [frame_ends[k-1],
+ * frame_ends[k]) of a world = 0 sink with a timestamp is a cticp_device_scan of that frame for
+ * cticp_odometry_register_device.
+ * Refusals of both, before anything is written or enqueued: null pointers; n_rings or n_azimuth 0; a non-finite
+ * elevation, t0, period or range bound; a NaN or negative noise_sigma; unknown sink dtypes or fields outside point_step;
+ * a trajectory on another device (CTICP_ERR_INVALID_ARGUMENT); device pointers that are not memory of the scene's device,
+ * end past their allocation or are not aligned (ray_index 4, frame_ends 8) (CTICP_ERR_INVALID_ARGUMENT);
+ * m × n_rings × n_azimuth above 2^32 - 1 (CTICP_ERR_CAPACITY). */
+int cticp_lidar_generate_sweeps_device(cticp_lidar_scene *s, cticp_trajectory *t, const cticp_lidar_sensor *sensor,
+                                       const cticp_lidar_frame *frames, size_t m, uint64_t seed,
+                                       const cticp_cloud_sink *sink, uint32_t *ray_index, uint64_t *frame_ends,
+                                       void *stream);
+
 /* ---- Map (L2 boundary; used directly by the parity tests) ---------------------------------------------- */
 
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */
