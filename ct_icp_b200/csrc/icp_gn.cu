@@ -32,6 +32,27 @@ namespace cg = cooperative_groups;
 #endif
 constexpr int kGatherWarps = CTICP_GATHER_WARPS;
 
+// The warp-specialised layout of the single-GPU k_gn_persistent (gn_ws_loop): six warpgroups, 768 threads. Warpgroups
+// 0-4 are gather warps (phase B only), warpgroup 5 the math warps (the pose, phases A and C one keypoint per lane, and
+// in the solver CTA the 12x12 solve). setmaxnreg moves registers from the gather warps to the math warps: 80 per thread
+// at launch (65536 / 768, in steps of 8), then 72 for the gather warps and 120 for the math warps — 20 x 32 x 72 +
+// 4 x 32 x 120 = 768 x 80, the CTA's allocation at launch.
+constexpr int kWsGatherWarps = 20;
+constexpr int kWsMathWarps = 4;
+constexpr int kWsWarps = kWsGatherWarps + kWsMathWarps;
+#ifndef CTICP_WS_GATHER_REGS
+#define CTICP_WS_GATHER_REGS 72
+#endif
+constexpr int kWsGatherRegs = CTICP_WS_GATHER_REGS;
+constexpr int kWsMathRegs = (kWsWarps * 80 - kWsGatherWarps * kWsGatherRegs) / kWsMathWarps;
+static_assert(kWsGatherWarps % 4 == 0 && kWsMathWarps == 4 && kWsGatherWarps >= kGatherWarps, "warpgroups");
+static_assert(kWsMathRegs <= 256 && kWsMathRegs % 8 == 0, "setmaxnreg");
+// phase A of one keypoint: its world position and voxel
+struct WsQuery {
+    double x, y, z;
+    int kx, ky, kz;
+};
+
 
 
 struct GatherLaunch {
@@ -63,7 +84,7 @@ struct GnGroup {
 // dynamically — a warp whose keypoint has a sparse stencil takes the next one while a neighbour is still busy with a
 // dense one — and the registration stays bit-reproducible. Per-warp clock64 stamps of the static tiles of
 // two that came before showed a long tail of slow tiles, and every iteration waited for the slowest while half of the
-// warps had no tile at all. The exception (gn_pair_schedule): in k_gn_persistent, a range of more keypoints than warps but
+// warps had no tile at all. The exception (gn_pair_schedule): in the sharded k_gn_persistent, a range of more keypoints than warps but
 // at most two per warp gets one tile per warp from the last iteration's costs (the first iteration: in keypoint order) —
 // the heaviest keypoints alone, the others in pairs — instead of a few warps running a second whole chain after their
 // first.
@@ -84,11 +105,83 @@ constexpr int kTileMax = 16;   // keypoints per warp tile (phases A / C cost 1/W
 constexpr int kRowCap = 256;   // rows of a CTA's range held in shared memory at a time (longer ranges go in chunks)
 constexpr int kRowParts = 5;   // the row reduction splits the rows over 5 x 96 threads
 
+// The moments of one keypoint as phase B hands them to phase C: [0] the kept neighbours (low word) and the stencil points
+// (high word) — two integers in one slot, no int <-> double conversion —, [1..12] s*, f* of NeighborSums (only when at
+// least `need` neighbours were kept). As wide as a row of CtaRows::u, which the warp-specialised loop stores them in.
+constexpr int kMomentWords = 13;
+__device__ __forceinline__ void gn_store_moments(double *o, const NeighborSums &s, unsigned spts, int need) {
+    o[0] = __hiloint2double((int) spts, s.n);
+    if (s.n >= need) {
+        o[1] = s.sx; o[2] = s.sy; o[3] = s.sz;
+        o[4] = s.sxx; o[5] = s.sxy; o[6] = s.sxz; o[7] = s.syy; o[8] = s.syz; o[9] = s.szz;
+        o[10] = s.fx; o[11] = s.fy; o[12] = s.fz;
+    }
+}
+__device__ __forceinline__ unsigned moments_stencil_points(const double *o) { return (unsigned) __double2hiint(o[0]); }
+
+// ---- A: world_kpts[i] = InterpolatePose(begin, end, t_i) * raw_i  (ct_icp.cpp:964-966, types.h:361-366): the world
+// position of a keypoint (`kraw`: raw xyz in the sensor frame + alpha timestamp, load_raw) and its voxel. Every schedule
+// calls this one function, so the arithmetic is one instruction sequence.
+__device__ __forceinline__ void gn_phase_a(const GatherConfig &G, const RawPoint &kraw, const GnPose &pose, bool rigid,
+                                           double inv_res, V3 &p, int &kx, int &ky, int &kz) {
+    const V3 raw{kraw.x, kraw.y, kraw.z};
+    p = rigid ? qrot(qnormalized(pose.qe), raw) + pose.te
+              : ct_transform_c(pose.qb, pose.tb, pose.qe, pose.te, kraw.alpha, raw, pose.sc);
+    kx = voxel_coord_rcp(p.x, G.L.res, inv_res);
+    ky = voxel_coord_rcp(p.y, G.L.res, inv_res);
+    kz = voxel_coord_rcp(p.z, G.L.res, inv_res);
+}
+
+// ---- C (ct_icp.cpp:769-850): a keypoint's moments `o` (world position p) → covariance, closed-form eigen, normal, a2D,
+// residual and 12-vector Jacobian row u[0..12]; returns whether the row is used. `raw()` gives the keypoint's RawPoint
+// (called only for a used row). `o` may alias `u`: every moment is read before the first store. Every schedule calls
+// this one function.
+template <class RawFn>
+__device__ __forceinline__ bool gn_phase_c(const GnParams &P, RawFn raw, const GnPose &pose, const V3 &p, int need,
+                                           const double *o, double *u, GnWarpAcc &A) {
+    bool used = false;
+    NeighborSums mine;
+    mine.n = __double2loint(o[0]);
+    A.n_kp += 1;
+    A.n_stencil += moments_stencil_points(o);
+    if (mine.n >= need) {
+        A.n_valid += 1;
+        mine.sx = o[1]; mine.sy = o[2]; mine.sz = o[3];
+        mine.sxx = o[4]; mine.sxy = o[5]; mine.sxz = o[6]; mine.syy = o[7]; mine.syz = o[8]; mine.szz = o[9];
+        mine.fx = o[10]; mine.fy = o[11]; mine.fz = o[12]; mine.fd2 = 0;
+        const NeighborhoodDesc nd = describe_from_sums(mine);
+        V3 normal = nd.normal;
+        // orient towards the sensor position at frame begin (:782-784)
+        if (dot(normal, pose.tb - p) < 0) normal = -1.0 * normal;
+        const double weight = nd.a2D * nd.a2D;                       // :787-788
+        // p - closest_point, closest_point = points[0] = farthest kept (:791)
+        const V3 diff{-nd.far_rel.x, -nd.far_rel.y, -nd.far_rel.z};
+        const double dist_to_plane = dot(normal, diff);
+        if (fabs(dist_to_plane) < P.max_dist_to_plane) {              // :803
+            const V3 nw = weight * normal;
+            const double scalar = dot(nw, diff);
+            const RawPoint kraw = raw();
+            const V3 xyz{kraw.x, kraw.y, kraw.z};
+            const V3 ob = qrot(pose.qb, xyz), oe = qrot(pose.qe, xyz);   // :813-816
+            const double a = kraw.alpha, am = 1.0 - a;
+            const V3 cb = cross(ob, nw), ce = cross(oe, nw);
+            u[0] = am * cb.x; u[1] = am * cb.y; u[2] = am * cb.z;
+            u[3] = am * nw.x; u[4] = am * nw.y; u[5] = am * nw.z;
+            u[6] = a * ce.x;  u[7] = a * ce.y;  u[8] = a * ce.z;
+            u[9] = a * nw.x;  u[10] = a * nw.y; u[11] = a * nw.z;
+            u[12] = -scalar;   // b -= u * scalar (:849)
+            used = true;
+            A.n_used += 1;
+        }
+    }
+    return used;
+}
+
 // Per-warp shared memory of a tile: the gather's staging area and the moments of each keypoint of the tile (phase B hands
 // them to phase C through here instead of through 27 registers that would stay live across the gather).
 struct __align__(16) TileScratch {
     SelScratch sel;
-    double sums[kTileMax][14];   // NeighborSums of keypoint j: n, stencil points, s*, f*
+    double sums[kTileMax][kMomentWords];
 };
 // Per-CTA row table of the current chunk of the CTA's range
 struct __align__(16) CtaRows {
@@ -173,18 +266,9 @@ __device__ __forceinline__ void gn_gather_tiles(const GatherConfig &G, const GnP
             r = j0 + lane;
         }
         CT_STAMP(const long long t_a = clock64();)
-        // ---- A: world_kpts[i] = InterpolatePose(begin, end, t_i) * raw_i  (ct_icp.cpp:964-966, types.h:361-366)
         V3 p{0, 0, 0};
         int kx = 0, ky = 0, kz = 0;
-        if (lane < wt) {
-            const RawPoint kraw = load_raw(keypoints, P.kp_lo, lo + r);   // raw xyz (sensor frame) + alpha timestamp
-            const V3 raw{kraw.x, kraw.y, kraw.z};
-            p = rigid ? qrot(qnormalized(pose.qe), raw) + pose.te
-                      : ct_transform_c(pose.qb, pose.tb, pose.qe, pose.te, kraw.alpha, raw, pose.sc);
-            kx = voxel_coord_rcp(p.x, G.L.res, inv_res);
-            ky = voxel_coord_rcp(p.y, G.L.res, inv_res);
-            kz = voxel_coord_rcp(p.z, G.L.res, inv_res);
-        }
+        if (lane < wt) gn_phase_a(G, load_raw(keypoints, P.kp_lo, lo + r), pose, rigid, inv_res, p, kx, ky, kz);
         CT_STAMP(const long long t_b = clock64();)
         // ---- B
         for (int j = 0; j < wt; ++j) {
@@ -194,60 +278,15 @@ __device__ __forceinline__ void gn_gather_tiles(const GatherConfig &G, const GnP
             NeighborSums s;
             unsigned spts = 0;
             warp_gather_sums<false>(G, P.bucket_scale, stencil, q, qx, qy, qz, need, lane, T.sel, s, spts, V3{0, 0, 0}, bulk);
-            if (lane == 0) {
-                double *o = T.sums[j];
-                o[0] = __hiloint2double((int) spts, s.n);   // two integers in one slot: no int <-> double conversion
-                if (s.n >= need) {
-                    o[2] = s.sx; o[3] = s.sy; o[4] = s.sz;
-                    o[5] = s.sxx; o[6] = s.sxy; o[7] = s.sxz; o[8] = s.syy; o[9] = s.syz; o[10] = s.szz;
-                    o[11] = s.fx; o[12] = s.fy; o[13] = s.fz;
-                }
-            }
+            if (lane == 0) gn_store_moments(T.sums[j], s, spts, need);
         }
         __syncwarp();
         CT_STAMP(const long long t_c = clock64();)
-        // ---- C (ct_icp.cpp:769-850)
         if (lane < wt) {
-            bool used = false;
-            const double *o = T.sums[lane];
-            NeighborSums mine;
-            mine.n = __double2loint(o[0]);
-            A.n_kp += 1;
-            const unsigned spts = (unsigned) __double2hiint(o[0]);
-            A.n_stencil += spts;
+            const unsigned spts = moments_stencil_points(T.sums[lane]);
             R.cost[r] = spts;   // the next iteration's schedule (gn_pair_schedule)
-            if (mine.n >= need) {
-                A.n_valid += 1;
-                mine.sx = o[2]; mine.sy = o[3]; mine.sz = o[4];
-                mine.sxx = o[5]; mine.sxy = o[6]; mine.sxz = o[7]; mine.syy = o[8]; mine.syz = o[9]; mine.szz = o[10];
-                mine.fx = o[11]; mine.fy = o[12]; mine.fz = o[13]; mine.fd2 = 0;
-                const NeighborhoodDesc nd = describe_from_sums(mine);
-                V3 normal = nd.normal;
-                // orient towards the sensor position at frame begin (:782-784)
-                if (dot(normal, pose.tb - p) < 0) normal = -1.0 * normal;
-                const double weight = nd.a2D * nd.a2D;                       // :787-788
-                // p - closest_point, closest_point = points[0] = farthest kept (:791)
-                const V3 diff{-nd.far_rel.x, -nd.far_rel.y, -nd.far_rel.z};
-                const double dist_to_plane = dot(normal, diff);
-                if (fabs(dist_to_plane) < P.max_dist_to_plane) {              // :803
-                    const V3 nw = weight * normal;
-                    const double scalar = dot(nw, diff);
-                    const RawPoint kraw = load_raw(keypoints, P.kp_lo, lo + r);
-                    const V3 raw{kraw.x, kraw.y, kraw.z};
-                    const V3 ob = qrot(pose.qb, raw), oe = qrot(pose.qe, raw);   // :813-816
-                    const double a = kraw.alpha, am = 1.0 - a;
-                    const V3 cb = cross(ob, nw), ce = cross(oe, nw);
-                    double *u = R.u[r];
-                    u[0] = am * cb.x; u[1] = am * cb.y; u[2] = am * cb.z;
-                    u[3] = am * nw.x; u[4] = am * nw.y; u[5] = am * nw.z;
-                    u[6] = a * ce.x;  u[7] = a * ce.y;  u[8] = a * ce.z;
-                    u[9] = a * nw.x;  u[10] = a * nw.y; u[11] = a * nw.z;
-                    u[12] = -scalar;   // b -= u * scalar (:849)
-                    used = true;
-                    A.n_used += 1;
-                }
-            }
-            R.used[r] = used ? 1 : 0;
+            const auto raw = [&] { return load_raw(keypoints, P.kp_lo, lo + r); };
+            R.used[r] = gn_phase_c(P, raw, pose, p, need, T.sums[lane], R.u[r], A) ? 1 : 0;
         }
         __syncwarp();   // the moments are consumed before the next tile rewrites them
         CT_STAMP(const long long t_e = clock64();
@@ -260,10 +299,15 @@ __device__ __forceinline__ void gn_gather_tiles(const GatherConfig &G, const GnP
 // classes, the classes then in fixed order: deterministic whatever warp wrote a row. Thread t < kRowParts * kAcc handles
 // accumulator t % kAcc (entries 0..89: pairs of [A upper | b]; 90: rows used; 91: Σ scalar²) of class t / kAcc. The sum
 // of the chunk is ADDED to `carry` of the threads < kAcc. Called by all threads of the CTA; barriers inside.
-__device__ __forceinline__ void gn_cta_reduce_rows(CtaRows &R, int n, double &carry) {
+// `sync` is the CTA-wide barrier (the warp-specialised loop: gn_ws_sync, called by its math warps as well).
+struct GnCtaSync {
+    __device__ __forceinline__ void operator()() const { __syncthreads(); }
+};
+template <class Sync = GnCtaSync>
+__device__ __forceinline__ void gn_cta_reduce_rows(CtaRows &R, int n, double &carry, Sync sync = Sync{}) {
     const int t = threadIdx.x;
     const int a = t % kAcc, part = t / kAcc;
-    __syncthreads();   // every row of the chunk is written
+    sync();   // every row of the chunk is written
     if (part < kRowParts && a <= kAccSumSq) {
         const int pi = a < kAccUsed ? c_pair_i[a] : 12, pj = a < kAccUsed ? c_pair_j[a] : 12;
         double s = 0;
@@ -277,7 +321,7 @@ __device__ __forceinline__ void gn_cta_reduce_rows(CtaRows &R, int n, double &ca
         }
         R.red[part][a] = s;
     }
-    __syncthreads();
+    sync();
     if (t < kAcc && a <= kAccSumSq) {
         double s = R.red[0][a];
 #pragma unroll
@@ -301,7 +345,13 @@ __device__ __forceinline__ void gn_store_warp_row(double *row, const GnWarpAcc &
 // this CTA's partial row (kAcc doubles) in global memory. `R.next` is reset here; all threads call.
 // shared memory of the GN kernels (dynamic: the staging areas alone are 70 KB)
 struct GnShared {
-    TileScratch tile[kGatherWarps];
+    union {
+        TileScratch tile[kGatherWarps];   // one warp per tile of keypoints (k_gn_iterate, the sharded k_gn_persistent)
+        struct {                          // the warp-specialised k_gn_persistent (gn_ws_loop)
+            SelScratch sel[kWsGatherWarps];   // staging area of each gather warp
+            WsQuery q[kRowCap];               // phase A of row r of the chunk, for phases B and C
+        } ws;
+    };
     CtaRows rows;
     GnPose pose;
     double acc[kGatherWarps][kAcc];
@@ -324,19 +374,24 @@ struct GnShared {
 
 // the per-warp column sums of a row reduction (columns lane, lane + 32, lane + 64) → their sum in warp order in
 // sh.acc[0][0..kAcc). Called by all threads, after a barrier that follows every earlier read of sh.acc.
-__device__ __forceinline__ void gn_sum_warp_partials(GnShared &sh, double a0, double a1, double a2, int lane, int w) {
-    sh.acc[w][lane] = a0;
-    sh.acc[w][lane + 32] = a1;
-    sh.acc[w][lane + 64] = a2;
-    __syncthreads();
+// Warps w >= kGatherWarps (the warp-specialised solver CTA) have no partials and only join the barriers.
+template <class Sync = GnCtaSync>
+__device__ __forceinline__ void gn_sum_warp_partials(GnShared &sh, double a0, double a1, double a2, int lane, int w,
+                                                     Sync sync = Sync{}) {
+    if (w < kGatherWarps) {
+        sh.acc[w][lane] = a0;
+        sh.acc[w][lane + 32] = a1;
+        sh.acc[w][lane + 64] = a2;
+    }
+    sync();
     double sum = 0;
     if (threadIdx.x < kAcc) {
 #pragma unroll
         for (int ww = 0; ww < kGatherWarps; ++ww) sum += sh.acc[ww][threadIdx.x];
     }
-    __syncthreads();
+    sync();
     if (threadIdx.x < kAcc) sh.acc[0][threadIdx.x] = sum;
-    __syncthreads();
+    sync();
 }
 
 // deterministic reduction of `rows` partial rows by one CTA: warp g sums the rows b = g (mod kGatherWarps), three
@@ -488,6 +543,15 @@ k_gn_iterate(GatherLaunch cfg, const float4 *__restrict__ keypoints, const int *
 #ifndef CTICP_GN_GRID_BARRIERS
 #define CTICP_GN_FLAG_SYNC 1
 #endif
+// threads of a k_gn_persistent CTA: the warp-specialised layout (gn_ws_loop) for the single-GPU loop, one warp per tile of
+// keypoints for the sharded one (and for the -DCTICP_GN_GRID_BARRIERS variant)
+constexpr int gn_persistent_threads(bool peers) {
+#ifdef CTICP_GN_FLAG_SYNC
+    return peers ? kGatherWarps * 32 : kWsWarps * 32;
+#else
+    return (void) peers, kGatherWarps * 32;
+#endif
+}
 constexpr int kRowWords = 2 * kAcc;   // tagged words of a partial row
 // pose words of a group: the bytes of GnPose as 32-bit halves, then `done` (and an unused half), in word pairs
 constexpr int kPosePairs = 18;
@@ -515,9 +579,9 @@ struct GnGroups {
 // sh.acc[0][0..kAcc). Returns false (uniform) when a row has not arrived within kLoopSyncTimeout. Called by all threads.
 // One row per warp at a time: loads of more rows in flight need registers that this kernel's gather path then spills to
 // local memory (on the bench workload the GN launch took 161 us with five rows in flight, 157 us with two, 151 us with one).
-__device__ __forceinline__ bool gn_reduce_tagged_rows(GnShared &sh, const unsigned long long *rows, int n, unsigned int tag,
-                                                      int lane, int w) {
-    double a0 = 0, a1 = 0, a2 = 0;
+// warp w < kGatherWarps: its rows of the reduction below, summed into a0..a2; false when one did not arrive in time
+__device__ __forceinline__ bool gn_consume_tagged_rows(const unsigned long long *rows, int n, unsigned int tag, int lane,
+                                                       int w, double &a0, double &a1, double &a2) {
     bool ok = true;
     const long long t0 = clock64();
     for (int b = w; b < n && ok; b += kGatherWarps) {
@@ -539,6 +603,12 @@ __device__ __forceinline__ bool gn_reduce_tagged_rows(GnShared &sh, const unsign
             a2 += pair_double(c2);
         }
     }
+    return ok;
+}
+__device__ __forceinline__ bool gn_reduce_tagged_rows(GnShared &sh, const unsigned long long *rows, int n, unsigned int tag,
+                                                      int lane, int w) {
+    double a0 = 0, a1 = 0, a2 = 0;
+    const bool ok = gn_consume_tagged_rows(rows, n, tag, lane, w, a0, a1, a2);
     if (!__syncthreads_and(ok)) return false;
     gn_sum_warp_partials(sh, a0, a1, a2, lane, w);
     return true;
@@ -587,6 +657,282 @@ __device__ __forceinline__ void gn_fetch_pose(GnShared &sh, unsigned int tag, lo
         sh.done = ok ? (int) word_payload(v.x) : 1;
 }
 
+// ---- the warp-specialised loop of the single-GPU k_gn_persistent (kWsWarps warps: kWsGatherWarps gather warps, then the
+// kWsMathWarps math warps) -------------------------------------------------------------------------------------------------
+// From the setmaxnreg on, the two roles run separate code to the end of the kernel (ptxas gives a region the registers of
+// the setmaxnreg that leads to it only where the roles do not merge again) and meet at named barrier 1 of all kWsWarps
+// warps, which either role reaches from its own code: every barrier of one role has its partner in the other.
+// Per chunk of a gather CTA's range (kRowCap rows):
+//   math warps, thread m : phase A of rows m, m + 128 → sh.ws.q (first chunk: after the pose) | barrier
+//   gather warps         : phase B, one row per grab from sh.rows.next (no pairs while the range is at most
+//                          kWsGatherWarps rows: the bench's ranges are 18-20) → the row's moments in sh.rows.u | barrier
+//   math warps           : phase C of the same rows, the moments in sh.rows.u replaced by the row
+//   gather warps         : gn_cta_reduce_rows (barriers inside; the math warps join them)
+// The rows are the rows of gn_gather_tiles (one gn_phase_a / gn_phase_c) and their reduction is the same, so the partial
+// row is the same bit for bit. The solver CTA: gather warps 0..kGatherWarps-1 consume the tagged rows as
+// gn_reduce_tagged_rows does, the first math warp solves and publishes the pose (the registers are there).
+struct GnWsSync {
+    __device__ __forceinline__ void operator()() const {
+        asm volatile("barrier.sync 1, %0;" ::"n"(kWsWarps * 32) : "memory");
+    }
+};
+__device__ __forceinline__ bool gn_ws_sync_and(bool pred) {
+    unsigned r;
+    asm volatile("{\n.reg .pred p, q;\nsetp.ne.u32 p, %1, 0;\nbarrier.red.and.pred q, 1, %2, p;\nselp.u32 %0, 1, 0, q;\n}"
+                 : "=r"(r) : "r"((unsigned) pred), "n"(kWsWarps * 32) : "memory");
+    return r != 0;
+}
+
+// gather CTA, gather warp w: phase B of every chunk of every iteration, the reduction of the rows, the tagged partial row
+__device__ __forceinline__ void gn_ws_gather_warp(GnShared &sh, const GatherConfig &G, const int *stencil, int num_iters,
+                                                  int c_lo, int c_hi, unsigned int tag0, int lane, int w) {
+    const GnWsSync sync;
+    const GnParams &P = sh.group.cfg.P;
+    const int need = P.kmin > 5 ? P.kmin : 5;   // ct_icp.cpp:769 ; neighborhood.h:227
+    CtaRows &R = sh.rows;
+    for (int it = 0; it < num_iters; ++it) {
+        // (CTICP_DEBUG_FLAGS & 2, timing only: an empty range — the hand-off and the reduction without the gather work)
+        const bool skip = (P.debug_flags & 2) != 0;
+        const int lo = skip ? 0 : c_lo, hi = skip ? 0 : c_hi;
+        double carry = 0;
+        bool done = false;
+        for (int base = lo;; base += kRowCap) {
+            const int top = (hi - base) > kRowCap ? base + kRowCap : hi;
+            const int n = top > base ? top - base : 0;
+            sync();   // phase A of the chunk (the first chunk: also the pose and `done`)
+            if (sh.done) {
+                done = true;
+                break;
+            }
+            while (true) {
+                int r = 0;
+                if (lane == 0) r = atomicAdd(&R.next, 1);
+                r = __shfl_sync(0xffffffffu, r, 0);
+                if (r >= n) break;
+                const WsQuery &q = sh.ws.q[r];
+                NeighborSums s;
+                unsigned spts = 0;
+                warp_gather_sums<false>(G, P.bucket_scale, stencil, V3{q.x, q.y, q.z}, q.kx, q.ky, q.kz, need, lane,
+                                        sh.ws.sel[w], s, spts);
+                if (lane == 0) gn_store_moments(R.u[r], s, spts, need);
+            }
+            sync();   // phase B of the chunk
+            gn_cta_reduce_rows(R, n, carry, sync);   // (the math warps' counters are in sh.acc from its first barrier on)
+            if (top >= hi) break;
+            if (threadIdx.x == 0) R.next = 0;
+            sync();
+        }
+        if (done) break;
+        const int t = threadIdx.x;
+        if (t < kAcc) {
+            double s = 0;
+            if (t <= kAccSumSq) s = carry;
+            else if (t == kAccStencil || t == kAccKeypoints || t == kAccValidNb) {
+#pragma unroll
+                for (int ww = 0; ww < kWsMathWarps; ++ww) s += sh.acc[ww][t];
+            }
+            tagged_store_double(sh.grp.rows + 2 * t, tag0 + (unsigned int) it, s);
+        }
+        if (it == num_iters - 1) break;   // nothing left to wait for: the solver CTA finishes the registration alone
+    }
+}
+
+// math warps only (named barrier 2): the pose and `done` that the first math warp fetched
+__device__ __forceinline__ void gn_ws_math_sync() {
+    asm volatile("barrier.sync 2, %0;" ::"n"(kWsMathWarps * 32) : "memory");
+}
+constexpr int kWsRowsPerLane = kRowCap / (kWsMathWarps * 32);   // rows of a chunk per math thread
+static_assert(kWsRowsPerLane * kWsMathWarps * 32 == kRowCap, "rows per math thread");
+
+// gather CTA, math warp mw = w - kWsGatherWarps: the pose, phases A and C, the per-keypoint counters. Thread m does rows
+// m + 128 j of a chunk; their raw keypoints are loaded into registers before the pose is waited for (the range is the
+// same in every iteration), so neither phase waits for a keypoint load in the first chunk.
+__device__ __forceinline__ void gn_ws_gather_math(GnShared &sh, const GatherConfig &G, int num_iters, int c_lo, int c_hi,
+                                                  unsigned int tag0, int lane, int w) {
+    const GnWsSync sync;
+    const GnParams &P = sh.group.cfg.P;
+    const float4 *__restrict__ keypoints = sh.group.keypoints;
+    const int need = P.kmin > 5 ? P.kmin : 5;
+    const int mw = w - kWsGatherWarps, m = threadIdx.x - kWsGatherWarps * 32;
+    const double inv_res = 1.0 / G.L.res;
+    CtaRows &R = sh.rows;
+    for (int it = 0; it < num_iters; ++it) {
+        GnWarpAcc A;
+        const bool skip = (P.debug_flags & 2) != 0;
+        const int lo = skip ? 0 : c_lo, hi = skip ? 0 : c_hi;
+        const bool rigid = P.rigid_first && it == 0;
+        RawPoint kr[kWsRowsPerLane];
+        const auto load_chunk = [&](int base, int n) {
+#pragma unroll
+            for (int j = 0; j < kWsRowsPerLane; ++j) {
+                const int r = m + j * kWsMathWarps * 32;
+                if (r < n) kr[j] = load_raw(keypoints, P.kp_lo, base + r);
+            }
+        };
+        load_chunk(lo, (hi - lo) > kRowCap ? kRowCap : hi - lo);
+        if (mw == 0) {
+            if (it == 0) {   // the state the host uploaded
+                if (lane == 0) {
+                    const IcpState *gst = sh.grp.st;
+                    const int done = __ldcg(&gst->done);   // issued with the pose loads: one round trip, not two
+                    sh.pose = load_pose(gst);
+                    sh.done = done;
+                }
+            } else {
+                gn_fetch_pose(sh, tag0 + (unsigned int) it, kLoopSyncTimeout, lane);
+            }
+            if (lane == 0) R.next = 0;
+        }
+        gn_ws_math_sync();
+        const bool done = sh.done != 0;
+        for (int base = lo;; base += kRowCap) {
+            const int top = (hi - base) > kRowCap ? base + kRowCap : hi;
+            const int n = top > base ? top - base : 0;
+            if (!done) {
+                if (base != lo) load_chunk(base, n);
+#pragma unroll
+                for (int j = 0; j < kWsRowsPerLane; ++j) {
+                    const int r = m + j * kWsMathWarps * 32;
+                    if (r < n) {
+                        V3 p;
+                        int kx, ky, kz;
+                        gn_phase_a(G, kr[j], sh.pose, rigid, inv_res, p, kx, ky, kz);
+                        sh.ws.q[r] = WsQuery{p.x, p.y, p.z, kx, ky, kz};
+                    }
+                }
+            }
+            sync();   // phase A of the chunk
+            if (done) break;
+            sync();   // phase B of the chunk
+#pragma unroll
+            for (int j = 0; j < kWsRowsPerLane; ++j) {
+                const int r = m + j * kWsMathWarps * 32;
+                if (r < n) {
+                    const WsQuery &q = sh.ws.q[r];
+                    R.used[r] = gn_phase_c(P, [&] { return kr[j]; }, sh.pose, V3{q.x, q.y, q.z}, need, R.u[r], R.u[r], A) ? 1 : 0;
+                }
+            }
+            gn_store_warp_row(sh.acc[mw], A, lane);   // the counters so far: final after the last chunk
+            double unused = 0;   // (no accumulator of the reduction falls on a math warp: kRowParts * kAcc <= gather threads)
+            gn_cta_reduce_rows(R, n, unused, sync);
+            if (top >= hi) break;
+            sync();
+        }
+        if (done || it == num_iters - 1) break;
+    }
+}
+static_assert(kRowParts * kAcc <= kWsGatherWarps * 32, "the row reduction runs on the gather warps");
+
+// solver CTA, gather warp w: its tagged rows (warps < kGatherWarps) and the sum of the per-warp partials
+__device__ __forceinline__ void gn_ws_solver_gather(GnShared &sh, int num_iters, unsigned int tag0, int lane, int w) {
+    const GnWsSync sync;
+    for (int it = 0; it < num_iters; ++it) {
+        if (sh.state.done) break;
+        double a0 = 0, a1 = 0, a2 = 0;
+        bool ok = true;
+        if (w < kGatherWarps) ok = gn_consume_tagged_rows(sh.grp.rows, sh.grp.gather_ctas, tag0 + (unsigned int) it, lane, w, a0, a1, a2);
+        if (!gn_ws_sync_and(ok)) break;
+        gn_sum_warp_partials(sh, a0, a1, a2, lane, w, sync);
+        sync();   // the solve is done with sh.acc / sh.state
+    }
+}
+
+// solver CTA, math warps: the first one solves, publishes the pose, and after the loop the state and the frame's tail
+__device__ __forceinline__ void gn_ws_solver_math(GnShared &sh, int num_iters, unsigned int tag0, FrameTailArgs &tail,
+                                                  int lane, int w) {
+    const GnWsSync sync;
+    const GnParams &P = sh.group.cfg.P;
+    const bool solver = w == kWsGatherWarps;
+    long long t_loop = 0, t_solve = 0;
+    if (solver) {
+        if (!(P.debug_flags & 4)) {
+            // instruction-cache warm-up of the serial tail on a dummy well-posed system (results discarded)
+            for (int i = lane; i < kAcc; i += 32) sh.acc[1][i] = 0.0;
+            __syncwarp();
+            for (int e = lane; e < 78; e += 32)
+                if (c_pair_i[e] == c_pair_j[e]) sh.acc[1][e] = 200.0 * (1.0 + c_pair_i[e]);
+            if (lane < 12) sh.acc[1][78 + lane] = 1e-3 * (lane + 1);
+            if (lane == 0) {
+                sh.acc[1][kAccUsed] = 200.0;
+                sh.dummy = sh.state;
+            }
+            __syncwarp();
+            warp_gn_solve(sh.acc[1], sh.solve, &sh.dummy, P, 0, nullptr, lane);
+            __syncwarp();
+        }
+        t_loop = clock64();
+    }
+    for (int it = 0; it < num_iters; ++it) {
+        const unsigned int tag = tag0 + (unsigned int) it;
+        if (sh.state.done) break;
+        if (!gn_ws_sync_and(true)) {
+            // a gather CTA's row never arrived: give up (the host raises "Error During Optimization"); pose words of
+            // the next iteration with done = 1 release every gather CTA that waits for them
+            if (solver) {
+                if (lane == 0) {
+                    sh.state.failed = 2;
+                    sh.state.done = 1;
+                }
+                __syncwarp();
+                gn_publish_pose(sh.grp.pose, sh.state, tag + 1u, lane);
+            }
+            break;
+        }
+        gn_sum_warp_partials(sh, 0.0, 0.0, 0.0, lane, w, sync);
+        if (solver) {
+            const long long t_begin = clock64();
+            IcpState *ws = &sh.state;
+            if (P.debug_flags & 1) {
+                if (lane == 0) ws->iter += 1;
+            } else
+                warp_gn_solve(sh.acc[0], sh.solve, ws, P, 0, nullptr, lane);
+            __syncwarp();
+            // the gather CTAs wait for the pose words only when they have another iteration to run
+            if (it + 1 < num_iters) gn_publish_pose(sh.grp.pose, *ws, tag + 1u, lane);
+            if (lane == 0) {
+                t_solve += clock64() - t_begin;
+                ws->cycles_total = (unsigned long long) (clock64() - t_loop);
+                ws->cycles_solve = (unsigned long long) t_solve;
+            }
+        }
+        sync();
+    }
+    if (!solver) return;
+    // the registration's state, published once on every way out of the loop (the host, k_frame_policy and later launches
+    // read it after this kernel)
+    {
+        const int *src = reinterpret_cast<const int *>(&sh.state);
+        int *dst = reinterpret_cast<int *>(sh.grp.st);
+        for (int i = lane; i < (int) (sizeof(IcpState) / sizeof(int)); i += 32) dst[i] = src[i];
+    }
+    // ---- the tail of the registration (frame_policy.h): as in k_gn_persistent's other layout
+    if (tail.enabled) {
+        const int *src = reinterpret_cast<const int *>(&sh.state);
+        int *dst = reinterpret_cast<int *>(&sh.verdict.state);
+        for (int i = lane; i < (int) (sizeof(IcpState) / sizeof(int)); i += 32) dst[i] = src[i];
+        if (lane < 4) sh.verdict.counts[lane] = __ldcg(tail.counts + lane);
+        __syncwarp();
+        if (lane == 0) frame_policy_decide(sh.verdict, tail.in);
+        __syncwarp();
+        frame_verdict_publish(sh.verdict, tail.dv, tail.hv, lane);
+    }
+}
+
+// the whole loop of one CTA from the register split on; all kWsWarps warps call
+__device__ __forceinline__ void gn_ws_loop(GnShared &sh, const GatherConfig &gather_G, const int *stencil, int num_iters,
+                                           bool solver_cta, int c_lo, int c_hi, unsigned int tag0, FrameTailArgs &tail,
+                                           int lane, int w) {
+    if (w >= kWsGatherWarps) {
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWsMathRegs));
+        if (solver_cta) gn_ws_solver_math(sh, num_iters, tag0, tail, lane, w);
+        else gn_ws_gather_math(sh, gather_G, num_iters, c_lo, c_hi, tag0, lane, w);
+    } else {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kWsGatherRegs));
+        if (solver_cta) gn_ws_solver_gather(sh, num_iters, tag0, lane, w);
+        else gn_ws_gather_warp(sh, gather_G, stencil, num_iters, c_lo, c_hi, tag0, lane, w);
+    }
+}
+
 // ---- persistent variant: the WHOLE Gauss-Newton loop in one cooperative launch --------------------------------
 // CTA 0 is the solver CTA (deterministic reduction of the partials + 12x12 solve + pose update, by the same warp on
 // the same SM every iteration, so its instructions stay in that SM's instruction cache: executed cold, the serial tail
@@ -606,10 +952,11 @@ __device__ __forceinline__ void gn_fetch_pose(GnShared &sh, unsigned int tag, lo
 // with the other ranks' solver CTAs through NVLink peer memory (peer_exchange.cuh) — the all-reduce of SURVEY §8e
 // happens INSIDE the loop, so the sharded loop is still one launch and costs one NVLink round trip per iteration.
 template <bool kPeers, bool kGrouped>
-__global__ void __launch_bounds__(kGatherWarps * 32, 1)
+__global__ void __launch_bounds__(gn_persistent_threads(kPeers), 1)
 k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints, const int *__restrict__ d_num_keypoints,
                 IcpState *st, int solo_iters, PeerLinks links, GnLoopWords words, FrameTailArgs tail, GnGroups groups) {
     static_assert(!(kPeers && kGrouped), "the sharded loop is single-group");
+    constexpr bool kWs = gn_persistent_threads(kPeers) == kWsWarps * 32;   // the warp-specialised loop (gn_ws_loop)
 #ifndef CTICP_GN_FLAG_SYNC
     cg::grid_group grid = cg::this_grid();
 #endif
@@ -666,7 +1013,7 @@ k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints
         __syncthreads();
     }
     CT_STAMP(if (solver_cta && threadIdx.x < 4) sh.state.dbg_t[threadIdx.x] = 0; __syncthreads();)
-    if (solver_cta && w == 0 && !(P.debug_flags & 4)) {
+    if (!kWs && solver_cta && w == 0 && !(P.debug_flags & 4)) {
         // instruction-cache warm-up of the serial tail on a dummy well-posed system (results discarded)
         for (int i = lane; i < kAcc; i += 32) sh.acc[1][i] = 0.0;
         __syncwarp();
@@ -685,8 +1032,10 @@ k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints
     void *bulk_ptr = nullptr;
 #ifdef CTICP_SEL_BULK
     SelBulk bulk;
-    sel_bulk_init(bulk, &sh.mbar[w], lane);
-    bulk_ptr = &bulk;
+    if (!kWs) {
+        sel_bulk_init(bulk, &sh.mbar[w], lane);
+        bulk_ptr = &bulk;
+    }
 #endif
     long long t_loop = 0, t_solve = 0;
     if (solver_cta && threadIdx.x == 0) t_loop = clock64();
@@ -702,6 +1051,10 @@ k_gn_persistent(GatherLaunch solo_cfg, const float4 *__restrict__ solo_keypoints
     if (!solver_cta) {
         c_lo = kp_lo + (int) ((long long) (kp_hi - kp_lo) * (cta - 1) / gather_ctas);
         c_hi = kp_lo + (int) ((long long) (kp_hi - kp_lo) * cta / gather_ctas);
+    }
+    if constexpr (kWs) {
+        gn_ws_loop(sh, gather_G, stencil, num_iters, solver_cta, c_lo, c_hi, words.tag, tail, lane, w);
+        return;
     }
     for (int it = 0; it < num_iters; ++it) {
         const unsigned int tag = words.tag + (unsigned int) it;
@@ -1003,7 +1356,7 @@ int IcpSolver::GnCoresident(bool peers) {
     if (coresident == 0) {
         void *kernel = peers ? (void *) k_gn_persistent<true, false> : (void *) k_gn_persistent<false, false>;
         int per_sm = 0;
-        CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kGatherWarps * 32, sizeof(GnShared)));
+        CT_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, gn_persistent_threads(peers), sizeof(GnShared)));
         coresident = std::max(1, per_sm * num_sms_);
     }
     return coresident;
@@ -1109,7 +1462,7 @@ void IcpSolver::EnqueueGaussNewtonGroups(const GnProblem *problems, int batch) {
     FrameTailArgs tail_args{};
     GnGroups groups{reinterpret_cast<const GnGroup *>(d_gn_table_.data()), reinterpret_cast<const int *>(d_gn_table_.data() + cta_off), batch};
     void *args[] = {&cfg, &kp, &nk, &st, &iters, &links, &words, &tail_args, &groups};
-    CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_gn_persistent<false, true>, dim3(grid), dim3(kGatherWarps * 32), args,
+    CT_CUDA_CHECK(cudaLaunchCooperativeKernel((void *) k_gn_persistent<false, true>, dim3(grid), dim3(gn_persistent_threads(false)), args,
                                               sizeof(GnShared), stream_));
     gather_launches_ += 1;
     launches_ += 1;
@@ -1231,7 +1584,7 @@ bool IcpSolver::EnqueueGaussNewton(const DeviceMap &map, const cticp_icp_options
         void *args[] = {&cfg, &kp, &nk, &d_state, &iters, &links, &words, &tail_args, &groups};
         const bool timed = time_gather_ && ev_used_ < kMaxEvents;
         if (timed) cudaEventRecord(ev_begin_[ev_used_].get(), stream_);
-        CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(kGatherWarps * 32), args, sizeof(GnShared), stream_));
+        CT_CUDA_CHECK(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(gn_persistent_threads(peers)), args, sizeof(GnShared), stream_));
         if (timed) cudaEventRecord(ev_end_[ev_used_++].get(), stream_);
         gather_launches_ += 1;
         launches_ += 1;
