@@ -156,6 +156,25 @@ class LidarFrame(_Struct):   # cticp_lidar_frame: one sweep
     _fields_ = [("t0", C.c_double), ("frame_id", C.c_uint32), ("_pad0", C.c_uint32)]
 
 
+class NcltFrame(_Struct):   # cticp_nclt_frame: one frame of an NCLT velodyne_hits.bin stream
+    _fields_ = [("num_points", C.c_uint64), ("t_first", C.c_double), ("t_max", C.c_double)]
+
+
+def nclt_frame_dtype():
+    import numpy as np
+    return np.dtype([("num_points", "<u8"), ("t_first", "<f8"), ("t_max", "<f8")])
+
+
+class PlyLayout(_Struct):   # cticp_ply_layout: the vertex records of a binary_little_endian PLY file
+    _fields_ = [("body_offset", C.c_uint64), ("num_points", C.c_uint64), ("point_step", C.c_uint32),
+                ("xyz_offset", C.c_uint32), ("xyz_dtype", C.c_int32), ("t_offset", C.c_uint32), ("t_dtype", C.c_int32),
+                ("_pad0", C.c_int32)]
+
+
+# CTICP_DATASET_*: the reference's ct_icp::DATASET values (include/ct_icp/dataset.h)
+DATASET = {"KITTI_raw": 0, "KITTI_CARLA": 1, "KITTI": 2, "KITTI_360": 3, "NCLT": 4, "HILTI_2021": 5, "HILTI_2022": 6}
+
+
 def lidar_frame_dtype():
     import numpy as np
     return np.dtype({"names": ["t0", "frame_id"], "formats": [np.float64, np.uint32], "offsets": [0, 8],

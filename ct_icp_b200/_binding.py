@@ -300,6 +300,23 @@ class Binding:
             "lidar_generate_sweeps": (i64, [vp, vp, P(abi.LidarSensor), vp, sz, u64, P(abi.CloudSink), vp, vp]),
             "lidar_generate_sweeps_device": (C.c_int, [vp, vp, P(abi.LidarSensor), vp, sz, u64, P(abi.CloudSink), vp, vp,
                                                         vp]),
+            "nclt_open": (C.c_int, [vp, sz, u32, C.c_int, C.c_int, P(vp)]),
+            "nclt_open_device": (C.c_int, [vp, sz, u32, C.c_int, C.c_int, vp, P(vp)]),
+            "nclt_destroy": (None, [vp]),
+            "nclt_num_frames": (i64, [vp]),
+            "nclt_num_packets": (i64, [vp]),
+            "nclt_num_hits": (i64, [vp]),
+            "nclt_bytes_used": (i64, [vp]),
+            "nclt_index_walked": (C.c_int, [vp]),
+            "nclt_frame_info": (C.c_int, [vp, sz, sz, vp]),
+            "nclt_read_frames": (i64, [vp, sz, sz, P(abi.CloudSink), vp]),
+            "nclt_read_frames_device": (C.c_int, [vp, sz, sz, P(abi.CloudSink), vp, vp]),
+            "ply_layout_parse": (C.c_int, [vp, sz, P(abi.PlyLayout)]),
+            "kitti_frame_filter": (C.c_int, [C.c_int, P(abi.CloudView), P(abi.CloudSink)]),
+            "kitti_frame_filter_device": (C.c_int, [C.c_int, P(abi.DeviceScan), P(abi.CloudSink), vp]),
+            "scan_time_ranges": (C.c_int, [C.c_int, P(abi.CloudView), vp, sz, vp]),
+            "scan_time_ranges_device": (C.c_int, [C.c_int, P(abi.DeviceScan), vp, sz, vp, vp]),
+            "ground_truth_parse": (i64, [C.c_int, C.c_int, vp, sz, vp, sz]),
         })
         for name, (res, args) in sigs.items():
             if self.has(name):
@@ -538,6 +555,109 @@ class Binding:
         """A ray-cast scene on `device`: boxes (n, 7) x0 y0 z0 x1 y1 z1 mean_free_path, cylinders (n, 4) cx cy r h and
         the ground plane z = 0 (synthetic.UrbanScene's .boxes and .cyl load as they are)."""
         return LidarScene(self, boxes, cylinders, ground, device)
+
+    # ---- dataset sequences ------------------------------------------------------------------------------------
+    def nclt_hits(self, data, num_aggregated=220, final=True, device=0):
+        """An NCLT velodyne_hits.bin stream (bytes, a uint8 NumPy array, or a uint8 CUDA tensor on `device`, read after
+        torch's current stream), indexed on `device` into frames of num_aggregated packets (include/cticp.h, "Dataset
+        sequences"). With final=False only whole frames are kept and .bytes_used says where the next chunk starts."""
+        return NcltHits(self, data, num_aggregated, final, device)
+
+    def ply_layout(self, data):
+        """The vertex record layout of a binary_little_endian PLY file's bytes: an abi.PlyLayout"""
+        buf = np.frombuffer(bytes(data) if not isinstance(data, np.ndarray) else data.tobytes(), dtype=np.uint8)
+        out = abi.PlyLayout()
+        self.check(self.fn("ply_layout_parse")(buf.ctypes.data, len(buf), C.byref(out)))
+        return out
+
+    def ply_records(self, data):
+        """(layout, records): the vertex records of a PLY file as a NumPy structured array with fields x, y, z and t
+        (when the file has a timestamp), a view of a copy of the body"""
+        lay = self.ply_layout(data)
+        raw = np.frombuffer(bytes(data), dtype=np.uint8)
+        names = {v: k for k, v in abi.DTYPE.items()}
+        xs = np.dtype(names[lay.xyz_dtype]).itemsize
+        fields = {"names": ["x", "y", "z"], "formats": [names[lay.xyz_dtype]] * 3,
+                  "offsets": [lay.xyz_offset, lay.xyz_offset + xs, lay.xyz_offset + 2 * xs], "itemsize": lay.point_step}
+        if lay.t_dtype:
+            fields["names"].append("t")
+            fields["formats"].append(names[lay.t_dtype])
+            fields["offsets"].append(lay.t_offset)
+        body = raw[lay.body_offset:lay.body_offset + lay.num_points * lay.point_step].copy()
+        return lay, body.view(np.dtype(fields))
+
+    def kitti_frame_filter(self, scan, device=0, in_place=False):
+        """kitti_frame_filter of a scan: a NumPy structured array with fields x, y, z (host; returns a filtered copy) or
+        an (N, >=3) float32 / float64 CUDA tensor with unit column stride (on torch's current stream; a new tensor, or
+        the same one with in_place=True)"""
+        if _is_cuda_tensor(scan):
+            import torch
+            if scan.dim() != 2 or scan.shape[1] < 3 or scan.stride(1) != 1 or scan.dtype not in (torch.float32,
+                                                                                                  torch.float64):
+                raise ValueError("scan must be an (N, >=3) float32 / float64 tensor with unit column stride")
+            out = scan if in_place else torch.empty_like(scan)
+            code = abi.DTYPE["float32" if scan.dtype == torch.float32 else "float64"]
+            es = scan.element_size()
+            ds = abi.DeviceScan(scan.data_ptr(), scan.stride(0) * es, None, 0, scan.shape[0], code, 0)
+            sink = abi.CloudSink(out.data_ptr(), out.shape[0], out.stride(0) * es, 0, code, 0, 0, 0)
+            if not in_place and scan.shape[1] > 3:
+                out[:, 3:] = scan[:, 3:]
+            if scan.shape[0]:
+                self.check(self.fn("kitti_frame_filter_device")(device, C.byref(ds), C.byref(sink),
+                                                                C.c_void_p(torch.cuda.current_stream(device).cuda_stream)))
+            return out
+        rec = np.ascontiguousarray(scan)
+        f = rec.dtype.fields
+        xdt, xoff = f["x"][0], f["x"][1]
+        view = abi.CloudView(rec.ctypes.data, len(rec), rec.dtype.itemsize, xoff, abi.DTYPE[xdt.name], 0, 0, 0)
+        out = rec.view(np.uint8).copy().view(rec.dtype).reshape(-1)   # every byte of a record, named or not
+        sink = abi.CloudSink(out.ctypes.data, len(out), out.dtype.itemsize, xoff, abi.DTYPE[xdt.name], 0, 0, 0)
+        if len(rec):
+            self.check(self.fn("kitti_frame_filter")(device, C.byref(view), C.byref(sink)))
+        return out
+
+    def scan_time_ranges(self, t, frame_ends, device=0):
+        """(m, 2) per-frame (min, max) of timestamps t split at frame_ends: NumPy arrays on the host (a NaN timestamp
+        raises), or CUDA tensors (t 1-D, frame_ends int64 / uint64) on torch's current stream (NaN rows for NaN frames)"""
+        if _is_cuda_tensor(t):
+            import torch
+            codes = _torch_dtype_codes(torch)
+            ends = frame_ends.to(device=t.device, dtype=torch.int64).contiguous()
+            out = torch.empty((ends.shape[0], 2), dtype=torch.float64, device=t.device)
+            ds = abi.DeviceScan(None, 0, t.data_ptr() if t.shape[0] else None, t.stride(0) * t.element_size(), t.shape[0],
+                                abi.DTYPE["float64"], codes[t.dtype])
+            if ends.shape[0]:
+                self.check(self.fn("scan_time_ranges_device")(device, C.byref(ds), ends.data_ptr(), ends.shape[0],
+                                                              out.data_ptr(),
+                                                              C.c_void_p(torch.cuda.current_stream(device).cuda_stream)))
+            return out
+        tt = np.ascontiguousarray(t)
+        ends = np.ascontiguousarray(frame_ends, dtype=np.uint64)
+        out = np.zeros((len(ends), 2))
+        rec = np.zeros(len(tt), dtype=np.dtype({"names": ["x", "y", "z", "t"], "formats": ["<f8"] * 3 + [tt.dtype],
+                                                "offsets": [0, 8, 16, 24], "itemsize": 24 + tt.dtype.itemsize}))
+        rec["t"] = tt
+        view = abi.CloudView(rec.ctypes.data if len(rec) else None, len(rec), rec.dtype.itemsize, 0,
+                             abi.DTYPE["float64"], 24, abi.DTYPE[tt.dtype.name], 0)
+        if len(ends):
+            if len(rec) == 0:
+                rec = np.zeros(1, dtype=rec.dtype)
+                view.data = rec.ctypes.data
+            self.check(self.fn("scan_time_ranges")(device, C.byref(view), ends.ctypes.data, len(ends), out.ctypes.data))
+        return out
+
+    def ground_truth(self, dataset, text, sequence_id=0):
+        """LoadPoses of a ground-truth file's text (str or bytes) for `dataset` (a name of abi.DATASET or its value):
+        an array of abi.pose_dtype() in the LiDAR frame"""
+        ds = abi.DATASET[dataset] if isinstance(dataset, str) else int(dataset)
+        raw = text.encode() if isinstance(text, str) else bytes(text)
+        buf = np.frombuffer(raw, dtype=np.uint8)
+        n = self.check(self.fn("ground_truth_parse")(ds, int(sequence_id), buf.ctypes.data if len(buf) else None,
+                                                     len(buf), None, 0))
+        out = np.zeros(n, dtype=abi.pose_dtype())
+        if n:
+            self.check(self.fn("ground_truth_parse")(ds, int(sequence_id), buf.ctypes.data, len(buf), out.ctypes.data, n))
+        return out
 
     def apply_uniform_noise(self, poses, scale_rot_deg, scale_trans_m, seed=0):
         """slam::ApplyUniformNoise of every pose (a copy, as an array of abi.pose_dtype()); pose i draws under key
@@ -1710,3 +1830,107 @@ class LidarScene:
         self.sweeps_sink(trajectory, sensor, fr, seed, sink, idx, ends)
         return {"xyz": np.ascontiguousarray(rec["xyz"]), "t": np.ascontiguousarray(rec["t"]), "ray_index": idx,
                 "frame_ends": ends}
+
+
+class NcltHits:
+    """An indexed NCLT velodyne_hits.bin stream on one device (include/cticp.h, "Dataset sequences")."""
+
+    def __init__(self, binding, data, num_aggregated=220, final=True, device=0):
+        self.b = binding
+        self.device = device
+        self.h = C.c_void_p()
+        if _is_cuda_tensor(data):
+            import torch
+            if data.dtype != torch.uint8 or not data.is_contiguous() or data.device.index != device:
+                raise ValueError("data must be a contiguous uint8 tensor on cuda:%d" % device)
+            stream = torch.cuda.current_stream(device).cuda_stream
+            binding.check(binding.fn("nclt_open_device")(data.data_ptr() if data.numel() else None, data.numel(),
+                                                         int(num_aggregated), int(bool(final)), device,
+                                                         C.c_void_p(stream), C.byref(self.h)))
+        else:
+            buf = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else \
+                np.ascontiguousarray(data).view(np.uint8).reshape(-1)
+            binding.check(binding.fn("nclt_open")(buf.ctypes.data if len(buf) else None, len(buf), int(num_aggregated),
+                                                  int(bool(final)), device, C.byref(self.h)))
+
+    def close(self):
+        if self.h:
+            self.b.fn("nclt_destroy")(self.h)
+        self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def num_frames(self):
+        return self.b.check(self.b.fn("nclt_num_frames")(self.h))
+
+    @property
+    def num_packets(self):
+        return self.b.check(self.b.fn("nclt_num_packets")(self.h))
+
+    @property
+    def num_hits(self):
+        return self.b.check(self.b.fn("nclt_num_hits")(self.h))
+
+    @property
+    def bytes_used(self):
+        return self.b.check(self.b.fn("nclt_bytes_used")(self.h))
+
+    @property
+    def index_walked(self):
+        """True when the one-thread walk built the index (a chain link failed), False for the parallel chain check"""
+        return bool(self.b.check(self.b.fn("nclt_index_walked")(self.h)))
+
+    def frame_info(self, first=0, m=None):
+        """frames [first, first + m): an array of abi.nclt_frame_dtype() (num_points, t_first, t_max)"""
+        m = self.num_frames - first if m is None else m
+        out = np.zeros(max(m, 0), dtype=abi.nclt_frame_dtype())
+        self.b.check(self.b.fn("nclt_frame_info")(self.h, first, m, out.ctypes.data if m else None))
+        return out
+
+    def read_sink(self, first, m, sink, frame_ends):
+        """cticp_nclt_read_frames into an abi.CloudSink in host memory; frame_ends a (m,) uint64 array. Returns the count."""
+        return self.b.check(self.b.fn("nclt_read_frames")(self.h, first, m, C.byref(sink),
+                                                          frame_ends.ctypes.data if m else None))
+
+    def read_device(self, first, m, sink, frame_ends_ptr, stream=0):
+        """cticp_nclt_read_frames_device: an abi.CloudSink and frame_ends in device memory, ordered after and before
+        `stream`"""
+        return self.b.check(self.b.fn("nclt_read_frames_device")(self.h, first, m, C.byref(sink),
+                                                                 C.c_void_p(frame_ends_ptr or None),
+                                                                 C.c_void_p(stream or None)))
+
+    def read(self, first=0, m=None, dtype=np.float64, device=True):
+        """Frames [first, first + m) as a dict: xyz (N, 3) of `dtype`, t (N,) float64 in microseconds and frame_ends
+        (m,): torch CUDA tensors decoded on torch's current stream with device=True, NumPy arrays otherwise."""
+        m = self.num_frames - first if m is None else m
+        dt = np.dtype(dtype)
+        if dt not in (np.dtype(np.float32), np.dtype(np.float64)):
+            raise ValueError("dtype must be float32 or float64")
+        code = abi.DTYPE[dt.name]
+        size = dt.itemsize
+        step = 3 * size + 8 + (4 if size == 4 else 0)   # x y z, pad to 8, t
+        toff = step - 8
+        info = self.frame_info(first, m)
+        count = int(info["num_points"].sum())
+        if device:
+            import torch
+            dev = torch.device("cuda", self.device)
+            rec = torch.empty((count, step), dtype=torch.uint8, device=dev)
+            ends = torch.zeros(m, dtype=torch.int64, device=dev)
+            sink = abi.CloudSink(rec.data_ptr() if count else None, count, step, 0, code, toff, abi.DTYPE["float64"], 0)
+            if m:
+                self.read_device(first, m, sink, ends.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream)
+            return {"xyz": rec[:, :3 * size].view(getattr(torch, dt.name)),
+                    "t": rec[:, toff:].view(torch.float64).reshape(-1), "frame_ends": ends}
+        rec = np.zeros(count, dtype=np.dtype({"names": ["xyz", "t"], "formats": [(dt, 3), np.float64],
+                                              "offsets": [0, toff], "itemsize": step}))
+        ends = np.zeros(m, dtype=np.uint64)
+        sink = abi.CloudSink(rec.ctypes.data if count else None, count, step, 0, code, toff, abi.DTYPE["float64"], 0)
+        if m:
+            self.read_sink(first, m, sink, ends)
+        return {"xyz": np.ascontiguousarray(rec["xyz"]), "t": np.ascontiguousarray(rec["t"]), "frame_ends": ends}

@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "../../include/cticp.h"
+#include "dataset.h"
 #include "engine.h"
 #include "lidar_sim.h"
 #include "neighborhood.h"
@@ -58,6 +59,15 @@ void RequireDevice(int device) {
     CT_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9 || prop.minor != 0) throw std::runtime_error("NO_DEVICE: this build targets sm_90a (Hopper H100) only");
 }
+// RequireDevice without cudaGetDeviceProperties (milliseconds per call): for the per-frame dataset entry points
+void RequireDeviceCheap(int device) {
+    int count = 0, major = 0, minor = 0;
+    if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0 || device < 0 || device >= count)
+        throw std::runtime_error("NO_DEVICE: no usable CUDA device (this engine has no CPU fallback)");
+    CT_CUDA_CHECK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device));
+    CT_CUDA_CHECK(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device));
+    if (major != 9 || minor != 0) throw std::runtime_error("NO_DEVICE: this build targets sm_90a (Hopper H100) only");
+}
 }  // namespace
 
 struct cticp_map {
@@ -90,6 +100,9 @@ struct cticp_synthetic_scene {
 struct cticp_lidar_scene {
     std::unique_ptr<LidarScene> impl;
 };
+struct cticp_nclt {
+    std::unique_ptr<NcltHits> impl;
+};
 
 extern "C" {
 
@@ -107,6 +120,8 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_synthetic_frame") return sizeof(cticp_synthetic_frame);
     if (s == "cticp_lidar_sensor") return sizeof(cticp_lidar_sensor);
     if (s == "cticp_lidar_frame") return sizeof(cticp_lidar_frame);
+    if (s == "cticp_nclt_frame") return sizeof(cticp_nclt_frame);
+    if (s == "cticp_ply_layout") return sizeof(cticp_ply_layout);
     if (s == "cticp_strategy_options") return sizeof(cticp_strategy_options);
     if (s == "cticp_motion_model_options") return sizeof(cticp_motion_model_options);
     if (s == "cticp_odometry_options") return sizeof(cticp_odometry_options);
@@ -928,6 +943,120 @@ int cticp_lidar_generate_sweeps_device(cticp_lidar_scene *s, cticp_trajectory *t
                                       static_cast<cudaStream_t>(stream));
         return (int) CTICP_OK;
     });
+}
+
+/* ---- dataset sequences (dataset.cu) ---------------------------------------------------------------------------- */
+static int NcltOpen(const void *bytes, size_t n_bytes, uint32_t num_aggregated, int final, int device, bool on_device,
+                    void *stream, cticp_nclt **out) {
+    return Guard([&] {
+        if (!out) throw std::invalid_argument("null argument");
+        RequireDeviceCheap(device);
+        auto h = std::make_unique<cticp_nclt>();
+        h->impl = std::make_unique<NcltHits>(bytes, n_bytes, num_aggregated, final != 0, device, on_device,
+                                             static_cast<cudaStream_t>(stream));
+        *out = h.release();
+        return (int) CTICP_OK;
+    });
+}
+int cticp_nclt_open(const void *bytes, size_t n_bytes, uint32_t num_aggregated, int final, int device, cticp_nclt **out) {
+    return NcltOpen(bytes, n_bytes, num_aggregated, final, device, false, nullptr, out);
+}
+int cticp_nclt_open_device(const void *bytes, size_t n_bytes, uint32_t num_aggregated, int final, int device,
+                           void *stream, cticp_nclt **out) {
+    return NcltOpen(bytes, n_bytes, num_aggregated, final, device, true, stream, out);
+}
+void cticp_nclt_destroy(cticp_nclt *h) { delete h; }
+int64_t cticp_nclt_num_frames(const cticp_nclt *h) {
+    return h ? (int64_t) h->impl->NumFrames() : Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+}
+int64_t cticp_nclt_num_packets(const cticp_nclt *h) {
+    return h ? (int64_t) h->impl->NumPackets() : Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+}
+int64_t cticp_nclt_num_hits(const cticp_nclt *h) {
+    return h ? (int64_t) h->impl->NumHits() : Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+}
+int64_t cticp_nclt_bytes_used(const cticp_nclt *h) {
+    return h ? (int64_t) h->impl->BytesUsed() : Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+}
+int cticp_nclt_index_walked(const cticp_nclt *h) {
+    return h ? (h->impl->Walked() ? 1 : 0) : Fail(CTICP_ERR_INVALID_ARGUMENT, "null handle");
+}
+int cticp_nclt_frame_info(const cticp_nclt *h, size_t first, size_t m, cticp_nclt_frame *out) {
+    return Guard([&] {
+        if (!h) throw std::invalid_argument("null handle");
+        h->impl->FrameInfo(first, m, out);
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_nclt_read_frames(cticp_nclt *h, size_t first, size_t m, const cticp_cloud_sink *sink,
+                               uint64_t *frame_ends) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        if (!h || !sink) throw std::invalid_argument("null argument");
+        count = h->impl->ReadFrames(first, m, *sink, frame_ends);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
+}
+int cticp_nclt_read_frames_device(cticp_nclt *h, size_t first, size_t m, const cticp_cloud_sink *sink,
+                                  uint64_t *frame_ends, void *stream) {
+    return Guard([&] {
+        if (!h || !sink) throw std::invalid_argument("null argument");
+        h->impl->ReadFramesDevice(first, m, *sink, frame_ends, static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+}
+int cticp_ply_layout_parse(const void *bytes, size_t n, cticp_ply_layout *out) {
+    return Guard([&] {
+        PlyLayoutParse(static_cast<const char *>(bytes), n, out);
+        return (int) CTICP_OK;
+    });
+}
+int cticp_kitti_frame_filter_device(int device, const cticp_device_scan *scan, const cticp_cloud_sink *sink,
+                                    void *stream) {
+    return Guard([&] {
+        if (!scan || !sink) throw std::invalid_argument("null argument");
+        RequireDeviceCheap(device);
+        KittiFrameFilterDevice(device, *scan, *sink, static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+}
+int cticp_kitti_frame_filter(int device, const cticp_cloud_view *cloud, const cticp_cloud_sink *sink) {
+    return Guard([&] {
+        if (!cloud || !sink) throw std::invalid_argument("null argument");
+        RequireDeviceCheap(device);
+        KittiFrameFilter(device, *cloud, *sink);
+        return (int) CTICP_OK;
+    });
+}
+int cticp_scan_time_ranges_device(int device, const cticp_device_scan *scan, const uint64_t *frame_ends, size_t m,
+                                  double *out_minmax, void *stream) {
+    return Guard([&] {
+        if (!scan) throw std::invalid_argument("null argument");
+        RequireDeviceCheap(device);
+        ScanTimeRangesDevice(device, *scan, frame_ends, m, out_minmax, static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+}
+int cticp_scan_time_ranges(int device, const cticp_cloud_view *cloud, const uint64_t *frame_ends, size_t m,
+                           double *out_minmax) {
+    return Guard([&] {
+        if (!cloud) throw std::invalid_argument("null argument");
+        RequireDeviceCheap(device);
+        ScanTimeRanges(device, *cloud, frame_ends, m, out_minmax);
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_ground_truth_parse(int dataset, int sequence_id, const char *text, size_t n, cticp_pose *out, size_t cap) {
+    int64_t count = 0;
+    int rc = Guard([&] {
+        const std::vector<cticp_pose> poses = GroundTruthParse(dataset, sequence_id, text, n);
+        if (cap && !out) throw std::invalid_argument("null out");
+        std::copy(poses.begin(), poses.begin() + std::min(cap, poses.size()), out);
+        count = (int64_t) poses.size();
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
 }
 
 /* ---- neighbourhoods of a point cloud (neighborhood.cu) ---------------------------------------------------------- */

@@ -1435,3 +1435,97 @@ private:
 };
 
 }  // namespace slam
+
+// ---- Dataset sequences over cticp_nclt_*, cticp_ply_layout_parse, cticp_kitti_frame_filter, cticp_ground_truth_parse --
+// The readers of the reference's dataset.cpp (semantics, quirks and deviations: include/cticp.h, "Dataset sequences").
+namespace ct_icp {
+
+// An indexed NCLT velodyne_hits.bin stream on one device: frames of num_aggregated packets
+class NCLTHits {
+public:
+    NCLTHits(const void *bytes, size_t n, uint32_t num_aggregated = 220, bool final = true, int device = 0) {
+        cticp_check(cticp_nclt_open(bytes, n, num_aggregated, final ? 1 : 0, device, &h_));
+    }
+    ~NCLTHits() {
+        if (h_) cticp_nclt_destroy(h_);
+    }
+    NCLTHits(NCLTHits &&o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+    NCLTHits &operator=(NCLTHits &&o) noexcept {
+        std::swap(h_, o.h_);
+        return *this;
+    }
+    NCLTHits(const NCLTHits &) = delete;
+    NCLTHits &operator=(const NCLTHits &) = delete;
+    cticp_nclt *Handle() const { return h_; }
+
+    size_t NumFrames() const { return (size_t) Checked(cticp_nclt_num_frames(h_)); }
+    size_t NumPackets() const { return (size_t) Checked(cticp_nclt_num_packets(h_)); }
+    size_t NumHits() const { return (size_t) Checked(cticp_nclt_num_hits(h_)); }
+    size_t BytesUsed() const { return (size_t) Checked(cticp_nclt_bytes_used(h_)); }
+    std::vector<cticp_nclt_frame> FrameInfo(size_t first, size_t m) const {
+        std::vector<cticp_nclt_frame> out(m);
+        cticp_check(cticp_nclt_frame_info(h_, first, m, m ? out.data() : nullptr));
+        return out;
+    }
+    // frames [first, first + m) as the reference's point records: raw xyz and timestamp (microseconds), index_frame = the
+    // frame's index in the stream; frame_ends (nullable) gets each frame's end
+    std::vector<slam::WPoint3D> ReadFrames(size_t first, size_t m, std::vector<uint64_t> *frame_ends = nullptr) const {
+        std::vector<uint64_t> ends(m);
+        cticp_cloud_sink sink{nullptr, 0, sizeof(slam::WPoint3D), 0, CTICP_DTYPE_FLOAT64, 24, CTICP_DTYPE_FLOAT64, 0};
+        const int64_t count = Checked(cticp_nclt_read_frames(h_, first, m, &sink, m ? ends.data() : nullptr));
+        std::vector<slam::WPoint3D> points((size_t) count);
+        if (count) {
+            sink.data = points.data();
+            sink.capacity_points = points.size();
+            Checked(cticp_nclt_read_frames(h_, first, m, &sink, ends.data()));
+            size_t i = 0;
+            for (size_t k = 0; k < m; ++k)
+                for (; i < ends[k]; ++i) points[i].index_frame = (slam::frame_id_t) (first + k);
+        }
+        if (frame_ends) *frame_ends = ends;
+        return points;
+    }
+
+private:
+    static int64_t Checked(int64_t rc) {
+        if (rc < 0) cticp_check((int) rc);
+        return rc;
+    }
+    cticp_nclt *h_ = nullptr;
+};
+
+// the vertex record layout of a binary_little_endian PLY file (PLYSchemaMapper::Builder::BuilderFromPLYFile's rules)
+inline cticp_ply_layout ReadPLYLayout(const void *bytes, size_t n) {
+    cticp_ply_layout out{};
+    cticp_check(cticp_ply_layout_parse(bytes, n, &out));
+    return out;
+}
+
+// kitti_frame_filter of the raw points, in place, on `device`
+inline void KittiFrameFilter(std::vector<slam::WPoint3D> &points, int device = 0) {
+    if (points.empty()) return;
+    const cticp_cloud_view view{points.data(), points.size(), sizeof(slam::WPoint3D), 0, CTICP_DTYPE_FLOAT64, 24,
+                                CTICP_DTYPE_FLOAT64, 0};
+    const cticp_cloud_sink sink{points.data(), points.size(), sizeof(slam::WPoint3D), 0, CTICP_DTYPE_FLOAT64, 0, 0, 0};
+    cticp_check(cticp_kitti_frame_filter(device, &view, &sink));
+}
+
+// LoadPoses of a ground-truth file's text in the LiDAR frame; dataset is a CTICP_DATASET_* (the reference's DATASET)
+inline std::vector<slam::Pose> LoadGroundTruth(int dataset, const std::string &text, int sequence_id = 0) {
+    const int64_t n = cticp_ground_truth_parse(dataset, sequence_id, text.data(), text.size(), nullptr, 0);
+    if (n < 0) cticp_check((int) n);
+    std::vector<cticp_pose> raw((size_t) n);
+    if (n) cticp_ground_truth_parse(dataset, sequence_id, text.data(), text.size(), raw.data(), raw.size());
+    std::vector<slam::Pose> out(raw.size());
+    for (size_t i = 0; i < raw.size(); ++i) {
+        for (int k = 0; k < 4; ++k) out[i].pose.quat.c[k] = raw[i].quat[k];
+        for (int k = 0; k < 3; ++k) out[i].pose.tr.v[k] = raw[i].tr[k];
+        out[i].ref_timestamp = raw[i].ref_timestamp;
+        out[i].dest_timestamp = raw[i].dest_timestamp;
+        out[i].ref_frame_id = raw[i].ref_frame_id;
+        out[i].dest_frame_id = raw[i].dest_frame_id;
+    }
+    return out;
+}
+
+}  // namespace ct_icp

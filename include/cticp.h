@@ -969,6 +969,118 @@ int cticp_lidar_generate_sweeps_device(cticp_lidar_scene *s, cticp_trajectory *t
                                        const cticp_cloud_sink *sink, uint32_t *ray_index, uint64_t *frame_ends,
                                        void *stream);
 
+/* ---- Dataset sequences (src/ct_icp/dataset.cpp: NCLTIterator, kitti_frame_filter, LoadPoses) ------------------------
+ * NCLT velodyne_hits.bin: packets of a 24-byte header (4 x u16 magic 44444, u32 num_hits, u64 utime at byte 12, u32 pad)
+ * and num_hits hits of 8 bytes (u16 x, y, z, u8 intensity, u8 laser). A handle copies the bytes into its own device
+ * buffer and indexes the packets there: one thread per 8-byte word finds the magic words, the candidates are compacted
+ * in order, and each one's successor (c + 24 + 8 num_hits) must be the next candidate; otherwise (a hit whose bytes equal
+ * the magic) one device thread walks the packets from offset 0, as the reference reads them. Frame f is packets
+ * [f A, (f + 1) A), A = num_aggregated (the reference's nclt_num_aggregated_pc, 220), counted from the start of the bytes.
+ * final = 0 keeps whole frames only (bytes_used: where the next chunk starts, so chunking never shifts the grouping);
+ * final = 1 lets the last frame hold the complete packets that remain. Decoded points: x = (double) u 0.005 - 100.0 (an
+ * fp64 multiply then subtract, no FMA; y, z the same), t = (double) utime in microseconds, in packet then hit order;
+ * intensity and laser are dropped. Quirks and deviations:
+ *   - a packet with num_hits = 0 counts towards the A packets of its frame but adds no point and no timestamp;
+ *   - the sequence ends after the last complete packet (the reference's eof() test reads one header past it);
+ *   - a frame's begin time is its first point's timestamp (the reference's minmax of iterators), its end time the
+ *     maximum timestamp (the reference dereferences end() there). A frame without points has NaN for both.
+ * Refusals at open (CTICP_ERR_INVALID_ARGUMENT, no handle): num_aggregated 0, 32 GiB or more of bytes (the index's
+ * counts are 32-bit), a header whose magic is wrong (the message names its byte offset: a refused open returns no handle
+ * to read it from), with final = 1 a truncated last packet or trailing bytes. */
+typedef struct cticp_nclt cticp_nclt;   /* opaque: one device, its own stream */
+typedef struct cticp_nclt_frame {   /* one frame of cticp_nclt_frame_info */
+    uint64_t num_points;
+    double t_first;                     /* the first point's timestamp (begin_pose) */
+    double t_max;                       /* the largest timestamp (end_pose) */
+} cticp_nclt_frame;
+int cticp_nclt_open(const void *bytes, size_t n_bytes, uint32_t num_aggregated, int final, int device, cticp_nclt **out);
+/* the same on bytes in device memory of `device`, read after the work queued on `stream`; returns once indexed */
+int cticp_nclt_open_device(const void *bytes, size_t n_bytes, uint32_t num_aggregated, int final, int device,
+                           void *stream, cticp_nclt **out);
+void cticp_nclt_destroy(cticp_nclt *h);
+int64_t cticp_nclt_num_frames(const cticp_nclt *h);
+int64_t cticp_nclt_num_packets(const cticp_nclt *h);
+int64_t cticp_nclt_num_hits(const cticp_nclt *h);
+int64_t cticp_nclt_bytes_used(const cticp_nclt *h);
+/* 1 when the index came from the one-thread walk (a chain link failed), 0 when the parallel chain check built it */
+int cticp_nclt_index_walked(const cticp_nclt *h);
+/* frames [first, first + m) */
+int cticp_nclt_frame_info(const cticp_nclt *h, size_t first, size_t m, cticp_nclt_frame *out);
+/* The points of frames [first, first + m) into `sink` (world must be 0; t_dtype 0, FLOAT32 or FLOAT64), frame k's ending
+ * at frame_ends[k] (counted from the call's first point). Writes min(capacity_points, count) records. Host memory,
+ * synchronous; returns the count. CTICP_ERR_INVALID_ARGUMENT before anything is written: frames outside the handle,
+ * null pointers, unknown sink dtypes, fields outside point_step, world != 0. */
+int64_t cticp_nclt_read_frames(cticp_nclt *h, size_t first, size_t m, const cticp_cloud_sink *sink,
+                               uint64_t *frame_ends);
+/* The same bytes into device memory of the handle's device (sink and frame_ends, 8-byte aligned), enqueued after the
+ * work queued on `stream`, which is made to wait for the result; no host synchronisation. A frame's slice of the sink
+ * (with a timestamp) is a cticp_device_scan for cticp_odometry_register_device. */
+int cticp_nclt_read_frames_device(cticp_nclt *h, size_t first, size_t m, const cticp_cloud_sink *sink,
+                                  uint64_t *frame_ends, void *stream);
+
+/* A binary_little_endian PLY header (PLYSchemaMapper::Builder::BuilderFromPLYFile, src/SlamCore/io.cxx:1234-1325): the
+ * "vertex" element's record layout. x, y, z of one float type, each sizeof(scalar) after the previous; the timestamp is
+ * the property named "timestamp", "t" or "timestamps" (the first present), of any scalar type (t_dtype 0 when none);
+ * point_step is the sum of the property sizes. Host only. CTICP_ERR_UNSUPPORTED: ascii or binary_big_endian, list
+ * properties, an element other than vertex. CTICP_ERR_INVALID_ARGUMENT: no "ply" magic or end_header, x, y, z missing,
+ * mixed or not consecutive, an unknown property type, a body shorter than num_points records. */
+typedef struct cticp_ply_layout {
+    uint64_t body_offset;               /* the first record's byte offset */
+    uint64_t num_points;
+    uint32_t point_step;
+    uint32_t xyz_offset;
+    int32_t xyz_dtype;                  /* CTICP_DTYPE_FLOAT32 or CTICP_DTYPE_FLOAT64 */
+    uint32_t t_offset;
+    int32_t t_dtype;                    /* any CTICP_DTYPE_*, 0 = no timestamp */
+    int32_t _pad0;
+} cticp_ply_layout;
+int cticp_ply_layout_parse(const void *bytes, size_t n, cticp_ply_layout *out);
+
+/* kitti_frame_filter (src/ct_icp/dataset.cpp:85-110), one thread per record, in fp64 without FMA: a point with
+ * !(z > -5) becomes (0, 0, 0) (NaN points included); any other is rotated by AngleAxis(0.205 pi / 180, axis),
+ * axis = (p x (0, 0, 1)).normalized() (a zero axis stays zero, so a point on the z axis is scaled by cos), with Eigen's
+ * toRotationMatrix and sin / cos from the host C library. The result is written in the sink's xyz type (the reference
+ * writes through its XYZ<double>() proxy into the cloud's own type), with the scan's timestamp when sink->t_dtype != 0.
+ * The sink may be the scan's own records (same point_step and xyz offset) with t_dtype = 0: the filter runs in place.
+ * Device memory of `device`, enqueued on `stream`. CTICP_ERR_INVALID_ARGUMENT before anything is enqueued: null or
+ * out-of-allocation pointers, unknown dtypes, fields outside point_step, world != 0, capacity below the scan's count. */
+int cticp_kitti_frame_filter_device(int device, const cticp_device_scan *scan, const cticp_cloud_sink *sink,
+                                    void *stream);
+/* the same on host records (copied through the device; synchronous) */
+int cticp_kitti_frame_filter(int device, const cticp_cloud_view *cloud, const cticp_cloud_sink *sink);
+
+/* Per-frame (min, max) of the scan's timestamps (ProcessFrame's minmax_element, dataset.cpp:306-316): frame k is points
+ * [frame_ends[k-1], frame_ends[k]) (frame_ends[-1] = 0) and out_minmax[2k], [2k+1] its range; a frame without points
+ * gets (+inf, -inf). A NaN timestamp: the device variant writes (NaN, NaN) for its frame, the host variant returns
+ * CTICP_ERR_INVALID_ARGUMENT (the reference's answer depends on the NaN's position). frame_ends must be non-decreasing
+ * and end at most at num_points (checked by the host variant; the device one reads them on the device). The scan's
+ * x, y, z are not read (scan->xyz may be NULL). */
+int cticp_scan_time_ranges_device(int device, const cticp_device_scan *scan, const uint64_t *frame_ends, size_t m,
+                                  double *out_minmax, void *stream);
+int cticp_scan_time_ranges(int device, const cticp_cloud_view *cloud, const uint64_t *frame_ends, size_t m,
+                           double *out_minmax);
+
+/* Ground truth in the LiDAR frame (LoadPoses, dataset.cpp:998-1098). dataset: the reference's DATASET values. Returns
+ * the count and copies min(cap, count) poses. Host only.
+ *   - KITTI_raw, KITTI, KITTI_360, KITTI_CARLA: LoadPosesKITTIFormat (io.cxx:252-279): each non-empty line's 12 values
+ *     fill a 3x4 matrix over the identity, read as `istream >> double` reads them (decimal only: no nan, inf or hex; a
+ *     short line keeps the identity's values where it ends; a value that is not a number becomes 0 and ends the line);
+ *     Quaternion(R), then CalibI * M * Calib with the sequence's calibration
+ *     (KITTI / KITTI_raw: ids 0-2, 3, 4-21; KITTI_360: one; KITTI_CARLA: identity), quaternion normalised;
+ *     dest_timestamp (i + 0.5) 0.1 (KITTI_CARLA: i 0.1), dest_frame_id i.
+ *   - NCLT: ReadNCLTPoses (:319-381): 7 comma-separated values t, x, y, z, roll, pitch, yaw per line; rotation
+ *     Rz(yaw) Ry(pitch) Rx(roll); rows with a NaN skipped; each pose relative to the first, then kNCLT_Calib as above;
+ *     dest_frame_id stays 0xFFFFFFFF (the reference's -1). A row of another count or a token that is not a number:
+ *     CTICP_ERR_INVALID_ARGUMENT (the reference's CHECK / std::stod).
+ *   - HILTI_2021, HILTI_2022 (:642-677): t, x, y, z, qx, qy, qz, qw per line, the quaternion NOT normalised (the
+ *     reference discards quat.normalized()), then imu_to_lidar * pose * lidar_to_imu in SE3 arithmetic.
+ * One stated deviation: CalibI is the rigid inverse [R^T, -R^T t], where the reference takes Eigen's general
+ * Matrix4d::inverse(); the two differ in the last bits, so poses agree with the reference's to ~1e-15, not bit for bit.
+ * CTICP_ERR_INVALID_ARGUMENT: a dataset outside these, a KITTI sequence id outside [0, 21]. */
+enum { CTICP_DATASET_KITTI_RAW = 0, CTICP_DATASET_KITTI_CARLA = 1, CTICP_DATASET_KITTI = 2, CTICP_DATASET_KITTI_360 = 3,
+       CTICP_DATASET_NCLT = 4, CTICP_DATASET_HILTI_2021 = 5, CTICP_DATASET_HILTI_2022 = 6 };
+int64_t cticp_ground_truth_parse(int dataset, int sequence_id, const char *text, size_t n, cticp_pose *out, size_t cap);
+
 /* ---- Map (L2 boundary; used directly by the parity tests) ---------------------------------------------- */
 
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */
