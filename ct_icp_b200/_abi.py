@@ -171,7 +171,18 @@ class PlyLayout(_Struct):   # cticp_ply_layout: the vertex records of a binary_l
                 ("_pad0", C.c_int32)]
 
 
-# CTICP_DATASET_*: the reference's ct_icp::DATASET values (include/ct_icp/dataset.h)
+# source types of a PLY column (cticp.h CTICP_DTYPE_INT64 / _UINT64 are valid there only)
+PLY_SRC_DTYPE = dict(DTYPE, int64=9, uint64=10)
+# PLY property type names (tinyply's), by CTICP_DTYPE_*
+PLY_TYPE_NAME = {1: "char", 2: "uchar", 3: "short", 4: "ushort", 5: "int", 6: "uint", 7: "float", 8: "double"}
+
+
+class PlyProperty(_Struct):   # cticp_ply_property: one PLY property as a strided column of scalars
+    _fields_ = [("element", C.c_char_p), ("name", C.c_char_p), ("ply_dtype", C.c_int32), ("src_dtype", C.c_int32),
+                ("src", C.c_void_p), ("src_stride_bytes", C.c_uint64)]
+
+
+# CTICP_DATASET_*:the reference's ct_icp::DATASET values (include/ct_icp/dataset.h)
 DATASET = {"KITTI_raw": 0, "KITTI_CARLA": 1, "KITTI": 2, "KITTI_360": 3, "NCLT": 4, "HILTI_2021": 5, "HILTI_2022": 6}
 
 

@@ -140,6 +140,52 @@ def _snapshot_bytes(binding, fn, handle):
     return buf.raw
 
 
+def _ply_code(t):
+    """a PLY property type: a CTICP_DTYPE_* code, a tinyply name or a NumPy dtype name"""
+    if isinstance(t, (int, np.integer)):
+        return int(t)
+    names = {v: k for k, v in abi.PLY_TYPE_NAME.items()}
+    return names[t] if t in names else abi.DTYPE[np.dtype(t).name]
+
+
+def _ply_src_code(name):
+    if name not in abi.PLY_SRC_DTYPE:
+        raise ValueError("no PLY source type for %s" % name)
+    return abi.PLY_SRC_DTYPE[name]
+
+
+def _ply_num_items(shapes, num_items):
+    lengths = {s[0] for s in shapes if len(s) == 1}
+    if num_items is None:
+        if len(lengths) > 1:
+            raise ValueError("the columns have different lengths %s" % sorted(lengths))
+        return lengths.pop() if lengths else 1
+    if any(length < num_items for length in lengths):
+        raise ValueError("a column is shorter than num_items")
+    return int(num_items)
+
+
+def _ply_props(cols, src_codes, sources):
+    """a cticp_ply_property array (and the encoded names it points to) from (element, name, ply_dtype, _) columns and
+    (pointer, stride) sources"""
+    props = (abi.PlyProperty * len(cols))()
+    keep = []
+    for i, ((elem, name, ply, _), code, (ptr, stride)) in enumerate(zip(cols, src_codes, sources)):
+        e, nm = elem.encode(), name.encode()
+        keep += [e, nm]
+        props[i] = abi.PlyProperty(e, nm, _ply_code(ply), code, ptr, stride)
+    return props, keep
+
+
+def _pose_columns(arr):
+    """SavePosesAsPLY's eleven columns: strided views of a cticp_pose array, whose records are the file's records"""
+    cols = [("pose", nm, "double", arr["quat"][:, i]) for i, nm in enumerate(["qx", "qy", "qz", "qw"])]
+    cols += [("pose", nm, "double", arr["tr"][:, i]) for i, nm in enumerate(["x", "y", "z"])]
+    cols += [("pose", "ref_t", "double", arr["ref_timestamp"]), ("pose", "dest_t", "double", arr["dest_timestamp"]),
+             ("pose", "ref_fid", "int", arr["ref_frame_id"]), ("pose", "dest_fid", "int", arr["dest_frame_id"])]
+    return cols
+
+
 class Binding:
     def __init__(self, lib, prefix):
         self.lib = lib
@@ -317,6 +363,9 @@ class Binding:
             "scan_time_ranges": (C.c_int, [C.c_int, P(abi.CloudView), vp, sz, vp]),
             "scan_time_ranges_device": (C.c_int, [C.c_int, P(abi.DeviceScan), vp, sz, vp, vp]),
             "ground_truth_parse": (i64, [C.c_int, C.c_int, vp, sz, vp, sz]),
+            "ply_write": (i64, [C.c_int, P(abi.PlyProperty), sz, u64, vp, u64]),
+            "ply_write_device": (C.c_int, [C.c_int, P(abi.PlyProperty), sz, u64, vp, sz, vp, u64, vp, vp]),
+            "ply_read_poses": (i64, [vp, sz, vp, sz]),
         })
         for name, (res, args) in sigs.items():
             if self.has(name):
@@ -657,6 +706,97 @@ class Binding:
         out = np.zeros(n, dtype=abi.pose_dtype())
         if n:
             self.check(self.fn("ground_truth_parse")(ds, int(sequence_id), buf.ctypes.data, len(buf), out.ctypes.data, n))
+        return out
+
+    # ---- PLY files -------------------------------------------------------------------------------------------
+    def ply_write(self, columns, file_ends=None, device=0, num_items=None):
+        """PLY files of columns (include/cticp.h, "PLY files"): `columns` is an ordered list of (element, name,
+        ply_dtype, array), ply_dtype a CTICP_DTYPE_* code, a tinyply name ("float") or a NumPy dtype name ("float32");
+        each array is 1-D (any stride) or 0-d (one value for every item), NumPy arrays or torch CUDA tensors on `device`.
+        num_items defaults to the 1-D columns' common length. Host arrays: the bytes of one file, or with file_ends
+        (non-decreasing, at most num_items) (bytes of every file back to back, int64 offsets of m + 1). CUDA tensors: a
+        uint8 tensor of every file and an int64 tensor of the m + 1 offsets, written in order with torch's current
+        stream (one host synchronisation reads the total size)."""
+        cols = list(columns)
+        if not cols:
+            raise CticpError(abi.ERR_INVALID_ARGUMENT, "no columns")
+        if any(_is_cuda_tensor(c[3]) for c in cols):
+            return self._ply_write_device(cols, file_ends, device, num_items)
+        arrays = []
+        for c in cols:
+            a = np.asarray(c[3])
+            if a.ndim > 1:
+                raise ValueError("column %s: expected a 1-D or 0-d array" % c[1])
+            if a.ndim == 1 and a.strides[0] < 0:
+                a = np.ascontiguousarray(a)
+            arrays.append(a)
+        n = _ply_num_items([a.shape for a in arrays], num_items)
+        codes = [_ply_src_code(a.dtype.name) for a in arrays]
+
+        def encode(first, count):
+            props, keep = _ply_props(cols, codes, [(a.ctypes.data + (first * a.strides[0] if a.ndim else 0)
+                                                    if a.size else None, a.strides[0] if a.ndim else 0)
+                                                   for a in arrays])
+            size = self.check(self.fn("ply_write")(device, props, len(cols), count, None, 0))
+            buf = C.create_string_buffer(size)
+            self.check(self.fn("ply_write")(device, props, len(cols), count, buf, size))
+            return buf.raw
+
+        if file_ends is None:
+            return encode(0, n)
+        ends = np.asarray(file_ends, dtype=np.int64).reshape(-1)
+        if (np.diff(ends) < 0).any() or (len(ends) and (ends[0] < 0 or ends[-1] > n)):
+            raise CticpError(abi.ERR_INVALID_ARGUMENT, "file_ends must be non-decreasing and at most num_items")
+        files = [encode(int(b), int(e - b)) for b, e in zip(np.concatenate([[0], ends[:-1]]), ends)]
+        return b"".join(files), np.concatenate([[0], np.cumsum([len(f) for f in files])]).astype(np.int64)
+
+    def _ply_write_device(self, cols, file_ends, device, num_items):
+        import torch
+        dev = torch.device("cuda", device)
+        codes = {torch.int8: 1, torch.uint8: 2, torch.int16: 3, torch.int32: 5, torch.float32: 7, torch.float64: 8,
+                 torch.int64: 9}
+        for name, code in (("uint16", 4), ("uint32", 6), ("uint64", 10)):
+            if hasattr(torch, name):
+                codes[getattr(torch, name)] = code
+        tensors = []
+        for c in cols:
+            t = c[3]
+            if not _is_cuda_tensor(t) or t.device != dev:
+                raise ValueError("column %s: every column must be a CUDA tensor on cuda:%d" % (c[1], device))
+            if t.dim() > 1 or t.dtype not in codes:
+                raise ValueError("column %s: expected a 1-D or 0-d tensor of a scalar type" % c[1])
+            tensors.append(t)
+        n = _ply_num_items([tuple(t.shape) for t in tensors], num_items)
+        props, keep = _ply_props(cols, [codes[t.dtype] for t in tensors],
+                                 [(t.data_ptr() if t.numel() else None, t.stride(0) * t.element_size() if t.dim() else 0)
+                                  for t in tensors])
+        ends = torch.tensor([n], dtype=torch.int64, device=dev) if file_ends is None else \
+            torch.as_tensor(file_ends).to(device=dev, dtype=torch.int64).reshape(-1).contiguous()
+        m = ends.shape[0]
+        offsets = torch.empty(m + 1, dtype=torch.int64, device=dev)
+        stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+        fn = self.fn("ply_write_device")
+        self.check(fn(device, props, len(cols), n, ends.data_ptr() if m else None, m, None, 0, offsets.data_ptr(),
+                      stream))
+        out = torch.empty(int(offsets[-1].item()), dtype=torch.uint8, device=dev)
+        if out.numel():
+            self.check(fn(device, props, len(cols), n, ends.data_ptr() if m else None, m, out.data_ptr(), out.numel(),
+                          offsets.data_ptr(), stream))
+        return out, offsets
+
+    def save_poses_ply(self, poses, device=0):
+        """slam::SavePosesAsPLY: element pose with qx qy qz qw x y z ref_t dest_t (double) and ref_fid dest_fid (int),
+        eleven columns over the cticp_pose records; returns the file's bytes"""
+        arr = _pose_array(poses)
+        return self.ply_write(_pose_columns(arr), device=device, num_items=len(arr))
+
+    def read_poses_ply(self, data):
+        """slam::ReadPosesFromPLY of a file's bytes: an array of abi.pose_dtype()"""
+        buf = np.frombuffer(bytes(data), dtype=np.uint8)
+        n = self.check(self.fn("ply_read_poses")(buf.ctypes.data, len(buf), None, 0))
+        out = np.zeros(n, dtype=abi.pose_dtype())
+        if n:
+            self.check(self.fn("ply_read_poses")(buf.ctypes.data, len(buf), out.ctypes.data, n))
         return out
 
     def apply_uniform_noise(self, poses, scale_rot_deg, scale_trans_m, seed=0):
@@ -1448,6 +1588,38 @@ class WorldCloud:
                                  code if with_timestamps else 0, 1)
             self.export_sink(sink, src)
         return (out, src) if with_source_index else out
+
+    def export_ply(self, dtype=np.float32, with_timestamps=False, with_source_index=False, normals=None):
+        """The cloud as one PLY file's bytes, encoded on the device: element vertex with x y z in `dtype` (float32 ->
+        float, float64 -> double), then optionally timestamp (same type), source_index (uint: the low 32 bits of the
+        uint64 index) and nx ny nz (float) from `normals`, a Neighborhood.describe result over the export order (a
+        NumPy array of neighborhood_description_dtype() or the device variant's uint8 tensor). Everything stays on the
+        device until the file's one copy to the host."""
+        import torch
+        dtype = np.dtype(dtype)
+        if dtype not in (np.dtype(np.float32), np.dtype(np.float64)):
+            raise ValueError("dtype must be float32 or float64")
+        pts = self.export(np.float64, with_timestamps=True, with_source_index=with_source_index, device=True)
+        xyzt, src = pts if with_source_index else (pts, None)
+        n = xyzt.shape[0]
+        ply = "float" if dtype == np.float32 else "double"
+        cols = [("vertex", k, ply, xyzt[:, i]) for i, k in enumerate("xyz")]
+        if with_timestamps:
+            cols.append(("vertex", "timestamp", ply, xyzt[:, 3]))
+        if with_source_index:
+            cols.append(("vertex", "source_index", "uint", src))
+        if normals is not None:
+            dev = xyzt.device
+            rec = normals if _is_cuda_tensor(normals) else torch.from_numpy(
+                np.ascontiguousarray(normals).view(np.uint8).reshape(len(normals), -1)).to(dev)
+            if rec.shape[0] != n:
+                raise ValueError("normals has %d descriptions for %d points" % (rec.shape[0], n))
+            off = abi.neighborhood_description_dtype().fields["normal"][1]
+            nrm = rec.view(torch.float64)[:, off // 8:off // 8 + 3] if n else torch.zeros((0, 3), dtype=torch.float64,
+                                                                                         device=dev)
+            cols += [("vertex", k, "float", nrm[:, i]) for i, k in enumerate(("nx", "ny", "nz"))]
+        out, _ = self.b.ply_write(cols, device=self.device, num_items=n)
+        return out.cpu().numpy().tobytes()
 
 
 class Neighborhood:

@@ -11,6 +11,7 @@
 #include "engine.h"
 #include "lidar_sim.h"
 #include "neighborhood.h"
+#include "ply.h"
 #include "synthetic.h"
 #include "trajectory.h"
 #include "trajectory_eval.h"
@@ -122,6 +123,7 @@ size_t cticp_abi_sizeof(const char *name) {
     if (s == "cticp_lidar_frame") return sizeof(cticp_lidar_frame);
     if (s == "cticp_nclt_frame") return sizeof(cticp_nclt_frame);
     if (s == "cticp_ply_layout") return sizeof(cticp_ply_layout);
+    if (s == "cticp_ply_property") return sizeof(cticp_ply_property);
     if (s == "cticp_strategy_options") return sizeof(cticp_strategy_options);
     if (s == "cticp_motion_model_options") return sizeof(cticp_motion_model_options);
     if (s == "cticp_odometry_options") return sizeof(cticp_odometry_options);
@@ -1011,6 +1013,39 @@ int cticp_ply_layout_parse(const void *bytes, size_t n, cticp_ply_layout *out) {
         PlyLayoutParse(static_cast<const char *>(bytes), n, out);
         return (int) CTICP_OK;
     });
+}
+
+/* ---- PLY files (ply.cu) ---------------------------------------------------------------------------------------- */
+int64_t cticp_ply_write(int device, const cticp_ply_property *props, size_t n_props, uint64_t num_items, void *out,
+                        uint64_t capacity) {
+    int64_t size = 0;
+    const int rc = Guard([&] {
+        RequireDeviceCheap(device);
+        size = (int64_t) PlyWrite(device, props, n_props, num_items, out, capacity);
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : size;
+}
+int cticp_ply_write_device(int device, const cticp_ply_property *props, size_t n_props, uint64_t num_items,
+                           const uint64_t *file_ends, size_t m, void *out, uint64_t capacity, uint64_t *file_offsets,
+                           void *stream) {
+    return Guard([&] {
+        RequireDeviceCheap(device);
+        PlyWriteDevice(device, props, n_props, num_items, file_ends, m, out, capacity, file_offsets,
+                       static_cast<cudaStream_t>(stream));
+        return (int) CTICP_OK;
+    });
+}
+int64_t cticp_ply_read_poses(const void *bytes, size_t n, cticp_pose *out, size_t cap) {
+    int64_t count = 0;
+    const int rc = Guard([&] {
+        const std::vector<cticp_pose> poses = PlyReadPoses(static_cast<const char *>(bytes), n);
+        if (cap && !out) throw std::invalid_argument("null argument");
+        for (size_t i = 0; i < poses.size() && i < cap; ++i) out[i] = poses[i];
+        count = (int64_t) poses.size();
+        return (int) CTICP_OK;
+    });
+    return rc < 0 ? rc : count;
 }
 int cticp_kitti_frame_filter_device(int device, const cticp_device_scan *scan, const cticp_cloud_sink *sink,
                                     void *stream) {

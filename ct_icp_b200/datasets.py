@@ -188,6 +188,28 @@ class PLYDirectory(_Sequence):
         return {"xyz": xyz, "t": t, "begin_pose": begin, "end_pose": end}
 
 
+def write_ply_frames(binding, xyz, t, frame_ends, directory, digits=4, first_index=0, device=0):
+    """Frames of a scan sequence as frame_%0<digits>d.ply files in `directory` (numbered from first_index) in the
+    layout of the reference's WPoint3D::FloatSchemaMapper (io.cxx:842-855): element vertex, float x y z timestamp. xyz
+    (N, 3) and t (N,) are CUDA tensors or NumPy arrays of any float or integer type, frame_ends the frames' ends. All
+    frames are encoded in one device call and copied to the host once; PLYDirectory reads the directory back. Returns
+    the paths."""
+    cols = [("vertex", k, "float", xyz[:, i]) for i, k in enumerate("xyz")] + [("vertex", "timestamp", "float", t)]
+    if not any(hasattr(c[3], "is_cuda") and c[3].is_cuda for c in cols):
+        import torch
+        dev = torch.device("cuda", device)
+        cols = [(e, k, p, torch.as_tensor(np.asarray(a)).to(dev)) for e, k, p, a in cols]
+    data, offsets = binding.ply_write(cols, file_ends=frame_ends, device=device)
+    data, offsets = data.cpu().numpy(), offsets.cpu().numpy()
+    os.makedirs(directory, exist_ok=True)
+    paths = []
+    for k in range(len(offsets) - 1):
+        path = os.path.join(directory, ("frame_%0" + str(digits) + "d.ply") % (first_index + k))
+        with open(path, "wb") as f:
+            f.write(data[offsets[k]:offsets[k + 1]].tobytes())
+        paths.append(path)
+    return paths
+
 def _read_gt(binding, dataset, path, sequence_id):
     if not os.path.exists(path):
         return None

@@ -17,11 +17,15 @@
 #include <array>
 #include <cmath>
 #include <cstdint>
+#include <cstddef>
 #include <cstring>
+#include <fstream>
+#include <iterator>
 #include <limits>
 #include <map>
 #include <memory>
 #include <optional>
+#include <ostream>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -1529,3 +1533,136 @@ inline std::vector<slam::Pose> LoadGroundTruth(int dataset, const std::string &t
 }
 
 }  // namespace ct_icp
+
+// ---- PLY files over cticp_ply_write, cticp_ply_read_poses -----------------------------------------------------------
+// slam::WritePLY / SavePosesAsPLY / ReadPosesFromPLY (src/SlamCore/io.cxx). The file layout, conversions and deviations:
+// include/cticp.h, "PLY files". The bytes are encoded on `device`.
+namespace slam {
+
+// one PLY property of a WPoint3D file: a scalar at `offset` in each 64-byte record
+struct PLYColumn {
+    std::string element, name;
+    int ply_dtype, src_dtype;
+    size_t offset;
+};
+struct PLYSchemaMapper {
+    std::vector<PLYColumn> columns;   // in file order
+};
+
+// WPoint3D::FloatSchemaMapper (io.cxx:842-855): vertex x y z timestamp from the raw point, all float
+inline PLYSchemaMapper WPoint3DFloatSchema() {
+    return {{{"vertex", "x", CTICP_DTYPE_FLOAT32, CTICP_DTYPE_FLOAT64, 0},
+             {"vertex", "y", CTICP_DTYPE_FLOAT32, CTICP_DTYPE_FLOAT64, 8},
+             {"vertex", "z", CTICP_DTYPE_FLOAT32, CTICP_DTYPE_FLOAT64, 16},
+             {"vertex", "timestamp", CTICP_DTYPE_FLOAT32, CTICP_DTYPE_FLOAT64, 24}}};
+}
+// WPoint3D::DoubleSchemaMapper: the same properties as double
+inline PLYSchemaMapper WPoint3DDoubleSchema() {
+    PLYSchemaMapper m = WPoint3DFloatSchema();
+    for (PLYColumn &c : m.columns) c.ply_dtype = CTICP_DTYPE_FLOAT64;
+    return m;
+}
+// PLYSchemaMapper::BuildDefaultFromSchema(WPoint3D::DefaultSchema()) (types.h:571-590): every property of every
+// element, <name> or <name>_<dim>, double except index_frame (uint); elements in the std::map order of
+// WriteCollectionToPLY, properties in insertion order
+inline PLYSchemaMapper WPoint3DDefaultSchema() {
+    struct Property {
+        const char *name;
+        int type;
+        size_t offset;
+        int dim;
+    };
+    const std::map<std::string, std::vector<Property>> schema = {
+        {"xyzt", {{"xyz", CTICP_DTYPE_FLOAT64, 0, 3}, {"t", CTICP_DTYPE_FLOAT64, 24, 1}}},
+        {"raw_point", {{"x", CTICP_DTYPE_FLOAT64, 0, 1}, {"y", CTICP_DTYPE_FLOAT64, 8, 1}, {"z", CTICP_DTYPE_FLOAT64, 16, 1}}},
+        {"world_point",
+         {{"x", CTICP_DTYPE_FLOAT64, 32, 1}, {"y", CTICP_DTYPE_FLOAT64, 40, 1}, {"z", CTICP_DTYPE_FLOAT64, 48, 1}}},
+        {"properties",
+         {{"raw_xyz", CTICP_DTYPE_FLOAT64, 0, 3}, {"t", CTICP_DTYPE_FLOAT64, 24, 1}, {"world_xyz", CTICP_DTYPE_FLOAT64, 32, 3},
+          {"index_frame", CTICP_DTYPE_UINT32, 56, 1}}}};
+    PLYSchemaMapper m;
+    for (const auto &element : schema)
+        for (const Property &p : element.second)
+            for (int d = 0; d < p.dim; ++d)
+                m.columns.push_back({element.first, p.dim == 1 ? p.name : std::string(p.name) + "_" + std::to_string(d),
+                                     p.type, p.type, p.offset + 8 * (size_t) d});
+    return m;
+}
+
+namespace detail {
+inline std::string EncodePLY(const std::vector<PLYColumn> &columns, const void *records, size_t stride, size_t n,
+                             int device) {
+    std::vector<cticp_ply_property> props;
+    for (const PLYColumn &c : columns)
+        props.push_back({c.element.c_str(), c.name.c_str(), c.ply_dtype, c.src_dtype,
+                         n ? static_cast<const char *>(records) + c.offset : nullptr, stride});
+    const int64_t size = cticp_ply_write(device, props.data(), props.size(), n, nullptr, 0);
+    if (size < 0) ct_icp::cticp_check((int) size);
+    std::string out((size_t) size, '\0');
+    const int64_t rc = cticp_ply_write(device, props.data(), props.size(), n, &out[0], out.size());
+    if (rc < 0) ct_icp::cticp_check((int) rc);
+    return out;
+}
+}  // namespace detail
+
+// slam::WritePLY(os, points, schema); the default is WritePLY(os, points)'s mapper
+inline void WritePLY(std::ostream &os, const std::vector<WPoint3D> &points,
+                     const PLYSchemaMapper &schema = WPoint3DDefaultSchema(), int device = 0) {
+    const std::string bytes = detail::EncodePLY(schema.columns, points.data(), sizeof(WPoint3D), points.size(), device);
+    os.write(bytes.data(), (std::streamsize) bytes.size());
+}
+inline void WritePLY(const std::string &path, const std::vector<WPoint3D> &points,
+                     const PLYSchemaMapper &schema = WPoint3DDefaultSchema(), int device = 0) {
+    std::ofstream os(path, std::ios::out | std::ios::binary);
+    WritePLY(os, points, schema, device);
+}
+
+// SavePosesAsPLY (io.cxx:320-351): element pose, qx qy qz qw x y z ref_t dest_t as double, ref_fid dest_fid as int
+inline void SavePosesAsPLY(std::ostream &os, const std::vector<Pose> &poses, int device = 0) {
+    std::vector<cticp_pose> raw(poses.size());
+    for (size_t i = 0; i < poses.size(); ++i) {
+        for (int k = 0; k < 4; ++k) raw[i].quat[k] = poses[i].pose.quat.c[k];
+        for (int k = 0; k < 3; ++k) raw[i].tr[k] = poses[i].pose.tr.v[k];
+        raw[i].ref_timestamp = poses[i].ref_timestamp;
+        raw[i].dest_timestamp = poses[i].dest_timestamp;
+        raw[i].ref_frame_id = poses[i].ref_frame_id;
+        raw[i].dest_frame_id = poses[i].dest_frame_id;
+    }
+    const char *names[] = {"qx", "qy", "qz", "qw", "x", "y", "z", "ref_t", "dest_t"};
+    std::vector<PLYColumn> columns;
+    for (size_t k = 0; k < 9; ++k) columns.push_back({"pose", names[k], CTICP_DTYPE_FLOAT64, CTICP_DTYPE_FLOAT64, 8 * k});
+    columns.push_back({"pose", "ref_fid", CTICP_DTYPE_INT32, CTICP_DTYPE_UINT32, offsetof(cticp_pose, ref_frame_id)});
+    columns.push_back({"pose", "dest_fid", CTICP_DTYPE_INT32, CTICP_DTYPE_UINT32, offsetof(cticp_pose, dest_frame_id)});
+    const std::string bytes = detail::EncodePLY(columns, raw.data(), sizeof(cticp_pose), raw.size(), device);
+    os.write(bytes.data(), (std::streamsize) bytes.size());
+}
+inline void SavePosesAsPLY(const std::string &path, const std::vector<Pose> &poses, int device = 0) {
+    std::ofstream os(path, std::ios::out | std::ios::binary);
+    SavePosesAsPLY(os, poses, device);
+}
+
+// ReadPosesFromPLY (io.cxx:359-410), on the host
+inline std::vector<Pose> ReadPosesFromPLY(std::istream &is) {
+    const std::string bytes((std::istreambuf_iterator<char>(is)), std::istreambuf_iterator<char>());
+    const int64_t n = cticp_ply_read_poses(bytes.data(), bytes.size(), nullptr, 0);
+    if (n < 0) ct_icp::cticp_check((int) n);
+    std::vector<cticp_pose> raw((size_t) n);
+    if (n) cticp_ply_read_poses(bytes.data(), bytes.size(), raw.data(), raw.size());
+    std::vector<Pose> out(raw.size());
+    for (size_t i = 0; i < raw.size(); ++i) {
+        for (int k = 0; k < 4; ++k) out[i].pose.quat.c[k] = raw[i].quat[k];
+        for (int k = 0; k < 3; ++k) out[i].pose.tr.v[k] = raw[i].tr[k];
+        out[i].ref_timestamp = raw[i].ref_timestamp;
+        out[i].dest_timestamp = raw[i].dest_timestamp;
+        out[i].ref_frame_id = raw[i].ref_frame_id;
+        out[i].dest_frame_id = raw[i].dest_frame_id;
+    }
+    return out;
+}
+inline std::vector<Pose> ReadPosesFromPLY(const std::string &path) {
+    std::ifstream is(path, std::ios::in | std::ios::binary);
+    if (!is) throw ct_icp::CticpFailure(CTICP_ERR_INVALID_ARGUMENT, "cannot open " + path);
+    return ReadPosesFromPLY(is);
+}
+
+}  // namespace slam

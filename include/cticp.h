@@ -1081,6 +1081,56 @@ enum { CTICP_DATASET_KITTI_RAW = 0, CTICP_DATASET_KITTI_CARLA = 1, CTICP_DATASET
        CTICP_DATASET_NCLT = 4, CTICP_DATASET_HILTI_2021 = 5, CTICP_DATASET_HILTI_2022 = 6 };
 int64_t cticp_ground_truth_parse(int dataset, int sequence_id, const char *text, size_t n, cticp_pose *out, size_t cap);
 
+/* ---- PLY files (slam::WritePLY / WriteCollectionToPLY, src/SlamCore/io.cxx:654-716, over tinyply 2.x) ------------------
+ * A file is described as a table of columns: each PLY property is one scalar per item, taken from a strided source and
+ * converted to the property's type. The layout is tinyply 2.x's binary writer:
+ *     ply\n format binary_little_endian 1.0\n
+ *     element <name> <count>\n property <type> <name>\n ...      (per element)
+ *     end_header\n
+ * then per element `count` packed records, the properties one after the other, no padding. Type names are
+ * char uchar short ushort int uint float double. Elements come in order of first appearance in the table (tinyply's
+ * add_properties_to_element), properties in table order, and every element of a file has the file's item count (the
+ * reference's writer always gives every element kNumItems).
+ * Conversions are static_cast as g++ on x86-64 computes them: fp64 -> fp32 rounds to nearest even, integer -> integer is
+ * modular, integer -> float rounds to nearest, float -> integer truncates toward zero.
+ * Deviation: a float -> integer conversion out of the target's range saturates, and NaN gives 0 (undefined behaviour in
+ * the reference).
+ * CTICP_DTYPE_INT64 / CTICP_DTYPE_UINT64 are source types of cticp_ply_property only (64-bit indices such as a world
+ * cloud's source index); PLY has no 64-bit integers, and every other entry point refuses them. */
+enum { CTICP_DTYPE_INT64 = 9, CTICP_DTYPE_UINT64 = 10 };
+typedef struct cticp_ply_property {
+    const char *element;        /* PLY element name ("vertex", "pose", ...) */
+    const char *name;           /* PLY property name */
+    int32_t ply_dtype;          /* CTICP_DTYPE_INT8 .. CTICP_DTYPE_FLOAT64 */
+    int32_t src_dtype;          /* CTICP_DTYPE_INT8 .. CTICP_DTYPE_UINT64 */
+    const void *src;            /* item 0's scalar (any alignment) */
+    uint64_t src_stride_bytes;  /* bytes between items; 0 repeats one scalar */
+} cticp_ply_property;
+/* One file of num_items items from host sources into host bytes, encoded on `device` (synchronous). Returns the file's
+ * size and writes it to `out` only when capacity >= size (capacity 0: a size query; out may then be NULL). */
+int64_t cticp_ply_write(int device, const cticp_ply_property *props, size_t n_props, uint64_t num_items, void *out,
+                        uint64_t capacity);
+/* m files from device sources into device memory, back to back, enqueued on `stream` with no host synchronisation.
+ * File k holds items [file_ends[k-1], file_ends[k]) of every column (file_ends[-1] = 0); file_offsets[k] is where it
+ * starts in `out` and file_offsets[m] the total size. The first min(capacity, total) bytes are written; with capacity
+ * 0 only the offsets are (size once, allocate, encode). file_ends are read on the device: each end is clamped to
+ * [previous end, num_items], so a decreasing or oversized end gives a short or empty file and never a read past the
+ * sources (deviation: the host readers of frame ends refuse such ends). file_ends / file_offsets 8-byte aligned.
+ * Refusals of both variants (CTICP_ERR_INVALID_ARGUMENT, before anything is enqueued): null pointers (out may be NULL
+ * when capacity is 0, a source when num_items is 0), n_props 0 or above 32, unknown dtypes, an empty element or property
+ * name, one longer than 63 bytes or containing whitespace, the same property twice in an element; device pointers that
+ * are not memory of `device` or end past their allocation (a column spans (num_items - 1) stride + size bytes). */
+int cticp_ply_write_device(int device, const cticp_ply_property *props, size_t n_props, uint64_t num_items,
+                           const uint64_t *file_ends, size_t m, void *out, uint64_t capacity, uint64_t *file_offsets,
+                           void *stream);
+/* slam::ReadPosesFromPLY (io.cxx:359-410): the properties qx qy qz qw x y z ref_t dest_t ref_fid dest_fid of element
+ * "pose", found by name in any order (other elements and properties are skipped). Returns the count and copies
+ * min(count, cap) poses. Host only. The nine doubles must be FLOAT64 (the reference's CHECK); deviation: the fids must
+ * be int or uint (the reference reinterprets whatever is there as pair<int, int>). CTICP_ERR_UNSUPPORTED: ascii or
+ * binary_big_endian, list properties. CTICP_ERR_INVALID_ARGUMENT: a malformed header, a missing property, other
+ * types, a body shorter than the header says. */
+int64_t cticp_ply_read_poses(const void *bytes, size_t n, cticp_pose *out, size_t cap);
+
 /* ---- Map (L2 boundary; used directly by the parity tests) ---------------------------------------------- */
 
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */

@@ -3,9 +3,11 @@
 frame is read and filtered on the GPU (ct_icp_b200.datasets), registered with Odometry.register_device, and its end pose
 written in KITTI format as SavePosesKITTIFormat writes it (io.cxx:282-304). With ground truth, the estimate is scored
 with ComputeTrajectoryMetrics (cticp_trajectory_metrics) against the ground truth at the frames' end timestamps and the
-scores printed as one JSON line.
+scores printed as one JSON line. --out-ply writes the runner's <sequence>.PLY as SaveTrajectoryAndMetrics does
+(odometry_runner.cpp:318-340, save_mid_frame false): the first frame's begin pose, then every frame's end pose, through
+SavePosesAsPLY.
 usage: python tools/run_sequence.py --dataset NCLT --root DIR --sequence 2012-01-08 --out poses.txt
-       [--max-frames N] [--init-frame K] [--device 0]"""
+       [--out-ply poses.PLY] [--max-frames N] [--init-frame K] [--device 0]"""
 import argparse
 import json
 import os
@@ -34,8 +36,9 @@ def kitti_lines(poses):
     return out
 
 
-def run(binding, sequence, options, device=0):
-    """register every frame of `sequence`; returns the end poses, the frames' end timestamps and the summaries"""
+def run(binding, sequence, options, device=0, begin_poses=None):
+    """register every frame of `sequence`; returns the end poses, the frames' end timestamps and whether every frame
+    registered; each frame's begin pose is appended to `begin_poses` when given"""
     import torch
     od = binding.odometry(options, device=device)
     stream = torch.cuda.current_stream(device).cuda_stream
@@ -44,6 +47,8 @@ def run(binding, sequence, options, device=0):
         frame = sequence.NextFrame()
         sm = od.register_device(datasets.device_scan(frame), frame["frame_id"], stream=stream)
         ok = ok and bool(sm.success)
+        if begin_poses is not None:
+            begin_poses.append(sm.frame.begin_pose)
         poses.append(sm.frame.end_pose)
         stamps.append(float(frame["t"].max().item()) if frame["t"].numel() else float("nan"))
     return poses, np.array(stamps), ok
@@ -83,6 +88,7 @@ def main():
     ap.add_argument("--root", required=True)
     ap.add_argument("--sequence", required=True)
     ap.add_argument("--out", required=True)
+    ap.add_argument("--out-ply", default=None)
     ap.add_argument("--max-frames", type=int, default=-1)
     ap.add_argument("--init-frame", type=int, default=0)
     ap.add_argument("--device", type=int, default=0)
@@ -95,10 +101,15 @@ def main():
     seq.SetInitFrame(args.init_frame)
     seq.SetMaxNumFrames(args.max_frames)
     o = b.default_odometry_options()
-    poses, stamps, ok = run(b, seq, o, args.device)
+    begins = []
+    poses, stamps, ok = run(b, seq, o, args.device, begins)
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, "w") as f:
         f.write("\n".join(kitti_lines(poses)) + "\n")
+    if args.out_ply:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out_ply)), exist_ok=True)
+        with open(args.out_ply, "wb") as f:
+            f.write(b.save_poses_ply(begins[:1] + poses, device=args.device))
     print(json.dumps({"frames": len(poses), "success": ok, "scores": score(b, seq, poses, stamps, args.device)}))
 
 
