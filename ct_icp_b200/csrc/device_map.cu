@@ -60,12 +60,11 @@ __device__ __forceinline__ void insert_claim_dev(const MapLevel &L, MapCounters 
     const double inv_res = 1.0 / L.res;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const double px = world[3 * i], py = world[3 * i + 1], pz = world[3 * i + 2];
-        if (!(isfinite(px) && isfinite(py) && isfinite(pz))) {
+        unsigned long long key;
+        if (!voxel_key(px, py, pz, L.res, inv_res, key)) {   // non-finite, or a voxel the key cannot hold: skipped
             next[i] = kNil;
             continue;
         }
-        const unsigned long long key =
-            pack_voxel(voxel_coord_rcp(px, L.res, inv_res), voxel_coord_rcp(py, L.res, inv_res), voxel_coord_rcp(pz, L.res, inv_res));
         uint32_t h = hash_key(key) & L.cap_mask;
         int slot = -1;
         for (uint32_t probe = 0; probe <= L.cap_mask; ++probe) {

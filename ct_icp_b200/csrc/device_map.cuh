@@ -61,7 +61,8 @@ CT_HD uint32_t hash_key(unsigned long long k) {
     k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
     return (uint32_t) k;
 }
-// slam::Voxel::Coordinates (src/SlamCore/types.cxx:13-20): C int() truncation toward zero
+// slam::Voxel::Coordinates (src/SlamCore/types.cxx:13-20): C int() truncation toward zero (on the device a quotient beyond
+// the int range saturates, so such a query fails stencil_in_range)
 CT_HD int voxel_coord(double p, double res) { return int(p / res); }
 // the same integer from p * (1 / res): the product is within 2 ulp of the quotient, so the truncation can only differ when
 // the quotient is within ~1e-15 relative of an integer — those (and only those) take the division. Three fp64 divisions
@@ -77,6 +78,40 @@ CT_HD int voxel_coord_rcp(double p, double res, double inv_res) {
 #endif
     const double guard = 1e-12 * (1.0 + fabs(q));
     return (f < guard || f > 1.0 - guard) ? int(p / res) : k;
+}
+
+// A key holds 21 bits per axis: voxel coordinates in [-2^20, 2^20). slam::Voxel is an int, so the map skips what it cannot
+// key instead of letting a coordinate wrap onto a voxel on the far side of the range (or onto kEmptyKey).
+constexpr double kVoxelCoordLimit = 2097152.0;   // 2^21: a quotient |p / res| beyond it is out of range (and voxel_coord_rcp
+                                                 // converts only |p / res| < 2^31)
+CT_HD bool voxel_in_range(int v) { return v >= -kVoxelBias && v < kVoxelBias; }
+// the key of a point's voxel; false: a non-finite coordinate, or a voxel coordinate outside [-2^20, 2^20)
+CT_HD bool voxel_key(double x, double y, double z, double res, double inv_res, unsigned long long &key) {
+    if (!(fabs(x * inv_res) < kVoxelCoordLimit) || !(fabs(y * inv_res) < kVoxelCoordLimit) ||
+        !(fabs(z * inv_res) < kVoxelCoordLimit))
+        return false;
+    const int vx = voxel_coord_rcp(x, res, inv_res), vy = voxel_coord_rcp(y, res, inv_res), vz = voxel_coord_rcp(z, res, inv_res);
+    if (!voxel_in_range(vx) || !voxel_in_range(vy) || !voxel_in_range(vz)) return false;
+    key = pack_voxel(vx, vy, vz);
+    return true;
+}
+// a query's voxel coordinate: voxel_coord_rcp, or +-2^21 (outside the range) when |p / res| >= 2^21
+CT_HD int query_voxel_coord(double p, double res, double inv_res) {
+    const double q = p * inv_res;
+    if (fabs(q) >= kVoxelCoordLimit) return q < 0.0 ? -2 * kVoxelBias : 2 * kVoxelBias;
+    return voxel_coord_rcp(p, res, inv_res);
+}
+// whether the (2r+1)^3 stencil around voxel (kx, ky, kz) lies inside [-2^20, 2^20) on every axis. Checked once per query:
+// a query whose stencil leaves the range finds no neighbours, since its out-of-range keys would alias stored voxels.
+CT_HD bool stencil_in_range(int kx, int ky, int kz, int r) {
+    const int lo = -kVoxelBias + r, hi = kVoxelBias - 1 - r;
+    return kx >= lo && kx <= hi && ky >= lo && ky <= hi && kz >= lo && kz <= hi;
+}
+// the x coordinate a query whose stencil leaves the range is given (r < 2^20): every stencil key then has x + 2^20 in
+// [2^21, 2^22), so bit 63 set, which no stored key has; such a query finds nothing with the gather left as it is
+constexpr int kVoxelNowhere = 2 * kVoxelBias;
+CT_HD void confine_query(int &kx, int ky, int kz, int r) {
+    if (!stencil_in_range(kx, ky, kz, r)) kx = kVoxelNowhere;
 }
 
 #ifdef __CUDACC__

@@ -165,9 +165,9 @@ __device__ __forceinline__ int warp_gather_knn(const GatherConfig &G, const int 
                                                V3 to_sensor = V3{0, 0, 0}) {
     const MapLevel &L = G.L;
     const int side = 2 * G.r + 1;
-    const int nst = side * side * side;
     const V3 &q = ctx.q;
     const int kx = ctx.kx, ky = ctx.ky, kz = ctx.kz;
+    const int nst = stencil_in_range(kx, ky, kz, G.r) ? side * side * side : 0;
     best.d2 = kKnnInf;
     best.seq = 0x7fffffff;
     best.addr = 0;

@@ -127,9 +127,10 @@ __device__ __forceinline__ void gn_phase_a(const GatherConfig &G, const RawPoint
     const V3 raw{kraw.x, kraw.y, kraw.z};
     p = rigid ? qrot(qnormalized(pose.qe), raw) + pose.te
               : ct_transform_c(pose.qb, pose.tb, pose.qe, pose.te, kraw.alpha, raw, pose.sc);
-    kx = voxel_coord_rcp(p.x, G.L.res, inv_res);
-    ky = voxel_coord_rcp(p.y, G.L.res, inv_res);
-    kz = voxel_coord_rcp(p.z, G.L.res, inv_res);
+    kx = query_voxel_coord(p.x, G.L.res, inv_res);
+    ky = query_voxel_coord(p.y, G.L.res, inv_res);
+    kz = query_voxel_coord(p.z, G.L.res, inv_res);
+    confine_query(kx, ky, kz, G.r);
 }
 
 // ---- C (ct_icp.cpp:769-850): a keypoint's moments `o` (world position p) → covariance, closed-form eigen, normal, a2D,

@@ -189,6 +189,7 @@ __device__ __noinline__ void lm_gather_tiles(const GatherConfig &G0, const LmPar
             kx = voxel_coord(p.x, res);
             ky = voxel_coord(p.y, res);
             kz = voxel_coord(p.z, res);
+            confine_query(kx, ky, kz, rr);
         }
         // ---- all lanes: gather + selection, keypoint by keypoint
         for (int j = 0; j < wt; ++j) {
@@ -323,9 +324,10 @@ __device__ __noinline__ void rb_gather_tiles(const GatherConfig &G, const LmPara
         if (lane < wt) {
             const RawPoint kraw = load_raw(keypoints, P.kp_lo, t0 + lane);
             p = ct_transform_c(qb, tb, qe, te, kraw.alpha, V3{kraw.x, kraw.y, kraw.z}, sc);   // TransformKeyPoints, :1373-1393
-            kx = voxel_coord_rcp(p.x, G.L.res, inv_res);
-            ky = voxel_coord_rcp(p.y, G.L.res, inv_res);
-            kz = voxel_coord_rcp(p.z, G.L.res, inv_res);
+            kx = query_voxel_coord(p.x, G.L.res, inv_res);
+            ky = query_voxel_coord(p.y, G.L.res, inv_res);
+            kz = query_voxel_coord(p.z, G.L.res, inv_res);
+            confine_query(kx, ky, kz, G.r);
         }
         for (int j = 0; j < wt; ++j) {
             const V3 q{__shfl_sync(0xffffffffu, p.x, j), __shfl_sync(0xffffffffu, p.y, j), __shfl_sync(0xffffffffu, p.z, j)};

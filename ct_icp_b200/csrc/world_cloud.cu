@@ -41,7 +41,6 @@ constexpr int kScanTile = kThreads * kScanItems;
 constexpr uint32_t kRejected = 0xFFFFFFFFu;
 constexpr uint32_t kLocal = 0x80000000u;                // pv: a voxel of the call-local table (slot in the low bits)
 constexpr uint64_t kMaxCallPoints = 1ull << 30;
-constexpr double kCoordLimit = 2097152.0;               // 2^21: |p / grid_size| beyond it has a voxel coordinate outside
 
 int Blocks(uint64_t n) { return (int) std::max<uint64_t>(1, std::min<uint64_t>((n + kThreads - 1) / kThreads, 132 * 16)); }
 
@@ -49,16 +48,6 @@ uint64_t Pow2AtLeast(uint64_t n) {
     uint64_t p = 1;
     while (p < n) p <<= 1;
     return p;
-}
-
-// slam::Voxel::Coordinates of one point; false: non-finite, or a coordinate outside [-2^20, 2^20)
-__device__ __forceinline__ bool voxel_key(double x, double y, double z, double res, double inv, unsigned long long &key) {
-    if (!(fabs(x * inv) < kCoordLimit) || !(fabs(y * inv) < kCoordLimit) || !(fabs(z * inv) < kCoordLimit)) return false;
-    const int vx = voxel_coord_rcp(x, res, inv), vy = voxel_coord_rcp(y, res, inv), vz = voxel_coord_rcp(z, res, inv);
-    if (vx < -kVoxelBias || vx >= kVoxelBias || vy < -kVoxelBias || vy >= kVoxelBias || vz < -kVoxelBias || vz >= kVoxelBias)
-        return false;
-    key = pack_voxel(vx, vy, vz);
-    return true;
 }
 
 struct KeyArgs {

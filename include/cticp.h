@@ -1136,7 +1136,10 @@ int64_t cticp_ply_read_poses(const void *bytes, size_t n, cticp_pose *out, size_
 /* MultipleResolutionVoxelMap(const Options&), include/ct_icp/map.h:136-138 */
 int cticp_map_create(const cticp_map_options *options, int device, cticp_map **out);
 void cticp_map_destroy(cticp_map *m);
-/* InsertPointCloud (world points, given order), include/ct_icp/map.h:153-254,261-293 */
+/* InsertPointCloud (world points, given order), include/ct_icp/map.h:153-254,261-293. Deviation: voxel coordinates are
+ * kept in 21 bits per axis, so a point that is non-finite or whose voxel coordinate lies outside [-2^20, 2^20) on any axis
+ * is skipped (not stored, not counted), where the reference's int voxel would keep it; a search whose stencil reaches
+ * outside that range finds no neighbours. The same holds for the odometry's map update. */
 int cticp_map_insert(cticp_map *m, const double *xyz, size_t stride_bytes, size_t n);
 /* InsertPointCloud(pointcloud, frame_poses, ...) where the begin pose of the source frame matters: per-voxel normals
  * are oriented towards `origin` = frame_poses.front().tr (include/ct_icp/map.h:211-235). cticp_map_insert is the same
