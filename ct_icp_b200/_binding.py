@@ -480,7 +480,7 @@ class Binding:
         return out
 
     # ---- many handles, one frame each ------------------------------------------------------------------------
-    def register_batch(self, odometries, scans, frame_ids, initial_estimates=None, motion_models=None):
+    def register_batch(self, odometries, scans, frame_ids, initial_estimates=None, motion_models=None, statuses=None):
         """One frame on each Odometry of `odometries` in one call (cticp_odometry_register_batch): the eligible
         Gauss-Newton loops run in one grouped launch, the eligible CERES / ROBUST loops in one grouped launch per LM mode
         (CERES nearest neighbour, CERES distance-based, ROBUST); the attempts of robust_registration frames run in rounds
@@ -488,7 +488,10 @@ class Binding:
         scans[i]: (xyz, timestamps) NumPy arrays (RegisterFrame's host path), (xyz, timestamps) torch CUDA tensors (read
         after the work queued on torch's current stream, as RegisterFrame), or an int staged slot (RegisterStaged).
         initial_estimates / motion_models: None or one entry (abi.Frame / abi.MotionPrior or None) per item.
-        Returns the summaries; raises CticpError after the call when an item fails (.statuses: every item's status)."""
+        Returns the summaries; raises CticpError after the call when an item fails (.statuses: every item's status).
+        statuses: a list that receives every item's status instead of the raise, so the items that registered keep their
+        summaries (a failed item's summary is left zero; cticp_last_error() holds the first failing item's message). A
+        call refused before any item ran still raises."""
         B = len(odometries)
         for name, lst in (("scans", scans), ("frame_ids", frame_ids), ("initial_estimates", initial_estimates),
                           ("motion_models", motion_models)):
@@ -530,9 +533,12 @@ class Binding:
                 it.motion_model = C.addressof(motion_models[i])
             it.out = C.addressof(outs[i])
         rc = self.fn("odometry_register_batch")(items, B)
-        if rc < 0:
+        item_status = [items[i].status for i in range(B)]
+        if rc < 0 and (statuses is None or not any(item_status)):
             msg = self.fn("last_error")()
-            raise CticpError(rc, msg.decode("utf-8", "replace") if msg else "", [items[i].status for i in range(B)])
+            raise CticpError(rc, msg.decode("utf-8", "replace") if msg else "", item_status)
+        if statuses is not None:
+            statuses[:] = item_status
         return outs
 
     # ---- sampling ------------------------------------------------------------------------------------------

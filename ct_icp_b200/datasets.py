@@ -4,7 +4,8 @@ LoadDataset, LoadPoses), with every frame decoded and filtered on the device.
 A frame is a dict: "xyz" (N, 3) and "t" (N,) torch CUDA tensors (a cticp_device_scan for Odometry.register_device
 through `device_scan(frame)`), "frame_id", and "begin_pose" / "end_pose" (abi.Pose, or None without ground truth)
 interpolated on the ground truth at the frame's first and largest timestamps (NCLT) or its minimum and maximum (PLY).
-Options arrive as keyword arguments; no YAML is read.
+Options arrive as keyword arguments (load_dataset) or as a config.DatasetOptions read from a reference configuration
+(load_dataset_from_options, which also builds SYNTHETIC sequences from scene YAML files).
 """
 import os
 
@@ -85,6 +86,10 @@ class _Sequence:
     def GroundTruth(self):
         return self.gt
 
+    def close(self):
+        """releases the device memory the reader holds between frames (a later NextFrame reopens it)"""
+        self._traj = None
+
     def _poses(self, t_begin, t_end):
         if self.gt is None or len(self.gt) == 0:
             return None, None
@@ -137,6 +142,12 @@ class NCLTSequence(_Sequence):
 
     def _count(self):
         return sum(c[3] for c in self.chunks)
+
+    def close(self):
+        if self._open is not None:
+            self._open[1].close()
+            self._open = None
+        super().close()
 
     def _read(self, k):
         for (pos, used, first, nf, final) in self.chunks:
@@ -255,3 +266,73 @@ def load_dataset(binding, dataset, root, sequences=None, device=0, **options):
         out.append((name, PLYDirectory(binding, frames, sizes[dataset][i], digits,
                                        dataset in ("KITTI", "KITTI_raw", "KITTI_360"), gt, device)))
     return out
+
+
+class SyntheticSequence(_Sequence):
+    """SyntheticSequence (dataset.cpp:693-790) of a scene, the dict config.yaml_to_synthetic_scene reads: frame k spans
+    ground-truth poses k and k + 1, sampled at sample_frequency along the scene's trajectory, and its points are
+    generated on the device (Binding.synthetic_sequence, with `seed`) when the first frame is read. The ground truth
+    is the sampled poses relative to the first. As the reference's HasNext, max_num_frames does not shorten it."""
+
+    def __init__(self, binding, spec, seed=0, device=0):
+        super().__init__(binding, None, device)
+        self.spec, self.seed = spec, seed
+        self._data = None
+        self.gt = binding.synthetic_sequence(spec, seed=seed, num_frames=0, device_index=device)["ground_truth"]
+
+    def _count(self):
+        return max(len(self.gt) - 1, 0)
+
+    def NumFrames(self):
+        return len(self.gt)        # seq_info.sequence_size: the number of ground-truth poses
+
+    def HasNext(self):
+        return self.current < self._count()
+
+    def _read(self, k):
+        if self._data is None:
+            d = self.b.synthetic_sequence(self.spec, seed=self.seed, device=True, device_index=self.device)
+            self._data = (d["xyz"], d["t"], [0] + d["frame_ends"].tolist())
+        xyz, t, ends = self._data
+        begin, end = pose_list(self.gt[k:k + 2])
+        return {"xyz": xyz[ends[k]:ends[k + 1]], "t": t[ends[k]:ends[k + 1]], "begin_pose": begin, "end_pose": end}
+
+    def close(self):
+        self._data = None
+        super().close()
+
+
+def load_dataset_from_options(binding, options, device=0):
+    """Dataset::LoadDataset (dataset.cpp:1214-1260) of a config.DatasetOptions: the dataset's sequences found under
+    root_path, each labelled <DATASET>_<name> (e.g. KITTI_raw_00, NCLT_2012-01-08, SYNTHETIC_courtyard). With
+    use_all_datasets false only the sequences of sequence_options are kept, each with its start_frame_id and
+    max_num_frames, and a named sequence that is not found is an error. SYNTHETIC: every <root_path>/*.yaml is one
+    sequence, named by the file's stem. Sequences come in name order (the reference's order is the directory
+    iterator's). Returns a list of (label, sequence)."""
+    from . import config
+    if options.dataset is None or options.dataset == "PLY_DIRECTORY":
+        raise config.ConfigError("The dataset %s cannot be defined from the config" % (options.dataset,))
+    if not os.path.exists(options.root_path):
+        raise config.ConfigError("The path to the root directory does not exist: %s" % options.root_path)
+    wanted = None if options.use_all_datasets else {s.sequence_name: s for s in options.sequence_options}
+    if options.dataset == "SYNTHETIC":
+        found = []
+        for fname in sorted(os.listdir(options.root_path)):
+            path = os.path.join(options.root_path, fname)
+            stem, ext = os.path.splitext(fname)
+            if not os.path.isfile(path) or ext != ".yaml" or (wanted is not None and stem not in wanted):
+                continue
+            spec = config.yaml_to_synthetic_scene(config.load_config(path))
+            found.append((stem, SyntheticSequence(binding, spec, device=device)))
+    else:
+        kw = {"num_aggregated": options.nclt_num_aggregated_pc} if options.dataset == "NCLT" else {}
+        found = load_dataset(binding, options.dataset, options.root_path,
+                             None if wanted is None else list(wanted), device=device, **kw)
+        found.sort(key=lambda x: x[0])
+    if wanted is not None:
+        if len(found) != len(wanted):
+            raise config.ConfigError("Could not find all the sequences in `sequence_options`")
+        for name, seq in found:
+            seq.SetInitFrame(wanted[name].start_frame_id)
+            seq.SetMaxNumFrames(wanted[name].max_num_frames)
+    return [(options.dataset + "_" + name, seq) for name, seq in found]

@@ -1666,3 +1666,326 @@ inline std::vector<Pose> ReadPosesFromPLY(const std::string &path) {
 }
 
 }  // namespace slam
+
+// ---- The reference's YAML readers (src/ct_icp/config.cpp, src/ct_icp/map.cpp:10-77, neighborhood_strategy.h:51-114) ---
+// Templates over a node type with yaml-cpp's interface: `node[key]` (a node that converts to false when the key is
+// absent), IsMap(), IsSequence(), `as<T>()` and range-for iteration. With YAML::Node they are the reference's own
+// signatures, and the facade gains no dependency on yaml-cpp. Scalars convert through the node's `as<T>`; keys the
+// option structs do not carry (output_*, log_to_file, the old map keys, ...) are converted and dropped. The Python
+// readers (ct_icp_b200/config.py) are the same clauses; DESIGN.md §5.13 lists the quirks kept.
+namespace ct_icp {
+
+// ct_icp::SequenceOptions / DatasetOptions (include/ct_icp/dataset.h:270-293); `dataset` is DATASETEnumToString's
+// name ("KITTI_raw", "NCLT", "SYNTHETIC", ...), empty when the node names none
+struct SequenceOptions {
+    std::string sequence_name;
+    int start_frame_id = 0;
+    int max_num_frames = -1;
+};
+struct DatasetOptions {
+    std::string dataset;
+    std::string root_path;
+    bool fail_if_incomplete = false;
+    double min_dist_lidar_center = 3.0;
+    double max_dist_lidar_center = 100.0;
+    int nclt_num_aggregated_pc = 220;
+    bool use_all_datasets = true;
+    std::vector<SequenceOptions> sequence_options;
+};
+
+namespace detail {
+template <class T, class Node, class F>
+inline void yaml_clause(const Node &node, const char *key, F &field) {   // OPTION_CLAUSE / FIND_OPTION
+    if (node[key]) field = (F) node[key].template as<T>();
+}
+template <class Node>
+inline void yaml_flag(const Node &node, const char *key, int32_t &field) {   // a bool clause into an int32 field
+    if (node[key]) field = node[key].template as<bool>() ? 1 : 0;
+}
+template <class T, class Node>
+inline void yaml_dropped(const Node &node, const char *key) {   // a clause into a field the structs do not carry
+    if (node[key]) (void) node[key].template as<T>();
+}
+template <class Node>
+inline bool yaml_enum(const Node &node, const char *key, std::string &out) {
+    if (!node[key]) return false;
+    out = node[key].template as<std::string>();
+    return true;
+}
+inline int trunc_int(double x, const char *key) {   // the reference's double → int assignment (out of range refused)
+    if (!(x > -2147483648.0 && x < 2147483648.0))
+        throw std::runtime_error(std::string("`") + key + "` does not fit an int");
+    return (int) x;
+}
+inline void check_enum(bool ok, const std::string &key, std::initializer_list<const char *> names, const std::string &got) {
+    if (ok) return;
+    std::string msg = "Check failed: ";
+    bool first = true;
+    for (const char *n : names) {
+        msg += (first ? "" : " || ") + key + " == \"" + n + "\"";
+        first = false;
+    }
+    throw std::runtime_error(msg + " (got " + got + ")");
+}
+}  // namespace detail
+
+template <class Node>
+CTICPOptions yaml_to_ct_icp_options(const Node &icp_node) {   // config.cpp:26-122
+    using namespace detail;
+    CTICPOptions o;
+    yaml_clause<int>(icp_node, "threshold_voxel_occupancy", o.threshold_voxel_occupancy);
+    yaml_clause<int>(icp_node, "num_iters_icp", o.num_iters_icp);
+    yaml_clause<int>(icp_node, "min_number_neighbors", o.min_number_neighbors);
+    yaml_clause<int>(icp_node, "max_number_neighbors", o.max_number_neighbors);
+    yaml_clause<double>(icp_node, "max_dist_to_plane_ct_icp", o.max_dist_to_plane_ct_icp);
+    yaml_clause<double>(icp_node, "threshold_orientation_norm", o.threshold_orientation_norm);
+    yaml_clause<double>(icp_node, "threshold_translation_norm", o.threshold_translation_norm);
+    yaml_flag(icp_node, "debug_print", o.debug_print);
+    yaml_flag(icp_node, "point_to_plane_with_distortion", o.point_to_plane_with_distortion);
+    yaml_clause<int>(icp_node, "num_closest_neighbors", o.num_closest_neighbors);
+    yaml_clause<int>(icp_node, "ls_max_num_iters", o.ls_max_num_iters);
+    yaml_clause<int>(icp_node, "ls_num_threads", o.ls_num_threads);
+    yaml_clause<double>(icp_node, "ls_sigma", o.ls_sigma);
+    yaml_clause<int>(icp_node, "min_num_residuals", o.min_num_residuals);
+    yaml_clause<int>(icp_node, "max_num_residuals", o.max_num_residuals);
+    yaml_clause<double>(icp_node, "weight_alpha", o.weight_alpha);
+    yaml_clause<double>(icp_node, "weight_neighborhood", o.weight_neighborhood);
+    yaml_clause<double>(icp_node, "ls_tolerant_min_threshold", o.ls_tolerant_min_threshold);
+    yaml_clause<double>(icp_node, "power_planarity", o.power_planarity);
+    yaml_flag(icp_node, "point_to_plane_with_distortion", o.point_to_plane_with_distortion);
+    for (const char *k : {"output_normals", "output_lines", "output_weights", "output_residuals",
+                          "output_neighborhood_info"})
+        yaml_dropped<bool>(icp_node, k);
+    yaml_clause<double>(icp_node, "threshold_linearity", o.threshold_linearity);
+    yaml_clause<double>(icp_node, "threshold_planarity", o.threshold_planarity);
+    yaml_clause<double>(icp_node, "weight_point_to_point", o.weight_point_to_point);
+    yaml_clause<double>(icp_node, "outlier_distance", o.outlier_distance);
+    yaml_flag(icp_node, "use_barycenter", o.use_barycenter);
+    std::string s;
+    if (yaml_enum(icp_node, "distance", s)) {
+        if (s == "POINT_TO_PLANE") o.distance = CTICP_DIST_POINT_TO_PLANE;
+        else if (s == "POINT_TO_LINE") o.distance = CTICP_DIST_POINT_TO_LINE;
+        else if (s == "POINT_TO_POINT") o.distance = CTICP_DIST_POINT_TO_POINT;
+        else if (s == "POINT_TO_DISTRIBUTION") o.distance = CTICP_DIST_POINT_TO_DISTRIBUTION;
+        else throw std::runtime_error("Distance " + s + " not recognized as a valid distance");
+    }
+    if (yaml_enum(icp_node, "parametrization", s)) {
+        if (s == "SIMPLE") o.parametrization = CTICP_PARAM_SIMPLE;
+        else if (s == "CONTINUOUS_TIME") o.parametrization = CTICP_PARAM_CONTINUOUS_TIME;
+        else throw std::runtime_error("Parametrization is not supported !");
+    }
+    if (yaml_enum(icp_node, "solver", s)) {
+        if (s == "GN") o.solver = CTICP_SOLVER_GN;
+        else if (s == "CERES") o.solver = CTICP_SOLVER_CERES;
+        else if (s == "ROBUST") o.solver = CTICP_SOLVER_ROBUST;
+        else throw std::runtime_error("Invalid Solver Options found: " + s + " Not in [GN, CERES, ROBUST]");
+    }
+    if (yaml_enum(icp_node, "loss_function", s)) {
+        const char *names[] = {"STANDARD", "CAUCHY", "HUBER", "TOLERANT", "TRUNCATED"};
+        int found = -1;
+        for (int i = 0; i < 5; ++i)
+            if (s == names[i]) found = i;
+        if (found < 0) throw std::runtime_error("Unrecognised loss function " + s);
+        o.loss_function = found;
+    }
+    return o;
+}
+
+template <class Node>
+cticp_motion_model_options yaml_to_motion_model_options(const Node &node) {   // config.cpp:304-318
+    using namespace detail;
+    cticp_motion_model_options o = OdometryOptions().default_motion_model;
+    yaml_clause<double>(node, "beta_location_consistency", o.beta_location_consistency);
+    yaml_clause<double>(node, "beta_small_velocity", o.beta_small_velocity);
+    yaml_clause<double>(node, "beta_orientation_consistency", o.beta_orientation_consistency);
+    yaml_clause<double>(node, "beta_constant_velocity", o.beta_constant_velocity);
+    yaml_clause<double>(node, "threshold_orientation_deg", o.threshold_orientation_deg);
+    yaml_clause<double>(node, "threshold_translation_diff", o.threshold_translation_diff);
+    yaml_flag(node, "log_if_invalid", o.log_if_invalid);
+    std::string s;
+    if (yaml_enum(node, "model", s)) {
+        if (s == "CONSTANT_VELOCITY") o.model = CTICP_MM_CONSTANT_VELOCITY;
+        else if (s == "SMALL_VELOCITY") o.model = CTICP_MM_SMALL_VELOCITY;
+        else throw std::runtime_error("[ERROR] The option " + s +
+                                      " is not a valid option. Valid options are: {CONSTANT_VELOCITY, SMALL_VELOCITY}");
+    }
+    return o;
+}
+
+// yaml_to_map_options (map.cpp:68-77): MULTI_RESOLUTION_VOXEL_HASHMAP, the old options without a map_type. The
+// resolutions are sorted stably; the slots past the last one are zero; more than CTICP_MAX_RESOLUTIONS is refused.
+template <class Node>
+cticp_map_options yaml_to_map_options(const Node &node) {
+    using namespace detail;
+    cticp_map_options o;
+    cticp_default_map_options(&o);
+    if (!node["map_type"]) {   // old_map_options_from_yaml: one resolution (the default's first), one frame kept
+        double size = o.resolutions[0].resolution, dmin = o.resolutions[0].min_distance_between_points;
+        int npts = o.resolutions[0].max_num_points;
+        yaml_clause<double>(node, "size_voxel_map", size);
+        if (node["max_num_points_in_voxel"])
+            npts = trunc_int(node["max_num_points_in_voxel"].template as<double>(), "max_num_points_in_voxel");
+        yaml_clause<double>(node, "min_distance_points", dmin);
+        cticp_legacy_map_options(&o, size, npts, dmin);
+        return o;
+    }
+    if (node["map_type"].template as<std::string>() != "MULTI_RESOLUTION_VOXEL_HASHMAP")
+        throw std::runtime_error("Not implemented error");
+    if (node["resolutions"]) {
+        const auto res = node["resolutions"];
+        if (!res.IsSequence()) throw std::runtime_error("The node 'resolutions' in the yaml is not a sequence");
+        std::vector<cticp_resolution_param> params;
+        for (const auto &child : res) {
+            if (!child.IsMap()) throw std::runtime_error("The following child node is not a Map");
+            cticp_resolution_param p{};
+            p.resolution = 0.5;   // ResolutionParam() (map.h:109-113)
+            p.min_distance_between_points = 0.1;
+            p.max_num_points = 40;
+            yaml_clause<double>(child, "min_distance_between_points", p.min_distance_between_points);
+            if (child["max_num_points"])
+                p.max_num_points = trunc_int(child["max_num_points"].template as<double>(), "max_num_points");
+            if (!child["resolution"]) throw std::runtime_error("Invalid Resolution Param in the yaml");
+            p.resolution = child["resolution"].template as<double>();
+            params.push_back(p);
+        }
+        if (params.empty()) throw std::runtime_error("The yaml does not define a valid set of resolutions for the map");
+        if (params.size() > CTICP_MAX_RESOLUTIONS)
+            throw std::runtime_error("the engine's map holds at most " + std::to_string(CTICP_MAX_RESOLUTIONS) +
+                                     " resolutions");
+        std::stable_sort(params.begin(), params.end(), [](const cticp_resolution_param &l,
+                                                          const cticp_resolution_param &r) {
+            return l.resolution < r.resolution;
+        });
+        o.num_resolutions = (int32_t) params.size();
+        for (int i = 0; i < CTICP_MAX_RESOLUTIONS; ++i) o.resolutions[i] = i < (int) params.size() ? params[i]
+                                                                                                  : cticp_resolution_param{};
+    }
+    yaml_clause<int>(node, "max_frames_to_keep", o.max_frames_to_keep);
+    yaml_clause<double>(node, "default_radius", o.default_radius);
+    return o;
+}
+
+// the neighborhood_strategy clause of yaml_to_odometry_options (config.cpp:155-168) and the strategies' FromYAML
+template <class Node>
+cticp_strategy_options yaml_to_strategy_options(const Node &node, const cticp_strategy_options &current) {
+    using namespace detail;
+    cticp_strategy_options o = current;
+    std::string type = o.type == CTICP_STRATEGY_DISTANCE_BASED ? "DISTANCE_BASED_STRATEGY" : "NEAREST_NEIGHBOR_STRATEGY";
+    yaml_enum(node, "type", type);
+    if (type == "DISTANCE_BASED_STRATEGY")   // a fresh DistanceBasedStrategy::Options
+        o = cticp_strategy_options{CTICP_STRATEGY_DISTANCE_BASED, 20, 8, 0, 60.0, 0.1, 2.0, 1.0};
+    yaml_clause<int>(node, "max_num_neighbors", o.max_num_neighbors);
+    yaml_clause<int>(node, "min_num_neighbors", o.min_num_neighbors);
+    if (o.type == CTICP_STRATEGY_DISTANCE_BASED) {
+        yaml_clause<double>(node, "distance_max", o.distance_max);
+        yaml_clause<double>(node, "radius_min", o.radius_min);
+        yaml_clause<double>(node, "radius_max", o.radius_max);
+        yaml_clause<double>(node, "exponent", o.exponent);
+    }
+    return o;
+}
+
+template <class Node>
+OdometryOptions yaml_to_odometry_options(const Node &odometry_node) {   // config.cpp:132-255
+    using namespace detail;
+    OdometryOptions o;
+    yaml_clause<double>(odometry_node, "voxel_size", o.voxel_size);
+    yaml_clause<double>(odometry_node, "max_distance", o.max_distance);
+    yaml_clause<double>(odometry_node, "distance_error_threshold", o.distance_error_threshold);
+    yaml_clause<double>(odometry_node, "orientation_error_threshold", o.orientation_error_threshold);
+    yaml_clause<int>(odometry_node, "max_num_keypoints", o.max_num_keypoints);
+    yaml_clause<double>(odometry_node, "sample_voxel_size", o.sample_voxel_size);
+    o.map_options = odometry_node["map_options"] ? yaml_to_map_options(odometry_node["map_options"])
+                                                 : yaml_to_map_options(odometry_node);
+    if (odometry_node["neighborhood_strategy"])
+        o.neighborhood_strategy = yaml_to_strategy_options(odometry_node["neighborhood_strategy"], o.neighborhood_strategy);
+    yaml_dropped<double>(odometry_node, "min_distance_points");
+    yaml_dropped<int>(odometry_node, "max_num_points_in_voxel");
+    yaml_dropped<double>(odometry_node, "size_voxel_map");
+    yaml_dropped<int>(odometry_node, "voxel_neighborhood");
+    yaml_dropped<double>(odometry_node, "max_radius_neighborhood");
+    yaml_clause<int>(odometry_node, "init_num_frames", o.init_num_frames);
+    yaml_clause<double>(odometry_node, "init_voxel_size", o.init_voxel_size);
+    yaml_clause<double>(odometry_node, "init_sample_voxel_size", o.init_sample_voxel_size);
+    yaml_dropped<bool>(odometry_node, "log_to_file");
+    yaml_dropped<std::string>(odometry_node, "log_file_destination");
+    yaml_flag(odometry_node, "debug_print", o.debug_print);
+    yaml_dropped<bool>(odometry_node, "debug_viz");
+    yaml_flag(odometry_node, "do_no_insert", o.do_no_insert);
+    yaml_flag(odometry_node, "always_insert", o.always_insert);
+    yaml_clause<int>(odometry_node, "robust_minimal_level", o.robust_minimal_level);
+    yaml_flag(odometry_node, "robust_registration", o.robust_registration);
+    yaml_clause<double>(odometry_node, "robust_full_voxel_threshold", o.robust_full_voxel_threshold);
+    yaml_flag(odometry_node, "robust_fail_early", o.robust_fail_early);
+    yaml_clause<int>(odometry_node, "robust_num_attempts", o.robust_num_attempts);
+    yaml_clause<int>(odometry_node, "robust_max_voxel_neighborhood", o.robust_max_voxel_neighborhood);
+    yaml_clause<double>(odometry_node, "robust_threshold_relative_orientation", o.robust_threshold_relative_orientation);
+    yaml_clause<double>(odometry_node, "robust_threshold_ego_orientation", o.robust_threshold_ego_orientation);
+    if (odometry_node["default_motion_model"])
+        o.default_motion_model = yaml_to_motion_model_options(odometry_node["default_motion_model"]);
+    std::string s;
+    if (yaml_enum(odometry_node, "motion_compensation", s)) {
+        const bool ok = s == "NONE" || s == "CONSTANT_VELOCITY" || s == "ITERATIVE" || s == "CONTINUOUS";
+        check_enum(ok, "motion_compensation", {"NONE", "CONSTANT_VELOCITY", "ITERATIVE", "CONTINUOUS"}, s);
+        o.motion_compensation = s == "NONE" ? CTICP_MC_NONE : s == "CONSTANT_VELOCITY" ? CTICP_MC_CONSTANT_VELOCITY
+                              : s == "ITERATIVE" ? CTICP_MC_ITERATIVE : CTICP_MC_CONTINUOUS;
+    }
+    if (yaml_enum(odometry_node, "sampling", s)) {
+        check_enum(s == "GRID" || s == "ADAPTIVE" || s == "NONE", "sampling", {"GRID", "ADAPTIVE", "NONE"}, s);
+        o.sampling = s == "NONE" ? CTICP_SAMPLING_NONE : s == "GRID" ? CTICP_SAMPLING_GRID : CTICP_SAMPLING_ADAPTIVE;
+    }
+    if (yaml_enum(odometry_node, "initialization", s)) {
+        check_enum(s == "INIT_NONE" || s == "INIT_CONSTANT_VELOCITY", "initialization",
+                   {"INIT_NONE", "INIT_CONSTANT_VELOCITY"}, s);
+        o.initialization = s == "INIT_NONE" ? CTICP_INIT_NONE : CTICP_INIT_CONSTANT_VELOCITY;
+    }
+    if (odometry_node["ct_icp_options"]) {
+        const CTICPOptions icp = yaml_to_ct_icp_options(odometry_node["ct_icp_options"]);
+        o.ct_icp_options = icp;
+    }
+    return o;
+}
+
+template <class Node>
+DatasetOptions yaml_to_dataset_options(const Node &dataset_node) {   // config.cpp:264-291
+    using namespace detail;
+    DatasetOptions o;
+    if (dataset_node["dataset"]) {   // DATASETFromString: case-insensitive, hilti is HILTI_2021
+        const std::string name = dataset_node["dataset"].template as<std::string>();
+        std::string lc = name;
+        std::transform(lc.begin(), lc.end(), lc.begin(), [](unsigned char c) { return (char) std::tolower(c); });
+        const std::map<std::string, std::string> names = {
+            {"kitti_carla", "KITTI_CARLA"}, {"kitti_360", "KITTI_360"}, {"kitti", "KITTI"}, {"hilti", "HILTI_2021"},
+            {"hilti_2021", "HILTI_2021"}, {"hilti_2022", "HILTI_2022"}, {"kitti_raw", "KITTI_raw"}, {"nclt", "NCLT"},
+            {"synthetic", "SYNTHETIC"}, {"ply_directory", "PLY_DIRECTORY"}};
+        auto it = names.find(lc);
+        if (it == names.end()) throw std::runtime_error("The `dataset` name: " + name + " is invalid.");
+        o.dataset = it->second;
+    }
+    yaml_clause<std::string>(dataset_node, "root_path", o.root_path);
+    yaml_clause<bool>(dataset_node, "fail_if_incomplete", o.fail_if_incomplete);
+    yaml_clause<float>(dataset_node, "min_dist_lidar_center", o.min_dist_lidar_center);
+    yaml_clause<int>(dataset_node, "nclt_num_aggregated_pc", o.nclt_num_aggregated_pc);
+    yaml_clause<float>(dataset_node, "max_dist_lidar_center", o.max_dist_lidar_center);
+    yaml_clause<bool>(dataset_node, "use_all_datasets", o.use_all_datasets);
+    if (dataset_node["sequence_options"]) {
+        o.sequence_options.clear();
+        for (const auto &seq_node : dataset_node["sequence_options"]) {
+            SequenceOptions s;
+            yaml_clause<std::string>(seq_node, "sequence_name", s.sequence_name);
+            yaml_clause<int>(seq_node, "start_frame_id", s.start_frame_id);
+            yaml_clause<int>(seq_node, "max_num_frames", s.max_num_frames);
+            o.sequence_options.push_back(s);
+        }
+    }
+    return o;
+}
+
+template <class Node>
+std::vector<DatasetOptions> yaml_to_dataset_options_vector(const Node &node) {   // config.cpp:294-301
+    std::vector<DatasetOptions> out;
+    for (const auto &child : node) out.push_back(yaml_to_dataset_options(child));
+    return out;
+}
+
+}  // namespace ct_icp
